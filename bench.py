@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- decoded cimbar frames/s (1024x1024 mode B) on N B200s, with roofline and CPU baseline.
+"""bench.py -- decoded cimbar frames/s (1024x1024 mode B) on N H100s, with roofline and CPU baseline.
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run, one rank per GPU)
     python bench.py --impl reference ...                      (the CPU restatement of the reference on the host cores)
@@ -7,7 +7,10 @@
 One "step" = one pass of the decode hot path over one batch of synthetic frames resident in HBM:
   K1 fused preprocess+ahash+colour -> K1x exact-walk check -> bit pack -> RS(155,125) -> fountain-chunk masks,
   then (N>1) one NCCL gather of the decoded chunk records to rank 0.
-Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for the definitions of every field."""
+Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for the definitions of every field.
+
+    --dump-outputs DIR   after the timed steps, write what the last timed step returned as DIR/<name>.npy (see dump_outputs);
+                         the inputs are generated from fixed seeds, so two builds run with the same arguments can be compared."""
 import argparse
 import json
 import os
@@ -30,7 +33,7 @@ def metric_name(mode_val):
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--frames", type=int, default=10000, help="frames per GPU per step (BASELINE config: 10k)")
@@ -60,7 +63,14 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--ref-sample", type=int, default=0, help="frames per step for --impl reference (0 = auto)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the decoded chunks, chunk masks and fallback flags of the last timed step to DIR/*.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "ours" or args.camera or args.fountain):
+        ap.error("--dump-outputs is written by the frame-decode benchmark (not --impl reference, --camera or --fountain)")
+    return args
 
 
 def measured_peak_gbs():
@@ -70,18 +80,27 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not a measured peak)"
 
 
-def k1_traffic_bytes():
-    """dram bytes per K1 launch from the committed ncu capture, scaled per frame; None until one exists."""
-    p = os.path.join(ROOT, "profiles", "k1_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+DUMP_BYTES = 48 << 20     # float32 chunk bytes of the sampled frames; with the per-frame arrays well under 64 MB in all
+
+
+def dump_outputs(out_dir, chunks, mask, fflags):
+    """what the timed path hands its caller, from the last timed step: the decoded chunk bytes (n x data_bytes), the chunk
+    bitmask of every frame and the per-frame flags (bit 0: the frame went through the exact flood walk).  The chunk bytes of
+    a large batch are a fixed, seeded sample of frames (frame_index.npy says which); every value is exact in float32/64."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n, row = chunks.shape
+    keep = min(n, max(1, DUMP_BYTES // (4 * row)))
+    idx = np.arange(n) if keep == n else np.sort(np.random.default_rng(0).choice(n, keep, replace=False))
+    sel = chunks[torch.from_numpy(idx).to(chunks.device)].cpu().numpy()
+    np.save(os.path.join(out_dir, "chunks.npy"), sel.astype(np.float32))
+    np.save(os.path.join(out_dir, "frame_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "chunk_mask.npy"), mask.cpu().numpy().astype(np.uint32).astype(np.float64))
+    np.save(os.path.join(out_dir, "frame_flags.npy"), fflags.cpu().numpy().astype(np.float32))
 
 
 class ClockSampler(threading.Thread):
@@ -436,7 +455,6 @@ def run_ours(args):
     stage_ms = [sum(r[i] for r in k_ms) / len(k_ms) for i in range(len(k_ms[0]))]
     peak, peak_src = measured_peak_gbs()
     achieved = B * K1_ALGO_BYTES / (k1_ms * 1e-3) / 1e9
-    traffic = k1_traffic_bytes()
     out = {
         "metric": metric_name(MV), "value": world * B * K / (elapsed_ms * 1e-3), "unit": UNIT, "n_gpus": world, "steps": K, "warmup": max(W, 3),
         "ms_per_step": elapsed_ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -448,7 +466,7 @@ def run_ours(args):
                    "(K1 fused threshold+ahash+colour, K1x exact-walk check, RS(%d,%d) with fused de-interleave, chunk masks)" % (
                        B, info.image_size_x, info.image_size_y, MODE_NAMES[MV], info.ecc_block_size, info.ecc_block_size - info.ecc_bytes),
                    "mode": "%s (%d)" % (MODE_NAMES[MV], MV), "frames_per_gpu_per_step": B, "color_correction": args.color_correction, "sharpen": bool(args.sharpen),
-                   "l2": "input %.1f GB per step >> 126 MB L2 (no flush needed)" % (B * info.frame_bytes / 1e9),
+                   "l2": "input %.1f GB per step >> 50 MB L2 (no flush needed)" % (B * info.frame_bytes / 1e9),
                    "parallelism": "frames sharded one-per-GPU (dp%d); chunk records to rank 0 by %s" % (world, {
                        None: "nothing (one GPU)", "window": "copy-engine pushes into a window in rank 0's HBM (CUDA IPC peer mapping over NVLink, device-side epochs, side stream: overlaps the next decode)",
                        "window-direct": "direct NVLink stores of the RS kernels into rank 0's HBM (CUDA IPC window, device-side epochs)",
@@ -461,17 +479,16 @@ def run_ours(args):
         "roofline": {"kernel": "k1_decode_kernel", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                      "frac": achieved / peak, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": B * K1_ALGO_BYTES,
-                     "traffic": (traffic["dram_bytes_per_frame"] * B if traffic else None),
-                     "traffic_source": (traffic["source"] if traffic else None),
-                     "note": "K1 is bound by instruction issue and dependency latency, not by HBM: the same TMA pipeline with the decode "
-                             "switched off (CB200_K1_L2_AHEAD=4096, tools/k1_sweep.py) copies at 7.4-7.5 TB/s on this GPU "
-                             "(profiles/r02_results.md)"},
+                     "note": "algorithmic bytes (each frame read once, one result byte per cell) over K1's event-timed "
+                             "kernel time"},
         "clocks": sampler.summary(),
     }
     if e2e:
         out["e2e"] = e2e
     if e2e_single:
         out["e2e_single_frame"] = e2e_single
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, chunks, mask, fflags)
     if world == 1 and not args.no_cpu_baseline:
         out["cpu_baseline"] = cpu_baseline_from_device_frames(frames, info, MV, stage_ms[3] / B)
     print(json.dumps(out))

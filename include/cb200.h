@@ -1,5 +1,5 @@
 /*
- * cb200.h -- C ABI of libcb200.so: the B200 (sm_100a) implementation of libcimbar's per-frame decode hot path.
+ * cb200.h -- C ABI of libcb200.so: the H100 (sm_90a) implementation of libcimbar's per-frame decode hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference (sz3/libcimbar) has no plugin registry: the path sits
  * behind header-only C++ templates (Decoder / CimbReader / CimbDecoder) and one facade C ABI (cimbard_*,

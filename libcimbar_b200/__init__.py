@@ -1,4 +1,4 @@
-"""libcimbar_b200 -- B200 (sm_100a) implementation of libcimbar's per-frame decode hot path.
+"""libcimbar_b200 -- H100 (sm_90a) implementation of libcimbar's per-frame decode hot path.
 
 This Python module is only plumbing around the C ABI of lib/libcb200.so (include/cb200.h): it loads the
 shared library with ctypes and passes raw pointers (numpy host buffers or torch device pointers).  There is

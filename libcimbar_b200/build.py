@@ -1,10 +1,11 @@
-"""Builds libcimbar_b200/lib/libcb200.so (the C-ABI shared library) with nvcc for sm_100a, in-tree.
+"""Builds libcimbar_b200/lib/libcb200.so (the C-ABI shared library) with nvcc for sm_90a (H100), in-tree.
 
     python -m libcimbar_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the built .so is git-ignored but travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU; the built .so is git-ignored.
 Every .cu is compiled to its own object (in parallel, only when it or a header changed) and the objects are linked."""
 import os
+import shutil
 import subprocess
 import sys
 from concurrent.futures import ThreadPoolExecutor
@@ -15,8 +16,8 @@ OBJ = os.path.join(HERE, "lib", "obj")
 LIB = os.path.join(HERE, "lib", "libcb200.so")
 SOURCES = ["api.cu", "k1_decode.cu", "k1x_flood.cu", "k2_rs.cu", "render.cu", "encode.cu", "host_sink.cu", "ccm.cu",
            "gather.cu", "deskew.cu", "scan.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC"]
-NVCC_FLAGS += os.environ.get("CB200_NVCC_EXTRA", "").split()      # tuning only: -D switches of compile-time variants (A/B on the GPU box)
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC"]
+NVCC_FLAGS += os.environ.get("CB200_NVCC_EXTRA", "").split()      # tuning only: -D switches of compile-time variants (A/B comparisons)
 
 
 def _nvcc():
@@ -62,7 +63,7 @@ def build(force=False, verbose=False):
         for rc in ex.map(lambda j: subprocess.call(j), jobs):
             if rc != 0:
                 raise subprocess.CalledProcessError(rc, "nvcc")
-    link = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + \
+    link = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB] + \
            [os.path.join(OBJ, s[:-3] + ".o") for s in _sources()] + ["-ldl"]
     if verbose:
         print(" ".join(link))
@@ -88,25 +89,21 @@ def build_facade(force=False, verbose=False):
 
 
 WIREHAIR_LIB = os.path.join(HERE, "lib", "libwirehair.so")
-WIREHAIR_SRC = "/root/reference/src/third_party_lib/wirehair"
+ORACLE_DIR = os.path.join(HERE, "..", "oracle")
+WIREHAIR_REF = os.path.join(ORACLE_DIR, "_ref", "libwirehair.so")
 
 
 def build_wirehair(force=False, verbose=False):
-    """wirehair -- the reference's third-party fountain codec (P15, stays on the rank-0 host) -- as a shared library of its own:
-    its four translation units compiled UNMODIFIED from where they lie in the reference checkout (nothing is copied into this
-    repository).  Where the checkout is absent (the GPU box) the prebuilt file that travelled with the snapshot is used.
-    The product binds it at run time (cb200_sink_create_wirehair), exactly as libcimbar links it."""
-    if not os.path.isdir(WIREHAIR_SRC):
+    """lib/libwirehair.so: wirehair -- the reference's third-party fountain codec (P15, stays on the rank-0 host) -- as a shared
+    library of its own, which the product binds at run time (cb200_sink_create_wirehair), exactly as libcimbar links it.
+    oracle/Makefile (target ref) compiles its four translation units unmodified from a checkout of the reference into
+    oracle/_ref/ (nothing is copied into this repository); that build is copied next to libcb200.so.  Returns None where
+    neither a checkout nor a built oracle/_ref/libwirehair.so exists."""
+    if not os.path.exists(WIREHAIR_REF):
         return WIREHAIR_LIB if os.path.exists(WIREHAIR_LIB) else None
-    srcs = [os.path.join(WIREHAIR_SRC, f) for f in ("wirehair.cpp", "gf256.cpp", "WirehairCodec.cpp", "WirehairTools.cpp")]
-    if not force and os.path.exists(WIREHAIR_LIB) and all(os.path.getmtime(x) <= os.path.getmtime(WIREHAIR_LIB) for x in srcs):
-        return WIREHAIR_LIB
-    os.makedirs(os.path.dirname(WIREHAIR_LIB), exist_ok=True)
-    cmd = ["g++", "-std=c++11", "-O3", "-mavx2", "-mssse3", "-fPIC", "-shared", "-I" + os.path.join(WIREHAIR_SRC, "include"),
-           "-I" + WIREHAIR_SRC, "-o", WIREHAIR_LIB] + srcs
-    if verbose:
-        print(" ".join(cmd))
-    subprocess.check_call(cmd)
+    if force or not os.path.exists(WIREHAIR_LIB) or os.path.getmtime(WIREHAIR_LIB) < os.path.getmtime(WIREHAIR_REF):
+        os.makedirs(os.path.dirname(WIREHAIR_LIB), exist_ok=True)
+        shutil.copy2(WIREHAIR_REF, WIREHAIR_LIB)
     return WIREHAIR_LIB
 
 

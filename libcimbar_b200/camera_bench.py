@@ -181,7 +181,7 @@ def run(args, ClockSampler, measured_peak_gbs):
         "data": "the reference's sample photographs 6bit/4_30_f0_627.jpg and 4_30_f2_246.jpg (960 x 1280), replicated",
         "config": {"workload": "camera path (SURVEY 8f-2): %d photographs of %d x %d per step: Scanner::scan (k_scan_blur, k_scan_otsu, "
                                "k_scan_anchors) -> corners -> k_deskew -> decode (K1 sharpen + exact walk K1x + RS)" % (B, w, h),
-                   "mode": "4C (4)", "pictures_per_step": B, "l2": "input %.2f GB per step >> 126 MB L2" % (B * w * h * 3 / 1e9)},
+                   "mode": "4C (4)", "pictures_per_step": B, "l2": "input %.2f GB per step >> 50 MB L2" % (B * w * h * 3 / 1e9)},
         "parity": "%d of %d chunks decoded per step (tests/test_gpu_scan.py checks the bytes against the CPU pipeline)" % (good_chunks, B * info.chunks_per_frame),
         "gpu_launches": launches,
         "kernel_ms_per_step": {"scan_blur_hist": blur_ms, "scan_otsu": otsu_ms, "scan_anchors": anch_ms},

@@ -1,6 +1,6 @@
 // api.cu -- the C ABI of libcb200.so (include/cb200.h): context, tables, and the kernel pipelines.
 // There is no CPU decode path in this library: every entry point that produces decode results launches the
-// sm_100a kernels, and cb200_create fails with CB200_ERR_NODEVICE when no CUDA device is usable.
+// sm_90a kernels, and cb200_create fails with CB200_ERR_NODEVICE when no CUDA device is usable.
 #include "ctx.cuh"
 #include "k1_decode.cuh"
 #include "k2_rs.cuh"
@@ -379,7 +379,7 @@ static int create_impl(cb200_ctx* c, int device, int mode_val, int max_frames)
     if (const char* e = getenv("CB200_K1_CTAS_PER_SM")) c->k1_ctas_per_sm = atoi(e);
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
-    if (prop.major < 10) return fail(CB200_ERR_NODEVICE, "libcb200 is built for sm_100a only");
+    if (prop.major != 9 || prop.minor != 0) return fail(CB200_ERR_NODEVICE, "libcb200 is built for sm_90a (compute capability 9.0) only");
     c->sm_count = prop.multiProcessorCount;
     CK(cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking), "cudaStreamCreate");
     c->stream = c->own_stream;

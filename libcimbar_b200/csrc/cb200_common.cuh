@@ -1,4 +1,4 @@
-// cb200_common.cuh -- shared definitions for the sm_100a decode kernels.
+// cb200_common.cuh -- shared definitions for the sm_90a decode kernels.
 // Geometry mirrors cimbar::conf (reference: src/lib/cimb_translator/GridConf.h:8-190, Config.h:20-175).
 #pragma once
 

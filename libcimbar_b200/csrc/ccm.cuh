@@ -1,4 +1,4 @@
-// ccm.cuh -- colour correction matrix (CCM): the float side path of the colour decode, sm_100a.
+// ccm.cuh -- colour correction matrix (CCM): the float side path of the colour decode, sm_90a.
 //
 // Reference (file:line relative to /root/reference/):
 //   color_correction::transform            src/lib/chromatic_adaptation/color_correction.h:64-68  (cv::Matx<float,3,3> * vec)

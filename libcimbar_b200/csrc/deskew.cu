@@ -1,4 +1,4 @@
-// deskew.cu -- the extractor's deskew in front of the decode path (SURVEY.md 8f-2), sm_100a.
+// deskew.cu -- the extractor's deskew in front of the decode path (SURVEY.md 8f-2), sm_90a.
 //
 // Replaces (reference file:line relative to /root/reference/):
 //   Deskewer::deskew        src/lib/extractor/Deskewer.h:25-40: cv::getPerspectiveTransform(corners, outputPoints) +

@@ -9,7 +9,7 @@
 //   push   (cb200_gather_push, the default of the drivers): the decode writes into local buffers, and a copy-engine transfer on
 //          a side stream of the context moves them through the peer mapping -- no SM is involved, the transfer of step i runs
 //          under the decode of step i + 1, and eight ranks finishing their RS kernels at the same moment do not pile their
-//          stores up on rank 0's NVLink ingress (measured on 8 GPUs: the direct stores below cost 1 ms per 6 ms step);
+//          stores up on rank 0's NVLink ingress;
 //   direct (cb200_gather_slot gives the pointers to hand to cb200_decode_chunks_dev): the RS kernel of rank r writes its
 //          corrected bytes, and the chunk-mask kernel its masks, STRAIGHT INTO rank 0's memory, tile by tile while the decode
 //          runs.  Fine for two to four ranks.

@@ -1,4 +1,4 @@
-// k1_decode.cu -- K1: fused preprocess + average-hash + colour kernel for clean (drift-0) frames, sm_100a.
+// k1_decode.cu -- K1: fused preprocess + average-hash + colour kernel for clean (drift-0) frames, sm_90a.
 //
 // Replaces, for one RGB8 frame resident in HBM (reference file:line relative to /root/reference/):
 //   P1  preprocessSymbolGrid            src/lib/cimb_translator/CimbReader.cpp:30-46  (cvtColor + adaptiveThreshold(5, C=0))
@@ -219,12 +219,11 @@ __device__ __forceinline__ uint32_t thread_symbol_search(const K1Smem& s, uint32
 }
 
 // ---------------------------------------------------------------------------------------------- the kernel
-// 128 threads (8 px each), 4 CTAs/SM.  The kernel is bound by instruction issue and dependency latency, not by HBM: the same
-// TMA pipeline with the decode switched off copies at 7.4-7.5 TB/s (CB200_K1_L2_AHEAD=4096), with it 5.6 TB/s.  Shared memory
-// per CTA is 41 KB -- the raw rows of exactly one stage (every raw byte is consumed before the stage barrier, so the next
+// 128 threads (8 px each), 4 CTAs/SM.  On an H100 it reads frames at 0.90 of the 3.35 TB/s data-sheet HBM3 bandwidth.  Shared
+// memory per CTA is 41 KB -- the raw rows of exactly one stage (every raw byte is consumed before the stage barrier, so the next
 // stage lands in the same place while the box sums and the symbols run) plus a 9 KB exchange array for the box-filter halo
-// words -- which would admit five CTAs per SM; measured, five CTAs at the 96 registers that requires lose to four at 128
-// (5.96 vs 5.63 ms per 10 000 frames: the scheduler needs the registers to keep a stage's loads in flight), so the cap is 128.
+// words -- which would admit five CTAs per SM; five CTAs would need 96 registers, and the scheduler needs 128 to keep a stage's
+// loads in flight, so the cap is 128.
 // One barrier per stage.  Iteration for stage `it` (cell row k, raw rows [y_k+2, y_k+10]):
 //   wait full[it&1]
 //   A(k):   gray of the thread's 8 px in each of the 9 rows -> packed pairs in registers; one halo word E_r per row

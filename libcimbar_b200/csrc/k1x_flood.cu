@@ -1,4 +1,4 @@
-// k1x_flood.cu -- K1x: the exact flood-walk decode for frames the drift-0 pass (K1) cannot prove exact, sm_100a.
+// k1x_flood.cu -- K1x: the exact flood-walk decode for frames the drift-0 pass (K1) cannot prove exact, sm_90a.
 //
 // Restates the reference's serial semantics on the device (reference file:line relative to /root/reference/):
 //   P1  preprocessSymbolGrid (+ sharpen)      src/lib/cimb_translator/CimbReader.cpp:17-46 (full frame, OpenCV borders)

@@ -1,4 +1,4 @@
-// k2_rs.cu -- K2: de-interleave/bit-pack + Reed-Solomon block correction + fountain-chunk masks, sm_100a.
+// k2_rs.cu -- K2: de-interleave/bit-pack + Reed-Solomon block correction + fountain-chunk masks, sm_90a.
 //
 // Replaces (reference file:line relative to /root/reference/):
 //   P7/P10 Decoder::do_decode bit packing     src/lib/encoder/Decoder.h:77-117 (:121-161 coupled), Interleave.h:8-36,

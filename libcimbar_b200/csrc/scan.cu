@@ -1,4 +1,4 @@
-// scan.cu -- the extractor's anchor scan on the device (SURVEY.md 8f-2: the step in front of the deskew), sm_100a.
+// scan.cu -- the extractor's anchor scan on the device (SURVEY.md 8f-2: the step in front of the deskew), sm_90a.
 //
 // Replaces, for a batch of camera pictures resident in HBM (reference file:line relative to /root/reference/src/lib/extractor/):
 //   Scanner::Scanner / preprocess_image(fast)   Scanner.h:146-174   cvtColor(RGB2GRAY) + GaussianBlur(unit x unit, sigma 0) + Otsu
@@ -14,8 +14,8 @@
 //   k_scan_anchors   one CTA per picture runs scan_core.cuh's scan_picture: the rows of a t1 pass and the confirmation chains
 //                    of its hits are spread over the threads, the order-dependent tail (on_t1_scan's shadow test, libstdc++'s
 //                    std::sort, the bottom-right window) runs on thread 0
-// The pixel work (gray/blur/histogram) moves 3 bytes in and 1 out per pixel (measured: 0.36 of the HBM copy peak, bound by
-// instruction issue); the scan itself touches ~60 rows and a few hundred short lines of the blurred picture.
+// The pixel work (gray/blur/histogram) moves 3 bytes in and 1 out per pixel (bound by
+// instruction issue, not by HBM); the scan itself touches ~60 rows and a few hundred short lines of the blurred picture.
 #include "ctx.cuh"
 #include "scan_core.cuh"
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Everything goes through the C ABI of libcb200.so and is
+"""GPU parity tests (run on an H100: pytest -m gpu).  Everything goes through the C ABI of libcb200.so and is
 compared bit for bit with the CPU oracle (itself pinned to the reference's goldens, tests/test_oracle_goldens.py),
 with the reference's SHA-256 goldens directly, and with size-independent round-trip properties."""
 import ctypes as C
@@ -139,7 +139,7 @@ def test_whole_frame_schedule_every_mode(cb, mode_val):
     run_cells); every mode -- incl. the non-1024x1024 geometries 66 (736x637) and 67 (1024x720) and the legacy coupled
     layouts 4C / 8C (Decoder.h:121-161, GridConf.h:144-189) -- must give the same bits there as the oracle."""
     m, payloads, frames = synth_frames(mode_val, 5, seed=200 + mode_val)
-    n = 640                                                     # > 4 x 148 CTAs
+    n = 640                                                     # > 4 x 132 CTAs (H100)
     big = np.concatenate([frames] * (n // 5))
     ctx = cb.Context(mode_val, max_frames=n)
     assert n >= 4 * ctx.info.sm_count, "test sized for <= 160 SMs"
