@@ -17,7 +17,6 @@ LIB = os.path.join(HERE, "lib", "libcb200.so")
 SOURCES = ["api.cu", "k1_decode.cu", "k1x_flood.cu", "k2_rs.cu", "render.cu", "encode.cu", "host_sink.cu", "ccm.cu",
            "gather.cu", "deskew.cu", "scan.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC"]
-NVCC_FLAGS += os.environ.get("CB200_NVCC_EXTRA", "").split()      # tuning only: -D switches of compile-time variants (A/B comparisons)
 
 
 def _nvcc():

@@ -10,7 +10,6 @@
 #include <atomic>
 #include <cmath>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -297,21 +296,18 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, CellTra
         int rc = ccm_arg(c, cc); if (rc) return rc;
     }
     const bool sharpen = (flags & CB200_FLAG_SHARPEN) != 0;
-    // a cell trace needs the walk itself; CB200_K1_SHARPEN=0 (tests, A/B) sends sharpened frames straight to the exact-walk kernel
-    // as rounds 1-2 did
-    const bool k1_sharpen = !(getenv("CB200_K1_SHARPEN") && atoi(getenv("CB200_K1_SHARPEN")) == 0);
-    const bool exact_only = (sharpen && !k1_sharpen) || d_trace != nullptr;
+    const bool exact_only = d_trace != nullptr;   // a cell trace needs the walk itself
     CK(cudaMemsetAsync(c->d_dirty, 0, sizeof(uint32_t) * (size_t)n, st), "memset dirty");
     if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; }
     mark(c);                                   // ev0: before K1
     if (!exact_only) {
         // bands: whole frames when there are enough of them to fill the machine, else split frames into bands of cell rows
-        int ctas = c->sm_count * k1_ctas_per_sm(sharpen, c->k1_ctas_per_sm);
+        int ctas = c->sm_count * k1_ctas_per_sm(sharpen);
         int bands = 1;
         if (n < ctas) { bands = (ctas + n - 1) / n; if (bands > m.cells_y / 4) bands = m.cells_y / 4; if (bands < 1) bands = 1; }
         int units = n * bands;
         int grid = units < ctas ? units : ctas;
-        CK(k1_launch(m, d_rgb, n, bands, grid, c->l2_ahead, sharpen, c->d_cellvals, c->d_dirty, cc, st), "k1 launch");
+        CK(k1_launch(m, d_rgb, n, bands, grid, sharpen, c->d_cellvals, c->d_dirty, cc, st), "k1 launch");
     }
     mark(c);                                   // ev1: after K1
     // frames K1 flagged (or all of them when exact_only) are re-done by the exact walk on the same preprocessing (sharpen or not)
@@ -375,8 +371,6 @@ static int create_impl(cb200_ctx* c, int device, int mode_val, int max_frames)
     if (!mode_init(c->mode, mode_val)) return fail(CB200_ERR_MODE, "unsupported mode_val");
     const Mode& m = c->mode;
     c->device = device; c->max_frames = max_frames;
-    if (const char* e = getenv("CB200_K1_L2_AHEAD")) c->l2_ahead = atoi(e);
-    if (const char* e = getenv("CB200_K1_CTAS_PER_SM")) c->k1_ctas_per_sm = atoi(e);
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
     if (prop.major != 9 || prop.minor != 0) return fail(CB200_ERR_NODEVICE, "libcb200 is built for sm_90a (compute capability 9.0) only");

@@ -39,8 +39,6 @@ struct cb200_ctx {
     uint8_t* d_gen = nullptr;        // RS generator polynomial, ecc_bytes+1 coefficients
     uint8_t* d_rho = nullptr;        // 4 x 64 bytes: x^(D+j) mod x^pad g, the basis of K2's remainder tables (k2_remainder_basis)
     // per-kernel timing (cb200_set_timing): events around every launch of the last pipeline call
-    int l2_ahead = 0;                // K1: TMA L2-prefetch distance in stages (CB200_K1_L2_AHEAD overrides, tuning only)
-    int k1_ctas_per_sm = 4;          // K1: resident CTAs per SM the grid is sized for (CB200_K1_CTAS_PER_SM, tuning only)
     bool timing = false;
     static constexpr int kEvSets = 64;
     cudaEvent_t ev[kEvSets][8] = {};

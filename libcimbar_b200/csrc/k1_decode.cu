@@ -23,14 +23,11 @@
 #include "cb200_common.cuh"
 #include "k1_decode.cuh"
 #include "ccm.cuh"
-#include <cstdlib>
 
 namespace cb200 {
 
 constexpr int kK1Threads = 128;            // 128 threads x 8 px = one full 1024-px row
-#ifndef CB200_K1_MIN_CTAS
-#define CB200_K1_MIN_CTAS 4                // resident CTAs per SM the register allocation is capped for (4 -> 128 registers, 5 -> 96)
-#endif
+constexpr int kK1CtasPerSm = 4;            // resident CTAs per SM without sharpen: caps the registers at 128 (5 -> 96)
 constexpr int kStageRows = 9;              // raw rows per cell row (stage)
 constexpr int kMaxW = 1024;
 constexpr int kRastPitch = 144;            // bytes per raster row: 1024 bits + funnel-shift overread pad
@@ -84,12 +81,6 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
 {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-// TMA prefetch of a linear global range into L2 (no shared memory needed): keeps DRAM requests in flight several stages
-// ahead of the shared-memory ring (SASS: UBLKPF)
-__device__ __forceinline__ void tma_prefetch_l2(const void* src_gmem, uint32_t bytes)
-{
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src_gmem), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void consumer_sync() { __syncthreads(); }
 
@@ -246,9 +237,9 @@ __device__ __forceinline__ uint32_t thread_symbol_search(const K1Smem& s, uint32
 //   a0-4 .. a0+4 = y_k .. y_k+8, S(k-1).  Frame borders are never reached: the cell windows stay 3 pixels inside.
 // A lane-level numpy model of exactly this schedule is checked against the oracle in tests/test_k1_sharpen_model.py.
 template <int NC, bool G1024, int CM, bool SH>
-__global__ void __launch_bounds__(kK1Threads, SH ? 3 : CB200_K1_MIN_CTAS)
-k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, int bands, int l2_ahead_arg,
-                 uint8_t* __restrict__ cellvals, uint32_t* __restrict__ dirty_flags, const CcmArg cc)
+__global__ void __launch_bounds__(kK1Threads, SH ? 3 : kK1CtasPerSm)
+k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, int bands, uint8_t* __restrict__ cellvals,
+                 uint32_t* __restrict__ dirty_flags, const CcmArg cc)
 {
     // G1024: the 1024x1024 / 112x112-cell geometry of modes B, 4C and 8C as compile-time constants (GridConf.h:121-141);
     // the other modes (Bm 1024x720, Bu 736x637) take every dimension from the Mode struct
@@ -327,24 +318,11 @@ k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, i
         mbar_expect_tx(bar, stage_bytes);
         tma_bulk_g2s(s.ring, c.src, stage_bytes, bar);
     };
-    // two cursors over that stream, each owned by one thread: thread 0 feeds the shared-memory ring (TMA), the first thread of
-    // warp 1 runs l2_ahead stages further ahead and only prefetches into L2 -- the per-stage cursor arithmetic is spread over
-    // two warps, so no warp arrives at the stage barrier much later than the others.
-    // (l2_ahead carries two tuning bits: 0x1000 = copy only, no decode: the ceiling of the load pipeline; 0x2000 = both cursors
-    //  in thread 0, as in round 1)
-    const bool load_only = (l2_ahead_arg & 0x1000) != 0;
-    const int l2_ahead = l2_ahead_arg & 0xFFF;
-    const int pf_tid = (l2_ahead_arg & 0x2000) ? 0 : 32;
-    Cursor nxt, pre;                              // next stage to load into shared memory / to prefetch into L2
-    nxt.u = blockIdx.x; nxt.valid = false; pre.u = blockIdx.x; pre.valid = false;
+    Cursor nxt;                                   // next stage to load into shared memory (thread 0's)
+    nxt.u = blockIdx.x; nxt.valid = false;
     if (tid == 0) {
         cursor_unit(nxt);
         if (nxt.valid) { issue_stage(nxt, 0u); cursor_next(nxt); }
-    }
-    if (tid == pf_tid && l2_ahead > 0) {
-        cursor_unit(pre);
-        if (pre.valid) cursor_next(pre);
-        for (int i = 0; i < l2_ahead && pre.valid; ++i) { tma_prefetch_l2(pre.src, stage_bytes); cursor_next(pre); }
     }
 
     // symbol stage for one cell row from a finished raster (P5/P6 at drift 0) + the colour decided earlier.
@@ -435,12 +413,6 @@ k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, i
             const uint32_t buf = it & 1u, ph = (it >> 1) & 1u;
             uint8_t* const ub[3] = {s.ring, s.ring + 3u * row_bytes, s.ring + 6u * row_bytes};   // stage rows 0-2, 3-5, 6-8
             mbar_wait(&s.full_bar[buf], ph);
-            if (load_only) {                               // tuning only: the stage is dropped as soon as it has landed
-                __syncthreads();
-                if (tid == 0 && nxt.valid) { issue_stage(nxt, it + 1u); cursor_next(nxt); }
-                if (tid == pf_tid && l2_ahead > 0 && pre.valid) { tma_prefetch_l2(pre.src, stage_bytes); cursor_next(pre); }
-                continue;
-            }
 
             // ---------------- A(k): gray, packed pairs P[r][j] = (g[j], g[j+4]); halo word E_r = (g0,g1,g6,g7)
             uint32_t P[kStageRows][4];
@@ -504,7 +476,6 @@ k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, i
             __syncthreads();
             // the raw rows are dead now (gray is in registers, the colour sums are taken): the next stage may overwrite them
             if (tid == 0 && nxt.valid) { issue_stage(nxt, it + 1u); cursor_next(nxt); }
-            if (tid == pf_tid && l2_ahead > 0 && pre.valid) { tma_prefetch_l2(pre.src, stage_bytes); cursor_next(pre); }
 
             // ---------------- B(k): 5x5 box sum, threshold, raster rows 1..9 (row 0 = row 9 of the previous stage)
             if constexpr (!SH) {
@@ -614,7 +585,6 @@ k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, i
         }
         // the last cell row of the unit still needs its symbols: one more barrier to see its complete raster
         __syncthreads();
-        if (load_only) continue;
         symbol_stage(k1 - 1, (it - 1u) & 1u, col_prev, out, any_dirty);
         if (any_dirty) atomicOr(&dirty_flags[f], (uint32_t)kFrameDirtyK1);
     }
@@ -670,7 +640,7 @@ cudaError_t k1_colors_launch(const Mode& m, const uint8_t* d_rgb, int n, uint8_t
 
 constexpr size_t kSharpenExtraSmem = sizeof(uint32_t) * kStageRows * kK1Threads;   // the second halo word of the sharpened rows
 size_t k1_smem_bytes(bool sharpen) { return sizeof(K1Smem) + (sharpen ? kSharpenExtraSmem : 0); }
-int k1_ctas_per_sm(bool sharpen, int plain) { return sharpen ? 3 : plain; }
+int k1_ctas_per_sm(bool sharpen) { return sharpen ? 3 : kK1CtasPerSm; }
 
 cudaError_t k1_init_tables(const float* adjust256, const unsigned long long* tiles_L16)
 {
@@ -678,7 +648,7 @@ cudaError_t k1_init_tables(const float* adjust256, const unsigned long long* til
     if (e != cudaSuccess) return e;
     e = cudaMemcpyToSymbol(c_tiles_L, tiles_L16, sizeof(unsigned long long) * 16);
     if (e != cudaSuccess) return e;
-    const int smem_max = (int)(sizeof(K1Smem) + kSharpenExtraSmem) + 64 * 1024;
+    const int smem_max = (int)(sizeof(K1Smem) + kSharpenExtraSmem);
 #define CB200_K1_ATTR2(NC, G, C, S) \
     if ((e = cudaFuncSetAttribute(k1_decode_kernel<NC, G, C, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)) != cudaSuccess) return e;
 #define CB200_K1_ATTR(NC, G, C) CB200_K1_ATTR2(NC, G, C, false) CB200_K1_ATTR2(NC, G, C, true)
@@ -690,15 +660,14 @@ cudaError_t k1_init_tables(const float* adjust256, const unsigned long long* til
     return cudaSuccess;
 }
 
-cudaError_t k1_launch(const Mode& m, const uint8_t* d_rgb, int n_frames, int bands, int grid, int l2_ahead, bool sharpen,
+cudaError_t k1_launch(const Mode& m, const uint8_t* d_rgb, int n_frames, int bands, int grid, bool sharpen,
                       uint8_t* d_cellvals, uint32_t* d_dirty, const CcmArg& cc, cudaStream_t stream)
 {
-    const int extra = getenv("CB200_K1_EXTRA_SMEM") ? atoi(getenv("CB200_K1_EXTRA_SMEM")) : 0;   // tuning only: lowers CTAs/SM
-    const size_t smem = k1_smem_bytes(sharpen) + extra;
+    const size_t smem = k1_smem_bytes(sharpen);
     const bool g1024 = m.width == 1024 && m.height == 1024 && m.cells_x == 112 && m.cells_y == 112 && m.corner == 6 &&
                        m.cell_offset == 8 && m.symbol_bits == 4;
     const int cm = cc.means ? 2 : (cc.active ? 1 : 0);
-#define CB200_K1_GO(NC, G, C, S) k1_decode_kernel<NC, G, C, S><<<grid, kK1Threads, smem, stream>>>(m, d_rgb, n_frames, bands, l2_ahead, d_cellvals, d_dirty, cc)
+#define CB200_K1_GO(NC, G, C, S) k1_decode_kernel<NC, G, C, S><<<grid, kK1Threads, smem, stream>>>(m, d_rgb, n_frames, bands, d_cellvals, d_dirty, cc)
 #define CB200_K1_SH(NC, G, C) do { if (sharpen) CB200_K1_GO(NC, G, C, true); else CB200_K1_GO(NC, G, C, false); } while (0)
 #define CB200_K1_CM(NC, G) do { if (cm == 2) CB200_K1_SH(NC, G, 2); else if (cm == 1) CB200_K1_SH(NC, G, 1); else CB200_K1_SH(NC, G, 0); } while (0)
     if (m.color_bits == 3) { if (g1024) CB200_K1_CM(8, true); else CB200_K1_CM(8, false); }

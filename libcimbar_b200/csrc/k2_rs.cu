@@ -16,7 +16,6 @@
 #include "cb200_common.cuh"
 #include "k2_rs.cuh"
 #include <cstring>
-#include <cstdlib>
 #include <cstdint>
 
 namespace cb200 {
@@ -783,10 +782,9 @@ cudaError_t k2_rs_fused_launch(const Mode& m, const uint8_t* d_cellvals, const u
                                uint8_t* d_ok, const uint8_t* d_rho, int sm_count, cudaStream_t st, int b_begin, int b_count)
 {
     if (b_count < 0) b_count = m.nblocks;
-    static const bool frames_off = getenv("CB200_K2_FRAMES") && atoi(getenv("CB200_K2_FRAMES")) == 0;   // tuning / A-B only
     const bool whole = b_begin == 0 && b_count == m.nblocks;
     const bool bits_ok = m.symbol_bits == 4 && m.color_bits == 2 && (!m.legacy || (size_t)m.num_cells * 6 == (size_t)m.cap_all * 8);
-    if (!frames_off && whole && bits_ok && m.ecc_block == kFrBlk && m.ecc_bytes <= 32 &&
+    if (whole && bits_ok && m.ecc_block == kFrBlk && m.ecc_bytes <= 32 &&
         m.ecc_bytes <= kLaDim && m.nblocks % 4 == 0 && kFrFrames * (m.nblocks / 4) <= kFrWarps && m.num_cells % 16 == 0 &&
         m.cap_sym % kFrBlk == 0 && (m.nblocks * m.msg_len) % 4 == 0 && ((uintptr_t)d_data & 3u) == 0 && n_frames > 0) {
         const int cell_pitch = m.num_cells;

@@ -6,8 +6,7 @@
 //                                                                   filter_candidates, sort_top_to_bottom) + add_bottom_right_corner
 //   Extractor::extract                          Extractor.h:30-46   scan -> Corners -> Deskewer (deskew.cu) -> NEEDS_SHARPEN test
 // Three kernels:
-//   k_scan_blur4<R>  (k_scan_blur<R>: the one-pixel-per-element first version, CB200_SCAN_BLUR=0)
-//                    gray + separable fixed-point Gaussian (OpenCV's 8-bit path: coefficients / 256 from its small-kernel
+//   k_scan_blur4<R>  gray + separable fixed-point Gaussian (OpenCV's 8-bit path: coefficients / 256 from its small-kernel
 //                    table, BORDER_REFLECT_101, (sum + 2^15) >> 16) in 128 x 32 tiles staged in shared memory, plus the
 //                    picture's 256-bin histogram (shared-memory atomics, one global atomic per bin and tile)
 //   k_scan_otsu      getThreshVal_Otsu_8u in double precision, one thread per picture (no FMA contraction)
@@ -19,7 +18,6 @@
 #include "ctx.cuh"
 #include "scan_core.cuh"
 
-#include <cstdlib>
 #include <vector>
 
 namespace cb200 {
@@ -64,56 +62,10 @@ __device__ __forceinline__ int reflect101_clamped(int p, int n)
 
 constexpr int kBlurTW = 128, kBlurTH = 32, kBlurThreads = 256;
 
-template <int R>
-__global__ void __launch_bounds__(kBlurThreads)
-k_scan_blur(const uint8_t* __restrict__ rgb, int w, int h, uint8_t* __restrict__ out, unsigned* __restrict__ hist)
-{
-    constexpr int GW = kBlurTW + 2 * R, GH = kBlurTH + 2 * R, KS = 2 * R + 1;
-    __shared__ uint8_t g[GH][GW];
-    __shared__ uint16_t hs[GH][kBlurTW];
-    __shared__ unsigned lh[256];
-    const int tid = threadIdx.x, pic = blockIdx.z, tx0 = blockIdx.x * kBlurTW, ty0 = blockIdx.y * kBlurTH;
-    const size_t npx = (size_t)w * (size_t)h;
-    const uint8_t* src = rgb + (size_t)pic * npx * 3;
-    lh[tid] = 0;
-    for (int i = tid; i < GH * GW; i += kBlurThreads) {
-        const int r = i / GW, c = i - r * GW;
-        const int y = reflect101_clamped(ty0 - R + r, h), x = reflect101_clamped(tx0 - R + c, w);
-        const uint8_t* p = src + ((size_t)y * w + x) * 3;
-        g[r][c] = (uint8_t)((9798u * p[0] + 19235u * p[1] + 3735u * p[2] + 16384u) >> 15);      // cvtColor(RGB2GRAY), 8 bit
-    }
-    __syncthreads();
-    for (int i = tid; i < GH * kBlurTW; i += kBlurThreads) {
-        const int r = i / kBlurTW, c = i - r * kBlurTW;
-        unsigned s = 0;
-#pragma unroll
-        for (int k = 0; k < KS; ++k) s += BlurK<R>::c(k) * g[r][c + k];
-        hs[r][c] = (uint16_t)s;                                   // <= 255 * 256
-    }
-    __syncthreads();
-    uint8_t* dst = out + (size_t)pic * npx;
-    for (int i = tid; i < kBlurTH * kBlurTW; i += kBlurThreads) {
-        const int r = i / kBlurTW, c = i - r * kBlurTW;
-        const int y = ty0 + r, x = tx0 + c;
-        if (y < h && x < w) {
-            unsigned s = 0;
-#pragma unroll
-            for (int k = 0; k < KS; ++k) s += BlurK<R>::c(k) * hs[r + k][c];
-            const unsigned v = (s + 32768u) >> 16;
-            dst[(size_t)y * w + x] = (uint8_t)v;
-            atomicAdd(&lh[v], 1u);
-        }
-    }
-    __syncthreads();
-    if (lh[tid]) atomicAdd(&hist[(size_t)pic * 256 + tid], lh[tid]);
-}
-
-// ---------------------------------------------------------------------------------------------- the same, four pixels per thread
-// k_scan_blur is bound by instruction issue (ncu: 85 % of the issue slots, 14 % of the DRAM bandwidth): a division per element for the
-// tile indexing, three byte loads and three multiplies per pixel of gray, byte-wise filter taps.  This version gives every thread four
-// consecutive pixels: the twelve RGB bytes come as three aligned words and are converted with K1's IDP.2A form (8 instructions per four
-// pixels), the horizontal taps are IDP.4A dot products of realigned gray words with the packed coefficients, the vertical pass reads
-// four 16-bit sums per 64-bit load, and a warp owns a tile row (no divisions).  Same arithmetic, same results.
+// The pixel work is bound by instruction issue, not by HBM, so every thread takes four consecutive pixels: the twelve RGB bytes come
+// as three aligned words and are converted with K1's IDP.2A form (8 instructions per four pixels), the horizontal taps are IDP.4A dot
+// products of realigned gray words with the packed coefficients, the vertical pass reads four 16-bit sums per 64-bit load, and a warp
+// owns a tile row (no divisions).
 // The word path needs 4-byte aligned rows: a picture width that is a multiple of four and an aligned base (checked by the caller);
 // otherwise, and in tiles that cross the right edge, pixels are fetched one by one.
 template <int R> struct BlurKW {     // the 2R+1 coefficients as bytes of up to three words (IDP.4A operands)
@@ -338,24 +290,13 @@ static int scan_run(cb200_ctx* c, const uint8_t* d_pics, int w, int h, int n)
     if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; }
     mark();
     const dim3 bgrid((unsigned)((w + kBlurTW - 1) / kBlurTW), (unsigned)((h + kBlurTH - 1) / kBlurTH), (unsigned)n);
-    // CB200_SCAN_BLUR=0 (tests, A/B): the one-pixel-per-element kernel
-    const bool blur4 = !(getenv("CB200_SCAN_BLUR") && atoi(getenv("CB200_SCAN_BLUR")) == 0);
     // aligned 32-bit accesses need rows that start on a word: width a multiple of four, base pointers aligned
     const int words_ok = (w % 4 == 0) && (reinterpret_cast<uintptr_t>(d_pics) % 4 == 0) && (reinterpret_cast<uintptr_t>(s->d_blur) % 4 == 0);
-    if (blur4) {
-        switch (R) {
-        case 1: k_scan_blur4<1><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
-        case 2: k_scan_blur4<2><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
-        case 3: k_scan_blur4<3><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
-        default: k_scan_blur4<4><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
-        }
-    } else {
-        switch (R) {
-        case 1: k_scan_blur<1><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, s->d_blur, s->d_hist); break;
-        case 2: k_scan_blur<2><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, s->d_blur, s->d_hist); break;
-        case 3: k_scan_blur<3><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, s->d_blur, s->d_hist); break;
-        default: k_scan_blur<4><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, s->d_blur, s->d_hist); break;
-        }
+    switch (R) {
+    case 1: k_scan_blur4<1><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
+    case 2: k_scan_blur4<2><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
+    case 3: k_scan_blur4<3><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
+    default: k_scan_blur4<4><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
     }
     count_launch();
     mark();

@@ -775,22 +775,21 @@ def test_sharpen_clean_batches_stay_on_k1(cb, mode_val, n):
     ctx.close()
 
 
-def test_sharpen_mixed_batch_and_the_old_route(cb, monkeypatch):
-    """camera frames in a sharpened batch are flagged by K1 and re-done by the exact walk on the sharpened raster; with
-    CB200_K1_SHARPEN=0 every frame takes that route (rounds 1-2): same bytes either way, and as the oracle's"""
+def test_sharpen_mixed_batch_and_the_walk_on_every_frame(cb):
+    """camera frames in a sharpened batch are flagged by K1 and re-done by the exact walk on the sharpened raster, with the
+    oracle's bytes; the walk forced on every frame (decode_cells) gives the oracle's cells and trace on the clean frames too"""
     m, payloads, frames = synth_frames(68, 3, seed=331)
     batch = np.stack([frames[0], load_sample("b/ex2434.jpg"), frames[1], load_sample("b/ex380.jpg"), frames[2]])
-    want = [ORA.decode_raw(m, fr, sharpen=True) for fr in batch]
+    want = [ORA.decode_raw(m, fr, sharpen=True, want_cells=True) for fr in batch]
     ctx = cb.Context(68, max_frames=5)
     raw, ff = ctx.decode_raw(batch, flags=cb.FLAG_SHARPEN)
     assert [int(x & cb.FRAME_FALLBACK) for x in ff] == [0, 1, 0, 1, 0]
-    monkeypatch.setenv("CB200_K1_SHARPEN", "0")
-    raw0, ff0 = ctx.decode_raw(batch, flags=cb.FLAG_SHARPEN)
-    monkeypatch.delenv("CB200_K1_SHARPEN")
-    assert all(int(x) & cb.FRAME_FALLBACK for x in ff0)
-    for f in range(5):
-        assert np.array_equal(raw[f], want[f]), f
-        assert np.array_equal(raw0[f], want[f]), f
+    cells, trace = ctx.decode_cells(batch, flags=cb.FLAG_SHARPEN)
+    for f, (want_raw, ocells) in enumerate(want):
+        assert np.array_equal(raw[f], want_raw), f
+        for k in ("order", "x", "y", "drift_offset", "distance"):
+            assert np.array_equal(trace[f][k], ocells[k]), (f, k)
+        assert np.array_equal(cells[f] & 15, ocells["symbol"]) and np.array_equal((cells[f] >> 4) & 7, ocells["color"]), f
     ctx.close()
 
 
@@ -814,10 +813,10 @@ def test_sharpen_with_noise_tiles_and_colour_correction(cb):
 
 
 @pytest.mark.parametrize("mode_val", [68, 66])
-def test_sharpen_raster_of_the_exact_walk(cb, mode_val, monkeypatch):
+def test_sharpen_raster_of_the_exact_walk(cb, mode_val):
     """K1x's streaming sharpen raster (k_flood_raster_fast_sharpen: OpenCV's borders, reflect for the filter, replicate for the
-    box sum) against the oracle and against the round-1 shared-memory kernel (CB200_K1X_SHARPEN_RASTER=0), on frames whose cells
-    reach the borders' influence (noise everywhere) and, for mode Bu, on the 736 x 637 geometry with its 61-row last band"""
+    box sum) against the oracle, on frames whose cells reach the borders' influence (noise everywhere) and, for mode Bu, on the
+    736 x 637 geometry with its 61-row last band"""
     m = ORA.mode(mode_val)
     rng = np.random.default_rng(400 + mode_val)
     frames = rng.integers(0, 256, (5, m.image_size_y, m.image_size_x, 3), dtype=np.uint8)
@@ -827,12 +826,7 @@ def test_sharpen_raster_of_the_exact_walk(cb, mode_val, monkeypatch):
         frames[3] = load_sample("b/ex2434.jpg"); frames[4] = load_sample("b/ex380.jpg")
     ctx = cb.Context(mode_val, max_frames=5)
     raw, ff = ctx.decode_raw(frames, flags=cb.FLAG_SHARPEN)
-    monkeypatch.setenv("CB200_K1X_SHARPEN_RASTER", "0")
-    raw0, ff0 = ctx.decode_raw(frames, flags=cb.FLAG_SHARPEN)
-    monkeypatch.delenv("CB200_K1X_SHARPEN_RASTER")
     assert all(int(x) & cb.FRAME_FALLBACK for x in ff)
     for f in range(5):
-        want = ORA.decode_raw(m, frames[f], sharpen=True)
-        assert np.array_equal(raw[f], want), f
-        assert np.array_equal(raw0[f], want), f
+        assert np.array_equal(raw[f], ORA.decode_raw(m, frames[f], sharpen=True)), f
     ctx.close()
