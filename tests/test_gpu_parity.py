@@ -210,12 +210,15 @@ def test_one_percent_tile_errors_config3(cb):
     ctx.close()
 
 
-@pytest.mark.parametrize("rate", [0.01, 0.08])
-def test_noise_tiles_and_rs_failures_match_oracle(cb, rate):
-    # noise tiles may break the centre-wins proof (-> exact walk) and, at 8 %, overwhelm RS: good/bad masks must match
-    m, payloads, frames = synth_frames(68, 4, seed=11, error_rate=rate, noise_tiles=True)
-    ctx = cb.Context(68, max_frames=4)
+@pytest.mark.parametrize("rate,mode_val", [pytest.param(r, mv, id=str(r) if mv == 68 else f"{r}-m{mv}")
+                                            for mv in (68, 4, 8, 66, 67) for r in (0.01, 0.08)])
+def test_noise_tiles_and_rs_failures_match_oracle(cb, mode_val, rate):
+    """noise tiles break the centre-wins proof (-> exact walk, k_flood_raster_fast on every geometry, k_flood_colour with every
+    palette) and, at 8 %, overwhelm RS: good/bad masks must match; then colour correction 1 (one matrix per frame) on the walk"""
+    m, payloads, frames = synth_frames(mode_val, 4, seed=11, error_rate=rate, noise_tiles=True)
+    ctx = cb.Context(mode_val, max_frames=4)
     raw, ff = ctx.decode_raw(frames)
+    assert all(int(x) & cb.FRAME_FALLBACK for x in ff)
     data, ok, _ = ctx.decode(frames)
     chunks, count, mask, _ = ctx.decode_fountain(frames)
     for f in range(4):
@@ -225,6 +228,14 @@ def test_noise_tiles_and_rs_failures_match_oracle(cb, rate):
         good, ochunks, omask = ORA.decode_fountain(m, frames[f])
         assert mask[f] == omask and count[f] * m.chunk_size == good
         assert np.array_equal(chunks[f][:count[f]], ochunks[:count[f]])
+    tinted = _tint(frames, (0.75, 1.0, 0.85))
+    raw1, ff1 = ctx.decode_raw(tinted, flags=cb.FLAG_CC_SIMPLE)
+    assert all(int(x) & cb.FRAME_FALLBACK for x in ff1)
+    try:
+        for f in range(4):
+            assert np.array_equal(raw1[f], ORA.decode_raw(m, tinted[f], color_correction=1)), f
+    finally:
+        ORA.set_ccm(None)
     ctx.close()
 
 
@@ -476,18 +487,24 @@ def test_degenerate_frames_match_oracle(cb):
 
 
 def test_cell_trace_matches_oracle_walk(cb):
-    """cb200_decode_cells == the reference's CimbReader loop: same walk order, positions, drift offsets and distances"""
-    for sample, mode in (("b/ex2434.jpg", 68), ("6bit/4_30_f0_627_extract.jpg", 4), ("b/tr_1.png", 68)):
+    """cb200_decode_cells == the reference's CimbReader loop: same walk order, positions, drift offsets and distances; on
+    photographs, a clean sample frame and frames with noise tiles in the 8-colour mode and the two smaller geometries"""
+    cases = [(sample, mode, load_sample(sample)) for sample, mode in
+             (("b/ex2434.jpg", 68), ("6bit/4_30_f0_627_extract.jpg", 4), ("b/tr_1.png", 68))]
+    for mode, rate in ((8, 0.01), (66, 0.08), (67, 0.01)):
+        cases.append((f"noise tiles {rate:.0%}", mode, synth_frames(mode, 1, seed=450 + mode, error_rate=rate, noise_tiles=True)[2][0]))
+    for sample, mode, rgb in cases:
         m = ORA.mode(mode)
-        rgb = load_sample(sample)
         ctx = cb.Context(mode, max_frames=1)
         cells, trace = ctx.decode_cells(rgb)
         _, ocells = ORA.decode_raw(m, rgb, want_cells=True)
-        assert np.array_equal(trace[0]["order"], ocells["order"]), sample
-        assert np.array_equal(trace[0]["x"], ocells["x"]) and np.array_equal(trace[0]["y"], ocells["y"])
-        assert np.array_equal(trace[0]["drift_offset"], ocells["drift_offset"])
-        assert np.array_equal(trace[0]["distance"], ocells["distance"])
-        assert np.array_equal(cells[0] & 15, ocells["symbol"]) and np.array_equal((cells[0] >> 4) & 7, ocells["color"])
+        assert np.array_equal(trace[0]["order"], ocells["order"]), (sample, mode)
+        assert np.array_equal(trace[0]["x"], ocells["x"]) and np.array_equal(trace[0]["y"], ocells["y"]), (sample, mode)
+        assert np.array_equal(trace[0]["drift_offset"], ocells["drift_offset"]), (sample, mode)
+        assert np.array_equal(trace[0]["distance"], ocells["distance"]), (sample, mode)
+        sb = m.symbol_bits
+        assert np.array_equal(cells[0] & ((1 << sb) - 1), ocells["symbol"]), (sample, mode)
+        assert np.array_equal((cells[0] >> sb) & ((1 << m.color_bits) - 1), ocells["color"]), (sample, mode)
         ctx.close()
 
 
@@ -812,12 +829,15 @@ def test_sharpen_with_noise_tiles_and_colour_correction(cb):
     ctx.close()
 
 
-@pytest.mark.parametrize("mode_val", [68, 66])
-def test_sharpen_raster_of_the_exact_walk(cb, mode_val):
-    """K1x's streaming sharpen raster (k_flood_raster_fast_sharpen: OpenCV's borders, reflect for the filter, replicate for the
-    box sum) against the oracle, on frames whose cells reach the borders' influence (noise everywhere) and, for mode Bu, on the
-    736 x 637 geometry with its 61-row last band"""
+@pytest.mark.parametrize("mode_val,sharpen", [pytest.param(mv, sh, id=str(mv) if sh else f"{mv}-plain")
+                                              for sh in (True, False) for mv in (68, 66, 67)])
+def test_sharpen_raster_of_the_exact_walk(cb, mode_val, sharpen):
+    """K1x's streaming rasters against the oracle: with sharpen k_flood_raster_fast_sharpen (OpenCV's borders, reflect for the
+    filter, replicate for the box sum), without it k_flood_raster_fast (replicate borders); on frames whose cells reach the
+    borders' influence (noise everywhere), on the 736 x 637 geometry of mode Bu with its 61-row last band and on the 1024 x 720
+    geometry of mode Bm with its 16-row last band"""
     m = ORA.mode(mode_val)
+    flags = cb.FLAG_SHARPEN if sharpen else 0
     rng = np.random.default_rng(400 + mode_val)
     frames = rng.integers(0, 256, (5, m.image_size_y, m.image_size_x, 3), dtype=np.uint8)
     frames[1, :, ::3] //= 4
@@ -825,8 +845,8 @@ def test_sharpen_raster_of_the_exact_walk(cb, mode_val):
     if mode_val == 68:
         frames[3] = load_sample("b/ex2434.jpg"); frames[4] = load_sample("b/ex380.jpg")
     ctx = cb.Context(mode_val, max_frames=5)
-    raw, ff = ctx.decode_raw(frames, flags=cb.FLAG_SHARPEN)
+    raw, ff = ctx.decode_raw(frames, flags=flags)
     assert all(int(x) & cb.FRAME_FALLBACK for x in ff)
     for f in range(5):
-        assert np.array_equal(raw[f], ORA.decode_raw(m, frames[f], sharpen=True)), f
+        assert np.array_equal(raw[f], ORA.decode_raw(m, frames[f], sharpen=sharpen)), f
     ctx.close()
