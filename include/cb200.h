@@ -55,6 +55,13 @@ extern "C" {
 
 #define CB200_FLAG_NO_INTERLEAVE 0x10u /* Decoder(use_ecc, interleave=false): cells map to stream slots in linear order
                                          (Interleave::interleave_indices with num_chunks == 0, Interleave.h:10-16; Decoder.h:68) */
+#define CB200_FLAG_SHARPEN_IF_NEEDED 0x20u /* the cimbar CLI's `--preprocess -1` (its default, src/exe/cimbar/cimbar.cpp:124-160):
+                                         camera picture i is decoded with should_preprocess = true iff Extractor::extract returns
+                                         NEEDS_SHARPEN for it, i.e. its corners fail Corners::is_granular_scale (Extractor.h:30-46),
+                                         and without sharpening otherwise, all in one batch, in order (the CCM of CC_FIT still
+                                         carries from picture to picture).  Honoured by the camera entry points
+                                         (cb200_scan_extract_decode_fountain, cb200_extract_decode_fountain[_dev]); with
+                                         CB200_FLAG_SHARPEN, or on an entry point that takes extracted frames, CB200_ERR_ARG. */
 
 /* per-frame status bits written to frame_flags[] */
 #define CB200_FRAME_FALLBACK    0x1u  /* frame was decoded by the exact flood-walk kernel (drift tracking needed) */
@@ -118,6 +125,14 @@ int cb200_rs_correct_dev(cb200_ctx* ctx, const uint8_t* d_raw, int n, uint8_t* d
 int cb200_decode_chunks_dev(cb200_ctx* ctx, const uint8_t* d_rgb, int n, uint32_t flags,
                             uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags);
 
+/* The same with a per-frame choice of preprocessing: frame f is decoded with should_preprocess = (sharpen[f] != 0), exactly as
+   Decoder::decode_fountain(img_f, stream, sharpen[f], color_correction) decodes it, and everything that depends on order (the
+   CCM carry of CC_FIT, the outputs) stays in batch order.  sharpen: n bytes in HOST memory, read before the call returns (the
+   caller may reuse it at once); the call stays enqueue-only.  `flags` must not contain CB200_FLAG_SHARPEN.  A batch of both
+   kinds runs K1 twice, once over each kind's frames; a selection of one kind only is the call without / with CB200_FLAG_SHARPEN. */
+int cb200_decode_chunks_sharpen_dev(cb200_ctx* ctx, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen,
+                                    uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags);
+
 /* ---- host-pointer entry points: H2D + kernels + D2H, synchronous ---------------------------------------------- */
 
 /* == Decoder(false).decode(img, stream): raw cell bits (Decoder.h:163-168 with _useEcc=false) */
@@ -131,6 +146,11 @@ int cb200_decode(cb200_ctx* ctx, const uint8_t* rgb, int n, uint32_t flags, uint
    NULL); good bytes = count * chunk_size == the reference's return value (aligned_stream::tellp) */
 int cb200_decode_fountain(cb200_ctx* ctx, const uint8_t* rgb, int n, uint32_t flags, uint8_t* chunks_out,
                           uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
+
+/* cb200_decode_fountain with a per-frame sharpen selection (n host bytes, as cb200_decode_chunks_sharpen_dev): the batched
+   form of the loop `for f: decoder.decode_fountain(img_f, stream, should_preprocess_f, color_correction)` */
+int cb200_decode_fountain_sharpen(cb200_ctx* ctx, const uint8_t* rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
+                                  uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
 
 /* the same with frames that are already in device memory (the output of cb200_deskew_dev): results to host memory */
 int cb200_decode_fountain_from_dev(cb200_ctx* ctx, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* chunks_out,
@@ -153,7 +173,9 @@ int cb200_deskew_dev(cb200_ctx* ctx, const uint8_t* d_src, int src_w, int src_h,
 /* host pointers in and out (H2D + kernel + D2H): what Deskewer::deskew returns */
 int cb200_deskew(cb200_ctx* ctx, const uint8_t* src, int src_w, int src_h, int n, const double* m9, uint8_t* dst);
 /* Extractor's deskew + Decoder::decode_fountain in one call: camera images (host) and their four anchor centres
-   (n x 8 floats) in, fountain chunks out; the deskewed frames stay on the device.  Outputs as cb200_decode_fountain. */
+   (n x 8 floats) in, fountain chunks out; the deskewed frames stay on the device.  Outputs as cb200_decode_fountain.
+   With CB200_FLAG_SHARPEN_IF_NEEDED picture i is sharpened iff its corners fail Corners::is_granular_scale (some side of the
+   quadrilateral spans no more than the frame's width in x and its height in y, Corners.h:57-75). */
 int cb200_extract_decode_fountain(cb200_ctx* ctx, const uint8_t* src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
                                   uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
 
@@ -183,9 +205,10 @@ int cb200_scan_blurred(cb200_ctx* ctx, uint8_t* blurred_out, int32_t* thresholds
 /* Extractor::extract (src/lib/extractor/Extractor.h:30-46) + Decoder::decode_fountain for n camera pictures in host memory:
    scan -> Corners (the anchors' centres) -> deskew to the mode's frame size -> decode; one H2D copy of the pictures, nothing
    but anchors and chunks comes back.  extract_status: n int32 with the reference's return values -- 0 FAILURE (fewer than four
-   anchors; no chunks), 1 SUCCESS, 2 NEEDS_SHARPEN (Corners::is_granular_scale false: the caller of the reference then decodes
-   with should_preprocess = true, i.e. CB200_FLAG_SHARPEN) -- or -1 for a capacity overflow (see cb200_scan).  `flags` applies
-   to the whole batch.  The other outputs are as cb200_decode_fountain. */
+   anchors; no chunks), 1 SUCCESS, 2 NEEDS_SHARPEN (Corners::is_granular_scale false: the reference's CLI then decodes that
+   picture with should_preprocess = true) -- or -1 for a capacity overflow (see cb200_scan).  CB200_FLAG_SHARPEN_IF_NEEDED does
+   exactly that per picture (sharpen iff status 2); CB200_FLAG_SHARPEN sharpens every picture.  The other flags apply to the
+   whole batch.  The other outputs are as cb200_decode_fountain. */
 int cb200_scan_extract_decode_fountain(cb200_ctx* ctx, const uint8_t* pictures, int w, int h, int n, uint32_t flags,
                                        uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
                                        int32_t* extract_status);
@@ -265,7 +288,7 @@ int cb200_encode_cells_dev(cb200_ctx* ctx, const uint8_t* d_payload, int n, uint
 
 /* when enabled, CUDA events are recorded on the context's stream around every kernel of every pipeline call (a ring of
    the last 64 calls).  cb200_get_timing returns the milliseconds of the call `calls_back` calls ago (0 = last) in launch
-   order: [0] K1 fused decode, [1] K1x exact-walk kernel, [2] pack, [3] RS, [4] chunk mask (decode_raw_dev stops after [2]) */
+   order: [0] K1 fused decode (both K1 launches of a batch with a per-frame sharpen choice), [1] K1x exact-walk kernel, [2] pack, [3] RS, [4] chunk mask (decode_raw_dev stops after [2]) */
 int cb200_set_timing(cb200_ctx* ctx, int enable);
 /* kernels launched by this library in this process so far (every launch site counts itself): bench.py reports the
    difference across its timed region as "gpu_launches" */

@@ -16,6 +16,7 @@ FLAG_SHARPEN = 0x2
 FLAG_CC_SIMPLE = 0x4
 FLAG_CC_FIT = 0x8
 FLAG_NO_INTERLEAVE = 0x10
+FLAG_SHARPEN_IF_NEEDED = 0x20     # camera entry points only: sharpen the pictures Extractor::extract calls NEEDS_SHARPEN
 FRAME_FALLBACK = 0x1
 FRAME_INEXACT = 0x2
 
@@ -31,6 +32,7 @@ EXPORTS = [
     "cb200_gather_root_create", "cb200_gather_peer_open", "cb200_gather_slot", "cb200_gather_publish", "cb200_gather_push", "cb200_gather_wait",
     "cb200_gather_release", "cb200_gather_acquire",
     "cb200_gather_status", "cb200_comm_unique_id", "cb200_comm_init", "cb200_gather_chunks", "cb200_gather_chunks_wait",
+    "cb200_decode_chunks_sharpen_dev", "cb200_decode_fountain_sharpen",
 ]
 
 
@@ -73,6 +75,8 @@ def load_library():
     lib.cb200_decode_raw.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, u8p]
     lib.cb200_decode.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, u8p, u8p]
     lib.cb200_decode_fountain.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, u32p, u32p, u8p]
+    lib.cb200_decode_chunks_sharpen_dev.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, u8p, u32p, u8p]
+    lib.cb200_decode_fountain_sharpen.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, u8p, u32p, u32p, u8p]
     lib.cb200_decode_cells.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, vp]
     lib.cb200_decode_symbols.argtypes = [vp, u16p, u8p, C.c_int, u8p, u8p, u8p]
     lib.cb200_best_colors.argtypes = [vp, u8p, C.c_int, u8p]
@@ -171,6 +175,14 @@ def _hptr(a):
     return a.ctypes.data if a is not None else None
 
 
+def _selection(sharpen, n):
+    """a per-frame sharpen choice as the C ABI takes it: n bytes, nonzero = should_preprocess"""
+    sel = np.ascontiguousarray(np.asarray(sharpen).astype(bool), dtype=np.uint8).reshape(-1)
+    if sel.size != n:
+        raise Cb200Error(f"sharpen must have one entry per frame ({n}), got {sel.size}")
+    return sel
+
+
 class Context:
     """One decode context = one GPU + one stream (cb200_create / cb200_destroy)."""
 
@@ -223,14 +235,21 @@ class Context:
         _check(self.lib.cb200_decode(self._h, rgb.ctypes.data, n, flags, data.ctypes.data, ok.ctypes.data, ff.ctypes.data))
         return data, ok, ff
 
-    def decode_fountain(self, rgb, flags=0):
+    def decode_fountain(self, rgb, flags=0, sharpen=None):
+        """Decoder::decode_fountain over a batch.  sharpen: None = as `flags` says for every frame; else one bool per frame
+        (should_preprocess of that frame; `flags` must not contain FLAG_SHARPEN then)"""
         rgb, n = self._frames(rgb)
         chunks = np.zeros((n, self.info.chunks_per_frame, self.info.chunk_size), dtype=np.uint8)
         count = np.zeros(n, dtype=np.uint32)
         mask = np.zeros(n, dtype=np.uint32)
         ff = np.zeros(n, dtype=np.uint8)
-        _check(self.lib.cb200_decode_fountain(self._h, rgb.ctypes.data, n, flags, chunks.ctypes.data, count.ctypes.data,
-                                              mask.ctypes.data, ff.ctypes.data))
+        if sharpen is None:
+            _check(self.lib.cb200_decode_fountain(self._h, rgb.ctypes.data, n, flags, chunks.ctypes.data, count.ctypes.data,
+                                                  mask.ctypes.data, ff.ctypes.data))
+        else:
+            sel = _selection(sharpen, n)
+            _check(self.lib.cb200_decode_fountain_sharpen(self._h, rgb.ctypes.data, n, flags, sel.ctypes.data, chunks.ctypes.data,
+                                                          count.ctypes.data, mask.ctypes.data, ff.ctypes.data))
         return chunks, count, mask, ff
 
     def deskew(self, src, m9):
@@ -361,8 +380,13 @@ class Context:
     def rs_correct_dev(self, d_raw, n, d_data_out, d_ok=None):
         _check(self.lib.cb200_rs_correct_dev(self._h, d_raw, n, d_data_out, d_ok))
 
-    def decode_chunks_dev(self, d_rgb, n, d_chunks, d_mask, d_flags=None, flags=0):
-        _check(self.lib.cb200_decode_chunks_dev(self._h, d_rgb, n, flags, d_chunks, d_mask, d_flags))
+    def decode_chunks_dev(self, d_rgb, n, d_chunks, d_mask, d_flags=None, flags=0, sharpen=None):
+        """sharpen: None = as `flags` says; else one bool per frame, host memory (see decode_fountain)"""
+        if sharpen is None:
+            _check(self.lib.cb200_decode_chunks_dev(self._h, d_rgb, n, flags, d_chunks, d_mask, d_flags))
+        else:
+            sel = _selection(sharpen, n)
+            _check(self.lib.cb200_decode_chunks_sharpen_dev(self._h, d_rgb, n, flags, sel.ctypes.data, d_chunks, d_mask, d_flags))
 
     def encode_cells_dev(self, d_payload, n, d_cellvals):
         _check(self.lib.cb200_encode_cells_dev(self._h, d_payload, n, d_cellvals))
@@ -371,7 +395,7 @@ class Context:
         _check(self.lib.cb200_set_timing(self._h, int(enable)))
 
     def get_timing(self, calls_back=0):
-        """ms per kernel of the pipeline call `calls_back` calls ago: [K1, K1x, pack, RS, mask]"""
+        """ms per kernel of the pipeline call `calls_back` calls ago: [K1 (both launches of a mixed batch), K1x, pack, RS, mask]"""
         ms = (C.c_float * 8)()
         n = C.c_int(0)
         _check(self.lib.cb200_get_timing(self._h, calls_back, ms, 8, C.byref(n)))

@@ -222,6 +222,21 @@ void mark(cb200_ctx* c)
     if (c->timing && c->ev_count[c->cur] < 8) cudaEventRecord(c->ev[c->cur][c->ev_count[c->cur]++], c->stream);
 }
 
+// CB200_FLAG_SHARPEN_IF_NEEDED is a decision about camera pictures: the entry points that take extracted frames refuse it
+int check_frame_flags(uint32_t flags)
+{
+    if (flags & CB200_FLAG_SHARPEN_IF_NEEDED) return fail(CB200_ERR_ARG, "CB200_FLAG_SHARPEN_IF_NEEDED applies to camera pictures, not to frames");
+    return CB200_OK;
+}
+// the frame entry points with a per-frame selection
+int check_selection_args(uint32_t flags, const uint8_t* sharpen)
+{
+    int rc = check_frame_flags(flags); if (rc) return rc;
+    if (flags & CB200_FLAG_SHARPEN) return fail(CB200_ERR_ARG, "CB200_FLAG_SHARPEN with a per-frame sharpen selection");
+    if (!sharpen) return fail(CB200_ERR_ARG, "null sharpen selection");
+    return CB200_OK;
+}
+
 int check_n(const cb200_ctx* c, int n)
 {
     if (!c) return fail(CB200_ERR_ARG, "null context");
@@ -273,8 +288,43 @@ int ccm_buffers(cb200_ctx* c)
     return CB200_OK;
 }
 
-// d_means != nullptr: first pass of a CC_FIT batch -- no colour decisions, the cells' mean colours go to d_means
-int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, CellTrace* d_trace = nullptr, uint32_t* d_means = nullptr)
+// a mixed sharpen selection on the device: the batch indices of the plain frames (d_list[0], nl[0] of them) and of the
+// sharpened ones (d_list[1]), both in batch order, and one 0 / 1 byte per frame (d_sharp).  The host copy is staged in a
+// pinned slot of the context, so the caller may reuse `sel` at once and nothing waits for the stream, except when a slot's
+// copy from two calls ago has not run yet.
+int upload_selection(cb200_ctx* c, const uint8_t* sel, int n, const int nl[2], const uint32_t* d_list[2], const uint8_t** d_sharp)
+{
+    const size_t bytes = (size_t)c->max_frames * 5;
+    if (!c->d_sel) CK(cudaMalloc(&c->d_sel, bytes), "cudaMalloc selection");
+    const int slot = c->sel_next;
+    c->sel_next = (slot + 1) % cb200_ctx::kSelSlots;
+    if (!c->h_sel[slot]) {
+        CK(cudaMallocHost(&c->h_sel[slot], bytes), "cudaMallocHost selection");
+        CK(cudaEventCreateWithFlags(&c->sel_ev[slot], cudaEventDisableTiming), "cudaEventCreate selection");
+    } else {
+        CK(cudaEventSynchronize(c->sel_ev[slot]), "sync (selection slot)");
+    }
+    uint32_t* h_list = reinterpret_cast<uint32_t*>(c->h_sel[slot]);
+    uint8_t* h_sharp = c->h_sel[slot] + (size_t)n * 4;
+    int at[2] = {0, nl[0]};
+    for (int f = 0; f < n; ++f) {
+        const int k = sel[f] != 0;
+        h_list[at[k]++] = (uint32_t)f;
+        h_sharp[f] = (uint8_t)k;
+    }
+    CK(cudaMemcpyAsync(c->d_sel, c->h_sel[slot], (size_t)n * 5, cudaMemcpyHostToDevice, c->stream), "H2D selection");
+    CK(cudaEventRecord(c->sel_ev[slot], c->stream), "record selection");
+    d_list[0] = reinterpret_cast<const uint32_t*>(c->d_sel);
+    d_list[1] = d_list[0] + nl[0];
+    *d_sharp = c->d_sel + (size_t)n * 4;
+    return CB200_OK;
+}
+
+// d_means != nullptr: first pass of a CC_FIT batch -- no colour decisions, the cells' mean colours go to d_means.
+// sel: NULL = every frame is preprocessed as CB200_FLAG_SHARPEN says; else n host bytes, nonzero = sharpen that frame (flags
+// must not carry CB200_FLAG_SHARPEN then).  A selection of one kind only takes the list-less path of that kind.
+int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sel, CellTrace* d_trace = nullptr,
+              uint32_t* d_means = nullptr)
 {
     const Mode& m = c->mode;
     cudaStream_t st = c->stream;
@@ -295,23 +345,36 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, CellTra
     } else {
         int rc = ccm_arg(c, cc); if (rc) return rc;
     }
-    const bool sharpen = (flags & CB200_FLAG_SHARPEN) != 0;
+    bool sharpen = (flags & CB200_FLAG_SHARPEN) != 0;
     const bool exact_only = d_trace != nullptr;   // a cell trace needs the walk itself
+    // nl[k] frames of kind k (0 = plain, 1 = sharpened), listed in d_list[k] (NULL: all n frames of the batch)
+    int nl[2] = {sharpen ? 0 : n, sharpen ? n : 0};
+    const uint32_t* d_list[2] = {nullptr, nullptr};
+    const uint8_t* d_sharp = nullptr;
+    if (sel) {
+        nl[1] = 0;
+        for (int f = 0; f < n; ++f) nl[1] += sel[f] != 0;
+        nl[0] = n - nl[1];
+        sharpen = nl[1] == n;
+        if (nl[0] && nl[1]) { int rc = upload_selection(c, sel, n, nl, d_list, &d_sharp); if (rc) return rc; }
+    }
     CK(cudaMemsetAsync(c->d_dirty, 0, sizeof(uint32_t) * (size_t)n, st), "memset dirty");
     if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; }
     mark(c);                                   // ev0: before K1
-    if (!exact_only) {
+    for (int k = 0; k < 2 && !exact_only; ++k) {
+        const int nk = nl[k];
+        if (nk == 0) continue;
         // bands: whole frames when there are enough of them to fill the machine, else split frames into bands of cell rows
-        int ctas = c->sm_count * k1_ctas_per_sm(sharpen);
+        int ctas = c->sm_count * k1_ctas_per_sm(k == 1);
         int bands = 1;
-        if (n < ctas) { bands = (ctas + n - 1) / n; if (bands > m.cells_y / 4) bands = m.cells_y / 4; if (bands < 1) bands = 1; }
-        int units = n * bands;
+        if (nk < ctas) { bands = (ctas + nk - 1) / nk; if (bands > m.cells_y / 4) bands = m.cells_y / 4; if (bands < 1) bands = 1; }
+        int units = nk * bands;
         int grid = units < ctas ? units : ctas;
-        CK(k1_launch(m, d_rgb, n, bands, grid, sharpen, c->d_cellvals, c->d_dirty, cc, st), "k1 launch");
+        CK(k1_launch(m, d_rgb, d_list[k], nk, bands, grid, k == 1, c->d_cellvals, c->d_dirty, cc, st), "k1 launch");
     }
     mark(c);                                   // ev1: after K1
     // frames K1 flagged (or all of them when exact_only) are re-done by the exact walk on the same preprocessing (sharpen or not)
-    CK(flood_launch(m, c->flood, d_rgb, n, (flags & CB200_FLAG_NO_FALLBACK) != 0, exact_only, sharpen,
+    CK(flood_launch(m, c->flood, d_rgb, n, (flags & CB200_FLAG_NO_FALLBACK) != 0, exact_only, sharpen, d_sharp,
                     c->d_cellvals, c->d_dirty, c->d_flags, d_trace, cc, st), "flood launch");
     mark(c);                                   // ev2: after K1x
     return CB200_OK;
@@ -478,6 +541,8 @@ int cb200_destroy(cb200_ctx* c)
     gather_destroy(c->gather);
     deskew_destroy(c->deskew); scan_destroy(c->scan);
     if (c->h_pinned) cudaFreeHost(c->h_pinned);
+    cudaFree(c->d_sel);
+    for (int k = 0; k < cb200_ctx::kSelSlots; ++k) { if (c->h_sel[k]) cudaFreeHost(c->h_sel[k]); if (c->sel_ev[k]) cudaEventDestroy(c->sel_ev[k]); }
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     delete c;
     return CB200_OK;
@@ -506,13 +571,14 @@ int cb200_sync(cb200_ctx* c)
 
 int cb200_decode_raw_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* d_raw_out, uint8_t* d_frame_flags)
 {
-    int rc = check_n(c, n); if (rc) return rc;
+    int rc = check_frame_flags(flags); if (rc) return rc;
+    rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
     if (!d_rgb || !d_raw_out) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const uint16_t* idx;
     rc = idx_for(c, flags, &idx); if (rc) return rc;
-    rc = run_cells(c, d_rgb, n, flags); if (rc) return rc;
+    rc = run_cells(c, d_rgb, n, flags, nullptr); if (rc) return rc;
     CK(k2_pack_launch(c->mode, c->d_cellvals, idx, n, d_raw_out, c->stream), "pack launch");
     mark(c);                                   // ev3: after pack
     if (d_frame_flags) CK(cudaMemcpyAsync(d_frame_flags, c->d_flags, (size_t)n, cudaMemcpyDeviceToDevice, c->stream), "copy flags");
@@ -530,7 +596,12 @@ int cb200_rs_correct_dev(cb200_ctx* c, const uint8_t* d_raw, int n, uint8_t* d_d
     return CB200_OK;
 }
 
-int cb200_decode_chunks_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
+}  // extern "C"
+
+namespace {
+// cb200_decode_chunks_dev with an optional per-frame selection (run_cells)
+int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
+                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
 {
     int rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
@@ -543,7 +614,7 @@ int cb200_decode_chunks_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t 
     const uint16_t* idx;
     rc = idx_for(c, flags, &idx); if (rc) return rc;
     if (!fit) {
-        rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT); if (rc) return rc;
+        rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen); if (rc) return rc;
         mark(c);                               // ev3: (no separate pack kernel on this path: the RS kernel gathers from the cell bytes)
         CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
     } else {
@@ -556,7 +627,7 @@ int cb200_decode_chunks_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t 
         if (!c->d_ccm_active) CK(cudaMalloc(&c->d_ccm_active, (size_t)c->max_frames), "cudaMalloc ccm flags");
         CcmArg initial;
         rc = ccm_arg(c, initial); if (rc) return rc;        // the decoder's CCM going into frame 0
-        rc = run_cells(c, d_rgb, n, flags & ~(CB200_FLAG_CC_FIT | CB200_FLAG_CC_SIMPLE), nullptr, c->d_means); if (rc) return rc;
+        rc = run_cells(c, d_rgb, n, flags & ~(CB200_FLAG_CC_FIT | CB200_FLAG_CC_SIMPLE), sharpen, nullptr, c->d_means); if (rc) return rc;
         mark(c);                               // ev3
         CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream, 0, m.nblocks_sym), "rs launch (symbols)");
         CK(ccm_fit_launch(m, d_rgb, d_chunks, c->d_ok, idx, n, c->d_fit, c->d_fit_valid, c->stream), "ccm fit");
@@ -576,11 +647,28 @@ int cb200_decode_chunks_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t 
     if (d_frame_flags) CK(cudaMemcpyAsync(d_frame_flags, c->d_flags, (size_t)n, cudaMemcpyDeviceToDevice, c->stream), "copy flags");
     return CB200_OK;
 }
+}  // namespace
+
+extern "C" {
+
+int cb200_decode_chunks_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
+{
+    int rc = check_frame_flags(flags); if (rc) return rc;
+    return decode_chunks(c, d_rgb, n, flags, nullptr, d_chunks, d_chunk_mask, d_frame_flags);
+}
+
+int cb200_decode_chunks_sharpen_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
+                                    uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
+{
+    int rc = check_selection_args(flags, sharpen); if (rc) return rc;
+    return decode_chunks(c, d_rgb, n, flags, sharpen, d_chunks, d_chunk_mask, d_frame_flags);
+}
 
 // ---- host-pointer entry points
 int cb200_decode_raw(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* raw_out, uint8_t* frame_flags)
 {
-    int rc = check_n(c, n); if (rc) return rc;
+    int rc = check_frame_flags(flags); if (rc) return rc;
+    rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
     if (!rgb || !raw_out) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
@@ -594,7 +682,8 @@ int cb200_decode_raw(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, ui
 
 int cb200_decode(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* data_out, uint8_t* block_ok, uint8_t* frame_flags)
 {
-    int rc = check_n(c, n); if (rc) return rc;
+    int rc = check_frame_flags(flags); if (rc) return rc;
+    rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
     if (!rgb || !data_out) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
@@ -607,27 +696,32 @@ int cb200_decode(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_
     return CB200_OK;
 }
 
-int cb200_decode_fountain(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count,
-                          uint32_t* chunk_mask, uint8_t* frame_flags)
+}  // extern "C"
+
+namespace {
+// the host-pointer fountain entry points: H2D of the frames, then the device-frame path
+int decode_fountain_from_host(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
+                              uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
     int rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
     if (!rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = upload_frames(c, rgb, n); if (rc) return rc;
-    return cb200_decode_fountain_from_dev(c, c->d_rgb, n, flags, chunks_out, chunk_count, chunk_mask, frame_flags);
+    return decode_fountain_to_host(c, c->d_rgb, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
+}  // namespace
 
 // frames already on the device (the staging buffer, or the deskew kernel's output), results to host memory
-int cb200_decode_fountain_from_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count,
-                                   uint32_t* chunk_mask, uint8_t* frame_flags)
+int cb200::decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
+                                   uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
     int rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
     if (!d_rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
-    rc = cb200_decode_chunks_dev(c, d_rgb, n, flags, c->d_data, c->d_mask, nullptr); if (rc) return rc;
+    rc = decode_chunks(c, d_rgb, n, flags, sharpen, c->d_data, c->d_mask, nullptr); if (rc) return rc;
     size_t need = (size_t)n * m.data_bytes + (size_t)n * sizeof(uint32_t);
     if (c->h_pinned_bytes < need) {
         if (c->h_pinned) cudaFreeHost(c->h_pinned);
@@ -654,6 +748,29 @@ int cb200_decode_fountain_from_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, ui
     return CB200_OK;
 }
 
+extern "C" {
+
+int cb200_decode_fountain(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count,
+                          uint32_t* chunk_mask, uint8_t* frame_flags)
+{
+    int rc = check_frame_flags(flags); if (rc) return rc;
+    return decode_fountain_from_host(c, rgb, n, flags, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags);
+}
+
+int cb200_decode_fountain_sharpen(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
+                                  uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
+{
+    int rc = check_selection_args(flags, sharpen); if (rc) return rc;
+    return decode_fountain_from_host(c, rgb, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
+}
+
+int cb200_decode_fountain_from_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count,
+                                   uint32_t* chunk_mask, uint8_t* frame_flags)
+{
+    int rc = check_frame_flags(flags); if (rc) return rc;
+    return decode_fountain_to_host(c, d_rgb, n, flags, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags);
+}
+
 int cb200_decode_cells(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* cellvals_out, cb200_cell_trace* trace_out)
 {
     return cb200_decode_cells_means(c, rgb, n, flags, cellvals_out, trace_out, nullptr);
@@ -662,7 +779,8 @@ int cb200_decode_cells(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, 
 int cb200_decode_cells_means(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* cellvals_out, cb200_cell_trace* trace_out,
                              uint32_t* means_out)
 {
-    int rc = check_n(c, n); if (rc) return rc;
+    int rc = check_frame_flags(flags); if (rc) return rc;
+    rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
     if (!rgb || !cellvals_out || !trace_out) return fail(CB200_ERR_ARG, "null buffer");
     static_assert(sizeof(cb200_cell_trace) == sizeof(CellTrace), "trace layout");
@@ -682,7 +800,7 @@ int cb200_decode_cells_means(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t f
         CK(cudaEventRecord(c->ccm_ev, c->stream), "record ccm");
         c->ccm_pending = true; c->ccm_pending_flag = false; c->ccm_active = true;
     }
-    rc = run_cells(c, c->d_rgb, n, flags & ~(CB200_FLAG_NO_FALLBACK | (d_means ? CB200_FLAG_CC_SIMPLE : 0u)), d_trace, d_means); if (rc) return rc;
+    rc = run_cells(c, c->d_rgb, n, flags & ~(CB200_FLAG_NO_FALLBACK | (d_means ? CB200_FLAG_CC_SIMPLE : 0u)), nullptr, d_trace, d_means); if (rc) return rc;
     if (means_out) CK(cudaMemcpyAsync(means_out, d_means, mb, cudaMemcpyDeviceToHost, c->stream), "D2H means");
     CK(cudaMemcpyAsync(cellvals_out, c->d_cellvals, (size_t)n * c->mode.num_cells, cudaMemcpyDeviceToHost, c->stream), "D2H cells");
     CK(cudaMemcpyAsync(trace_out, d_trace, tb, cudaMemcpyDeviceToHost, c->stream), "D2H trace");

@@ -17,6 +17,15 @@ struct ScanScratch;      // scan.cu
 void gather_destroy(GatherState* g);
 void deskew_destroy(DeskewState* d);
 void scan_destroy(ScanScratch* s);
+// cb200_decode_fountain_from_dev with an optional per-frame sharpen selection: `sharpen` = n host bytes (nonzero =
+// should_preprocess) or NULL (the batch-wide CB200_FLAG_SHARPEN decides).  The flags are checked by the caller (api.cu)
+int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
+                            uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
+// CB200_ERR_ARG for CB200_FLAG_SHARPEN together with CB200_FLAG_SHARPEN_IF_NEEDED (deskew.cu)
+int check_camera_flags(uint32_t flags);
+// cb200_extract_decode_fountain_dev with the same selection (deskew.cu)
+int extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
+                           const uint8_t* sharpen, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
 }  // namespace cb200
 #define CK(call, what) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cb200::fail_cuda(e__, what); } while (0)
 
@@ -50,6 +59,13 @@ struct cb200_ctx {
     void* d_scratch = nullptr; size_t scratch_bytes = 0;
     // pinned host staging for results of the host-pointer entry points
     uint8_t* h_pinned = nullptr; size_t h_pinned_bytes = 0;
+    // per-frame sharpen selection of a mixed batch: the two frame lists and the sharpen bytes, staged in one of two pinned
+    // slots (each reused once the copy enqueued from it two calls ago has run) and copied to d_sel on the call's stream
+    static constexpr int kSelSlots = 2;
+    uint8_t* h_sel[kSelSlots] = {};
+    cudaEvent_t sel_ev[kSelSlots] = {};
+    int sel_next = 0;
+    uint8_t* d_sel = nullptr;        // max_frames x (4 + 1): plain list, sharpened list, then one sharpen byte per frame
     // colour correction (the reference's thread-local CimbDecoder CCM, CimbDecoder.cpp:69-85)
     float ccm[9] = {};               // active matrix, row-major
     bool ccm_active = false;

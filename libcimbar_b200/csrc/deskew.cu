@@ -272,9 +272,19 @@ int cb200_deskew(cb200_ctx* c, const uint8_t* src, int src_w, int src_h, int n, 
     return CB200_OK;
 }
 
+}  // extern "C"
+
+// both sharpen flags together are a contradiction (CB200_FLAG_SHARPEN_IF_NEEDED is the CLI's --preprocess -1, SHARPEN its 1)
+int cb200::check_camera_flags(uint32_t flags)
+{
+    if ((flags & CB200_FLAG_SHARPEN) && (flags & CB200_FLAG_SHARPEN_IF_NEEDED))
+        return fail(CB200_ERR_ARG, "CB200_FLAG_SHARPEN and CB200_FLAG_SHARPEN_IF_NEEDED are exclusive");
+    return CB200_OK;
+}
+
 // the pictures are already in device memory (the scan entry points stage them once for scan + deskew)
-int cb200_extract_decode_fountain_dev(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
-                                      uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
+int cb200::extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
+                                  const uint8_t* sharpen, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
     if (!c || !d_src || !corners || !chunks_out || !chunk_count || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
     if (n == 0) return CB200_OK;
@@ -292,12 +302,39 @@ int cb200_extract_decode_fountain_dev(cb200_ctx* c, const uint8_t* d_src, int sr
     if (db > d->dst_bytes) { cudaFree(d->d_dst); d->d_dst = nullptr; d->dst_bytes = 0; CK(cudaMalloc(&d->d_dst, db), "cudaMalloc deskew output"); d->dst_bytes = db; }
     int rc = cb200_deskew_dev(c, d_src, src_w, src_h, n, m9.data(), d->d_dst); if (rc) return rc;
     // the deskewed frames never leave the device: straight into the decode
-    return cb200_decode_fountain_from_dev(c, d->d_dst, n, flags, chunks_out, chunk_count, chunk_mask, frame_flags);
+    return decode_fountain_to_host(c, d->d_dst, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
+}
+
+extern "C" {
+
+int cb200_extract_decode_fountain_dev(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
+                                      uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
+{
+    int rc = check_camera_flags(flags); if (rc) return rc;
+    if (!(flags & CB200_FLAG_SHARPEN_IF_NEEDED) || !c || !corners || n < 0 || n > c->max_frames)
+        return extract_decode_to_host(c, d_src, src_w, src_h, n, corners, flags, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags);
+    // Extractor::extract (Extractor.h:30-46): NEEDS_SHARPEN unless every side of the corner quadrilateral spans more than the
+    // frame in x or in y (Corners::is_granular_scale, Corners.h:57-75)
+    const Mode& m = c->mode;
+    std::vector<uint8_t> sharpen((size_t)n);
+    const int pairs[4][2] = {{0, 1}, {1, 3}, {3, 2}, {2, 0}};              // tl-tr, tr-br, br-bl, bl-tl
+    for (int i = 0; i < n; ++i) {
+        const float* xy = corners + 8 * (size_t)i;
+        bool granular = true;
+        for (int k = 0; k < 4; ++k) {
+            const int p = pairs[k][0], q = pairs[k][1];
+            granular = granular && (std::fabs(xy[2 * p] - xy[2 * q]) > (float)m.width || std::fabs(xy[2 * p + 1] - xy[2 * q + 1]) > (float)m.height);
+        }
+        sharpen[(size_t)i] = granular ? 0 : 1;
+    }
+    return extract_decode_to_host(c, d_src, src_w, src_h, n, corners, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, sharpen.data(), chunks_out,
+                                  chunk_count, chunk_mask, frame_flags);
 }
 
 int cb200_extract_decode_fountain(cb200_ctx* c, const uint8_t* src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
                                   uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
+    int rc = check_camera_flags(flags); if (rc) return rc;
     if (!c || !src || !corners || !chunks_out || !chunk_count || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
     if (n == 0) return CB200_OK;
     CK(cudaSetDevice(c->device), "cudaSetDevice");

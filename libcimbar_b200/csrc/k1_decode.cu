@@ -236,10 +236,12 @@ __device__ __forceinline__ uint32_t thread_symbol_search(const K1Smem& s, uint32
 //   (two carried), their halo words (s0,s1,s2 | s5,s6,s7) -> smem  ---- barrier 2 ----  7x7 box sums, threshold rows
 //   a0-4 .. a0+4 = y_k .. y_k+8, S(k-1).  Frame borders are never reached: the cell windows stay 3 pixels inside.
 // A lane-level numpy model of exactly this schedule is checked against the oracle in tests/test_k1_sharpen_model.py.
+// frame_list: NULL = the n_frames frames of the batch; else the batch indices of the n_frames frames this launch decodes (one
+// kind of a batch that mixes sharpened and plain frames).  Every output stays batch-indexed.
 template <int NC, bool G1024, int CM, bool SH>
 __global__ void __launch_bounds__(kK1Threads, SH ? 3 : kK1CtasPerSm)
-k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, int bands, uint8_t* __restrict__ cellvals,
-                 uint32_t* __restrict__ dirty_flags, const CcmArg cc)
+k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, const uint32_t* __restrict__ frame_list, int n_frames, int bands,
+                 uint8_t* __restrict__ cellvals, uint32_t* __restrict__ dirty_flags, const CcmArg cc)
 {
     // G1024: the 1024x1024 / 112x112-cell geometry of modes B, 4C and 8C as compile-time constants (GridConf.h:121-141);
     // the other modes (Bm 1024x720, Bu 736x637) take every dimension from the Mode struct
@@ -302,7 +304,8 @@ k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, i
     auto cursor_unit = [&](Cursor& c) {          // position at the first (virtual) stage of unit c.u
         c.valid = c.u < n_units;
         if (!c.valid) return;
-        int f = c.u / bands, b = c.u - f * bands;
+        const int e = c.u / bands, b = c.u - e * bands;
+        const int f = frame_list ? (int)frame_list[e] : e;
         c.k = (m.cells_y() * b) / bands - 1;
         c.kend = (m.cells_y() * (b + 1)) / bands;
         c.src = rgb + (size_t)f * frame_bytes + (size_t)(m.cell_offset() + kSpacing * c.k + kFirstRow) * row_bytes;
@@ -387,7 +390,8 @@ k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, int n_frames, i
 
     uint32_t it = 0;
     for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-        int f = u / bands, b = u - f * bands;
+        const int e = u / bands, b = u - e * bands;
+        const int f = frame_list ? (int)frame_list[e] : e;
         int k0 = (m.cells_y() * b) / bands, k1 = (m.cells_y() * (b + 1)) / bands;
         uint8_t* out = cellvals + (size_t)f * (size_t)m.num_cells();
         if (CM == 1) {  // nobody reads s.ccm between the last colour pass of the previous unit and this barrier
@@ -660,14 +664,14 @@ cudaError_t k1_init_tables(const float* adjust256, const unsigned long long* til
     return cudaSuccess;
 }
 
-cudaError_t k1_launch(const Mode& m, const uint8_t* d_rgb, int n_frames, int bands, int grid, bool sharpen,
+cudaError_t k1_launch(const Mode& m, const uint8_t* d_rgb, const uint32_t* d_list, int n_frames, int bands, int grid, bool sharpen,
                       uint8_t* d_cellvals, uint32_t* d_dirty, const CcmArg& cc, cudaStream_t stream)
 {
     const size_t smem = k1_smem_bytes(sharpen);
     const bool g1024 = m.width == 1024 && m.height == 1024 && m.cells_x == 112 && m.cells_y == 112 && m.corner == 6 &&
                        m.cell_offset == 8 && m.symbol_bits == 4;
     const int cm = cc.means ? 2 : (cc.active ? 1 : 0);
-#define CB200_K1_GO(NC, G, C, S) k1_decode_kernel<NC, G, C, S><<<grid, kK1Threads, smem, stream>>>(m, d_rgb, n_frames, bands, d_cellvals, d_dirty, cc)
+#define CB200_K1_GO(NC, G, C, S) k1_decode_kernel<NC, G, C, S><<<grid, kK1Threads, smem, stream>>>(m, d_rgb, d_list, n_frames, bands, d_cellvals, d_dirty, cc)
 #define CB200_K1_SH(NC, G, C) do { if (sharpen) CB200_K1_GO(NC, G, C, true); else CB200_K1_GO(NC, G, C, false); } while (0)
 #define CB200_K1_CM(NC, G) do { if (cm == 2) CB200_K1_SH(NC, G, 2); else if (cm == 1) CB200_K1_SH(NC, G, 1); else CB200_K1_SH(NC, G, 0); } while (0)
     if (m.color_bits == 3) { if (g1024) CB200_K1_CM(8, true); else CB200_K1_CM(8, false); }

@@ -8,7 +8,8 @@ size_t k1_smem_bytes(bool sharpen);
 // resident CTAs per SM the grid is sized for: the kernel's launch bounds, four without sharpen, three with it
 int k1_ctas_per_sm(bool sharpen);
 cudaError_t k1_init_tables(const float* adjust256, const unsigned long long* tiles_L16);
-cudaError_t k1_launch(const Mode& m, const uint8_t* d_rgb, int n_frames, int bands, int grid, bool sharpen,
+// d_list: NULL = frames 0 .. n_frames-1 of d_rgb; else n_frames batch indices (device memory) -- results stay batch-indexed
+cudaError_t k1_launch(const Mode& m, const uint8_t* d_rgb, const uint32_t* d_list, int n_frames, int bands, int grid, bool sharpen,
                       uint8_t* d_cellvals, uint32_t* d_dirty, const CcmArg& cc, cudaStream_t stream);
 cudaError_t k1_symbols_launch(const uint16_t* d_windows, const uint8_t* d_cooldown, int n, uint8_t* d_sym, uint8_t* d_off, uint8_t* d_dist, cudaStream_t st);
 cudaError_t k1_colors_launch(const Mode& m, const uint8_t* d_rgb, int n, uint8_t* d_color, const CcmArg& cc, cudaStream_t st);

@@ -17,7 +17,8 @@
 //                   borders, rolling vertical sums in registers; output in 16x16-pixel TILES (32 B = one sector each) so that
 //                   a 10x10 window of the walk touches at most four sectors.  k_flood_raster_fast_sharpen is the same for
 //                   needs_sharpen (3x3 sharpen with reflected borders + block 7 with replicated ones, rows streamed through
-//                   registers, two barriers per row).
+//                   registers, two barriers per row).  A batch that mixes sharpened and plain frames launches both over the
+//                   same work list; each skips the items whose frame is of the other kind (one byte per frame).
 //   k_flood_walk    the serial 12 400-step walk, ONE WARP PER FRAME, up to 32 frames per SM in flight (the walk is a chain
 //                   of dependent heap and window accesses, so throughput comes from walking many frames at once):
 //                   binary heap in shared memory (+ global spill); the sift-down of a pop resolves FIVE heap levels per
@@ -125,7 +126,7 @@ __device__ __forceinline__ void gray8_packed(const uint2 q0, const uint2 q1, con
 
 __global__ void __launch_bounds__(kFastThreads)
 k_flood_raster_fast(const Mode m, const uint8_t* __restrict__ rgb, const uint32_t* __restrict__ list, const uint32_t* __restrict__ counters,
-                    int base, int cap, uint16_t* __restrict__ ws_raster)
+                    int base, int cap, const uint8_t* __restrict__ sharpen_of, uint16_t* __restrict__ ws_raster)
 {
     __shared__ uint32_t ex[2][kFastThreads];                       // halo words E of the row in flight (double buffered)
     __shared__ __align__(16) uint8_t outb[2][16][kFastThreads];    // threshold bytes of the 16-row group being collected
@@ -142,6 +143,7 @@ k_flood_raster_fast(const Mode m, const uint8_t* __restrict__ rgb, const uint32_
     for (int item = blockIdx.x; item < cnt * nb; item += gridDim.x) {
         const int e = item / nb, band = item - e * nb;
         const uint32_t f = list[base + e];
+        if (sharpen_of && sharpen_of[f]) continue;                // a sharpened frame of a mixed batch: the other raster's
         const uint8_t* frame = rgb + (size_t)f * row_bytes * (size_t)H;
         uint16_t* raster = ws_raster + (size_t)e * raster_words16(W, H);
         const int y0 = band * kFastBand, y1 = (y0 + kFastBand < H) ? y0 + kFastBand : H;
@@ -231,7 +233,7 @@ k_flood_raster_fast(const Mode m, const uint8_t* __restrict__ rgb, const uint32_
 // oracle over whole frames, borders included, in tests/test_k1x_sharpen_raster_model.py.
 __global__ void __launch_bounds__(kFastThreads)
 k_flood_raster_fast_sharpen(const Mode m, const uint8_t* __restrict__ rgb, const uint32_t* __restrict__ list, const uint32_t* __restrict__ counters,
-                            int base, int cap, uint16_t* __restrict__ ws_raster)
+                            int base, int cap, const uint8_t* __restrict__ sharpen_of, uint16_t* __restrict__ ws_raster)
 {
     __shared__ uint32_t ex[2][kFastThreads];                       // gray halo words E (double buffered by load parity)
     __shared__ uint32_t sx[2][2][kFastThreads];                    // sharpened halo words (s0,s1,s2) / (s5,s6,s7) (by row parity)
@@ -251,6 +253,7 @@ k_flood_raster_fast_sharpen(const Mode m, const uint8_t* __restrict__ rgb, const
     for (int item = blockIdx.x; item < cnt * nb; item += gridDim.x) {
         const int e = item / nb, band = item - e * nb;
         const uint32_t f = list[base + e];
+        if (sharpen_of && !sharpen_of[f]) continue;               // a plain frame of a mixed batch: the other raster's
         const uint8_t* frame = rgb + (size_t)f * row_bytes * (size_t)H;
         uint16_t* raster = ws_raster + (size_t)e * raster_words16(W, H);
         const int y0 = band * kFastBand, y1 = (y0 + kFastBand < H) ? y0 + kFastBand : H;
@@ -983,8 +986,8 @@ static cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int
 }
 
 cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb, int n_frames, bool no_fallback,
-                         bool force_all, bool sharpen, uint8_t* d_cellvals, const uint32_t* d_dirty, uint8_t* d_flags, CellTrace* d_trace,
-                         const CcmArg& cc, cudaStream_t st)
+                         bool force_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
+                         uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st)
 {
     if (n_frames <= 0) return cudaSuccess;
     cudaError_t e = flood_workspace_ensure(m, ws, n_frames);
@@ -997,9 +1000,9 @@ cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb
         const int cap = n_frames - base < ws.entry_cap ? n_frames - base : ws.entry_cap;
         const long long items = (long long)cap * ((m.height + kFastBand - 1) / kFastBand);
         const int rgrid = (int)(items < (long long)ws.sm_count * 8 ? items : (long long)ws.sm_count * 8);
-        if (sharpen) k_flood_raster_fast_sharpen<<<rgrid, kFastThreads, 0, st>>>(m, d_rgb, ws.list, ws.counters, base, cap, ws.raster);
-        else k_flood_raster_fast<<<rgrid, kFastThreads, 0, st>>>(m, d_rgb, ws.list, ws.counters, base, cap, ws.raster);
-        count_launch();
+        // a mixed batch runs both rasters over the chunk, each skipping the other kind's items
+        if (d_sharpen_of || !sharpen) { k_flood_raster_fast<<<rgrid, kFastThreads, 0, st>>>(m, d_rgb, ws.list, ws.counters, base, cap, d_sharpen_of, ws.raster); count_launch(); }
+        if (d_sharpen_of || sharpen) { k_flood_raster_fast_sharpen<<<rgrid, kFastThreads, 0, st>>>(m, d_rgb, ws.list, ws.counters, base, cap, d_sharpen_of, ws.raster); count_launch(); }
         int wgrid = cap < ws.slots ? cap : ws.slots;
         const bool few = cap <= ws.few_frames;              // at most one wave of big-heap walks: latency over occupancy
         k_flood_walk<<<wgrid, 32, few ? ws.walk_smem_few : ws.walk_smem, st>>>(m, ws.list, ws.counters, base, cap, ws.counters + 1 + c,

@@ -37,9 +37,10 @@ cudaError_t flood_init_tables(const float* adjust256, const unsigned long long* 
 cudaError_t flood_workspace_create(const Mode& m, int sm_count, const uint16_t* adj_host, FloodWorkspace* ws);
 void flood_workspace_destroy(FloodWorkspace* ws);
 // writes d_flags[f] for every frame: 0 = K1 result stands, CB200_FRAME_FALLBACK = re-decoded here,
-// CB200_FRAME_INEXACT = needed but skipped (no_fallback)
+// CB200_FRAME_INEXACT = needed but skipped (no_fallback).  d_sharpen_of: NULL = every frame is preprocessed as `sharpen` says;
+// else one byte per frame of the batch (device memory, nonzero = sharpen) and `sharpen` is ignored
 cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb, int n_frames, bool no_fallback,
-                         bool force_all, bool sharpen, uint8_t* d_cellvals, const uint32_t* d_dirty, uint8_t* d_flags, CellTrace* d_trace,
-                         const CcmArg& cc, cudaStream_t st);
+                         bool force_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
+                         uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st);
 
 }  // namespace cb200

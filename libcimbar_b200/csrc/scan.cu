@@ -381,13 +381,14 @@ int cb200_scan_extract_decode_fountain(cb200_ctx* c, const uint8_t* pictures, in
                                        uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
                                        int32_t* extract_status)
 {
+    int rc = check_camera_flags(flags); if (rc) return rc;
     if (!c || !pictures || !chunks_out || !chunk_count || !extract_status || n < 0 || n > c->max_frames || w < 2 || h < 2)
         return fail(CB200_ERR_ARG, "bad arguments");
     if (n == 0) return CB200_OK;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
     const uint8_t* d = nullptr;
-    int rc = stage_pictures(c, pictures, w, h, n, &d); if (rc) return rc;
+    rc = stage_pictures(c, pictures, w, h, n, &d); if (rc) return rc;
     rc = scan_run(c, d, w, h, n); if (rc) return rc;
     const ScanScratch* s = c->scan;
     // Extractor::extract (Extractor.h:30-46): fewer than four anchors -> FAILURE; Corners = the anchors' centres
@@ -413,7 +414,14 @@ int cb200_scan_extract_decode_fountain(cb200_ctx* c, const uint8_t* pictures, in
         double m9[9];
         if (cb200_perspective_transform(cr, ident, m9) != CB200_OK) { extract_status[i] = 0; memcpy(cr, ident, sizeof(ident)); }   // collinear anchors
     }
-    rc = cb200_extract_decode_fountain_dev(c, d, w, h, n, corners.data(), flags, chunks_out, chunk_count, chunk_mask, frame_flags);
+    // CB200_FLAG_SHARPEN_IF_NEEDED: the CLI's decode loop sharpens exactly the NEEDS_SHARPEN pictures (cimbar.cpp:124-160)
+    std::vector<uint8_t> sharpen;
+    if (flags & CB200_FLAG_SHARPEN_IF_NEEDED) {
+        sharpen.resize((size_t)n);
+        for (int i = 0; i < n; ++i) sharpen[(size_t)i] = extract_status[i] == 2;
+    }
+    rc = extract_decode_to_host(c, d, w, h, n, corners.data(), flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, sharpen.empty() ? nullptr : sharpen.data(),
+                                chunks_out, chunk_count, chunk_mask, frame_flags);
     if (rc) return rc;
     for (int i = 0; i < n; ++i)
         if (extract_status[i] <= 0) { chunk_count[i] = 0; if (chunk_mask) chunk_mask[i] = 0; }

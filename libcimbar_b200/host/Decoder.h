@@ -2,6 +2,7 @@
 // Same constructor and the same two templates
 //     unsigned decode(const MAT& img, STREAM& ostream, bool should_preprocess=false, int color_correction=2)
 //     unsigned decode_fountain(const MAT& img, FOUNTAINSTREAM& ostream, bool should_preprocess=false, int color_correction=2)
+// (plus batched decode_fountain overloads over n frames, with one should_preprocess for all of them or one per frame)
 // with the same stream protocol and the same return value (good bytes).  The frame is decoded on the GPU through the C ABI;
 // the host only hands the results to the caller's stream:
 //   decode()           good RS blocks are write()n, failed ones announced with `stream << BadChunk(n)` -- what the two
@@ -121,6 +122,24 @@ public:
 	template <typename MAT, typename FOUNTAINSTREAM>
 	unsigned decode_fountain(const MAT* imgs, unsigned n, FOUNTAINSTREAM& ostream, bool should_preprocess = false, int color_correction = 2)
 	{
+		return decode_fountain_batch(imgs, n, ostream, nullptr, should_preprocess, color_correction);
+	}
+
+	// The same with should_preprocess chosen per frame (n flags): the cimbar CLI's decode loop (cimbar.cpp:124-160) over
+	// cb200::Extractor results -- `should_preprocess[f] = extract(...) == Extractor::NEEDS_SHARPEN` -- in one call.
+	template <typename MAT, typename FOUNTAINSTREAM>
+	unsigned decode_fountain(const MAT* imgs, unsigned n, FOUNTAINSTREAM& ostream, const bool* should_preprocess, int color_correction = 2)
+	{
+		if (!should_preprocess) throw std::invalid_argument("cb200::Decoder: null should_preprocess");
+		return decode_fountain_batch(imgs, n, ostream, should_preprocess, false, color_correction);
+	}
+
+protected:
+	// each: n should_preprocess flags, or nullptr = should_preprocess for every frame
+	template <typename MAT, typename FOUNTAINSTREAM>
+	unsigned decode_fountain_batch(const MAT* imgs, unsigned n, FOUNTAINSTREAM& ostream, const bool* each, bool should_preprocess,
+	                               int color_correction)
+	{
 		const unsigned chunk_size = _info.chunk_size;
 		// Decoder.h:180-185: on a chunk-size mismatch the decode is eaten (it still runs, and still updates the CCM)
 		const bool deliver = ostream.chunk_size() == chunk_size;
@@ -160,12 +179,17 @@ public:
 			std::vector<uint8_t> ff(m);
 			detail::push_ccm(c);
 			// the fit of color_correction 2 needs this stream's chunk callbacks in the reference: they exist in decode_fountain only
-			const uint32_t flags = flags_for(should_preprocess, color_correction, true);
+			const uint32_t flags = flags_for(each ? false : should_preprocess, color_correction, true);
+			std::vector<uint8_t> sel;
+			if (each)
+				for (unsigned k = 0; k < m; ++k) sel.push_back(each[good_idx[k]] ? 1 : 0);
 			if (_useEcc)
 			{
 				std::vector<uint8_t> out((size_t)m * _info.data_bytes);
 				std::vector<uint32_t> cnt(m), mask(m);
-				if (cb200_decode_fountain(c, batch, (int)m, flags, out.data(), cnt.data(), mask.data(), ff.data()) != CB200_OK)
+				const int rc = each ? cb200_decode_fountain_sharpen(c, batch, (int)m, flags, sel.data(), out.data(), cnt.data(), mask.data(), ff.data())
+				                         : cb200_decode_fountain(c, batch, (int)m, flags, out.data(), cnt.data(), mask.data(), ff.data());
+				if (rc != CB200_OK)
 					throw std::runtime_error(std::string("cb200_decode_fountain: ") + cb200_last_error());
 				for (unsigned k = 0; k < m; ++k)
 				{
@@ -177,8 +201,31 @@ public:
 			{   // ecc_bytes = 0: the raw bit stream passes through reed_solomon_stream untouched and is re-chunked as it is;
 				// the tail that does not fill a chunk is never flushed.  No RS pass means no header for a CCM fit.
 				std::vector<uint8_t> raw((size_t)m * _info.raw_bytes);
-				if (cb200_decode_raw(c, batch, (int)m, flags & ~CB200_FLAG_CC_FIT, raw.data(), ff.data()) != CB200_OK)
-					throw std::runtime_error(std::string("cb200_decode_raw: ") + cb200_last_error());
+				if (!each)
+				{
+					if (cb200_decode_raw(c, batch, (int)m, flags & ~CB200_FLAG_CC_FIT, raw.data(), ff.data()) != CB200_OK)
+						throw std::runtime_error(std::string("cb200_decode_raw: ") + cb200_last_error());
+				}
+				else
+				{   // no fit, so nothing carries between frames except the CCM the last one leaves (color_correction 1): one call
+					// per kind, the kind of the last frame last
+					for (int pass = 0; pass < 2; ++pass)
+					{
+						const uint8_t kind = (uint8_t)(pass == 0 ? !sel[m - 1] : sel[m - 1]);
+						std::vector<unsigned> ks;
+						for (unsigned k = 0; k < m; ++k) if (sel[k] == kind) ks.push_back(k);
+						if (ks.empty()) continue;
+						std::vector<uint8_t> in(ks.size() * (size_t)_info.frame_bytes), part(ks.size() * (size_t)_info.raw_bytes), pff(ks.size());
+						for (size_t j = 0; j < ks.size(); ++j) std::memcpy(in.data() + j * _info.frame_bytes, batch + (size_t)ks[j] * _info.frame_bytes, _info.frame_bytes);
+						if (cb200_decode_raw(c, in.data(), (int)ks.size(), (flags & ~CB200_FLAG_CC_FIT) | (kind ? CB200_FLAG_SHARPEN : 0u), part.data(), pff.data()) != CB200_OK)
+							throw std::runtime_error(std::string("cb200_decode_raw: ") + cb200_last_error());
+						for (size_t j = 0; j < ks.size(); ++j)
+						{
+							std::memcpy(raw.data() + (size_t)ks[j] * _info.raw_bytes, part.data() + j * _info.raw_bytes, _info.raw_bytes);
+							ff[ks[j]] = pff[j];
+						}
+					}
+				}
 				if (flags & CB200_FLAG_CC_FIT) _warnings |= WARN_COLOR_CORRECTION_IGNORED;
 				for (unsigned k = 0; k < m; ++k)
 				{
@@ -202,7 +249,6 @@ public:
 		return total;
 	}
 
-protected:
 	cb200_ctx* ctx(int frames) const { return detail::thread_context(_device, _modeVal, frames); }
 
 	void check_mode() const
