@@ -213,6 +213,34 @@ int cb200_scan_extract_decode_fountain(cb200_ctx* ctx, const uint8_t* pictures, 
                                        uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
                                        int32_t* extract_status);
 
+/* ---- ragged batches: n camera pictures, each of its own size ----------------------------------------------------------
+
+   The reference CLI's decode loop (src/exe/cimbar/cimbar.cpp:124-160) takes files of any sizes -- landscape and portrait photographs
+   alternate -- and runs Extractor::extract + Decoder::decode_fountain on each, in order, with one decoder.  These entry points do
+   the same in one call.  wh: n x 2 int32 in HOST memory, (w_i, h_i) of picture i; the pictures are tightly packed RGB8.  The host
+   entry points take n host pointers (one buffer per picture, e.g. per file; packed into the library's staging buffer with one copy
+   each); the _dev entry points take one packed device buffer in which picture i starts at byte 3 * sum_{j<i} w_j h_j.  A uniform
+   batch gives exactly what the uniform entry point gives.  CB200_ERR_ARG, before any CUDA call, for n < 0, a null wh or pictures
+   (or a null picture pointer), a picture whose short side is under 60 or 4500 and up (the message names the picture's index),
+   n > max_frames on the decoding calls, and both sharpen flags together; a bad picture fails the whole call. */
+
+/* cb200_scan for a ragged batch: outputs as cb200_scan, one entry per picture */
+int cb200_scan_ragged(cb200_ctx* ctx, const uint8_t* const* pictures, const int32_t* wh, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff);
+int cb200_scan_ragged_dev(cb200_ctx* ctx, const uint8_t* d_pictures, const int32_t* wh, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff);
+/* cb200_scan_blurred after a ragged scan: the blurred gray pictures back to back (sum_i w_i h_i bytes) and n thresholds */
+int cb200_scan_blurred_ragged(cb200_ctx* ctx, uint8_t* blurred_out, int32_t* thresholds_out, const int32_t* wh, int n);
+/* cb200_extract_decode_fountain_dev for a ragged batch in device memory, with the caller's corners (n x 8 floats); honours
+   CB200_FLAG_SHARPEN_IF_NEEDED as that call does (sharpen iff the corners fail Corners::is_granular_scale) */
+int cb200_extract_decode_fountain_ragged_dev(cb200_ctx* ctx, const uint8_t* d_pictures, const int32_t* wh, int n, const float* corners,
+                                             uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
+                                             uint8_t* frame_flags);
+/* the CLI's decode loop in one call: cb200_scan_extract_decode_fountain for a ragged batch.  Outputs, extract_status and every flag
+   behave as there: CB200_FLAG_SHARPEN_IF_NEEDED sharpens exactly the NEEDS_SHARPEN pictures, and the CCM of CB200_FLAG_CC_FIT
+   carries from picture to picture in batch order. */
+int cb200_scan_extract_decode_fountain_ragged(cb200_ctx* ctx, const uint8_t* const* pictures, const int32_t* wh, int n, uint32_t flags,
+                                              uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
+                                              int32_t* extract_status);
+
 /* per-cell record of the exact flood walk: what CimbReader::read() hands back, step by step
    (src/lib/cimb_translator/CimbReader.cpp:139-162, PositionData.h:4-9) */
 typedef struct cb200_cell_trace {
@@ -288,7 +316,8 @@ int cb200_encode_cells_dev(cb200_ctx* ctx, const uint8_t* d_payload, int n, uint
 
 /* when enabled, CUDA events are recorded on the context's stream around every kernel of every pipeline call (a ring of
    the last 64 calls).  cb200_get_timing returns the milliseconds of the call `calls_back` calls ago (0 = last) in launch
-   order: [0] K1 fused decode (both K1 launches of a batch with a per-frame sharpen choice), [1] K1x exact-walk kernel, [2] pack, [3] RS, [4] chunk mask (decode_raw_dev stops after [2]) */
+   order: [0] K1 fused decode (both K1 launches of a batch with a per-frame sharpen choice), [1] K1x exact-walk kernel, [2] pack, [3] RS, [4] chunk mask (decode_raw_dev stops after [2]);
+   a scan call: [0] blur + histogram (all blur launches of a ragged batch), [1] Otsu, [2] anchors */
 int cb200_set_timing(cb200_ctx* ctx, int enable);
 /* kernels launched by this library in this process so far (every launch site counts itself): bench.py reports the
    difference across its timed region as "gpu_launches" */

@@ -33,6 +33,8 @@ EXPORTS = [
     "cb200_gather_release", "cb200_gather_acquire",
     "cb200_gather_status", "cb200_comm_unique_id", "cb200_comm_init", "cb200_gather_chunks", "cb200_gather_chunks_wait",
     "cb200_decode_chunks_sharpen_dev", "cb200_decode_fountain_sharpen",
+    "cb200_scan_ragged", "cb200_scan_ragged_dev", "cb200_scan_blurred_ragged", "cb200_extract_decode_fountain_ragged_dev",
+    "cb200_scan_extract_decode_fountain_ragged",
 ]
 
 
@@ -109,6 +111,11 @@ def load_library():
     lib.cb200_scan_dev.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     lib.cb200_scan_blurred.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
     lib.cb200_scan_extract_decode_fountain.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_uint32, vp, vp, vp, vp, vp]
+    lib.cb200_scan_ragged.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp]
+    lib.cb200_scan_ragged_dev.argtypes = [vp, vp, vp, C.c_int, vp, vp, vp]
+    lib.cb200_scan_blurred_ragged.argtypes = [vp, vp, vp, vp, C.c_int]
+    lib.cb200_extract_decode_fountain_ragged_dev.argtypes = [vp, vp, vp, C.c_int, vp, C.c_uint32, vp, vp, vp, vp]
+    lib.cb200_scan_extract_decode_fountain_ragged.argtypes = [vp, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp]
     lib.cb200_decode_cells_means.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, vp, vp]
     lib.cb200_fit_ccm.argtypes = [vp, u8p, u8p, C.c_uint32, C.c_uint32, C.c_void_p]
     lib.cb200_palette_color.argtypes = [C.c_int, C.c_uint, C.c_int, u8p]
@@ -173,6 +180,17 @@ def interleave_indices(mode_val=68):
 
 def _hptr(a):
     return a.ctypes.data if a is not None else None
+
+
+def _ragged(pictures):
+    """a list of (h, w, 3) uint8 pictures of any sizes -> (contiguous pictures, n host pointers, wh n x 2 int32 = (w, h))"""
+    pics = [np.ascontiguousarray(p, dtype=np.uint8) for p in pictures]
+    for i, p in enumerate(pics):
+        if p.ndim != 3 or p.shape[2] != 3:
+            raise Cb200Error(f"picture {i} must be (h, w, 3) RGB8, got {p.shape}")
+    ptrs = (C.c_void_p * max(len(pics), 1))(*[p.ctypes.data for p in pics])
+    wh = np.array([(p.shape[1], p.shape[0]) for p in pics], dtype=np.int32).reshape(-1, 2)
+    return pics, ptrs, wh
 
 
 def _selection(sharpen, n):
@@ -297,6 +315,42 @@ class Context:
         thr = np.zeros(n, dtype=np.int32)
         _check(self.lib.cb200_scan_blurred(self._h, blurred.ctypes.data, thr.ctypes.data, w, h, n))
         return blurred, thr
+
+    def scan_ragged(self, pictures):
+        """scan() for a list of (h, w, 3) uint8 pictures of any sizes, in one call"""
+        pics, ptrs, wh = _ragged(pictures)
+        n = len(pics)
+        anchors = np.zeros((n, 4, 4), dtype=np.int32)
+        count = np.zeros(n, dtype=np.int32)
+        cutoff = np.zeros(n, dtype=np.uint32)
+        _check(self.lib.cb200_scan_ragged(self._h, ptrs, wh.ctypes.data, n, anchors.ctypes.data, count.ctypes.data, cutoff.ctypes.data))
+        return anchors, count, cutoff
+
+    def scan_blurred_ragged(self, shapes):
+        """the blurred gray pictures (a list, one (h, w) array each) and Otsu thresholds of the last scan call; shapes: its (h, w)s"""
+        wh = np.array([(w, h) for h, w in (tuple(s)[:2] for s in shapes)], dtype=np.int32).reshape(-1, 2)
+        n = wh.shape[0]
+        flat = np.zeros(int((wh[:, 0].astype(np.int64) * wh[:, 1]).sum()), dtype=np.uint8)
+        thr = np.zeros(n, dtype=np.int32)
+        _check(self.lib.cb200_scan_blurred_ragged(self._h, flat.ctypes.data, thr.ctypes.data, wh.ctypes.data, n))
+        out, at = [], 0
+        for w, h in wh.tolist():
+            out.append(flat[at:at + w * h].reshape(h, w))
+            at += w * h
+        return out, thr
+
+    def scan_extract_decode_fountain_ragged(self, pictures, flags=0):
+        """scan_extract_decode_fountain for a list of (h, w, 3) uint8 pictures of any sizes, in order (the CLI's decode loop)"""
+        pics, ptrs, wh = _ragged(pictures)
+        n = len(pics)
+        chunks = np.zeros((n, self.info.chunks_per_frame, self.info.chunk_size), dtype=np.uint8)
+        count = np.zeros(n, dtype=np.uint32)
+        mask = np.zeros(n, dtype=np.uint32)
+        ff = np.zeros(n, dtype=np.uint8)
+        status = np.zeros(n, dtype=np.int32)
+        _check(self.lib.cb200_scan_extract_decode_fountain_ragged(self._h, ptrs, wh.ctypes.data, n, flags, chunks.ctypes.data, count.ctypes.data,
+                                                                  mask.ctypes.data, ff.ctypes.data, status.ctypes.data))
+        return chunks, count, mask, ff, status
 
     def scan_extract_decode_fountain(self, pictures, flags=0):
         """Extractor::extract + Decoder::decode_fountain: camera pictures in, chunks out -> (chunks, count, mask, frame_flags, extract_status)"""

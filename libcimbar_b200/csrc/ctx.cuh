@@ -6,6 +6,7 @@
 #include "ccm.cuh"
 
 #include <string>
+#include <vector>
 
 namespace cb200 {
 // thread-local error text behind cb200_last_error(); both return `code`
@@ -23,9 +24,25 @@ int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t 
                             uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
 // CB200_ERR_ARG for CB200_FLAG_SHARPEN together with CB200_FLAG_SHARPEN_IF_NEEDED (deskew.cu)
 int check_camera_flags(uint32_t flags);
-// cb200_extract_decode_fountain_dev with the same selection (deskew.cu)
-int extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
+// one camera picture of a batch as the extractor kernels (scan.cu, deskew.cu) read it.  The host builds the table per call, for
+// uniform batches too: picture i of a packed batch starts at byte 3 * sum_{j<i} w_j h_j, its blurred gray at sum_{j<i} w_j h_j
+struct PicDesc {
+    uint64_t src;        // byte offset of the RGB8 picture in the source buffer
+    uint64_t blur;       // byte offset of its blurred gray picture in the scan's buffer (k_scan_blur4 / k_scan_anchors)
+    int w, h;
+    int words;           // k_scan_blur4's word path: w % 4 == 0 and both bases 4-byte aligned
+    int tile0;           // first tile of the picture in the blur launch of its radius
+};
+// wh: n x (w, h) on the host.  CB200_ERR_ARG naming the picture if a size is outside what the scan restates (short side 60 ..
+// 4499) (scan.cu); no CUDA call
+int check_picture_sizes(const int32_t* wh, int n);
+// the uniform batch as a ragged one: n x (w, h)
+std::vector<int32_t> uniform_sizes(int w, int h, int n);
+// cb200_extract_decode_fountain_dev with the same selection, for pictures of sizes wh (n x (w, h)) packed in d_src (deskew.cu)
+int extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int n, const float* corners, uint32_t flags,
                            const uint8_t* sharpen, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
+// CB200_FLAG_SHARPEN_IF_NEEDED on given corners: sharpen[i] = 1 iff picture i's corners fail Corners::is_granular_scale (deskew.cu)
+std::vector<uint8_t> sharpen_from_corners(const cb200_ctx* c, const float* corners, int n);
 }  // namespace cb200
 #define CK(call, what) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cb200::fail_cuda(e__, what); } while (0)
 

@@ -18,6 +18,7 @@
 #include "ctx.cuh"
 #include "scan_core.cuh"
 
+#include <string>
 #include <vector>
 
 namespace cb200 {
@@ -32,6 +33,8 @@ struct ScanScratch {                 // per-context scratch of the scan entry po
     int ws_pics = 0, ws_rows_cap = 0;
     int4* d_anchors = nullptr; int* d_count = nullptr; unsigned* d_cutoff = nullptr; int* d_status = nullptr;
     int4* h_anchors = nullptr; int* h_count = nullptr;      // pinned results: [n][4] anchors, then count / cutoff / status per picture
+    uint8_t* d_table = nullptr;                             // n PicDesc, then the pictures grouped by blur radius (n int)
+    std::vector<uint8_t> h_table;                           // its host image, built per call
 };
 
 void scan_destroy(ScanScratch* s)
@@ -39,7 +42,7 @@ void scan_destroy(ScanScratch* s)
     if (!s) return;
     cudaFree(s->d_pics); cudaFree(s->d_blur); cudaFree(s->d_hist); cudaFree(s->d_thr);
     cudaFree(s->d_rowbuf); cudaFree(s->d_rowcnt); cudaFree(s->d_pts); cudaFree(s->d_res); cudaFree(s->d_nres);
-    cudaFree(s->d_anchors); cudaFree(s->d_count); cudaFree(s->d_cutoff); cudaFree(s->d_status);
+    cudaFree(s->d_anchors); cudaFree(s->d_count); cudaFree(s->d_cutoff); cudaFree(s->d_status); cudaFree(s->d_table);
     cudaFreeHost(s->h_anchors); cudaFreeHost(s->h_count);
     delete s;
 }
@@ -66,8 +69,9 @@ constexpr int kBlurTW = 128, kBlurTH = 32, kBlurThreads = 256;
 // as three aligned words and are converted with K1's IDP.2A form (8 instructions per four pixels), the horizontal taps are IDP.4A dot
 // products of realigned gray words with the packed coefficients, the vertical pass reads four 16-bit sums per 64-bit load, and a warp
 // owns a tile row (no divisions).
-// The word path needs 4-byte aligned rows: a picture width that is a multiple of four and an aligned base (checked by the caller);
-// otherwise, and in tiles that cross the right edge, pixels are fetched one by one.
+// The word path needs 4-byte aligned rows: a picture width that is a multiple of four and aligned source and blurred bases (decided
+// per picture by the host: in a packed batch a picture that follows one of odd area starts unaligned); otherwise, and in tiles that
+// cross the right edge, pixels are fetched one by one.
 template <int R> struct BlurKW {     // the 2R+1 coefficients as bytes of up to three words (IDP.4A operands)
     __device__ static constexpr uint32_t w(int i)
     {
@@ -81,18 +85,34 @@ __device__ __forceinline__ uint32_t gray_scalar(const uint8_t* p)
     return (9798u * p[0] + 19235u * p[1] + 3735u * p[2] + 16384u) >> 15;
 }
 
+// One launch per radius over the flattened tiles of that radius' pictures: order[0 .. npics) lists them (batch indices into the
+// descriptor table, in batch order), their tiles are numbered consecutively from desc[order[k]].tile0, row-major inside a picture.
+// A CTA finds its picture by division when all listed pictures have one size (uniform_tiles tiles each), else by binary search.
 template <int R>
 __global__ void __launch_bounds__(kBlurThreads)
-k_scan_blur4(const uint8_t* __restrict__ rgb, int w, int h, int words_ok, uint8_t* __restrict__ out, unsigned* __restrict__ hist)
+k_scan_blur4(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out, const PicDesc* __restrict__ desc, const int* __restrict__ order,
+             int npics, int uniform_tiles, unsigned* __restrict__ hist)
 {
     constexpr int GH = kBlurTH + 2 * R, GP = kBlurTW + 8, NW = (2 * R + 1 + 3) / 4;      // gray pitch: interior at byte 4
     __shared__ __align__(16) uint8_t g[GH][GP];
     __shared__ __align__(16) uint16_t hs[GH][kBlurTW];
     __shared__ unsigned lh[256];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int pic = blockIdx.z, tx0 = blockIdx.x * kBlurTW, ty0 = blockIdx.y * kBlurTH;
-    const size_t npx = (size_t)w * (size_t)h;
-    const uint8_t* src = rgb + (size_t)pic * npx * 3;
+    const int t = (int)blockIdx.x;
+    int k;
+    if (uniform_tiles) {
+        k = t / uniform_tiles;
+    } else {
+        int lo = 0, hi = npics - 1;
+        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (__ldg(&desc[__ldg(order + mid)].tile0) <= t) lo = mid; else hi = mid - 1; }
+        k = lo;
+    }
+    const int pic = __ldg(order + k);
+    const PicDesc* d = desc + pic;
+    const int w = __ldg(&d->w), h = __ldg(&d->h), words_ok = __ldg(&d->words);
+    const int tiles_x = (w + kBlurTW - 1) / kBlurTW, tl = t - __ldg(&d->tile0), tyi = tl / tiles_x;
+    const int tx0 = (tl - tyi * tiles_x) * kBlurTW, ty0 = tyi * kBlurTH;
+    const uint8_t* src = rgb + __ldg(&d->src);
     lh[tid] = 0;
     // ---- gray of the tile and its halo
     const int x = tx0 + 4 * lane;
@@ -143,7 +163,7 @@ k_scan_blur4(const uint8_t* __restrict__ rgb, int w, int h, int words_ok, uint8_
     }
     __syncthreads();
     // ---- vertical pass, histogram, store
-    uint8_t* dst = out + (size_t)pic * npx;
+    uint8_t* dst = out + __ldg(&d->blur);
     for (int r = warp; r < kBlurTH; r += kBlurThreads / 32) {
         const int y = ty0 + r;
         if (y >= h) break;
@@ -172,11 +192,12 @@ k_scan_blur4(const uint8_t* __restrict__ rgb, int w, int h, int words_ok, uint8_
 
 // ---------------------------------------------------------------------------------------------- Otsu
 // cv::threshold(THRESH_OTSU) -> getThreshVal_Otsu_8u (modules/imgproc/src/thresh.cpp), double precision, operation for operation
-__global__ void k_scan_otsu(const unsigned* __restrict__ hist, int n, double npx, int* __restrict__ thr)
+__global__ void k_scan_otsu(const unsigned* __restrict__ hist, const PicDesc* __restrict__ desc, int n, int* __restrict__ thr)
 {
     const int pic = blockIdx.x * blockDim.x + threadIdx.x;
     if (pic >= n) return;
     const unsigned* hh = hist + (size_t)pic * 256;
+    const double npx = (double)((long long)desc[pic].w * desc[pic].h);
     const double scale = ddiv(1., npx);
     double mu = 0;
     for (int i = 0; i < 256; ++i) mu = dadd(mu, dmul((double)i, (double)hh[i]));
@@ -204,23 +225,23 @@ __global__ void k_scan_otsu(const unsigned* __restrict__ hist, int n, double npx
 constexpr int kScanThreads = 256;
 
 __global__ void __launch_bounds__(kScanThreads)
-k_scan_anchors(const uint8_t* __restrict__ blurred, const int* __restrict__ thr, int w, int h, int rows_cap,
+k_scan_anchors(const uint8_t* __restrict__ blurred, const PicDesc* __restrict__ desc, const int* __restrict__ thr, int rows_cap,
                Anchor* rowbuf, int* rowcnt, Anchor* pts, Anchor* res, int* nres,
                int4* __restrict__ anchors_out, int* __restrict__ count_out, unsigned* __restrict__ cutoff_out, int* __restrict__ status_out)
 {
     __shared__ PicShared sh;
     const int pic = blockIdx.x;
+    Anchor* out = reinterpret_cast<Anchor*>(anchors_out + (size_t)pic * 4);
+    if (threadIdx.x < 4) out[threadIdx.x] = mk(0, 0, 0, 0);
+    __syncthreads();
     Img im;
-    im.px = blurred + (size_t)pic * (size_t)w * (size_t)h; im.w = w; im.h = h; im.thr = thr[pic];
+    im.px = blurred + desc[pic].blur; im.w = desc[pic].w; im.h = desc[pic].h; im.thr = thr[pic];
     PicWs ws;
     ws.rowbuf = rowbuf + (size_t)pic * rows_cap * kRowCap; ws.rowcnt = rowcnt + (size_t)pic * rows_cap;
     ws.pts = pts + (size_t)pic * kPtsCap; ws.res = res + (size_t)pic * kPtsCap * kResCap; ws.nres = nres + (size_t)pic * kPtsCap;
     ws.rows_cap = rows_cap;
     Exec ex;
-    ex.tid = threadIdx.x; ex.nthreads = blockDim.x;
-    Anchor* out = reinterpret_cast<Anchor*>(anchors_out + (size_t)pic * 4);
-    if (threadIdx.x < 4) out[threadIdx.x] = mk(0, 0, 0, 0);
-    __syncthreads();
+    ex.tid = threadIdx.x; ex.nthreads = kScanThreads;
     const int count = scan_picture(ex, im, ws, sh, out, cutoff_out + pic, status_out + pic);
     if (threadIdx.x == 0) count_out[pic] = count;
 }
@@ -241,42 +262,67 @@ static int scan_blur_radius(int w, int h)               // Scanner.h:93-103, :15
     return (int)(unit / 2);
 }
 
-// blurred pictures + thresholds + anchors for n pictures in device memory; results land in the pinned host arrays of the state
-static int scan_run(cb200_ctx* c, const uint8_t* d_pics, int w, int h, int n)
+int check_picture_sizes(const int32_t* wh, int n)
+{
+    for (int i = 0; i < n; ++i) {
+        const int w = wh[2 * i], h = wh[2 * i + 1];
+        if ((w < h ? w : h) < 60)
+            return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " is " + std::to_string(w) + " x " + std::to_string(h) +
+                                           ": smaller than 60 pixels on its short side (Scanner's row step would be 0)");
+        if (scan_blur_radius(w, h) > 4)
+            return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " is " + std::to_string(w) + " x " + std::to_string(h) +
+                                           ": pictures with a short side of 4500 pixels or more need a Gaussian kernel beyond 9 taps, which is not restated");
+    }
+    return CB200_OK;
+}
+
+std::vector<int32_t> uniform_sizes(int w, int h, int n)
+{
+    std::vector<int32_t> wh(2 * (size_t)(n > 0 ? n : 0));
+    for (int i = 0; i < n; ++i) { wh[2 * (size_t)i] = w; wh[2 * (size_t)i + 1] = h; }
+    return wh;
+}
+
+// blurred pictures + thresholds + anchors for n pictures of sizes wh (checked by check_picture_sizes) packed in device memory;
+// results land in the pinned host arrays of the state
+static int scan_run(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n)
 {
     ScanScratch* s = sstate(c);
     cudaStream_t st = c->stream;
-    const int R = scan_blur_radius(w, h);
-    if (R > 4) return fail(CB200_ERR_ARG, "pictures with a short side of 4500 pixels or more need a Gaussian kernel beyond 9 taps, which is not restated");
-    const int skip = (w < h ? w : h) / 60;
-    if (skip < 1) return fail(CB200_ERR_ARG, "picture smaller than 60 pixels on its short side (Scanner's row step would be 0)");
-    const size_t npx = (size_t)w * (size_t)h;
-    if (npx * (size_t)n > s->blur_bytes) {
+    size_t npx = 0;
+    int rows_cap = 0;
+    for (int i = 0; i < n; ++i) {
+        const int w = wh[2 * i], h = wh[2 * i + 1], skip = (w < h ? w : h) / 60;
+        npx += (size_t)w * (size_t)h;
+        // rows of a pass: the primary pass scans h / skip rows, the bottom-right window at most 2 h / skip (half the step)
+        const int rc = 2 * ((h + skip - 1) / skip) + 4;
+        if (rc > rows_cap) rows_cap = rc;
+    }
+    if (npx > s->blur_bytes) {
         cudaFree(s->d_blur); s->d_blur = nullptr; s->blur_bytes = 0;
-        CK(cudaMalloc(&s->d_blur, npx * (size_t)n), "cudaMalloc blurred pictures");
-        s->blur_bytes = npx * (size_t)n;
+        CK(cudaMalloc(&s->d_blur, npx), "cudaMalloc blurred pictures");
+        s->blur_bytes = npx;
     }
     if (n > s->thr_cap) {
         cudaFree(s->d_hist); cudaFree(s->d_thr); cudaFree(s->d_anchors); cudaFree(s->d_count); cudaFree(s->d_cutoff); cudaFree(s->d_status);
-        cudaFreeHost(s->h_anchors); cudaFreeHost(s->h_count);
+        cudaFree(s->d_table); cudaFreeHost(s->h_anchors); cudaFreeHost(s->h_count);
         s->d_hist = nullptr; s->d_thr = nullptr; s->d_anchors = nullptr; s->d_count = nullptr; s->d_cutoff = nullptr; s->d_status = nullptr;
-        s->h_anchors = nullptr; s->h_count = nullptr; s->thr_cap = 0;
+        s->d_table = nullptr; s->h_anchors = nullptr; s->h_count = nullptr; s->thr_cap = 0;
         CK(cudaMalloc(&s->d_hist, sizeof(unsigned) * 256 * (size_t)n), "cudaMalloc histograms");
         CK(cudaMalloc(&s->d_thr, sizeof(int) * (size_t)n), "cudaMalloc thresholds");
         CK(cudaMalloc(&s->d_anchors, sizeof(int4) * 4 * (size_t)n), "cudaMalloc anchors");
         CK(cudaMalloc(&s->d_count, sizeof(int) * (size_t)n), "cudaMalloc counts");
         CK(cudaMalloc(&s->d_cutoff, sizeof(unsigned) * (size_t)n), "cudaMalloc cutoffs");
         CK(cudaMalloc(&s->d_status, sizeof(int) * (size_t)n), "cudaMalloc status");
+        CK(cudaMalloc(&s->d_table, (sizeof(PicDesc) + sizeof(int)) * (size_t)n), "cudaMalloc picture table");
         CK(cudaMallocHost(&s->h_anchors, sizeof(int4) * 4 * (size_t)n), "cudaMallocHost anchors");
         CK(cudaMallocHost(&s->h_count, sizeof(int) * 3 * (size_t)n), "cudaMallocHost counts");
         s->thr_cap = n;
     }
-    // rows of a pass: the primary pass scans h / skip rows, the bottom-right window at most 2 h / skip (half the step)
-    const int rows_cap = 2 * ((h + skip - 1) / skip) + 4;
     if (n > s->ws_pics || rows_cap > s->ws_rows_cap) {
         cudaFree(s->d_rowbuf); cudaFree(s->d_rowcnt); cudaFree(s->d_pts); cudaFree(s->d_res); cudaFree(s->d_nres);
-        s->d_rowbuf = nullptr; s->d_rowcnt = nullptr; s->d_pts = nullptr; s->d_res = nullptr; s->d_nres = nullptr; s->ws_pics = 0; s->ws_rows_cap = 0;
         const int np = n > s->ws_pics ? n : s->ws_pics, rc = rows_cap > s->ws_rows_cap ? rows_cap : s->ws_rows_cap;
+        s->d_rowbuf = nullptr; s->d_rowcnt = nullptr; s->d_pts = nullptr; s->d_res = nullptr; s->d_nres = nullptr; s->ws_pics = 0; s->ws_rows_cap = 0;
         CK(cudaMalloc(&s->d_rowbuf, sizeof(Anchor) * (size_t)np * rc * kRowCap), "cudaMalloc scan rows");
         CK(cudaMalloc(&s->d_rowcnt, sizeof(int) * (size_t)np * rc), "cudaMalloc scan row counts");
         CK(cudaMalloc(&s->d_pts, sizeof(Anchor) * (size_t)np * kPtsCap), "cudaMalloc scan points");
@@ -284,25 +330,61 @@ static int scan_run(cb200_ctx* c, const uint8_t* d_pics, int w, int h, int n)
         CK(cudaMalloc(&s->d_nres, sizeof(int) * (size_t)np * kPtsCap), "cudaMalloc scan result counts");
         s->ws_pics = np; s->ws_rows_cap = rc;
     }
+    // the descriptor table (batch order), then the pictures grouped by blur radius (batch order inside a group); the tiles of one
+    // radius are numbered across its pictures
+    s->h_table.resize((sizeof(PicDesc) + sizeof(int)) * (size_t)n);
+    PicDesc* desc = reinterpret_cast<PicDesc*>(s->h_table.data());
+    int* order = reinterpret_cast<int*>(desc + n);
+    int first[5] = {}, count[5] = {};
+    long long tiles[5] = {};
+    bool same[5] = {true, true, true, true, true};
+    for (int i = 0; i < n; ++i) {
+        const int R = scan_blur_radius(wh[2 * i], wh[2 * i + 1]);
+        if (!count[R]) first[R] = i;
+        else same[R] = same[R] && wh[2 * i] == wh[2 * first[R]] && wh[2 * i + 1] == wh[2 * first[R] + 1];
+        ++count[R];
+    }
+    size_t off = 0;
+    int next[5] = {};
+    for (int R = 1, at = 0; R <= 4; ++R) { next[R] = at; at += count[R]; }
+    int group0[5] = {};
+    for (int R = 1; R <= 4; ++R) group0[R] = next[R];
+    for (int i = 0; i < n; ++i) {
+        const int w = wh[2 * i], h = wh[2 * i + 1], R = scan_blur_radius(w, h);
+        PicDesc& d = desc[i];
+        d.src = 3 * off; d.blur = off; d.w = w; d.h = h;
+        d.words = (w % 4 == 0) && (reinterpret_cast<uintptr_t>(d_pics + d.src) % 4 == 0) && (reinterpret_cast<uintptr_t>(s->d_blur + d.blur) % 4 == 0);
+        d.tile0 = (int)tiles[R];
+        tiles[R] += (long long)((w + kBlurTW - 1) / kBlurTW) * ((h + kBlurTH - 1) / kBlurTH);
+        if (tiles[R] > 0x7FFFFFFFll) return fail(CB200_ERR_ARG, "more than 2^31 blur tiles in one batch");
+        order[next[R]++] = i;
+        off += (size_t)w * (size_t)h;
+    }
+    CK(cudaMemcpyAsync(s->d_table, s->h_table.data(), s->h_table.size(), cudaMemcpyHostToDevice, st), "H2D picture table");
+    const PicDesc* d_desc = reinterpret_cast<const PicDesc*>(s->d_table);
+    const int* d_order = reinterpret_cast<const int*>(d_desc + n);
     CK(cudaMemsetAsync(s->d_hist, 0, sizeof(unsigned) * 256 * (size_t)n, st), "memset histograms");
-    // cb200_set_timing: one event set per scan -- [blur + histogram, Otsu, anchors] through cb200_get_timing
+    // cb200_set_timing: one event set per scan -- [blur + histogram (all radii), Otsu, anchors] through cb200_get_timing
     auto mark = [&]() { if (c->timing && c->ev_count[c->cur] < 8) cudaEventRecord(c->ev[c->cur][c->ev_count[c->cur]++], st); };
     if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; }
     mark();
-    const dim3 bgrid((unsigned)((w + kBlurTW - 1) / kBlurTW), (unsigned)((h + kBlurTH - 1) / kBlurTH), (unsigned)n);
-    // aligned 32-bit accesses need rows that start on a word: width a multiple of four, base pointers aligned
-    const int words_ok = (w % 4 == 0) && (reinterpret_cast<uintptr_t>(d_pics) % 4 == 0) && (reinterpret_cast<uintptr_t>(s->d_blur) % 4 == 0);
-    switch (R) {
-    case 1: k_scan_blur4<1><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
-    case 2: k_scan_blur4<2><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
-    case 3: k_scan_blur4<3><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
-    default: k_scan_blur4<4><<<bgrid, kBlurThreads, 0, st>>>(d_pics, w, h, words_ok, s->d_blur, s->d_hist); break;
+    for (int R = 1; R <= 4; ++R) {
+        if (!count[R]) continue;
+        const int uniform = same[R] ? (int)(tiles[R] / count[R]) : 0;
+        const unsigned grid = (unsigned)tiles[R];
+        const int* ord = d_order + group0[R];
+        switch (R) {
+        case 1: k_scan_blur4<1><<<grid, kBlurThreads, 0, st>>>(d_pics, s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
+        case 2: k_scan_blur4<2><<<grid, kBlurThreads, 0, st>>>(d_pics, s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
+        case 3: k_scan_blur4<3><<<grid, kBlurThreads, 0, st>>>(d_pics, s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
+        default: k_scan_blur4<4><<<grid, kBlurThreads, 0, st>>>(d_pics, s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
+        }
+        count_launch();
     }
-    count_launch();
     mark();
-    k_scan_otsu<<<(n + 63) / 64, 64, 0, st>>>(s->d_hist, n, (double)npx, s->d_thr); count_launch();
+    k_scan_otsu<<<(n + 63) / 64, 64, 0, st>>>(s->d_hist, d_desc, n, s->d_thr); count_launch();
     mark();
-    k_scan_anchors<<<n, kScanThreads, 0, st>>>(s->d_blur, s->d_thr, w, h, s->ws_rows_cap, s->d_rowbuf, s->d_rowcnt, s->d_pts, s->d_res, s->d_nres,
+    k_scan_anchors<<<n, kScanThreads, 0, st>>>(s->d_blur, d_desc, s->d_thr, s->ws_rows_cap, s->d_rowbuf, s->d_rowcnt, s->d_pts, s->d_res, s->d_nres,
                                                s->d_anchors, s->d_count, s->d_cutoff, s->d_status); count_launch();
     mark();
     CK(cudaGetLastError(), "scan launch");
@@ -326,70 +408,41 @@ static int scan_results(cb200_ctx* c, int n, int32_t* anchors, int32_t* count, u
     return CB200_OK;
 }
 
-static int stage_pictures(cb200_ctx* c, const uint8_t* pics, int w, int h, int n, const uint8_t** d_out)
+// the host pictures, packed into the staging buffer with one copy each
+static int stage_pictures(cb200_ctx* c, const uint8_t* const* pics, const int32_t* wh, int n, const uint8_t** d_out)
 {
     ScanScratch* s = sstate(c);
-    const size_t bytes = (size_t)w * h * 3 * (size_t)n;
+    size_t bytes = 0;
+    for (int i = 0; i < n; ++i) bytes += (size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3;
     if (bytes > s->pics_bytes) {
         cudaFree(s->d_pics); s->d_pics = nullptr; s->pics_bytes = 0;
         CK(cudaMalloc(&s->d_pics, bytes), "cudaMalloc picture staging");
         s->pics_bytes = bytes;
     }
-    CK(cudaMemcpyAsync(s->d_pics, pics, bytes, cudaMemcpyHostToDevice, c->stream), "H2D pictures");
+    size_t off = 0;
+    for (int i = 0; i < n; ++i) {
+        const size_t b = (size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3;
+        CK(cudaMemcpyAsync(s->d_pics + off, pics[i], b, cudaMemcpyHostToDevice, c->stream), "H2D pictures");
+        off += b;
+    }
     *d_out = s->d_pics;
     return CB200_OK;
 }
 
-}  // namespace cb200
-
-using namespace cb200;
-
-extern "C" {
-
-int cb200_scan_dev(cb200_ctx* c, const uint8_t* d_pictures, int w, int h, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
+// the host pointers of a uniform batch (picture i at pics + i w h 3)
+static std::vector<const uint8_t*> uniform_pointers(const uint8_t* pics, int w, int h, int n)
 {
-    if (!c || !d_pictures || !count || n < 0 || w < 1 || h < 1) return fail(CB200_ERR_ARG, "bad arguments");
-    if (n == 0) return CB200_OK;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    int rc = scan_run(c, d_pictures, w, h, n); if (rc) return rc;
-    return scan_results(c, n, anchors, count, cutoff);
+    std::vector<const uint8_t*> p((size_t)n);
+    for (int i = 0; i < n; ++i) p[(size_t)i] = pics + (size_t)i * w * h * 3;
+    return p;
 }
 
-int cb200_scan(cb200_ctx* c, const uint8_t* pictures, int w, int h, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
+// Extractor::extract (Extractor.h:30-46) + Decoder::decode_fountain for n pictures of sizes wh packed in device memory
+static int scan_extract_decode(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* chunks_out,
+                               uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags, int32_t* extract_status)
 {
-    if (!c || !pictures || !count || n < 0 || w < 1 || h < 1) return fail(CB200_ERR_ARG, "bad arguments");
-    if (n == 0) return CB200_OK;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    const uint8_t* d = nullptr;
-    int rc = stage_pictures(c, pictures, w, h, n, &d); if (rc) return rc;
-    rc = scan_run(c, d, w, h, n); if (rc) return rc;
-    return scan_results(c, n, anchors, count, cutoff);
-}
-
-int cb200_scan_blurred(cb200_ctx* c, uint8_t* blurred_out, int32_t* thresholds_out, int w, int h, int n)
-{
-    if (!c || !c->scan || n < 0 || (size_t)w * h * (size_t)n > c->scan->blur_bytes || n > c->scan->thr_cap) return fail(CB200_ERR_ARG, "no scan of that size to read back");
-    if (n == 0) return CB200_OK;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    if (blurred_out) CK(cudaMemcpyAsync(blurred_out, c->scan->d_blur, (size_t)w * h * (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H blurred");
-    if (thresholds_out) CK(cudaMemcpyAsync(thresholds_out, c->scan->d_thr, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H thresholds");
-    CK(cudaStreamSynchronize(c->stream), "sync");
-    return CB200_OK;
-}
-
-int cb200_scan_extract_decode_fountain(cb200_ctx* c, const uint8_t* pictures, int w, int h, int n, uint32_t flags,
-                                       uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
-                                       int32_t* extract_status)
-{
-    int rc = check_camera_flags(flags); if (rc) return rc;
-    if (!c || !pictures || !chunks_out || !chunk_count || !extract_status || n < 0 || n > c->max_frames || w < 2 || h < 2)
-        return fail(CB200_ERR_ARG, "bad arguments");
-    if (n == 0) return CB200_OK;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    int rc = scan_run(c, d, wh, n); if (rc) return rc;
     const Mode& m = c->mode;
-    const uint8_t* d = nullptr;
-    rc = stage_pictures(c, pictures, w, h, n, &d); if (rc) return rc;
-    rc = scan_run(c, d, w, h, n); if (rc) return rc;
     const ScanScratch* s = c->scan;
     // Extractor::extract (Extractor.h:30-46): fewer than four anchors -> FAILURE; Corners = the anchors' centres
     // (Corners.h:13-16); NEEDS_SHARPEN unless every side of the quadrilateral is longer than the frame (is_granular_scale, :57-75).
@@ -420,12 +473,139 @@ int cb200_scan_extract_decode_fountain(cb200_ctx* c, const uint8_t* pictures, in
         sharpen.resize((size_t)n);
         for (int i = 0; i < n; ++i) sharpen[(size_t)i] = extract_status[i] == 2;
     }
-    rc = extract_decode_to_host(c, d, w, h, n, corners.data(), flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, sharpen.empty() ? nullptr : sharpen.data(),
+    rc = extract_decode_to_host(c, d, wh, n, corners.data(), flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, sharpen.empty() ? nullptr : sharpen.data(),
                                 chunks_out, chunk_count, chunk_mask, frame_flags);
     if (rc) return rc;
     for (int i = 0; i < n; ++i)
         if (extract_status[i] <= 0) { chunk_count[i] = 0; if (chunk_mask) chunk_mask[i] = 0; }
     return CB200_OK;
+}
+
+// the argument checks of the ragged entry points, all before any CUDA call
+static int check_ragged(const int32_t* wh, const void* pictures, int n)
+{
+    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
+    if (!wh) return fail(CB200_ERR_ARG, "null wh");
+    if (!pictures) return fail(CB200_ERR_ARG, "null pictures");
+    return check_picture_sizes(wh, n);
+}
+
+static int check_host_pictures(const uint8_t* const* pictures, int n)
+{
+    for (int i = 0; i < n; ++i)
+        if (!pictures[i]) return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " is a null pointer");
+    return CB200_OK;
+}
+
+}  // namespace cb200
+
+using namespace cb200;
+
+extern "C" {
+
+int cb200_scan_dev(cb200_ctx* c, const uint8_t* d_pictures, int w, int h, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
+{
+    if (!c || !d_pictures || !count || n < 0 || w < 1 || h < 1) return fail(CB200_ERR_ARG, "bad arguments");
+    if (n == 0) return CB200_OK;
+    const std::vector<int32_t> wh = uniform_sizes(w, h, n);
+    int rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    rc = scan_run(c, d_pictures, wh.data(), n); if (rc) return rc;
+    return scan_results(c, n, anchors, count, cutoff);
+}
+
+int cb200_scan(cb200_ctx* c, const uint8_t* pictures, int w, int h, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
+{
+    if (!c || !pictures || !count || n < 0 || w < 1 || h < 1) return fail(CB200_ERR_ARG, "bad arguments");
+    if (n == 0) return CB200_OK;
+    const std::vector<int32_t> wh = uniform_sizes(w, h, n);
+    int rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    const uint8_t* d = nullptr;
+    rc = stage_pictures(c, uniform_pointers(pictures, w, h, n).data(), wh.data(), n, &d); if (rc) return rc;
+    rc = scan_run(c, d, wh.data(), n); if (rc) return rc;
+    return scan_results(c, n, anchors, count, cutoff);
+}
+
+int cb200_scan_ragged_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32_t* wh, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
+{
+    int rc = check_ragged(wh, d_pictures, n); if (rc) return rc;
+    if (!c || !count) return fail(CB200_ERR_ARG, !c ? "null context" : "null count");
+    if (n == 0) return CB200_OK;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    rc = scan_run(c, d_pictures, wh, n); if (rc) return rc;
+    return scan_results(c, n, anchors, count, cutoff);
+}
+
+int cb200_scan_ragged(cb200_ctx* c, const uint8_t* const* pictures, const int32_t* wh, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
+{
+    int rc = check_ragged(wh, pictures, n); if (rc) return rc;
+    rc = check_host_pictures(pictures, n); if (rc) return rc;
+    if (!c || !count) return fail(CB200_ERR_ARG, !c ? "null context" : "null count");
+    if (n == 0) return CB200_OK;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    const uint8_t* d = nullptr;
+    rc = stage_pictures(c, pictures, wh, n, &d); if (rc) return rc;
+    rc = scan_run(c, d, wh, n); if (rc) return rc;
+    return scan_results(c, n, anchors, count, cutoff);
+}
+
+// the first npx blurred bytes and n thresholds of the last scan
+static int read_blurred(cb200_ctx* c, uint8_t* blurred_out, int32_t* thresholds_out, size_t npx, int n)
+{
+    if (!c || !c->scan || n < 0 || npx > c->scan->blur_bytes || n > c->scan->thr_cap) return fail(CB200_ERR_ARG, "no scan of that size to read back");
+    if (n == 0) return CB200_OK;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    if (blurred_out) CK(cudaMemcpyAsync(blurred_out, c->scan->d_blur, npx, cudaMemcpyDeviceToHost, c->stream), "D2H blurred");
+    if (thresholds_out) CK(cudaMemcpyAsync(thresholds_out, c->scan->d_thr, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H thresholds");
+    CK(cudaStreamSynchronize(c->stream), "sync");
+    return CB200_OK;
+}
+
+int cb200_scan_blurred(cb200_ctx* c, uint8_t* blurred_out, int32_t* thresholds_out, int w, int h, int n)
+{
+    return read_blurred(c, blurred_out, thresholds_out, (size_t)w * h * (size_t)(n < 0 ? 0 : n), n);
+}
+
+int cb200_scan_blurred_ragged(cb200_ctx* c, uint8_t* blurred_out, int32_t* thresholds_out, const int32_t* wh, int n)
+{
+    if (n < 0 || !wh) return fail(CB200_ERR_ARG, n < 0 ? "n < 0" : "null wh");
+    size_t npx = 0;
+    for (int i = 0; i < n; ++i) npx += (size_t)wh[2 * i] * (size_t)wh[2 * i + 1];
+    return read_blurred(c, blurred_out, thresholds_out, npx, n);
+}
+
+int cb200_scan_extract_decode_fountain(cb200_ctx* c, const uint8_t* pictures, int w, int h, int n, uint32_t flags,
+                                       uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
+                                       int32_t* extract_status)
+{
+    int rc = check_camera_flags(flags); if (rc) return rc;
+    if (!c || !pictures || !chunks_out || !chunk_count || !extract_status || n < 0 || n > c->max_frames || w < 2 || h < 2)
+        return fail(CB200_ERR_ARG, "bad arguments");
+    if (n == 0) return CB200_OK;
+    const std::vector<int32_t> wh = uniform_sizes(w, h, n);
+    rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    const uint8_t* d = nullptr;
+    rc = stage_pictures(c, uniform_pointers(pictures, w, h, n).data(), wh.data(), n, &d); if (rc) return rc;
+    return scan_extract_decode(c, d, wh.data(), n, flags, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
+}
+
+int cb200_scan_extract_decode_fountain_ragged(cb200_ctx* c, const uint8_t* const* pictures, const int32_t* wh, int n, uint32_t flags,
+                                              uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
+                                              int32_t* extract_status)
+{
+    int rc = check_camera_flags(flags); if (rc) return rc;
+    rc = check_ragged(wh, pictures, n); if (rc) return rc;
+    rc = check_host_pictures(pictures, n); if (rc) return rc;
+    if (!c) return fail(CB200_ERR_ARG, "null context");
+    if (!chunks_out || !chunk_count || !extract_status) return fail(CB200_ERR_ARG, "null output");
+    if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
+    if (n == 0) return CB200_OK;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    const uint8_t* d = nullptr;
+    rc = stage_pictures(c, pictures, wh, n, &d); if (rc) return rc;
+    return scan_extract_decode(c, d, wh, n, flags, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
 }
 
 }  // extern "C"
