@@ -10,6 +10,35 @@ namespace cb200 {
 // kernel launches issued by this library in this process (cb200_launch_count): every `<<<>>>` is followed by count_launch()
 void count_launch(int n = 1);
 
+// A grow-only buffer of `T` in device memory (pinned host memory with kPinned) that owns its allocation.  ensure() keeps the
+// buffer, and what it holds, when it is large enough; otherwise it frees the old memory before it allocates -- cudaFree
+// synchronises the device, so no kernel still reads the old buffer, and the peak stays one buffer.
+template <typename T, bool kPinned = false>
+class Buffer {
+public:
+    Buffer() = default;
+    Buffer(const Buffer&) = delete;
+    Buffer& operator=(const Buffer&) = delete;
+    ~Buffer() { release(); }
+    cudaError_t ensure(size_t count)
+    {
+        if (count <= cap_) return cudaSuccess;
+        release();
+        const cudaError_t e = kPinned ? cudaMallocHost((void**)&p_, count * sizeof(T)) : cudaMalloc((void**)&p_, count * sizeof(T));
+        if (e == cudaSuccess) cap_ = count; else p_ = nullptr;
+        return e;
+    }
+    T* get() const { return p_; }
+    operator T*() const { return p_; }
+    size_t capacity() const { return cap_; }   // elements
+private:
+    void release() { if (p_) { if (kPinned) cudaFreeHost(p_); else cudaFree(p_); } p_ = nullptr; cap_ = 0; }
+    T* p_ = nullptr;
+    size_t cap_ = 0;
+};
+template <typename T> using DevBuf = Buffer<T>;
+template <typename T> using PinnedBuf = Buffer<T, true>;
+
 constexpr int kMaxCells = 12544;   // 112*112
 constexpr int kCellSize = 8;       // Config::cell_size() is constexpr 8 (Config.h:106-110)
 constexpr int kSpacing = 9;        // every 8x8 mode uses cell_size+1 (GridConf.h:121-189)

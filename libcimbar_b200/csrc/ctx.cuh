@@ -16,8 +16,8 @@ struct GatherState;      // gather.cu
 struct DeskewState;      // deskew.cu
 struct ScanScratch;      // scan.cu
 void gather_destroy(GatherState* g);
-void deskew_destroy(DeskewState* d);
-void scan_destroy(ScanScratch* s);
+void deskew_destroy(DeskewState* d);     // delete: its buffers free themselves
+void scan_destroy(ScanScratch* s);       // likewise
 // cb200_decode_fountain_from_dev with an optional per-frame sharpen selection: `sharpen` = n host bytes (nonzero =
 // should_preprocess) or NULL (the batch-wide CB200_FLAG_SHARPEN decides).  The flags are checked by the caller (api.cu)
 int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
@@ -46,24 +46,25 @@ std::vector<uint8_t> sharpen_from_corners(const cb200_ctx* c, const float* corne
 }  // namespace cb200
 #define CK(call, what) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cb200::fail_cuda(e__, what); } while (0)
 
+// Every buffer of the context is a cb200::Buffer and frees itself; cb200_destroy only destroys the streams and events
 struct cb200_ctx {
     cb200::Mode mode;
     int device = 0, max_frames = 0, sm_count = 0;
     cudaStream_t own_stream = nullptr, stream = nullptr;
     // device workspaces
-    uint8_t* d_rgb = nullptr;        // host-pointer entry points only: max_frames frames
-    uint8_t* d_cellvals = nullptr;   // max_frames * num_cells
-    uint32_t* d_dirty = nullptr;     // max_frames
-    uint8_t* d_raw = nullptr;        // max_frames * cap_all
-    uint8_t* d_data = nullptr;       // max_frames * data_bytes
-    uint8_t* d_ok = nullptr;         // max_frames * nblocks
-    uint32_t* d_mask = nullptr;      // max_frames
-    uint8_t* d_flags = nullptr;      // max_frames
-    uint16_t* d_idx = nullptr;       // num_cells: slot -> cell (Interleave::interleave_indices)
-    uint16_t* d_inv = nullptr;       // num_cells: cell -> slot (Interleave::interleave_reverse)
-    uint16_t* d_idx_ident = nullptr; // identity map for CB200_FLAG_NO_INTERLEAVE (created on first use)
-    uint8_t* d_gen = nullptr;        // RS generator polynomial, ecc_bytes+1 coefficients
-    uint8_t* d_rho = nullptr;        // 4 x 64 bytes: x^(D+j) mod x^pad g, the basis of K2's remainder tables (k2_remainder_basis)
+    cb200::DevBuf<uint8_t> d_rgb;           // host-pointer entry points only: max_frames frames
+    cb200::DevBuf<uint8_t> d_cellvals;      // max_frames * num_cells
+    cb200::DevBuf<uint32_t> d_dirty;        // max_frames
+    cb200::DevBuf<uint8_t> d_raw;           // max_frames * cap_all
+    cb200::DevBuf<uint8_t> d_data;          // max_frames * data_bytes
+    cb200::DevBuf<uint8_t> d_ok;            // max_frames * nblocks
+    cb200::DevBuf<uint32_t> d_mask;         // max_frames
+    cb200::DevBuf<uint8_t> d_flags;         // max_frames
+    cb200::DevBuf<uint16_t> d_idx;          // num_cells: slot -> cell (Interleave::interleave_indices)
+    cb200::DevBuf<uint16_t> d_inv;          // num_cells: cell -> slot (Interleave::interleave_reverse)
+    cb200::DevBuf<uint16_t> d_idx_ident;    // identity map for CB200_FLAG_NO_INTERLEAVE (created on first use)
+    cb200::DevBuf<uint8_t> d_gen;           // RS generator polynomial, ecc_bytes+1 coefficients
+    cb200::DevBuf<uint8_t> d_rho;           // 4 x 64 bytes: x^(D+j) mod x^pad g, the basis of K2's remainder tables (k2_remainder_basis)
     // per-kernel timing (cb200_set_timing): events around every launch of the last pipeline call
     bool timing = false;
     static constexpr int kEvSets = 64;
@@ -73,30 +74,42 @@ struct cb200_ctx {
     int cur = 0;                     // event set of the call in progress
     cb200::FloodWorkspace flood;            // exact-walk fallback scratch
     // small scratch for the single-cell entry points
-    void* d_scratch = nullptr; size_t scratch_bytes = 0;
+    cb200::DevBuf<uint8_t> d_scratch;
     // pinned host staging for results of the host-pointer entry points
-    uint8_t* h_pinned = nullptr; size_t h_pinned_bytes = 0;
-    // per-frame sharpen selection of a mixed batch: the two frame lists and the sharpen bytes, staged in one of two pinned
-    // slots (each reused once the copy enqueued from it two calls ago has run) and copied to d_sel on the call's stream
-    static constexpr int kSelSlots = 2;
-    uint8_t* h_sel[kSelSlots] = {};
-    cudaEvent_t sel_ev[kSelSlots] = {};
-    int sel_next = 0;
-    uint8_t* d_sel = nullptr;        // max_frames x (4 + 1): plain list, sharpened list, then one sharpen byte per frame
+    cb200::PinnedBuf<uint8_t> h_pinned;
+    // host-built tables of a call (sharpen lists, picture tables, inverse maps) on their way to the device: a ring of pinned
+    // slots, each reused once the copy enqueued from it has run (stage_take / stage_send).  A call uploads at most three tables
+    // (the camera calls: picture table, deskew table, selection), so no call waits for a copy it enqueued itself
+    struct StageSlot { cb200::PinnedBuf<uint8_t> h; cudaEvent_t ev = nullptr; };
+    static constexpr int kStageSlots = 3;
+    StageSlot stage[kStageSlots];
+    int stage_next = 0;
+    cb200::DevBuf<uint8_t> d_sel;           // max_frames x (4 + 1): plain list, sharpened list, then one sharpen byte per frame
     // colour correction (the reference's thread-local CimbDecoder CCM, CimbDecoder.cpp:69-85)
     float ccm[9] = {};               // active matrix, row-major
     bool ccm_active = false;
     bool ccm_pending = false;        // the last CC_SIMPLE batch's final matrix is still on its way to h_ccm
     bool ccm_pending_flag = false;   // ... and so is whether that frame had a CCM at all (CC_FIT batches)
-    float* d_ccm = nullptr;          // per-frame matrices of a CC_SIMPLE / CC_FIT batch (the ones used): max_frames x 9
-    float* h_ccm = nullptr;          // pinned: 9 floats + 1 activity byte (at float index 9)
+    cb200::DevBuf<float> d_ccm;             // per-frame matrices of a CC_SIMPLE / CC_FIT batch (the ones used): max_frames x 9
+    cb200::PinnedBuf<float> h_ccm;          // 9 floats + 1 activity byte (at float index 9)
     // CC_FIT scratch: per-cell mean colours of the first pass, per-frame fits
-    uint32_t* d_means = nullptr;     // max_frames x num_cells
-    float* d_fit = nullptr;          // max_frames x 9
-    uint8_t* d_fit_valid = nullptr;  // max_frames
-    uint8_t* d_ccm_active = nullptr; // max_frames: the frame is decoded with d_ccm[f]
+    cb200::DevBuf<uint32_t> d_means;        // max_frames x num_cells
+    cb200::DevBuf<float> d_fit;             // max_frames x 9
+    cb200::DevBuf<uint8_t> d_fit_valid;     // max_frames
+    cb200::DevBuf<uint8_t> d_ccm_active;    // max_frames: the frame is decoded with d_ccm[f]
     cudaEvent_t ccm_ev = nullptr;    // recorded after the D2H copies of the last batch's CCM (ccm_resolve waits on it)
     cb200::GatherState* gather = nullptr;   // multi-GPU chunk-record window (gather.cu)
     cb200::DeskewState* deskew = nullptr;   // extractor scratch (deskew.cu)
     cb200::ScanScratch* scan = nullptr;     // anchor-scan scratch (scan.cu)
 };
+
+namespace cb200 {
+// cb200_set_timing: begin_timed_call starts the event set of a pipeline call, mark records its next event on the call's stream
+inline void begin_timed_call(cb200_ctx* c) { if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; } }
+inline void mark(cb200_ctx* c) { if (c->timing && c->ev_count[c->cur] < 8) cudaEventRecord(c->ev[c->cur][c->ev_count[c->cur]++], c->stream); }
+// a host-built table for this call: stage_take hands out the next pinned slot with room for `bytes` (after the copy last
+// enqueued from it has run); the caller fills *h, and stage_send enqueues the copy of its first `bytes` to d_dst on the call's
+// stream and records the slot's event.  The caller's own host inputs are free again when the call returns
+int stage_take(cb200_ctx* c, size_t bytes, int* slot, uint8_t** h);
+int stage_send(cb200_ctx* c, int slot, void* d_dst, size_t bytes, const char* what);
+}  // namespace cb200

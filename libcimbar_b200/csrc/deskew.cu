@@ -26,20 +26,12 @@
 namespace cb200 {
 
 struct DeskewState {
-    uint8_t* d_table = nullptr;    // n x 9 inverse maps (destination -> source) in double, then n PicDesc (the sources)
-    int cap = 0;
-    uint8_t* d_src = nullptr;      // staging for the host-pointer entry point
-    size_t src_bytes = 0;
-    uint8_t* d_dst = nullptr;      // deskewed frames of the host-pointer entry points
-    size_t dst_bytes = 0;
+    DevBuf<uint8_t> d_table;       // n x 9 inverse maps (destination -> source) in double, then n PicDesc (the sources)
+    DevBuf<uint8_t> d_src;         // staging for the host-pointer entry point
+    DevBuf<uint8_t> d_dst;         // deskewed frames of the host-pointer entry points
 };
 
-void deskew_destroy(DeskewState* d)
-{
-    if (!d) return;
-    cudaFree(d->d_table); cudaFree(d->d_src); cudaFree(d->d_dst);
-    delete d;
-}
+void deskew_destroy(DeskewState* d) { delete d; }
 
 // hal::LU64f (modules/core/src/matrix_decomp.cpp, LUImpl<double>) for an m x m system with one right-hand side
 static bool lu_solve(double* A, int m, double* b)
@@ -193,6 +185,23 @@ static DeskewState* dstate(cb200_ctx* c)
     return c->deskew;
 }
 
+// the host-pointer entry points: n source pictures of w x h into the staging buffer
+static int stage_sources(cb200_ctx* c, const uint8_t* src, int w, int h, int n)
+{
+    DeskewState* d = dstate(c);
+    const size_t sb = (size_t)n * w * h * 3;
+    CK(d->d_src.ensure(sb), "cudaMalloc deskew source");
+    CK(cudaMemcpyAsync(d->d_src, src, sb, cudaMemcpyHostToDevice, c->stream), "H2D camera frames");
+    return CB200_OK;
+}
+
+// room for n deskewed frames in the output buffer
+static int ensure_frames(cb200_ctx* c, int n)
+{
+    CK(dstate(c)->d_dst.ensure((size_t)n * c->mode.width * c->mode.height * 3), "cudaMalloc deskew output");
+    return CB200_OK;
+}
+
 // warpPerspective of n source pictures of sizes wh (n x (w, h), host) packed in d_src, one frame each
 static int deskew_run(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int n, const double* m9, uint8_t* d_dst)
 {
@@ -208,16 +217,13 @@ static int deskew_run(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int
     const Mode& m = c->mode;
     DeskewState* d = dstate(c);
     const size_t table_bytes = (sizeof(double) * 9 + sizeof(PicDesc)) * (size_t)n;
-    if (n > d->cap) {
-        cudaFree(d->d_table); d->d_table = nullptr; d->cap = 0;
-        CK(cudaMalloc(&d->d_table, table_bytes), "cudaMalloc transforms");
-        d->cap = n;
-    }
+    CK(d->d_table.ensure(table_bytes), "cudaMalloc transforms");
     // warpPerspective inverts the transform it is given (no WARP_INVERSE_MAP): cv::invert, DECOMP_LU; a singular matrix maps
     // everything to (0, 0) there (invert leaves zeros) -- reported here instead
-    static thread_local std::vector<uint8_t> table;
-    table.resize(table_bytes);
-    double* inv = reinterpret_cast<double*>(table.data());
+    int slot;
+    uint8_t* table;
+    int rc = stage_take(c, table_bytes, &slot, &table); if (rc) return rc;
+    double* inv = reinterpret_cast<double*>(table);
     PicDesc* desc = reinterpret_cast<PicDesc*>(inv + 9 * (size_t)n);
     size_t off = 0;
     for (int f = 0; f < n; ++f) {
@@ -225,14 +231,13 @@ static int deskew_run(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int
         desc[f] = PicDesc{off, 0, wh[2 * f], wh[2 * f + 1], 0, 0};
         off += (size_t)wh[2 * f] * (size_t)wh[2 * f + 1] * 3;
     }
-    CK(cudaMemcpyAsync(d->d_table, table.data(), table_bytes, cudaMemcpyHostToDevice, c->stream), "H2D transforms");
-    CK(cudaStreamSynchronize(c->stream), "sync (transforms staged from a host vector)");
+    rc = stage_send(c, slot, d->d_table, table_bytes, "H2D transforms"); if (rc) return rc;
     // OpenCV's block geometry (WarpPerspectiveInvoker): bh0 = min(16, H); bw0 = min(1024 / bh0, W)
     const int bh0 = m.height < 16 ? m.height : 16;
     int bw0 = 1024 / bh0; if (bw0 > m.width) bw0 = m.width;
     const int per_frame = m.height * (m.width / 4);
     const dim3 grid((unsigned)((per_frame + 255) / 256), (unsigned)(n < 32768 ? n : 32768));
-    const double* d_inv = reinterpret_cast<const double*>(d->d_table);
+    const double* d_inv = reinterpret_cast<const double*>(d->d_table.get());
     k_deskew<<<grid, 256, 0, c->stream>>>(d_src, src_bytes, d_inv, reinterpret_cast<const PicDesc*>(d_inv + 9 * (size_t)n), n, m.width, m.height, bw0, d_dst);
     count_launch();
     CK(cudaGetLastError(), "deskew launch");
@@ -286,13 +291,11 @@ int cb200_deskew(cb200_ctx* c, const uint8_t* src, int src_w, int src_h, int n, 
     if (!c || !src || !dst || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
     if (n == 0) return CB200_OK;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
-    DeskewState* d = dstate(c);
-    const size_t sb = (size_t)n * src_w * src_h * 3, db = (size_t)n * c->mode.width * c->mode.height * 3;
-    if (sb > d->src_bytes) { cudaFree(d->d_src); d->d_src = nullptr; d->src_bytes = 0; CK(cudaMalloc(&d->d_src, sb), "cudaMalloc deskew source"); d->src_bytes = sb; }
-    if (db > d->dst_bytes) { cudaFree(d->d_dst); d->d_dst = nullptr; d->dst_bytes = 0; CK(cudaMalloc(&d->d_dst, db), "cudaMalloc deskew output"); d->dst_bytes = db; }
-    CK(cudaMemcpyAsync(d->d_src, src, sb, cudaMemcpyHostToDevice, c->stream), "H2D camera frames");
-    int rc = cb200_deskew_dev(c, d->d_src, src_w, src_h, n, m9, d->d_dst); if (rc) return rc;
-    CK(cudaMemcpyAsync(dst, d->d_dst, db, cudaMemcpyDeviceToHost, c->stream), "D2H frames");
+    int rc = stage_sources(c, src, src_w, src_h, n); if (rc) return rc;
+    rc = ensure_frames(c, n); if (rc) return rc;
+    const DeskewState* d = c->deskew;
+    rc = cb200_deskew_dev(c, d->d_src, src_w, src_h, n, m9, d->d_dst); if (rc) return rc;
+    CK(cudaMemcpyAsync(dst, d->d_dst, (size_t)n * c->mode.width * c->mode.height * 3, cudaMemcpyDeviceToHost, c->stream), "D2H frames");
     CK(cudaStreamSynchronize(c->stream), "sync");
     return CB200_OK;
 }
@@ -315,7 +318,6 @@ int cb200::extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, const int3
     if (n == 0) return CB200_OK;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
-    DeskewState* d = dstate(c);
     // Deskewer::deskew (Deskewer.h:27-39) with padding 0: the anchor centres go to (anchor, anchor) ... (W - anchor, H - anchor)
     const float an = 30.0f;                                     // Config::anchor_size() (Config.h)
     const float outp[8] = {an, an, (float)m.width - an, an, an, (float)m.height - an, (float)m.width - an, (float)m.height - an};
@@ -323,11 +325,10 @@ int cb200::extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, const int3
     for (int f = 0; f < n; ++f) {
         int rc = cb200_perspective_transform(corners + (size_t)f * 8, outp, m9.data() + (size_t)f * 9); if (rc) return rc;
     }
-    const size_t db = (size_t)n * m.width * m.height * 3;
-    if (db > d->dst_bytes) { cudaFree(d->d_dst); d->d_dst = nullptr; d->dst_bytes = 0; CK(cudaMalloc(&d->d_dst, db), "cudaMalloc deskew output"); d->dst_bytes = db; }
-    int rc = deskew_run(c, d_src, wh, n, m9.data(), d->d_dst); if (rc) return rc;
+    int rc = ensure_frames(c, n); if (rc) return rc;
+    rc = deskew_run(c, d_src, wh, n, m9.data(), c->deskew->d_dst); if (rc) return rc;
     // the deskewed frames never leave the device: straight into the decode
-    return decode_fountain_to_host(c, d->d_dst, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
+    return decode_fountain_to_host(c, c->deskew->d_dst, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
 // Extractor::extract (Extractor.h:30-46): NEEDS_SHARPEN unless every side of the corner quadrilateral spans more than the frame in x
@@ -386,11 +387,8 @@ int cb200_extract_decode_fountain(cb200_ctx* c, const uint8_t* src, int src_w, i
     if (!c || !src || !corners || !chunks_out || !chunk_count || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
     if (n == 0) return CB200_OK;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
-    DeskewState* d = dstate(c);
-    const size_t sb = (size_t)n * src_w * src_h * 3;
-    if (sb > d->src_bytes) { cudaFree(d->d_src); d->d_src = nullptr; d->src_bytes = 0; CK(cudaMalloc(&d->d_src, sb), "cudaMalloc deskew source"); d->src_bytes = sb; }
-    CK(cudaMemcpyAsync(d->d_src, src, sb, cudaMemcpyHostToDevice, c->stream), "H2D camera frames");
-    return cb200_extract_decode_fountain_dev(c, d->d_src, src_w, src_h, n, corners, flags, chunks_out, chunk_count, chunk_mask, frame_flags);
+    rc = stage_sources(c, src, src_w, src_h, n); if (rc) return rc;
+    return cb200_extract_decode_fountain_dev(c, c->deskew->d_src, src_w, src_h, n, corners, flags, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
 }  // extern "C"

@@ -919,7 +919,6 @@ static void flood_build_cinfo(const Mode& m, const uint16_t* adj, std::vector<ui
 
 cudaError_t flood_workspace_create(const Mode& m, int sm_count, const uint16_t* adj_host, FloodWorkspace* ws)
 {
-    memset(ws, 0, sizeof(*ws));
     ws->sm_count = sm_count;
     // shared-memory heap entries per walking warp (must be odd): 1023 = the ten top levels; deeper levels go to the
     // per-slot spill area in L2.  Shared memory per walk decides how many walks an SM holds (at most 32 blocks).
@@ -943,19 +942,13 @@ cudaError_t flood_workspace_create(const Mode& m, int sm_count, const uint16_t* 
     cudaError_t e;
     if ((e = cudaFuncSetAttribute(k_flood_walk, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)(ws->walk_smem > ws->walk_smem_few ? ws->walk_smem : ws->walk_smem_few))) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&ws->spill, ws->spill_cap * (size_t)ws->slots * sizeof(uint32_t))) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&ws->prio, (size_t)kMaxCells * (size_t)ws->slots)) != cudaSuccess) return e;
+    if ((e = ws->spill.ensure(ws->spill_cap * (size_t)ws->slots)) != cudaSuccess) return e;
+    if ((e = ws->prio.ensure((size_t)kMaxCells * (size_t)ws->slots)) != cudaSuccess) return e;
     std::vector<uint16_t> cinfo;
     flood_build_cinfo(m, adj_host, cinfo);
-    if ((e = cudaMalloc(&ws->cinfo, cinfo.size() * sizeof(uint16_t))) != cudaSuccess) return e;
+    if ((e = ws->cinfo.ensure(cinfo.size())) != cudaSuccess) return e;
     if ((e = cudaMemcpy(ws->cinfo, cinfo.data(), cinfo.size() * sizeof(uint16_t), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
     return cudaSuccess;
-}
-
-void flood_workspace_destroy(FloodWorkspace* ws)
-{
-    cudaFree(ws->spill); cudaFree(ws->prio); cudaFree(ws->cinfo); cudaFree(ws->list); cudaFree(ws->counters); cudaFree(ws->raster); cudaFree(ws->result);
-    memset(ws, 0, sizeof(*ws));
 }
 
 // grows the per-batch buffers (cudaFree synchronises, so no kernel still reads the old ones)
@@ -963,23 +956,19 @@ static cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int
 {
     cudaError_t e;
     const size_t rw = raster_words16(m.width, m.height);
-    if (n_frames > ws.list_cap) {
-        int cap = ws.list_cap ? ws.list_cap : 256;
-        while (cap < n_frames) cap *= 2;
-        cudaFree(ws.list); cudaFree(ws.counters); ws.list = nullptr; ws.counters = nullptr; ws.list_cap = 0;
-        if ((e = cudaMalloc(&ws.list, (size_t)cap * sizeof(uint32_t))) != cudaSuccess) return e;
-        if ((e = cudaMalloc(&ws.counters, (size_t)(2 + cap) * sizeof(uint32_t))) != cudaSuccess) return e;   // 1 + one per chunk (>= 1 frame each)
-        ws.list_cap = cap;
-    }
+    size_t list_cap = ws.list.capacity() ? ws.list.capacity() : 256;
+    while (list_cap < (size_t)n_frames) list_cap *= 2;
+    if ((e = ws.list.ensure(list_cap)) != cudaSuccess) return e;
+    if ((e = ws.counters.ensure(2 + list_cap)) != cudaSuccess) return e;   // 1 + one per chunk (>= 1 frame each)
     const int want = n_frames < ws.max_entries ? n_frames : ws.max_entries;
     if (want > ws.entry_cap) {
         int cap = (want + 1023) / 1024 * 1024;          // in steps of 1024 frames (185 MB)
         if (want <= 64) cap = 64; else if (want <= 256) cap = 256;
         if (cap > ws.max_entries) cap = ws.max_entries;
-        cudaFree(ws.raster); cudaFree(ws.result); ws.raster = nullptr; ws.result = nullptr; ws.entry_cap = 0;
-        if ((e = cudaMalloc(&ws.raster, rw * (size_t)cap * sizeof(uint16_t))) != cudaSuccess) return e;
+        ws.entry_cap = 0;
+        if ((e = ws.raster.ensure(rw * (size_t)cap)) != cudaSuccess) return e;
         if ((e = cudaMemset(ws.raster, 0, rw * (size_t)cap * sizeof(uint16_t))) != cudaSuccess) return e;
-        if ((e = cudaMalloc(&ws.result, (size_t)m.num_cells * (size_t)cap * sizeof(uint32_t))) != cudaSuccess) return e;
+        if ((e = ws.result.ensure((size_t)m.num_cells * (size_t)cap)) != cudaSuccess) return e;
         ws.entry_cap = cap;
     }
     return cudaSuccess;

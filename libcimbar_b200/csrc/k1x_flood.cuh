@@ -17,25 +17,24 @@ struct CellTrace {
 };
 
 struct FloodWorkspace {
-    int sm_count;
-    int slots;                 // walking warps resident at once (one frame each)
-    int heap_smem;             // heap entries per walk kept in shared memory (odd)
-    size_t walk_smem;          // dynamic shared memory of one walking warp
-    int heap_smem_few; size_t walk_smem_few; int few_frames;   // batches of at most few_frames listed frames: the whole heap in shared memory
-    size_t spill_cap;          // heap spill entries per slot
-    int serial_above;          // heap sizes above this use the one-level-per-step pop (65536; tests lower it)
-    uint32_t* spill;           // [slots][spill_cap]
-    uint8_t* prio;             // [slots][kMaxCells] per-cell priority bytes of the walk in that slot
-    uint16_t* cinfo;           // [num_cells][16] update candidates in push order (0xFFFF = none)
-    int list_cap; uint32_t* list; uint32_t* counters;   // work list; counters[0] = listed frames, [1 + c] = chunk c's work counter
-    int max_entries;           // upper bound of entry_cap (one chunk); larger work lists are processed chunk by chunk
-    int entry_cap; uint16_t* raster; uint32_t* result;  // per listed frame of a chunk: 1-bit raster in 16x16 tiles, per-cell x | y<<11 | sym<<22
+    int sm_count = 0;
+    int slots = 0;             // walking warps resident at once (one frame each)
+    int heap_smem = 0;         // heap entries per walk kept in shared memory (odd)
+    size_t walk_smem = 0;      // dynamic shared memory of one walking warp
+    int heap_smem_few = 0; size_t walk_smem_few = 0; int few_frames = 0;   // batches of at most few_frames listed frames: the whole heap in shared memory
+    size_t spill_cap = 0;      // heap spill entries per slot
+    int serial_above = 0;      // heap sizes above this use the one-level-per-step pop (65536; tests lower it)
+    DevBuf<uint32_t> spill;    // [slots][spill_cap]
+    DevBuf<uint8_t> prio;      // [slots][kMaxCells] per-cell priority bytes of the walk in that slot
+    DevBuf<uint16_t> cinfo;    // [num_cells][16] update candidates in push order (0xFFFF = none)
+    DevBuf<uint32_t> list, counters;   // work list; counters[0] = listed frames, [1 + c] = chunk c's work counter
+    int max_entries = 0;       // upper bound of entry_cap (one chunk); larger work lists are processed chunk by chunk
+    int entry_cap = 0; DevBuf<uint16_t> raster; DevBuf<uint32_t> result;  // per listed frame of a chunk: 1-bit raster in 16x16 tiles, per-cell x | y<<11 | sym<<22
 };
 
 cudaError_t flood_init_tables(const float* adjust256, const unsigned long long* tiles_L16, uint32_t hash_mul);
 // adj_host: [num_cells][4] = AdjacentCellFinder::find for every cell (built by the caller from the cell geometry)
 cudaError_t flood_workspace_create(const Mode& m, int sm_count, const uint16_t* adj_host, FloodWorkspace* ws);
-void flood_workspace_destroy(FloodWorkspace* ws);
 // writes d_flags[f] for every frame: 0 = K1 result stands, CB200_FRAME_FALLBACK = re-decoded here,
 // CB200_FRAME_INEXACT = needed but skipped (no_fallback).  d_sharpen_of: NULL = every frame is preprocessed as `sharpen` says;
 // else one byte per frame of the batch (device memory, nonzero = sharpen) and `sharpen` is ignored

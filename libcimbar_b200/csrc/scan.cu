@@ -26,26 +26,17 @@ namespace cb200 {
 using namespace scan;
 
 struct ScanScratch {                 // per-context scratch of the scan entry points
-    uint8_t* d_pics = nullptr; size_t pics_bytes = 0;       // staging of host pictures
-    uint8_t* d_blur = nullptr; size_t blur_bytes = 0;       // blurred gray, n x h x w
-    unsigned* d_hist = nullptr; int* d_thr = nullptr; int thr_cap = 0;
-    Anchor* d_rowbuf = nullptr; int* d_rowcnt = nullptr; Anchor* d_pts = nullptr; Anchor* d_res = nullptr; int* d_nres = nullptr;
+    DevBuf<uint8_t> d_pics;                                 // staging of host pictures
+    DevBuf<uint8_t> d_blur;                                 // blurred gray, n x h x w
+    DevBuf<unsigned> d_hist; DevBuf<int> d_thr;
+    DevBuf<Anchor> d_rowbuf; DevBuf<int> d_rowcnt; DevBuf<Anchor> d_pts; DevBuf<Anchor> d_res; DevBuf<int> d_nres;
     int ws_pics = 0, ws_rows_cap = 0;
-    int4* d_anchors = nullptr; int* d_count = nullptr; unsigned* d_cutoff = nullptr; int* d_status = nullptr;
-    int4* h_anchors = nullptr; int* h_count = nullptr;      // pinned results: [n][4] anchors, then count / cutoff / status per picture
-    uint8_t* d_table = nullptr;                             // n PicDesc, then the pictures grouped by blur radius (n int)
-    std::vector<uint8_t> h_table;                           // its host image, built per call
+    DevBuf<int4> d_anchors; DevBuf<int> d_count; DevBuf<unsigned> d_cutoff; DevBuf<int> d_status;
+    PinnedBuf<int4> h_anchors; PinnedBuf<int> h_count;      // results: [n][4] anchors, then count / cutoff / status per picture
+    DevBuf<uint8_t> d_table;                                // n PicDesc, then the pictures grouped by blur radius (n int)
 };
 
-void scan_destroy(ScanScratch* s)
-{
-    if (!s) return;
-    cudaFree(s->d_pics); cudaFree(s->d_blur); cudaFree(s->d_hist); cudaFree(s->d_thr);
-    cudaFree(s->d_rowbuf); cudaFree(s->d_rowcnt); cudaFree(s->d_pts); cudaFree(s->d_res); cudaFree(s->d_nres);
-    cudaFree(s->d_anchors); cudaFree(s->d_count); cudaFree(s->d_cutoff); cudaFree(s->d_status); cudaFree(s->d_table);
-    cudaFreeHost(s->h_anchors); cudaFreeHost(s->h_count);
-    delete s;
-}
+void scan_destroy(ScanScratch* s) { delete s; }
 
 // ---------------------------------------------------------------------------------------------- gray + blur + histogram
 template <int R> struct BlurK;
@@ -298,42 +289,32 @@ static int scan_run(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int 
         const int rc = 2 * ((h + skip - 1) / skip) + 4;
         if (rc > rows_cap) rows_cap = rc;
     }
-    if (npx > s->blur_bytes) {
-        cudaFree(s->d_blur); s->d_blur = nullptr; s->blur_bytes = 0;
-        CK(cudaMalloc(&s->d_blur, npx), "cudaMalloc blurred pictures");
-        s->blur_bytes = npx;
-    }
-    if (n > s->thr_cap) {
-        cudaFree(s->d_hist); cudaFree(s->d_thr); cudaFree(s->d_anchors); cudaFree(s->d_count); cudaFree(s->d_cutoff); cudaFree(s->d_status);
-        cudaFree(s->d_table); cudaFreeHost(s->h_anchors); cudaFreeHost(s->h_count);
-        s->d_hist = nullptr; s->d_thr = nullptr; s->d_anchors = nullptr; s->d_count = nullptr; s->d_cutoff = nullptr; s->d_status = nullptr;
-        s->d_table = nullptr; s->h_anchors = nullptr; s->h_count = nullptr; s->thr_cap = 0;
-        CK(cudaMalloc(&s->d_hist, sizeof(unsigned) * 256 * (size_t)n), "cudaMalloc histograms");
-        CK(cudaMalloc(&s->d_thr, sizeof(int) * (size_t)n), "cudaMalloc thresholds");
-        CK(cudaMalloc(&s->d_anchors, sizeof(int4) * 4 * (size_t)n), "cudaMalloc anchors");
-        CK(cudaMalloc(&s->d_count, sizeof(int) * (size_t)n), "cudaMalloc counts");
-        CK(cudaMalloc(&s->d_cutoff, sizeof(unsigned) * (size_t)n), "cudaMalloc cutoffs");
-        CK(cudaMalloc(&s->d_status, sizeof(int) * (size_t)n), "cudaMalloc status");
-        CK(cudaMalloc(&s->d_table, (sizeof(PicDesc) + sizeof(int)) * (size_t)n), "cudaMalloc picture table");
-        CK(cudaMallocHost(&s->h_anchors, sizeof(int4) * 4 * (size_t)n), "cudaMallocHost anchors");
-        CK(cudaMallocHost(&s->h_count, sizeof(int) * 3 * (size_t)n), "cudaMallocHost counts");
-        s->thr_cap = n;
-    }
-    if (n > s->ws_pics || rows_cap > s->ws_rows_cap) {
-        cudaFree(s->d_rowbuf); cudaFree(s->d_rowcnt); cudaFree(s->d_pts); cudaFree(s->d_res); cudaFree(s->d_nres);
-        const int np = n > s->ws_pics ? n : s->ws_pics, rc = rows_cap > s->ws_rows_cap ? rows_cap : s->ws_rows_cap;
-        s->d_rowbuf = nullptr; s->d_rowcnt = nullptr; s->d_pts = nullptr; s->d_res = nullptr; s->d_nres = nullptr; s->ws_pics = 0; s->ws_rows_cap = 0;
-        CK(cudaMalloc(&s->d_rowbuf, sizeof(Anchor) * (size_t)np * rc * kRowCap), "cudaMalloc scan rows");
-        CK(cudaMalloc(&s->d_rowcnt, sizeof(int) * (size_t)np * rc), "cudaMalloc scan row counts");
-        CK(cudaMalloc(&s->d_pts, sizeof(Anchor) * (size_t)np * kPtsCap), "cudaMalloc scan points");
-        CK(cudaMalloc(&s->d_res, sizeof(Anchor) * (size_t)np * kPtsCap * kResCap), "cudaMalloc scan results");
-        CK(cudaMalloc(&s->d_nres, sizeof(int) * (size_t)np * kPtsCap), "cudaMalloc scan result counts");
-        s->ws_pics = np; s->ws_rows_cap = rc;
-    }
+    CK(s->d_blur.ensure(npx), "cudaMalloc blurred pictures");
+    const size_t table_bytes = (sizeof(PicDesc) + sizeof(int)) * (size_t)n;
+    CK(s->d_hist.ensure(256 * (size_t)n), "cudaMalloc histograms");
+    CK(s->d_thr.ensure((size_t)n), "cudaMalloc thresholds");
+    CK(s->d_anchors.ensure(4 * (size_t)n), "cudaMalloc anchors");
+    CK(s->d_count.ensure((size_t)n), "cudaMalloc counts");
+    CK(s->d_cutoff.ensure((size_t)n), "cudaMalloc cutoffs");
+    CK(s->d_status.ensure((size_t)n), "cudaMalloc status");
+    CK(s->d_table.ensure(table_bytes), "cudaMalloc picture table");
+    CK(s->h_anchors.ensure(4 * (size_t)n), "cudaMallocHost anchors");
+    CK(s->h_count.ensure(3 * (size_t)n), "cudaMallocHost counts");
+    // the per-picture scan lists: k_scan_anchors strides them by the largest row count seen so far
+    if (n > s->ws_pics) s->ws_pics = n;
+    if (rows_cap > s->ws_rows_cap) s->ws_rows_cap = rows_cap;
+    const size_t np = (size_t)s->ws_pics, rows = (size_t)s->ws_rows_cap;
+    CK(s->d_rowbuf.ensure(np * rows * kRowCap), "cudaMalloc scan rows");
+    CK(s->d_rowcnt.ensure(np * rows), "cudaMalloc scan row counts");
+    CK(s->d_pts.ensure(np * kPtsCap), "cudaMalloc scan points");
+    CK(s->d_res.ensure(np * kPtsCap * kResCap), "cudaMalloc scan results");
+    CK(s->d_nres.ensure(np * kPtsCap), "cudaMalloc scan result counts");
     // the descriptor table (batch order), then the pictures grouped by blur radius (batch order inside a group); the tiles of one
     // radius are numbered across its pictures
-    s->h_table.resize((sizeof(PicDesc) + sizeof(int)) * (size_t)n);
-    PicDesc* desc = reinterpret_cast<PicDesc*>(s->h_table.data());
+    int slot;
+    uint8_t* h_table;
+    int err = stage_take(c, table_bytes, &slot, &h_table); if (err) return err;
+    PicDesc* desc = reinterpret_cast<PicDesc*>(h_table);
     int* order = reinterpret_cast<int*>(desc + n);
     int first[5] = {}, count[5] = {};
     long long tiles[5] = {};
@@ -360,14 +341,13 @@ static int scan_run(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int 
         order[next[R]++] = i;
         off += (size_t)w * (size_t)h;
     }
-    CK(cudaMemcpyAsync(s->d_table, s->h_table.data(), s->h_table.size(), cudaMemcpyHostToDevice, st), "H2D picture table");
-    const PicDesc* d_desc = reinterpret_cast<const PicDesc*>(s->d_table);
+    err = stage_send(c, slot, s->d_table, table_bytes, "H2D picture table"); if (err) return err;
+    const PicDesc* d_desc = reinterpret_cast<const PicDesc*>(s->d_table.get());
     const int* d_order = reinterpret_cast<const int*>(d_desc + n);
     CK(cudaMemsetAsync(s->d_hist, 0, sizeof(unsigned) * 256 * (size_t)n, st), "memset histograms");
     // cb200_set_timing: one event set per scan -- [blur + histogram (all radii), Otsu, anchors] through cb200_get_timing
-    auto mark = [&]() { if (c->timing && c->ev_count[c->cur] < 8) cudaEventRecord(c->ev[c->cur][c->ev_count[c->cur]++], st); };
-    if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; }
-    mark();
+    begin_timed_call(c);
+    mark(c);
     for (int R = 1; R <= 4; ++R) {
         if (!count[R]) continue;
         const int uniform = same[R] ? (int)(tiles[R] / count[R]) : 0;
@@ -381,12 +361,12 @@ static int scan_run(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int 
         }
         count_launch();
     }
-    mark();
+    mark(c);
     k_scan_otsu<<<(n + 63) / 64, 64, 0, st>>>(s->d_hist, d_desc, n, s->d_thr); count_launch();
-    mark();
+    mark(c);
     k_scan_anchors<<<n, kScanThreads, 0, st>>>(s->d_blur, d_desc, s->d_thr, s->ws_rows_cap, s->d_rowbuf, s->d_rowcnt, s->d_pts, s->d_res, s->d_nres,
                                                s->d_anchors, s->d_count, s->d_cutoff, s->d_status); count_launch();
-    mark();
+    mark(c);
     CK(cudaGetLastError(), "scan launch");
     CK(cudaMemcpyAsync(s->h_anchors, s->d_anchors, sizeof(int4) * 4 * (size_t)n, cudaMemcpyDeviceToHost, st), "D2H anchors");
     CK(cudaMemcpyAsync(s->h_count, s->d_count, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st), "D2H counts");
@@ -414,11 +394,7 @@ static int stage_pictures(cb200_ctx* c, const uint8_t* const* pics, const int32_
     ScanScratch* s = sstate(c);
     size_t bytes = 0;
     for (int i = 0; i < n; ++i) bytes += (size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3;
-    if (bytes > s->pics_bytes) {
-        cudaFree(s->d_pics); s->d_pics = nullptr; s->pics_bytes = 0;
-        CK(cudaMalloc(&s->d_pics, bytes), "cudaMalloc picture staging");
-        s->pics_bytes = bytes;
-    }
+    CK(s->d_pics.ensure(bytes), "cudaMalloc picture staging");
     size_t off = 0;
     for (int i = 0; i < n; ++i) {
         const size_t b = (size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3;
@@ -553,7 +529,8 @@ int cb200_scan_ragged(cb200_ctx* c, const uint8_t* const* pictures, const int32_
 // the first npx blurred bytes and n thresholds of the last scan
 static int read_blurred(cb200_ctx* c, uint8_t* blurred_out, int32_t* thresholds_out, size_t npx, int n)
 {
-    if (!c || !c->scan || n < 0 || npx > c->scan->blur_bytes || n > c->scan->thr_cap) return fail(CB200_ERR_ARG, "no scan of that size to read back");
+    if (!c || !c->scan || n < 0 || npx > c->scan->d_blur.capacity() || (size_t)n > c->scan->d_thr.capacity())
+        return fail(CB200_ERR_ARG, "no scan of that size to read back");
     if (n == 0) return CB200_OK;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     if (blurred_out) CK(cudaMemcpyAsync(blurred_out, c->scan->d_blur, npx, cudaMemcpyDeviceToHost, c->stream), "D2H blurred");
