@@ -241,6 +241,37 @@ int cb200_scan_extract_decode_fountain_ragged(cb200_ctx* ctx, const uint8_t* con
                                               uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
                                               int32_t* extract_status);
 
+/* ---- enqueue-only camera decode -----------------------------------------------------------------------------------------
+
+   The camera path on the device from end to end: scan, Extractor::extract (one thread per picture), deskew and decode are only
+   enqueued on the context's stream, and the call returns without waiting for the device -- so a caller can queue a batch behind
+   other work, overlap the copy of the next batch with this one's decode, and hand the records to cb200_gather_push.
+     d_pictures: a ragged batch packed in device memory as for cb200_scan_ragged_dev; wh: n x 2 int32 in HOST memory, read before
+                 the call returns.
+     d_chunks, d_chunk_mask, d_frame_flags (may be NULL): the fixed-slot layout of cb200_decode_chunks_dev -- data_bytes per picture,
+                 slot q valid iff bit q of the mask is set.  A picture with status <= 0 gets mask 0.
+     d_extract_status: n int32 (4-byte aligned) with cb200_scan_extract_decode_fountain's statuses: -1, 0, 1 or 2.
+   Every flag behaves as on cb200_scan_extract_decode_fountain_ragged: CB200_FLAG_SHARPEN_IF_NEEDED sharpens exactly the
+   NEEDS_SHARPEN pictures, the CCM of CB200_FLAG_CC_FIT (and CC_SIMPLE's last matrix) carries in batch order, and from one call to
+   the next: a call enqueued while an earlier one that may change the CCM is still running takes that CCM from the device.
+   CB200_ERR_ARG before any CUDA call, with the checks and messages of the ragged entry points, for null outputs, and for
+   CC_SIMPLE with CC_FIT.
+   The call never waits for the device, with two exceptions:
+     1. a call that has to grow one of the context's buffers waits for the device (cudaFree synchronises); after one call with the
+        same or a larger batch (and the same pictures' sizes or smaller) nothing grows;
+     2. each call uploads one pinned table (its picture table) from a ring of three slots: a fourth call in flight waits until the
+        upload of the first has run.
+   The outputs, and the context's scratch buffers, belong to the stream: read them after cb200_sync or an event on that stream. */
+int cb200_scan_extract_decode_chunks_ragged_dev(cb200_ctx* ctx, const uint8_t* d_pictures, const int32_t* wh, int n, uint32_t flags,
+                                                uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+/* the same for n pictures of one size w x h */
+int cb200_scan_extract_decode_chunks_dev(cb200_ctx* ctx, const uint8_t* d_pictures, int w, int h, int n, uint32_t flags, uint8_t* d_chunks,
+                                         uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+/* diagnostic: the forward transforms (getPerspectiveTransform(corners, output points), n x 9 doubles, row-major) of the first n
+   pictures of the last camera call of this context; a picture with status <= 0 has the transform of the output points onto
+   themselves.  Synchronises the context's stream. */
+int cb200_camera_transforms(cb200_ctx* ctx, double* m9_out, int n);
+
 /* per-cell record of the exact flood walk: what CimbReader::read() hands back, step by step
    (src/lib/cimb_translator/CimbReader.cpp:139-162, PositionData.h:4-9) */
 typedef struct cb200_cell_trace {

@@ -34,7 +34,8 @@ EXPORTS = [
     "cb200_gather_status", "cb200_comm_unique_id", "cb200_comm_init", "cb200_gather_chunks", "cb200_gather_chunks_wait",
     "cb200_decode_chunks_sharpen_dev", "cb200_decode_fountain_sharpen",
     "cb200_scan_ragged", "cb200_scan_ragged_dev", "cb200_scan_blurred_ragged", "cb200_extract_decode_fountain_ragged_dev",
-    "cb200_scan_extract_decode_fountain_ragged",
+    "cb200_scan_extract_decode_fountain_ragged", "cb200_scan_extract_decode_chunks_ragged_dev", "cb200_scan_extract_decode_chunks_dev",
+    "cb200_camera_transforms",
 ]
 
 
@@ -116,6 +117,9 @@ def load_library():
     lib.cb200_scan_blurred_ragged.argtypes = [vp, vp, vp, vp, C.c_int]
     lib.cb200_extract_decode_fountain_ragged_dev.argtypes = [vp, vp, vp, C.c_int, vp, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_fountain_ragged.argtypes = [vp, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp]
+    lib.cb200_scan_extract_decode_chunks_ragged_dev.argtypes = [vp, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
+    lib.cb200_scan_extract_decode_chunks_dev.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_uint32, vp, vp, vp, vp]
+    lib.cb200_camera_transforms.argtypes = [vp, vp, C.c_int]
     lib.cb200_decode_cells_means.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, vp, vp]
     lib.cb200_fit_ccm.argtypes = [vp, u8p, u8p, C.c_uint32, C.c_uint32, C.c_void_p]
     lib.cb200_palette_color.argtypes = [C.c_int, C.c_uint, C.c_int, u8p]
@@ -441,6 +445,20 @@ class Context:
         else:
             sel = _selection(sharpen, n)
             _check(self.lib.cb200_decode_chunks_sharpen_dev(self._h, d_rgb, n, flags, sel.ctypes.data, d_chunks, d_mask, d_flags))
+
+    def scan_extract_decode_chunks_dev(self, d_pictures, wh, d_chunks, d_mask, d_status, d_flags=None, flags=0):
+        """scan_extract_decode_fountain_ragged, enqueue-only: a ragged batch packed in device memory (d_pictures), its sizes wh
+        (n x (w, h), host) -> fixed-slot chunks, masks, extract statuses (int32) and frame flags in device memory, on the context's
+        stream; returns without waiting for the device"""
+        wh = np.ascontiguousarray(wh, dtype=np.int32).reshape(-1, 2)
+        _check(self.lib.cb200_scan_extract_decode_chunks_ragged_dev(self._h, d_pictures, wh.ctypes.data, wh.shape[0], flags, d_chunks, d_mask,
+                                                                    d_flags, d_status))
+
+    def camera_transforms(self, n):
+        """the forward perspective transforms of the first n pictures of the last camera call: (n, 3, 3) float64 (synchronises)"""
+        out = np.zeros((n, 3, 3), dtype=np.float64)
+        _check(self.lib.cb200_camera_transforms(self._h, out.ctypes.data, n))
+        return out
 
     def encode_cells_dev(self, d_payload, n, d_cellvals):
         _check(self.lib.cb200_encode_cells_dev(self._h, d_payload, n, d_cellvals))

@@ -289,6 +289,7 @@ int idx_for(cb200_ctx* c, uint32_t flags, const uint16_t** out)
 int ccm_buffers(cb200_ctx* c)
 {
     CK(c->d_ccm.ensure(9 * (size_t)c->max_frames), "cudaMalloc ccm");
+    CK(c->d_carry.ensure(12), "cudaMalloc ccm carry");
     CK(c->h_ccm.ensure(12), "cudaMallocHost ccm");
     if (!c->ccm_ev) CK(cudaEventCreateWithFlags(&c->ccm_ev, cudaEventDisableTiming), "cudaEventCreate ccm");
     CK(c->d_fit.ensure(9 * (size_t)c->max_frames), "cudaMalloc fit");
@@ -297,11 +298,15 @@ int ccm_buffers(cb200_ctx* c)
 }
 
 // the decoder keeps the CCM of the batch's last frame (CimbDecoder.cpp:82-85): its matrix in d_ccm -- and with d_active (CC_FIT)
-// whether that frame had one at all -- goes to h_ccm behind the batch, for ccm_resolve
+// whether that frame had one at all -- goes to d_carry behind the batch (for the next batch enqueued before this one is done) and
+// from there to h_ccm (for ccm_resolve)
 int ccm_keep_last(cb200_ctx* c, int n, const uint8_t* d_active)
 {
-    CK(cudaMemcpyAsync(c->h_ccm, c->d_ccm + 9 * (size_t)(n - 1), sizeof(float) * 9, cudaMemcpyDeviceToHost, c->stream), "D2H ccm");
-    if (d_active) CK(cudaMemcpyAsync(c->h_ccm + 9, d_active + (n - 1), 1, cudaMemcpyDeviceToHost, c->stream), "D2H ccm flag");
+    uint8_t* d_flag = reinterpret_cast<uint8_t*>(c->d_carry + 9);
+    CK(cudaMemcpyAsync(c->d_carry, c->d_ccm + 9 * (size_t)(n - 1), sizeof(float) * 9, cudaMemcpyDeviceToDevice, c->stream), "copy ccm");
+    if (d_active) CK(cudaMemcpyAsync(d_flag, d_active + (n - 1), 1, cudaMemcpyDeviceToDevice, c->stream), "copy ccm flag");
+    else CK(cudaMemsetAsync(d_flag, 1, 1, c->stream), "set ccm flag");
+    CK(cudaMemcpyAsync(c->h_ccm, c->d_carry, sizeof(float) * 10, cudaMemcpyDeviceToHost, c->stream), "D2H ccm");
     CK(cudaEventRecord(c->ccm_ev, c->stream), "record ccm");
     c->ccm_pending = true; c->ccm_pending_flag = d_active != nullptr;
     if (!d_active) c->ccm_active = true;
@@ -316,24 +321,67 @@ int ccm_simple(cb200_ctx* c, const uint8_t* d_rgb, int n)
     return ccm_keep_last(c, n, nullptr);
 }
 
-// a mixed sharpen selection on the device: the batch indices of the plain frames (d_list[0], nl[0] of them) and of the
-// sharpened ones (d_list[1]), both in batch order, and one 0 / 1 byte per frame (d_sharp), uploaded through the context's
-// pinned slots (stage_take)
+// the frame lists of a sharpen selection (cb200_ctx::d_sel): an order-preserving compaction of the n selection bytes in one CTA
+// (every thread counts a contiguous segment, a block-wide scan of the counts gives each segment's first slot in both lists), the
+// bytes rewritten as 0 / 1, and per list {count, K1 bands, first entry} in sched -- the band count is run_cells' rule for a grid
+// of ctas[k] CTAs
+__global__ void __launch_bounds__(1024)
+k_select(uint8_t* __restrict__ sel, int n, int ctas0, int ctas1, int max_bands, int* __restrict__ sched)
+{
+    __shared__ int sums[1024];
+    uint32_t* list = reinterpret_cast<uint32_t*>(sel);
+    uint8_t* sharp = sel + (size_t)n * 4;
+    const int t = threadIdx.x;
+    const int seg = (n + 1023) / 1024, f0 = t * seg, f1 = min(f0 + seg, n);
+    int mine = 0;
+    for (int f = f0; f < f1; ++f) mine += sharp[f] != 0;
+    sums[t] = mine;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {                  // inclusive scan of the sharpened counts
+        const int v = t >= o ? sums[t - o] : 0;
+        __syncthreads();
+        sums[t] += v;
+        __syncthreads();
+    }
+    const int n1 = sums[1023], n0 = n - n1;
+    int at1 = sums[t] - mine, at0 = min(f0, n) - at1;     // sharpened / plain frames before this segment
+    for (int f = f0; f < f1; ++f) {
+        const bool k = sharp[f] != 0;
+        if (k) list[n0 + at1++] = (uint32_t)f; else list[at0++] = (uint32_t)f;
+        sharp[f] = k ? 1 : 0;
+    }
+    if (t < 2) {
+        const int nk = t ? n1 : n0, ctas = t ? ctas1 : ctas0;
+        int bands = 1;
+        if (nk > 0 && nk < ctas) { bands = (ctas + nk - 1) / nk; if (bands > max_bands) bands = max_bands; if (bands < 1) bands = 1; }
+        sched[3 * t] = nk; sched[3 * t + 1] = bands; sched[3 * t + 2] = t ? n0 : 0;
+    }
+}
+
+// K1's persistent grid for one kind of frame (0 = plain, 1 = sharpened)
+int k1_grid(const cb200_ctx* c, int k) { return c->sm_count * k1_ctas_per_sm(k == 1); }
+
+// the frame lists of a selection whose n bytes (nonzero = sharpen) are in c->d_sel + 4 n, built there by k_select
+int build_selection(cb200_ctx* c, int n)
+{
+    CK(c->d_sched.ensure(6), "cudaMalloc selection schedule");
+    k_select<<<1, 1024, 0, c->stream>>>(c->d_sel, n, k1_grid(c, 0), k1_grid(c, 1), c->mode.cells_y / 4, c->d_sched); count_launch();
+    CK(cudaGetLastError(), "selection launch");
+    return CB200_OK;
+}
+
+// a mixed sharpen selection from the host: its n bytes go up through the context's pinned slots (stage_take), k_select builds the
+// batch indices of the plain frames (d_list[0], nl[0] of them) and of the sharpened ones (d_list[1]), both in batch order, and
+// one 0 / 1 byte per frame (d_sharp)
 int upload_selection(cb200_ctx* c, const uint8_t* sel, int n, const int nl[2], const uint32_t* d_list[2], const uint8_t** d_sharp)
 {
     CK(c->d_sel.ensure((size_t)c->max_frames * 5), "cudaMalloc selection");
     int slot;
     uint8_t* h;
-    int rc = stage_take(c, (size_t)n * 5, &slot, &h); if (rc) return rc;
-    uint32_t* h_list = reinterpret_cast<uint32_t*>(h);
-    uint8_t* h_sharp = h + (size_t)n * 4;
-    int at[2] = {0, nl[0]};
-    for (int f = 0; f < n; ++f) {
-        const int k = sel[f] != 0;
-        h_list[at[k]++] = (uint32_t)f;
-        h_sharp[f] = (uint8_t)k;
-    }
-    rc = stage_send(c, slot, c->d_sel, (size_t)n * 5, "H2D selection"); if (rc) return rc;
+    int rc = stage_take(c, (size_t)n, &slot, &h); if (rc) return rc;
+    memcpy(h, sel, (size_t)n);
+    rc = stage_send(c, slot, c->d_sel + (size_t)n * 4, (size_t)n, "H2D selection"); if (rc) return rc;
+    rc = build_selection(c, n); if (rc) return rc;
     d_list[0] = reinterpret_cast<const uint32_t*>(c->d_sel.get());
     d_list[1] = d_list[0] + nl[0];
     *d_sharp = c->d_sel + (size_t)n * 4;
@@ -344,8 +392,10 @@ int upload_selection(cb200_ctx* c, const uint8_t* sel, int n, const int nl[2], c
 // d_means != nullptr: first pass of a CC_FIT batch -- no colour decisions, the cells' mean colours go to d_means.
 // sel: NULL = every frame is preprocessed as CB200_FLAG_SHARPEN says; else n host bytes, nonzero = sharpen that frame (flags
 // must not carry CB200_FLAG_SHARPEN then).  A selection of one kind only takes the list-less path of that kind.
+// d_sel_bytes (instead of sel): the selection is n bytes at c->d_sel + 4 n on the device; the lists are built there and K1 takes
+// their lengths from the device (both kinds are launched, one may be empty)
 int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sel, CellTrace* d_trace = nullptr,
-              uint32_t* d_means = nullptr)
+              uint32_t* d_means = nullptr, const uint8_t* d_sel_bytes = nullptr)
 {
     const Mode& m = c->mode;
     cudaStream_t st = c->stream;
@@ -366,7 +416,14 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const u
     int nl[2] = {sharpen ? 0 : n, sharpen ? n : 0};
     const uint32_t* d_list[2] = {nullptr, nullptr};
     const uint8_t* d_sharp = nullptr;
-    if (sel) {
+    const int* d_sched = nullptr;
+    if (d_sel_bytes) {
+        int rc = build_selection(c, n); if (rc) return rc;
+        d_list[0] = d_list[1] = reinterpret_cast<const uint32_t*>(c->d_sel.get());
+        d_sharp = d_sel_bytes;
+        d_sched = c->d_sched;
+        nl[0] = nl[1] = 1;                     // launched whatever the device counts are
+    } else if (sel) {
         nl[1] = 0;
         for (int f = 0; f < n; ++f) nl[1] += sel[f] != 0;
         nl[0] = n - nl[1];
@@ -380,12 +437,14 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const u
         const int nk = nl[k];
         if (nk == 0) continue;
         // bands: whole frames when there are enough of them to fill the machine, else split frames into bands of cell rows
-        int ctas = c->sm_count * k1_ctas_per_sm(k == 1);
+        // (k_select applies the same rule on the device)
+        int ctas = k1_grid(c, k);
         int bands = 1;
         if (nk < ctas) { bands = (ctas + nk - 1) / nk; if (bands > m.cells_y / 4) bands = m.cells_y / 4; if (bands < 1) bands = 1; }
         int units = nk * bands;
-        int grid = units < ctas ? units : ctas;
-        CK(k1_launch(m, d_rgb, d_list[k], nk, bands, grid, k == 1, c->d_cellvals, c->d_dirty, cc, st), "k1 launch");
+        int grid = d_sched || units > ctas ? ctas : units;
+        CK(k1_launch(m, d_rgb, d_list[k], nk, bands, grid, k == 1, c->d_cellvals, c->d_dirty, cc, st, d_sched ? d_sched + 3 * k : nullptr),
+           "k1 launch");
     }
     mark(c);                                   // ev1: after K1
     // frames K1 flagged (or all of them when exact_only) are re-done by the exact walk on the same preprocessing (sharpen or not)
@@ -607,9 +666,12 @@ int cb200_rs_correct_dev(cb200_ctx* c, const uint8_t* d_raw, int n, uint8_t* d_d
 }  // extern "C"
 
 namespace {
-// cb200_decode_chunks_dev with an optional per-frame selection (run_cells)
+// cb200_decode_chunks_dev with an optional per-frame selection (run_cells: sharpen on the host, or d_sel_bytes on the device).
+// enqueue_only: a CCM still on its way from an earlier batch (ccm_keep_last) is not waited for but read
+// from c->d_carry on the device -- through k_ccm_carry, so a batch without a fit then takes the fitted-CCM route with no fits
+// (mean colours, carry, colour decisions), which decides every colour as K1 would with that matrix or without one
 int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
-                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
+                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes = nullptr, bool enqueue_only = false)
 {
     int rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
@@ -619,10 +681,16 @@ int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
     if ((flags & CB200_FLAG_CC_FIT) && (flags & CB200_FLAG_CC_SIMPLE)) return fail(CB200_ERR_ARG, "CC_SIMPLE and CC_FIT are exclusive");
     // init_ccm is only reached from Decoder::do_decode (not the legacy coupled layout) and needs a header from the RS stream
     const bool fit = (flags & CB200_FLAG_CC_FIT) && !m.legacy && m.ecc_bytes > 0 && m.color_bits > 0;
+    bool carried = false;                      // the CCM going into frame 0 is only known on the device
+    if (enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->ccm_pending) {
+        const cudaError_t q = cudaEventQuery(c->ccm_ev);
+        if (q == cudaErrorNotReady) carried = true;
+        else if (q != cudaSuccess) return fail_cuda(q, "query ccm");
+    }
     const uint16_t* idx;
     rc = idx_for(c, flags, &idx); if (rc) return rc;
-    if (!fit) {
-        rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen); if (rc) return rc;
+    if (!fit && !carried) {
+        rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen, nullptr, nullptr, d_sel_bytes); if (rc) return rc;
         mark(c);                               // ev3: (no separate pack kernel on this path: the RS kernel gathers from the cell bytes)
         CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
     } else {
@@ -631,17 +699,31 @@ int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
         rc = ccm_buffers(c); if (rc) return rc;
         CK(c->d_means.ensure((size_t)c->max_frames * m.num_cells), "cudaMalloc means");
         CK(c->d_ccm_active.ensure((size_t)c->max_frames), "cudaMalloc ccm flags");
-        CcmArg initial;
-        rc = ccm_arg(c, initial); if (rc) return rc;        // the decoder's CCM going into frame 0
-        rc = run_cells(c, d_rgb, n, flags & ~(CB200_FLAG_CC_FIT | CB200_FLAG_CC_SIMPLE), sharpen, nullptr, c->d_means); if (rc) return rc;
+        CcmArg initial;                        // the decoder's CCM going into frame 0
+        if (carried) {
+            memset(&initial, 0, sizeof(initial));
+            initial.per_frame = c->d_carry;
+            initial.per_frame_active = reinterpret_cast<const uint8_t*>(c->d_carry + 9);
+        } else {
+            rc = ccm_arg(c, initial); if (rc) return rc;
+        }
+        rc = run_cells(c, d_rgb, n, flags & ~(CB200_FLAG_CC_FIT | CB200_FLAG_CC_SIMPLE), sharpen, nullptr, c->d_means, d_sel_bytes); if (rc) return rc;
         mark(c);                               // ev3
-        CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream, 0, m.nblocks_sym), "rs launch (symbols)");
-        CK(ccm_fit_launch(m, d_rgb, d_chunks, c->d_ok, idx, n, c->d_fit, c->d_fit_valid, c->stream), "ccm fit");
+        if (fit) {
+            CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream, 0, m.nblocks_sym), "rs launch (symbols)");
+            CK(ccm_fit_launch(m, d_rgb, d_chunks, c->d_ok, idx, n, c->d_fit, c->d_fit_valid, c->stream), "ccm fit");
+        } else {
+            CK(cudaMemsetAsync(c->d_fit_valid, 0, (size_t)n, c->stream), "memset fit flags");
+        }
         CK(ccm_carry_launch(n, c->d_fit, c->d_fit_valid, initial, c->d_ccm, c->d_ccm_active, c->stream), "ccm carry");
         CK(ccm_apply_launch(m, c->d_means, n, c->d_ccm, c->d_ccm_active, c->d_cellvals, c->stream), "ccm apply");
-        CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream, m.nblocks_sym, m.nblocks - m.nblocks_sym),
-           "rs launch (colours)");
-        rc = ccm_keep_last(c, n, c->d_ccm_active); if (rc) return rc;
+        if (fit) {
+            CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream, m.nblocks_sym, m.nblocks - m.nblocks_sym),
+               "rs launch (colours)");
+            rc = ccm_keep_last(c, n, c->d_ccm_active); if (rc) return rc;
+        } else {
+            CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
+        }
     }
     mark(c);                                   // ev4: after RS
     CK(k2_mask_launch(m, c->d_ok, n, d_chunk_mask, c->stream), "mask launch");
@@ -722,14 +804,27 @@ int cb200::decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, ui
     if (n == 0) return CB200_OK;
     if (!d_rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
-    const Mode& m = c->mode;
     rc = decode_chunks(c, d_rgb, n, flags, sharpen, c->d_data, c->d_mask, nullptr); if (rc) return rc;
+    return fetch_fountain(c, n, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags, nullptr);
+}
+
+int cb200::decode_chunks_enqueue(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* d_sharp, uint8_t* d_chunks,
+                                 uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
+{
+    return decode_chunks(c, d_rgb, n, flags, nullptr, d_chunks, d_chunk_mask, d_frame_flags, d_sharp, true);
+}
+
+int cb200::fetch_fountain(cb200_ctx* c, int n, const int32_t* d_status, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
+                          uint8_t* frame_flags, int32_t* extract_status)
+{
+    const Mode& m = c->mode;
     CK(c->h_pinned.ensure((size_t)n * m.data_bytes + (size_t)n * sizeof(uint32_t)), "cudaMallocHost");
     uint32_t* h_mask = reinterpret_cast<uint32_t*>(c->h_pinned.get());
     uint8_t* h_data = c->h_pinned + (size_t)n * sizeof(uint32_t);
     CK(cudaMemcpyAsync(h_data, c->d_data, (size_t)n * m.data_bytes, cudaMemcpyDeviceToHost, c->stream), "D2H chunks");
     CK(cudaMemcpyAsync(h_mask, c->d_mask, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream), "D2H mask");
     if (frame_flags) CK(cudaMemcpyAsync(frame_flags, c->d_flags, (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H flags");
+    if (d_status) CK(cudaMemcpyAsync(extract_status, d_status, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H status");
     CK(cudaStreamSynchronize(c->stream), "sync");
     // escrow_buffer_writer order: good chunks appended densely (src/lib/encoder/escrow_buffer_writer.h:44-60)
     for (int f = 0; f < n; ++f) {

@@ -335,11 +335,15 @@ k_ccm_fit(const Mode m, const uint8_t* __restrict__ rgb, const uint8_t* __restri
 }
 
 // the decoder's CCM is whatever the last successful fit left (thread-local state, CimbDecoder.cpp:69-85): frame f uses its own
-// fit if it has one, else the matrix of frame f-1 (frame 0: the context's)
+// fit if it has one, else the matrix of frame f-1 (frame 0: the context's).  The context's matrix is initial.m / initial.active,
+// or, with initial.per_frame set, 9 floats and an activity byte in device memory (an earlier batch still in flight left it there)
 __global__ void __launch_bounds__(1024)
 k_ccm_carry(int n_frames, const float* __restrict__ fit, const uint8_t* __restrict__ valid, const CcmArg initial,
             float* __restrict__ used, uint8_t* __restrict__ used_active)
 {
+    float im[9];
+    for (int i = 0; i < 9; ++i) im[i] = initial.per_frame ? initial.per_frame[i] : initial.m[i];
+    const bool iactive = initial.per_frame ? initial.per_frame_active[0] != 0 : initial.active != 0;
     // "index of the last frame <= f with a fit" is a running maximum: every thread scans a contiguous segment, the segment
     // results are combined by a block-wide inclusive max scan, then every thread replays its segment with the right start
     __shared__ int seg_last[1024];
@@ -358,8 +362,8 @@ k_ccm_carry(int n_frames, const float* __restrict__ fit, const uint8_t* __restri
     int cur = t > 0 ? seg_last[t - 1] : -1;
     for (int f = f0; f < f1; ++f) {
         if (valid[f]) cur = f;
-        for (int i = 0; i < 9; ++i) used[(size_t)f * 9 + i] = cur >= 0 ? fit[(size_t)cur * 9 + i] : initial.m[i];
-        used_active[f] = (cur >= 0 || initial.active) ? 1 : 0;
+        for (int i = 0; i < 9; ++i) used[(size_t)f * 9 + i] = cur >= 0 ? fit[(size_t)cur * 9 + i] : im[i];
+        used_active[f] = (cur >= 0 || iactive) ? 1 : 0;
     }
 }
 

@@ -43,6 +43,19 @@ int extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh
                            const uint8_t* sharpen, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
 // CB200_FLAG_SHARPEN_IF_NEEDED on given corners: sharpen[i] = 1 iff picture i's corners fail Corners::is_granular_scale (deskew.cu)
 std::vector<uint8_t> sharpen_from_corners(const cb200_ctx* c, const float* corners, int n);
+// room for n deskewed frames in the context's frame buffer, *frames = its base (deskew.cu)
+int deskew_frames(cb200_ctx* c, int n, uint8_t** frames);
+// k_deskew over n pictures described by d_desc (src, w, h; src_bytes in all) with the inverse maps d_minv (n x 9) into d_dst (deskew.cu)
+int deskew_launch(cb200_ctx* c, const uint8_t* d_src, size_t src_bytes, const double* d_minv, const PicDesc* d_desc, int n, uint8_t* d_dst);
+// the enqueue-only decode of n extracted frames (api.cu): cb200_decode_chunks_dev, but the sharpen selection, if any, is n bytes in
+// device memory (d_sharp, at c->d_sel + 4 n: k_select builds the frame lists there; NULL = as the flags say) and a CCM that an earlier call still in flight may
+// change is taken from the device (c->d_carry) instead of waiting for it
+int decode_chunks_enqueue(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* d_sharp, uint8_t* d_chunks,
+                          uint32_t* d_chunk_mask, uint8_t* d_frame_flags);
+// the results of the last decode (c->d_data, c->d_mask, c->d_flags, and d_status when given) to host memory with one synchronise,
+// the good chunks of each frame packed densely (api.cu)
+int fetch_fountain(cb200_ctx* c, int n, const int32_t* d_status, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
+                   uint8_t* frame_flags, int32_t* extract_status);
 }  // namespace cb200
 #define CK(call, what) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cb200::fail_cuda(e__, what); } while (0)
 
@@ -77,21 +90,27 @@ struct cb200_ctx {
     cb200::DevBuf<uint8_t> d_scratch;
     // pinned host staging for results of the host-pointer entry points
     cb200::PinnedBuf<uint8_t> h_pinned;
-    // host-built tables of a call (sharpen lists, picture tables, inverse maps) on their way to the device: a ring of pinned
-    // slots, each reused once the copy enqueued from it has run (stage_take / stage_send).  A call uploads at most three tables
-    // (the camera calls: picture table, deskew table, selection), so no call waits for a copy it enqueued itself
+    // host-built tables of a call (sharpen selections, picture tables, inverse maps) on their way to the device: a ring of pinned
+    // slots, each reused once the copy enqueued from it has run (stage_take / stage_send).  A call uploads at most two tables
+    // (cb200_deskew_dev: its table; a frame call with a mixed selection: the selection), so no call waits for a copy it enqueued
+    // itself; a camera call uploads one (its picture table), so three camera calls can be in flight before the fourth waits
     struct StageSlot { cb200::PinnedBuf<uint8_t> h; cudaEvent_t ev = nullptr; };
     static constexpr int kStageSlots = 3;
     StageSlot stage[kStageSlots];
     int stage_next = 0;
-    cb200::DevBuf<uint8_t> d_sel;           // max_frames x (4 + 1): plain list, sharpened list, then one sharpen byte per frame
+    // a sharpen selection of n frames: the plain frames' batch indices, then the sharpened ones' (both in batch order, 4 n bytes),
+    // then one sharpen byte per frame (n bytes); built from the bytes by k_select (api.cu), which also leaves the launch schedule
+    // of each list in d_sched: {count, K1 bands, first entry} for the plain and for the sharpened frames
+    cb200::DevBuf<uint8_t> d_sel;           // max_frames x (4 + 1)
+    cb200::DevBuf<int> d_sched;             // 6
     // colour correction (the reference's thread-local CimbDecoder CCM, CimbDecoder.cpp:69-85)
     float ccm[9] = {};               // active matrix, row-major
     bool ccm_active = false;
     bool ccm_pending = false;        // the last CC_SIMPLE batch's final matrix is still on its way to h_ccm
     bool ccm_pending_flag = false;   // ... and so is whether that frame had a CCM at all (CC_FIT batches)
     cb200::DevBuf<float> d_ccm;             // per-frame matrices of a CC_SIMPLE / CC_FIT batch (the ones used): max_frames x 9
-    cb200::PinnedBuf<float> h_ccm;          // 9 floats + 1 activity byte (at float index 9)
+    cb200::DevBuf<float> d_carry;           // the last such batch's final matrix + activity byte (at float index 9), stream-ordered
+    cb200::PinnedBuf<float> h_ccm;          // d_carry's copy on the host
     // CC_FIT scratch: per-cell mean colours of the first pass, per-frame fits
     cb200::DevBuf<uint32_t> d_means;        // max_frames x num_cells
     cb200::DevBuf<float> d_fit;             // max_frames x 9

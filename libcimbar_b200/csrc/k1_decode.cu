@@ -238,11 +238,14 @@ __device__ __forceinline__ uint32_t thread_symbol_search(const K1Smem& s, uint32
 // A lane-level numpy model of exactly this schedule is checked against the oracle in tests/test_k1_sharpen_model.py.
 // frame_list: NULL = the n_frames frames of the batch; else the batch indices of the n_frames frames this launch decodes (one
 // kind of a batch that mixes sharpened and plain frames).  Every output stays batch-indexed.
-template <int NC, bool G1024, int CM, bool SH>
+// DC: the list's length is only known on the device (a selection built there, k_select in api.cu): n_frames, bands and the
+// list's first entry come from sched[0..2] instead, and the launch is the persistent grid whatever the count.
+template <int NC, bool G1024, int CM, bool SH, bool DC>
 __global__ void __launch_bounds__(kK1Threads, SH ? 3 : kK1CtasPerSm)
 k1_decode_kernel(const Mode mm, const uint8_t* __restrict__ rgb, const uint32_t* __restrict__ frame_list, int n_frames, int bands,
-                 uint8_t* __restrict__ cellvals, uint32_t* __restrict__ dirty_flags, const CcmArg cc)
+                 uint8_t* __restrict__ cellvals, uint32_t* __restrict__ dirty_flags, const CcmArg cc, const int* __restrict__ sched)
 {
+    if constexpr (DC) { n_frames = __ldg(sched); bands = __ldg(sched + 1); frame_list += __ldg(sched + 2); }
     // G1024: the 1024x1024 / 112x112-cell geometry of modes B, 4C and 8C as compile-time constants (GridConf.h:121-141);
     // the other modes (Bm 1024x720, Bu 736x637) take every dimension from the Mode struct
     struct Geo {
@@ -653,25 +656,28 @@ cudaError_t k1_init_tables(const float* adjust256, const unsigned long long* til
     e = cudaMemcpyToSymbol(c_tiles_L, tiles_L16, sizeof(unsigned long long) * 16);
     if (e != cudaSuccess) return e;
     const int smem_max = (int)(sizeof(K1Smem) + kSharpenExtraSmem);
-#define CB200_K1_ATTR2(NC, G, C, S) \
-    if ((e = cudaFuncSetAttribute(k1_decode_kernel<NC, G, C, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)) != cudaSuccess) return e;
+#define CB200_K1_ATTR3(NC, G, C, S, D) \
+    if ((e = cudaFuncSetAttribute(k1_decode_kernel<NC, G, C, S, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)) != cudaSuccess) return e;
+#define CB200_K1_ATTR2(NC, G, C, S) CB200_K1_ATTR3(NC, G, C, S, false) CB200_K1_ATTR3(NC, G, C, S, true)
 #define CB200_K1_ATTR(NC, G, C) CB200_K1_ATTR2(NC, G, C, false) CB200_K1_ATTR2(NC, G, C, true)
     CB200_K1_ATTR(4, true, 0) CB200_K1_ATTR(4, false, 0) CB200_K1_ATTR(8, true, 0) CB200_K1_ATTR(8, false, 0)
     CB200_K1_ATTR(4, true, 1) CB200_K1_ATTR(4, false, 1) CB200_K1_ATTR(8, true, 1) CB200_K1_ATTR(8, false, 1)
     CB200_K1_ATTR(4, true, 2) CB200_K1_ATTR(4, false, 2) CB200_K1_ATTR(8, true, 2) CB200_K1_ATTR(8, false, 2)
 #undef CB200_K1_ATTR
 #undef CB200_K1_ATTR2
+#undef CB200_K1_ATTR3
     return cudaSuccess;
 }
 
 cudaError_t k1_launch(const Mode& m, const uint8_t* d_rgb, const uint32_t* d_list, int n_frames, int bands, int grid, bool sharpen,
-                      uint8_t* d_cellvals, uint32_t* d_dirty, const CcmArg& cc, cudaStream_t stream)
+                      uint8_t* d_cellvals, uint32_t* d_dirty, const CcmArg& cc, cudaStream_t stream, const int* d_sched)
 {
     const size_t smem = k1_smem_bytes(sharpen);
     const bool g1024 = m.width == 1024 && m.height == 1024 && m.cells_x == 112 && m.cells_y == 112 && m.corner == 6 &&
                        m.cell_offset == 8 && m.symbol_bits == 4;
     const int cm = cc.means ? 2 : (cc.active ? 1 : 0);
-#define CB200_K1_GO(NC, G, C, S) k1_decode_kernel<NC, G, C, S><<<grid, kK1Threads, smem, stream>>>(m, d_rgb, d_list, n_frames, bands, d_cellvals, d_dirty, cc)
+#define CB200_K1_GO2(NC, G, C, S, D) k1_decode_kernel<NC, G, C, S, D><<<grid, kK1Threads, smem, stream>>>(m, d_rgb, d_list, n_frames, bands, d_cellvals, d_dirty, cc, d_sched)
+#define CB200_K1_GO(NC, G, C, S) do { if (d_sched) CB200_K1_GO2(NC, G, C, S, true); else CB200_K1_GO2(NC, G, C, S, false); } while (0)
 #define CB200_K1_SH(NC, G, C) do { if (sharpen) CB200_K1_GO(NC, G, C, true); else CB200_K1_GO(NC, G, C, false); } while (0)
 #define CB200_K1_CM(NC, G) do { if (cm == 2) CB200_K1_SH(NC, G, 2); else if (cm == 1) CB200_K1_SH(NC, G, 1); else CB200_K1_SH(NC, G, 0); } while (0)
     if (m.color_bits == 3) { if (g1024) CB200_K1_CM(8, true); else CB200_K1_CM(8, false); }
@@ -679,6 +685,7 @@ cudaError_t k1_launch(const Mode& m, const uint8_t* d_rgb, const uint32_t* d_lis
 #undef CB200_K1_CM
 #undef CB200_K1_SH
 #undef CB200_K1_GO
+#undef CB200_K1_GO2
     count_launch();
     return cudaGetLastError();
 }
