@@ -267,6 +267,38 @@ int cb200_scan_extract_decode_chunks_ragged_dev(cb200_ctx* ctx, const uint8_t* d
 /* the same for n pictures of one size w x h */
 int cb200_scan_extract_decode_chunks_dev(cb200_ctx* ctx, const uint8_t* d_pictures, int w, int h, int n, uint32_t flags, uint8_t* d_chunks,
                                          uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+/* ---- JPEG files in: the CLI's input, decoded on the device ---------------------------------------------------------------
+
+   Replaces: cv::imread(file) + cv::cvtColor(BGR2RGB) (src/exe/cimbar/cimbar.cpp:132-133) for a batch of JPEG files in host memory:
+   the output is byte for byte the RGB8 picture cv2.imread + cvtColor(BGR2RGB) returns (libjpeg-turbo's JDCT_ISLOW IDCT, fancy
+   upsampling and fixed-point YCbCr -> RGB, and the EXIF orientation as imread applies it).
+     files, sizes: n pointers to whole JPEG files and their sizes in bytes, in HOST memory; read before the call returns.
+   Supported: baseline, extended-sequential Huffman and progressive (SOF0 / SOF1 / SOF2), 8-bit samples, one component (grey: the
+   three channels are equal) or three YCbCr components (JFIF, no APP marker, or Adobe APP14 with transform 1), luma sampling 1x1,
+   2x1, 1x2 or 2x2 with chroma 1x1 (4:4:4, 4:2:2, 4:4:0, 4:2:0), any restart interval, EXIF orientation 1-8, and output sizes the
+   camera path accepts (short side 60 .. 4499).  Anything else -- arithmetic coding, 12-bit, lossless, hierarchical, CMYK, Adobe
+   transform 0 / 2, other sampling layouts such as 4:1:1, a progressive script that leaves the first coefficients incomplete,
+   truncated headers, bytes that are not a JPEG file -- fails the whole call with CB200_ERR_ARG before any CUDA call, and
+   cb200_last_error names the picture and the reason.  Entropy-coded data that turn out corrupt or truncated are found on the
+   device: that picture gets status -2 (and is written black); the other pictures are unaffected. */
+
+/* the output size of one file (after the EXIF orientation), or CB200_ERR_ARG with the refusal reason.  Host only: no context,
+   no CUDA call */
+int cb200_jpeg_info(const uint8_t* file, uint64_t size, int32_t* w, int32_t* h);
+/* enqueue-only decode of n files into d_rgb_out, the packed ragged RGB8 batch of the _ragged_dev entry points: picture i at byte
+   3 * sum_{j<i} w_j h_j (sizes as cb200_jpeg_info).  d_status (may be NULL): n int32 in device memory, 0 = decoded, -2 = corrupt
+   data.  Waits for the device only as cb200_scan_extract_decode_chunks_ragged_dev does (a buffer that grows, the upload ring). */
+int cb200_jpeg_decode_dev(cb200_ctx* ctx, const uint8_t* const* files, const uint64_t* sizes, int n, uint8_t* d_rgb_out, int32_t* d_status);
+/* cb200_jpeg_decode_dev into a context buffer, then exactly cb200_scan_extract_decode_chunks_ragged_dev on the decoded pictures:
+   the same flags, CCM carry across calls, fixed-slot records, statuses and wait rules, plus extract status -2 and mask 0 for a
+   picture with corrupt data (which is otherwise treated as the black picture it decodes to: a status-0 picture).  Checks as
+   cb200_scan_extract_decode_chunks_ragged_dev, all before any CUDA call.  The files and their descriptors go up from a ring of
+   three pinned buffers of the JPEG calls (each grows to the largest batch's compressed size), the scan's picture table from the
+   context's ring: one slot of each per call, so, as on the RGB call, a fourth call in flight waits until the first one's
+   uploads have run. */
+int cb200_jpeg_scan_extract_decode_chunks_dev(cb200_ctx* ctx, const uint8_t* const* files, const uint64_t* sizes, int n, uint32_t flags,
+                                              uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+
 /* diagnostic: the forward transforms (getPerspectiveTransform(corners, output points), n x 9 doubles, row-major) of the first n
    pictures of the last camera call of this context; a picture with status <= 0 has the transform of the output points onto
    themselves.  Synchronises the context's stream. */

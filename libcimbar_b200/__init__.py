@@ -35,7 +35,7 @@ EXPORTS = [
     "cb200_decode_chunks_sharpen_dev", "cb200_decode_fountain_sharpen",
     "cb200_scan_ragged", "cb200_scan_ragged_dev", "cb200_scan_blurred_ragged", "cb200_extract_decode_fountain_ragged_dev",
     "cb200_scan_extract_decode_fountain_ragged", "cb200_scan_extract_decode_chunks_ragged_dev", "cb200_scan_extract_decode_chunks_dev",
-    "cb200_camera_transforms",
+    "cb200_camera_transforms", "cb200_jpeg_info", "cb200_jpeg_decode_dev", "cb200_jpeg_scan_extract_decode_chunks_dev",
 ]
 
 
@@ -120,6 +120,9 @@ def load_library():
     lib.cb200_scan_extract_decode_chunks_ragged_dev.argtypes = [vp, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_dev.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_camera_transforms.argtypes = [vp, vp, C.c_int]
+    lib.cb200_jpeg_info.argtypes = [vp, C.c_uint64, vp, vp]
+    lib.cb200_jpeg_decode_dev.argtypes = [vp, vp, vp, C.c_int, vp, vp]
+    lib.cb200_jpeg_scan_extract_decode_chunks_dev.argtypes = [vp, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_decode_cells_means.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, vp, vp]
     lib.cb200_fit_ccm.argtypes = [vp, u8p, u8p, C.c_uint32, C.c_uint32, C.c_void_p]
     lib.cb200_palette_color.argtypes = [C.c_int, C.c_uint, C.c_int, u8p]
@@ -195,6 +198,22 @@ def _ragged(pictures):
     ptrs = (C.c_void_p * max(len(pics), 1))(*[p.ctypes.data for p in pics])
     wh = np.array([(p.shape[1], p.shape[0]) for p in pics], dtype=np.int32).reshape(-1, 2)
     return pics, ptrs, wh
+
+
+def jpeg_info(data):
+    """(w, h) of a JPEG file (bytes) after its EXIF orientation, as cb200_jpeg_info: host only, no GPU.  Raises Cb200Error with
+    the reason for a file the device decoder refuses"""
+    w, h = C.c_int32(), C.c_int32()
+    _check(load_library().cb200_jpeg_info(data, len(data), C.byref(w), C.byref(h)))
+    return w.value, h.value
+
+
+def _files(files):
+    """a list of bytes -> (kept objects, n host pointers, n sizes)"""
+    files = [bytes(f) for f in files]
+    ptrs = (C.c_char_p * max(len(files), 1))(*files)
+    sizes = (C.c_uint64 * max(len(files), 1))(*[len(f) for f in files])
+    return files, ptrs, sizes
 
 
 def _selection(sharpen, n):
@@ -453,6 +472,20 @@ class Context:
         wh = np.ascontiguousarray(wh, dtype=np.int32).reshape(-1, 2)
         _check(self.lib.cb200_scan_extract_decode_chunks_ragged_dev(self._h, d_pictures, wh.ctypes.data, wh.shape[0], flags, d_chunks, d_mask,
                                                                     d_flags, d_status))
+
+    jpeg_info = staticmethod(jpeg_info)
+
+    def jpeg_decode_dev(self, files, d_rgb_out, d_status=None):
+        """cb200_jpeg_decode_dev, enqueue-only: a list of JPEG files (bytes) -> the packed ragged RGB8 batch at d_rgb_out (picture i at
+        3 * sum_{j<i} w_j h_j, sizes as jpeg_info) and n int32 statuses (0, or -2 for corrupt data) at d_status, on the context's stream"""
+        keep, ptrs, sizes = _files(files)
+        _check(self.lib.cb200_jpeg_decode_dev(self._h, ptrs, sizes, len(keep), d_rgb_out, d_status))
+
+    def jpeg_scan_extract_decode_chunks_dev(self, files, d_chunks, d_mask, d_status, d_flags=None, flags=0):
+        """scan_extract_decode_chunks_dev on a list of JPEG files (bytes) decoded on the device; enqueue-only.  A picture with corrupt
+        data gets status -2 and mask 0"""
+        keep, ptrs, sizes = _files(files)
+        _check(self.lib.cb200_jpeg_scan_extract_decode_chunks_dev(self._h, ptrs, sizes, len(keep), flags, d_chunks, d_mask, d_flags, d_status))
 
     def camera_transforms(self, n):
         """the forward perspective transforms of the first n pictures of the last camera call: (n, 3, 3) float64 (synchronises)"""

@@ -15,9 +15,11 @@ int fail_cuda(cudaError_t e, const char* what);
 struct GatherState;      // gather.cu
 struct DeskewState;      // deskew.cu
 struct ScanScratch;      // scan.cu
+struct JpegState;        // jpeg.cu
 void gather_destroy(GatherState* g);
 void deskew_destroy(DeskewState* d);     // delete: its buffers free themselves
 void scan_destroy(ScanScratch* s);       // likewise
+void jpeg_destroy(JpegState* j);         // likewise
 // cb200_decode_fountain_from_dev with an optional per-frame sharpen selection: `sharpen` = n host bytes (nonzero =
 // should_preprocess) or NULL (the batch-wide CB200_FLAG_SHARPEN decides).  The flags are checked by the caller (api.cu)
 int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
@@ -52,6 +54,14 @@ int deskew_launch(cb200_ctx* c, const uint8_t* d_src, size_t src_bytes, const do
 // change is taken from the device (c->d_carry) instead of waiting for it
 int decode_chunks_enqueue(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* d_sharp, uint8_t* d_chunks,
                           uint32_t* d_chunk_mask, uint8_t* d_frame_flags);
+// the argument checks of cb200_scan_extract_decode_chunks_ragged_dev beyond its pictures, all before any CUDA call (scan.cu): the
+// flags (both sharpen flags, CC_SIMPLE with CC_FIT), then the context, the outputs and n against max_frames
+int check_camera_dev_flags(uint32_t flags);
+int check_camera_dev_outputs(cb200_ctx* c, int n, const uint8_t* d_chunks, const uint32_t* d_chunk_mask, const int32_t* d_extract_status);
+// the enqueue-only camera path (scan, k_extract, deskew, decode, failed pictures' masks cleared) for n pictures of sizes wh packed
+// in device memory, arguments checked (scan.cu)
+int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
+                   uint8_t* d_frame_flags, int32_t* d_status);
 // the results of the last decode (c->d_data, c->d_mask, c->d_flags, and d_status when given) to host memory with one synchronise,
 // the good chunks of each frame packed densely (api.cu)
 int fetch_fountain(cb200_ctx* c, int n, const int32_t* d_status, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
@@ -120,6 +130,7 @@ struct cb200_ctx {
     cb200::GatherState* gather = nullptr;   // multi-GPU chunk-record window (gather.cu)
     cb200::DeskewState* deskew = nullptr;   // extractor scratch (deskew.cu)
     cb200::ScanScratch* scan = nullptr;     // anchor-scan scratch (scan.cu)
+    cb200::JpegState* jpeg = nullptr;       // JPEG decode scratch (jpeg.cu)
 };
 
 namespace cb200 {

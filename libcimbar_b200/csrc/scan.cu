@@ -453,8 +453,8 @@ __global__ void k_mask_failed(const int32_t* __restrict__ status, int n, uint32_
 // Extractor::extract + Decoder::decode_fountain for n pictures of sizes wh packed in device memory, enqueued on the context's stream
 // without a host round trip: scan, k_extract, deskew with the scan's picture table, decode (with CB200_FLAG_SHARPEN_IF_NEEDED the
 // frame lists are built on the device), masks of failed pictures cleared.  The arguments are checked by the caller
-static int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
-                          uint8_t* d_frame_flags, int32_t* d_status)
+int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
+                   uint8_t* d_frame_flags, int32_t* d_status)
 {
     const Mode& m = c->mode;
     size_t src_bytes = 0;
@@ -508,6 +508,30 @@ static int check_host_pictures(const uint8_t* const* pictures, int n)
     for (int i = 0; i < n; ++i)
         if (!pictures[i]) return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " is a null pointer");
     return CB200_OK;
+}
+
+int check_camera_dev_flags(uint32_t flags)
+{
+    int rc = check_camera_flags(flags); if (rc) return rc;
+    if ((flags & CB200_FLAG_CC_FIT) && (flags & CB200_FLAG_CC_SIMPLE)) return fail(CB200_ERR_ARG, "CC_SIMPLE and CC_FIT are exclusive");
+    return CB200_OK;
+}
+
+int check_camera_dev_outputs(cb200_ctx* c, int n, const uint8_t* d_chunks, const uint32_t* d_chunk_mask, const int32_t* d_extract_status)
+{
+    if (!c) return fail(CB200_ERR_ARG, "null context");
+    if (!d_chunks || !d_chunk_mask || !d_extract_status) return fail(CB200_ERR_ARG, "null output");
+    if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
+    return CB200_OK;
+}
+
+// the argument checks of the enqueue-only camera entry point, all before any CUDA call
+static int check_camera_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32_t* wh, int n, uint32_t flags, const uint8_t* d_chunks,
+                            const uint32_t* d_chunk_mask, const int32_t* d_extract_status)
+{
+    int rc = check_camera_dev_flags(flags); if (rc) return rc;
+    rc = check_ragged(wh, d_pictures, n); if (rc) return rc;
+    return check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status);
 }
 
 }  // namespace cb200
@@ -620,19 +644,6 @@ int cb200_scan_extract_decode_fountain_ragged(cb200_ctx* c, const uint8_t* const
     const uint8_t* d = nullptr;
     rc = stage_pictures(c, pictures, wh, n, &d); if (rc) return rc;
     return scan_extract_decode(c, d, wh, n, flags, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
-}
-
-// the argument checks of the enqueue-only camera entry point, all before any CUDA call
-static int check_camera_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32_t* wh, int n, uint32_t flags, const uint8_t* d_chunks,
-                            const uint32_t* d_chunk_mask, const int32_t* d_extract_status)
-{
-    int rc = check_camera_flags(flags); if (rc) return rc;
-    if ((flags & CB200_FLAG_CC_FIT) && (flags & CB200_FLAG_CC_SIMPLE)) return fail(CB200_ERR_ARG, "CC_SIMPLE and CC_FIT are exclusive");
-    rc = check_ragged(wh, d_pictures, n); if (rc) return rc;
-    if (!c) return fail(CB200_ERR_ARG, "null context");
-    if (!d_chunks || !d_chunk_mask || !d_extract_status) return fail(CB200_ERR_ARG, "null output");
-    if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
-    return CB200_OK;
 }
 
 int cb200_scan_extract_decode_chunks_ragged_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32_t* wh, int n, uint32_t flags,
