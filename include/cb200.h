@@ -299,6 +299,40 @@ int cb200_jpeg_decode_dev(cb200_ctx* ctx, const uint8_t* const* files, const uin
 int cb200_jpeg_scan_extract_decode_chunks_dev(cb200_ctx* ctx, const uint8_t* const* files, const uint64_t* sizes, int n, uint32_t flags,
                                               uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
 
+/* ---- PNG files decoded on the device (cv::imread + cvtColor(BGR2RGB) of the reference CLI, for PNG) -------------------------
+   The same three entry points for PNG files, byte for byte cv2.cvtColor(cv2.imread(file, IMREAD_COLOR), COLOR_BGR2RGB) as
+   OpenCV 4.13 with libpng 1.6 gives it: grey replicated, palettes looked up (an index past PLTE is black), alpha dropped (tRNS and
+   bKGD change nothing), 16 bit truncated to its high byte, gAMA / sRGB / iCCP ignored, the eXIf orientation applied as for JPEG.
+   Supported: non-interlaced files of colour type 0 (1, 2, 4, 8, 16 bit), 2 (8, 16), 3 (1, 2, 4, 8), 4 (8, 16) and 6 (8, 16), any
+   number and size of consecutive IDAT chunks, every deflate block type, ancillary chunks (skipped), and output sizes the camera path
+   accepts (short side 60 .. 4499).  Refused with CB200_ERR_ARG before any CUDA call, cb200_last_error naming the picture and the
+   reason: a bad signature; a missing, repeated, misplaced or invalid IHDR or a bad CRC in it; colour type 3 without PLTE, a repeated
+   PLTE, a PLTE after IDAT, of a bad size or with a bad CRC; an unknown critical chunk or an invalid chunk type; Adam7 interlace;
+   APNG (acTL, fcTL, fdAT); IDAT chunks that are not consecutive; more than one eXIf chunk; an invalid zlib header or a preset
+   dictionary; a truncated file (no IEND); a width or height above 1 000 000 (libpng's limit) or more than 2^30 pixels (OpenCV's).
+   Found on the device, status -2 and a black picture, the other pictures unaffected: an IDAT CRC mismatch, an invalid block type,
+   stored LEN / NLEN that do not match, bad code lengths, a code not in the table, a distance before the output or past zlib's
+   window as libpng calls zlib (the window of the zlib header, row by row), a stream that ends before its Adler-32 or gives fewer
+   bytes than the rows, a filter type above 4, and an Adler-32 mismatch where libpng fails the file for it (the check value read in
+   the same 8 KB read of the last IDAT data as the last row).  Corrupt data after the last row that libpng reads in a later zlib
+   call (where it only warns) are also reported -2.
+
+   Extracted frames (the encoder's output, the CLI's --no-deskew input) need no entry point of their own: when every file has the
+   mode's frame size, the packed ragged batch of cb200_png_decode_dev is the frame batch of cb200_decode_chunks_dev, so
+   cb200_png_decode_dev followed by cb200_decode_chunks_dev on the same stream is the CLI's --no-deskew loop on the device. */
+
+/* the output size of one file (after the eXIf orientation), or CB200_ERR_ARG with the refusal reason.  Host only */
+int cb200_png_info(const uint8_t* file, uint64_t size, int32_t* w, int32_t* h);
+/* enqueue-only decode of n files into d_rgb_out, the packed ragged RGB8 batch: picture i at byte 3 * sum_{j<i} w_j h_j (sizes as
+   cb200_png_info).  d_status (may be NULL): n int32 in device memory, 0 = decoded, -2 = corrupt data.  Waits for the device only
+   as cb200_jpeg_decode_dev does (a buffer that grows, the upload ring of the PNG calls). */
+int cb200_png_decode_dev(cb200_ctx* ctx, const uint8_t* const* files, const uint64_t* sizes, int n, uint8_t* d_rgb_out, int32_t* d_status);
+/* cb200_png_decode_dev into a context buffer, then exactly cb200_scan_extract_decode_chunks_ragged_dev on the decoded pictures, with
+   extract status -2 and mask 0 for a picture with corrupt data; arguments, flags and wait rules as
+   cb200_jpeg_scan_extract_decode_chunks_dev (the PNG calls have a ring of three pinned upload buffers of their own). */
+int cb200_png_scan_extract_decode_chunks_dev(cb200_ctx* ctx, const uint8_t* const* files, const uint64_t* sizes, int n, uint32_t flags,
+                                             uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+
 /* diagnostic: the forward transforms (getPerspectiveTransform(corners, output points), n x 9 doubles, row-major) of the first n
    pictures of the last camera call of this context; a picture with status <= 0 has the transform of the output points onto
    themselves.  Synchronises the context's stream. */

@@ -36,6 +36,7 @@ EXPORTS = [
     "cb200_scan_ragged", "cb200_scan_ragged_dev", "cb200_scan_blurred_ragged", "cb200_extract_decode_fountain_ragged_dev",
     "cb200_scan_extract_decode_fountain_ragged", "cb200_scan_extract_decode_chunks_ragged_dev", "cb200_scan_extract_decode_chunks_dev",
     "cb200_camera_transforms", "cb200_jpeg_info", "cb200_jpeg_decode_dev", "cb200_jpeg_scan_extract_decode_chunks_dev",
+    "cb200_png_info", "cb200_png_decode_dev", "cb200_png_scan_extract_decode_chunks_dev",
 ]
 
 
@@ -123,6 +124,9 @@ def load_library():
     lib.cb200_jpeg_info.argtypes = [vp, C.c_uint64, vp, vp]
     lib.cb200_jpeg_decode_dev.argtypes = [vp, vp, vp, C.c_int, vp, vp]
     lib.cb200_jpeg_scan_extract_decode_chunks_dev.argtypes = [vp, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
+    lib.cb200_png_info.argtypes = [vp, C.c_uint64, vp, vp]
+    lib.cb200_png_decode_dev.argtypes = [vp, vp, vp, C.c_int, vp, vp]
+    lib.cb200_png_scan_extract_decode_chunks_dev.argtypes = [vp, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_decode_cells_means.argtypes = [vp, u8p, C.c_int, C.c_uint32, u8p, vp, vp]
     lib.cb200_fit_ccm.argtypes = [vp, u8p, u8p, C.c_uint32, C.c_uint32, C.c_void_p]
     lib.cb200_palette_color.argtypes = [C.c_int, C.c_uint, C.c_int, u8p]
@@ -205,6 +209,14 @@ def jpeg_info(data):
     the reason for a file the device decoder refuses"""
     w, h = C.c_int32(), C.c_int32()
     _check(load_library().cb200_jpeg_info(data, len(data), C.byref(w), C.byref(h)))
+    return w.value, h.value
+
+
+def png_info(data):
+    """(w, h) of a PNG file (bytes) after its eXIf orientation, as cb200_png_info: host only, no GPU.  Raises Cb200Error with the
+    reason for a file the device decoder refuses"""
+    w, h = C.c_int32(), C.c_int32()
+    _check(load_library().cb200_png_info(data, len(data), C.byref(w), C.byref(h)))
     return w.value, h.value
 
 
@@ -486,6 +498,21 @@ class Context:
         data gets status -2 and mask 0"""
         keep, ptrs, sizes = _files(files)
         _check(self.lib.cb200_jpeg_scan_extract_decode_chunks_dev(self._h, ptrs, sizes, len(keep), flags, d_chunks, d_mask, d_flags, d_status))
+
+    png_info = staticmethod(png_info)
+
+    def png_decode_dev(self, files, d_rgb_out, d_status=None):
+        """cb200_png_decode_dev, enqueue-only: a list of PNG files (bytes) -> the packed ragged RGB8 batch at d_rgb_out (picture i at
+        3 * sum_{j<i} w_j h_j, sizes as png_info) and n int32 statuses (0, or -2 for corrupt data) at d_status, on the context's
+        stream.  Files of the mode's frame size give the frame batch of decode_chunks_dev (the CLI's --no-deskew)"""
+        keep, ptrs, sizes = _files(files)
+        _check(self.lib.cb200_png_decode_dev(self._h, ptrs, sizes, len(keep), d_rgb_out, d_status))
+
+    def png_scan_extract_decode_chunks_dev(self, files, d_chunks, d_mask, d_status, d_flags=None, flags=0):
+        """scan_extract_decode_chunks_dev on a list of PNG files (bytes) decoded on the device; enqueue-only.  A picture with corrupt
+        data gets status -2 and mask 0"""
+        keep, ptrs, sizes = _files(files)
+        _check(self.lib.cb200_png_scan_extract_decode_chunks_dev(self._h, ptrs, sizes, len(keep), flags, d_chunks, d_mask, d_flags, d_status))
 
     def camera_transforms(self, n):
         """the forward perspective transforms of the first n pictures of the last camera call: (n, 3, 3) float64 (synchronises)"""

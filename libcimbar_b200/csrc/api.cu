@@ -609,7 +609,7 @@ int cb200_destroy(cb200_ctx* c)
     for (const auto& s : c->stage) if (s.ev) cudaEventDestroy(s.ev);
     if (c->ccm_ev) cudaEventDestroy(c->ccm_ev);
     gather_destroy(c->gather);
-    deskew_destroy(c->deskew); scan_destroy(c->scan); jpeg_destroy(c->jpeg);
+    deskew_destroy(c->deskew); scan_destroy(c->scan); jpeg_destroy(c->jpeg); png_destroy(c->png);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     delete c;
     return CB200_OK;

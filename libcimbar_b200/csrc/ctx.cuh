@@ -16,10 +16,28 @@ struct GatherState;      // gather.cu
 struct DeskewState;      // deskew.cu
 struct ScanScratch;      // scan.cu
 struct JpegState;        // jpeg.cu
+struct PngState;         // png.cu
 void gather_destroy(GatherState* g);
 void deskew_destroy(DeskewState* d);     // delete: its buffers free themselves
 void scan_destroy(ScanScratch* s);       // likewise
 void jpeg_destroy(JpegState* j);         // likewise
+void png_destroy(PngState* p);           // likewise
+// the uploads of the file calls (descriptors + compressed data, jpeg.cu / png.cu): a ring of pinned buffers, each reused once the
+// copy enqueued from it has run -- one per call, so, as on the RGB camera call, a fourth call in flight waits until the first
+// one's upload has run.  take() hands out the next slot with room for `bytes`; send() enqueues the copy of its first `bytes` to
+// d_dst and records the slot's event
+struct FileUpload {
+    static constexpr int kSlots = 3;
+    PinnedBuf<uint8_t> h[kSlots];
+    cudaEvent_t ev[kSlots] = {};
+    int next = 0;
+    ~FileUpload() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+    int take(size_t bytes, int* slot, uint8_t** host);
+    int send(cudaStream_t st, int slot, void* d_dst, size_t bytes);
+};
+// status -2 (and, when d_mask is given, mask 0) for every picture whose flag in d_bad is set: the corrupt files of a file call
+// (files.cu, like FileUpload's members)
+int file_status(cb200_ctx* c, const int* d_bad, int n, int32_t* d_status, uint32_t* d_mask);
 // cb200_decode_fountain_from_dev with an optional per-frame sharpen selection: `sharpen` = n host bytes (nonzero =
 // should_preprocess) or NULL (the batch-wide CB200_FLAG_SHARPEN decides).  The flags are checked by the caller (api.cu)
 int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
@@ -131,6 +149,7 @@ struct cb200_ctx {
     cb200::DeskewState* deskew = nullptr;   // extractor scratch (deskew.cu)
     cb200::ScanScratch* scan = nullptr;     // anchor-scan scratch (scan.cu)
     cb200::JpegState* jpeg = nullptr;       // JPEG decode scratch (jpeg.cu)
+    cb200::PngState* png = nullptr;         // PNG decode scratch (png.cu)
 };
 
 namespace cb200 {

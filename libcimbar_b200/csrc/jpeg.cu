@@ -3,7 +3,8 @@
 // (src/exe/cimbar/cimbar.cpp:132-133, reference-relative), for a batch of files in host memory.
 //
 // The host parses the markers (jpeg_core.cuh parse: tables, scans, restart intervals, EXIF orientation) and uploads the picture,
-// scan, segment and table descriptors together with the compressed files in one copy from a pinned ring of its own.  Then,
+// scan, segment and table descriptors together with the compressed files in one copy from a pinned ring of its own (ctx.cuh
+// FileUpload, the type the PNG calls use too).  Then,
 // enqueued on the context's stream:
 //   k_jpeg_init     the per-picture corrupt flag from the parse (a file that ends inside its data)
 //   k_jpeg_unstuff  one CTA per segment (restart interval, or whole scan): FF 00 stuffing out by a flag + block-wide prefix sum
@@ -29,15 +30,9 @@ namespace cb200 {
 using namespace jpeg;
 
 constexpr int kSegThreads = 512;       // threads per segment in k_jpeg_unstuff / k_jpeg_decode
-constexpr int kUploadSlots = 3;        // pinned upload buffers of the JPEG calls
 
 struct JpegState {
-    // the calls' uploads (descriptors + files): a ring of pinned buffers, each reused once the copy enqueued from it has run --
-    // one per call, so, as on the RGB camera call, a fourth call in flight waits until the first one's upload has run
-    PinnedBuf<uint8_t> h_up[kUploadSlots];
-    cudaEvent_t up_ev[kUploadSlots] = {};
-    int up_next = 0;
-    ~JpegState() { for (cudaEvent_t e : up_ev) if (e) cudaEventDestroy(e); }
+    FileUpload up;                     // the calls' uploads (descriptors + files)
     DevBuf<uint8_t> d_blob;            // the call's upload (descriptors + files)
     DevBuf<uint8_t> d_unstuffed;       // the segments' bytes without FF 00 stuffing, at their offsets in the data section
     DevBuf<uint32_t> d_ulen;           // per segment: its unstuffed bytes
@@ -205,13 +200,6 @@ __global__ void k_jpeg_rgb(const Pic* __restrict__ pics, const uint8_t* __restri
     o[0] = rgb[0]; o[1] = rgb[1]; o[2] = rgb[2];
 }
 
-// a picture with corrupt data: status -2 and, on the camera call, no chunks
-__global__ void k_jpeg_status(const int* __restrict__ bad, int n, int32_t* __restrict__ status, uint32_t* __restrict__ mask)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && bad[i]) { status[i] = -2; if (mask) mask[i] = 0; }
-}
-
 // the files' headers, all before any CUDA call: CB200_ERR_ARG naming the picture for a refused file or size
 static int parse_files(const uint8_t* const* files, const uint64_t* sizes, int n, std::vector<Parsed>& ps, std::vector<int32_t>& wh)
 {
@@ -247,14 +235,11 @@ static int jpeg_enqueue(cb200_ctx* c, const std::vector<Parsed>& ps, const uint8
     CK(j->d_planes.ensure(L.planes), "cudaMalloc JPEG planes");
     CK(j->d_masks.ensure(4 * (L.coef / 64)), "cudaMalloc JPEG refinement masks");
     CK(j->d_bad.ensure((size_t)n), "cudaMalloc JPEG flags");
-    const int slot = j->up_next;
-    j->up_next = (slot + 1) % kUploadSlots;
-    if (!j->up_ev[slot]) CK(cudaEventCreateWithFlags(&j->up_ev[slot], cudaEventDisableTiming), "cudaEventCreate JPEG upload");
-    CK(cudaEventSynchronize(j->up_ev[slot]), "sync (JPEG upload slot)");   // the slot's last copy has run
-    CK(j->h_up[slot].ensure(L.bytes), "cudaMallocHost JPEG upload");
-    pack(ps, files, sizes, L, j->h_up[slot]);
-    CK(cudaMemcpyAsync(j->d_blob, j->h_up[slot], L.bytes, cudaMemcpyHostToDevice, st), "H2D JPEG files");
-    CK(cudaEventRecord(j->up_ev[slot], st), "record JPEG upload");
+    int slot, rc;
+    uint8_t* h;
+    rc = j->up.take(L.bytes, &slot, &h); if (rc) return rc;
+    pack(ps, files, sizes, L, h);
+    rc = j->up.send(st, slot, j->d_blob, L.bytes); if (rc) return rc;
     const uint8_t* b = j->d_blob;
     const Pic* pics = reinterpret_cast<const Pic*>(b + L.pics);
     const Seg* segs = reinterpret_cast<const Seg*>(b + L.segs);
@@ -311,9 +296,7 @@ int cb200_jpeg_decode_dev(cb200_ctx* c, const uint8_t* const* files, const uint6
     rc = jpeg_enqueue(c, ps, files, sizes, d_rgb_out); if (rc) return rc;
     if (d_status) {
         CK(cudaMemsetAsync(d_status, 0, sizeof(int32_t) * (size_t)n, c->stream), "memset status");
-        k_jpeg_status<<<(n + 127) / 128, 128, 0, c->stream>>>(c->jpeg->d_bad, n, d_status, nullptr);
-        count_launch();
-        CK(cudaGetLastError(), "JPEG status launch");
+        return file_status(c, c->jpeg->d_bad, n, d_status, nullptr);
     }
     return CB200_OK;
 }
@@ -334,10 +317,7 @@ int cb200_jpeg_scan_extract_decode_chunks_dev(cb200_ctx* c, const uint8_t* const
     CK(j->d_rgb.ensure(rgb), "cudaMalloc JPEG pictures");
     rc = jpeg_enqueue(c, ps, files, sizes, j->d_rgb); if (rc) return rc;
     rc = camera_enqueue(c, j->d_rgb, wh.data(), n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status); if (rc) return rc;
-    k_jpeg_status<<<(n + 127) / 128, 128, 0, c->stream>>>(j->d_bad, n, d_extract_status, d_chunk_mask);
-    count_launch();
-    CK(cudaGetLastError(), "JPEG status launch");
-    return CB200_OK;
+    return file_status(c, j->d_bad, n, d_extract_status, d_chunk_mask);
 }
 
 }  // extern "C"

@@ -551,20 +551,27 @@ JD_HD int sample(const uint8_t* planes, const Pic& P, const Comp& C, int x, int 
 
 JD_HD uint8_t clamp255(int v) { return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v); }
 
+// the decoded pixel (x, y) of a w x h picture shown at output pixel (ox, oy) under EXIF orientation `orient` (OpenCV's
+// ApplyExifOrientation: flips and transposes)
+JD_HD void orient_source(int orient, int w, int h, int ox, int oy, int& x, int& y)
+{
+    switch (orient) {
+    case 2: x = w - 1 - ox; y = oy; break;
+    case 3: x = w - 1 - ox; y = h - 1 - oy; break;
+    case 4: x = ox; y = h - 1 - oy; break;
+    case 5: x = oy; y = ox; break;
+    case 6: x = oy; y = h - 1 - ox; break;
+    case 7: x = w - 1 - oy; y = h - 1 - ox; break;
+    case 8: x = w - 1 - oy; y = ox; break;
+    default: x = ox; y = oy; break;
+    }
+}
+
 // output pixel (ox, oy) of picture P: EXIF orientation -> decoded pixel -> RGB (ycc_rgb_convert; gray replicated)
 JD_HD void pixel_rgb(const uint8_t* planes, const Pic& P, int ox, int oy, uint8_t* rgb)
 {
     int x, y;
-    switch (P.orient) {
-    case 2: x = P.w - 1 - ox; y = oy; break;
-    case 3: x = P.w - 1 - ox; y = P.h - 1 - oy; break;
-    case 4: x = ox; y = P.h - 1 - oy; break;
-    case 5: x = oy; y = ox; break;
-    case 6: x = oy; y = P.h - 1 - ox; break;
-    case 7: x = P.w - 1 - oy; y = P.h - 1 - ox; break;
-    case 8: x = P.w - 1 - oy; y = ox; break;
-    default: x = ox; y = oy; break;
-    }
+    orient_source(P.orient, P.w, P.h, ox, oy, x, y);
     const int Y = sample(planes, P, P.comp[0], x, y);
     if (P.ncomp == 1) { rgb[0] = rgb[1] = rgb[2] = (uint8_t)Y; return; }
     const int cb = sample(planes, P, P.comp[1], x, y) - 128, cr = sample(planes, P, P.comp[2], x, y) - 128;
