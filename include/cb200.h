@@ -393,6 +393,10 @@ int cb200_get_ccm(cb200_ctx* ctx, float* m9);
    and the anchor white on the device and runs the Moore-Penrose fit (OpenCV's float Jacobi SVD restated).  Returns 1 when a
    matrix was fitted -- it is then the context's CCM and copied to m9_out (may be NULL) --, 0 when the reference would have
    returned without one (no header, fewer than four colours seen), negative on error. */
+/* the matrices the first n frames of the last call that fitted CCMs (CB200_FLAG_CC_FIT, or a call reading a CCM still in flight)
+   were decoded with: n x 9 floats, row-major, and n activity bytes (0: that frame had no CCM).  Synchronises.  CB200_ERR_ARG for
+   n beyond that call's frames */
+int cb200_get_frame_ccms(cb200_ctx* ctx, int n, float* m9n, uint8_t* active);
 int cb200_fit_ccm(cb200_ctx* ctx, const uint8_t* rgb, const uint8_t* header6, uint32_t radioactive_block_id, uint32_t flags, float* m9_out);
 
 /* Replaces: CimbDecoder::get_color(i, color_mode) -> cimbar::getColor(i, num_colors, color_mode)
@@ -466,6 +470,31 @@ int cb200_comm_init(cb200_ctx* ctx, const uint8_t* id, int nranks, int rank);
 int cb200_gather_chunks(cb200_ctx* ctx, void* nccl_comm, int nranks, int rank, int buffer /* 0 | 1 */, const uint8_t* d_chunks,
                         const uint32_t* d_mask, int n, uint8_t* d_all_chunks, uint32_t* d_all_masks);
 int cb200_gather_chunks_wait(cb200_ctx* ctx, int buffer);
+
+/* ---- multi-GPU: the CC_FIT colour correction chained across ranks ------------------------------------------------
+
+   Under CB200_FLAG_CC_FIT a frame without a usable fountain header takes the CCM of the frame before it: the one state that
+   crosses frames.  When a batch is cut into contiguous stripes, one per rank in rank order, linking the ranks' contexts to a chain
+   makes every rank's records equal those of one context decoding the whole batch: the CCM entering rank r's stripe is the last fit
+   of the stripes of ranks 0 .. r-1 in the same step, or, when none of them fit, the CCM rank 0 entered the step with.
+   Rank 0 allocates a small region (cb200_ccm_chain_root_create) and hands the IPC handle to the other ranks
+   (cb200_ccm_chain_peer_open); every rank then links its context (cb200_ccm_chain_attach) and, before each CC_FIT call, sets the
+   call's step (cb200_ccm_chain_step: epochs start at >= 1 and increase; every rank uses the same epoch for the same step; a rank
+   with no frames in a step still makes the call with n = 0: every entry point that honours CB200_FLAG_CC_FIT, host-pointer and
+   camera ones included, then takes part in the step).  A chained call enqueues, with no host wait, a publish of the stripe's
+   last fit after its fit kernel, a bounded system-scope wait for the lower ranks' publishes of the step before its colour
+   decisions, and at its end a bounded wait for all ranks' publishes: afterwards the context's CCM (cb200_get_ccm, and the next
+   call) is the step's global exit on every rank.  A wait that gives up after 30 s records the missing rank;
+   cb200_ccm_chain_status (synchronises, any rank) reports it.  Calls without CB200_FLAG_CC_FIT are not chained.
+   CB200_ERR_ARG, before any CUDA call: a CC_FIT call on a linked context without a step set, cb200_set_ccm / cb200_fit_ccm on a
+   linked context, a step on a context that is not linked, rank >= nranks or values that differ from the region's. */
+int cb200_ccm_chain_root_create(cb200_ctx* ctx, int nranks, uint8_t* handle_out /* CB200_IPC_HANDLE_BYTES */);
+int cb200_ccm_chain_peer_open(cb200_ctx* ctx, int nranks, int rank, const uint8_t* handle);
+int cb200_ccm_chain_attach(cb200_ctx* ctx, int rank, int nranks);
+int cb200_ccm_chain_step(cb200_ctx* ctx, uint32_t epoch);
+int cb200_ccm_chain_status(cb200_ctx* ctx);
+/* with cb200_set_timing on: the milliseconds the last chained call's link kernel took (its wait for the lower ranks' fits) */
+int cb200_ccm_chain_link_ms(cb200_ctx* ctx, float* ms);
 
 /* ---- rank-0 fountain ingest (host only, no GPU) ------------------------------------------------------------------
 

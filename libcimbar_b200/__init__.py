@@ -37,6 +37,8 @@ EXPORTS = [
     "cb200_scan_extract_decode_fountain_ragged", "cb200_scan_extract_decode_chunks_ragged_dev", "cb200_scan_extract_decode_chunks_dev",
     "cb200_camera_transforms", "cb200_jpeg_info", "cb200_jpeg_decode_dev", "cb200_jpeg_scan_extract_decode_chunks_dev",
     "cb200_png_info", "cb200_png_decode_dev", "cb200_png_scan_extract_decode_chunks_dev",
+    "cb200_ccm_chain_root_create", "cb200_ccm_chain_peer_open", "cb200_ccm_chain_attach", "cb200_ccm_chain_step", "cb200_ccm_chain_status",
+    "cb200_ccm_chain_link_ms", "cb200_get_frame_ccms",
 ]
 
 
@@ -143,6 +145,13 @@ def load_library():
     lib.cb200_comm_init.argtypes = [vp, u8p, C.c_int, C.c_int]
     lib.cb200_gather_chunks.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, u8p, u32p, C.c_int, u8p, u32p]
     lib.cb200_gather_chunks_wait.argtypes = [vp, C.c_int]
+    lib.cb200_ccm_chain_root_create.argtypes = [vp, C.c_int, u8p]
+    lib.cb200_ccm_chain_peer_open.argtypes = [vp, C.c_int, C.c_int, u8p]
+    lib.cb200_ccm_chain_attach.argtypes = [vp, C.c_int, C.c_int]
+    lib.cb200_ccm_chain_step.argtypes = [vp, C.c_uint32]
+    lib.cb200_ccm_chain_status.argtypes = [vp]
+    lib.cb200_ccm_chain_link_ms.argtypes = [vp, C.POINTER(C.c_float)]
+    lib.cb200_get_frame_ccms.argtypes = [vp, C.c_int, vp, vp]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -454,6 +463,15 @@ class Context:
             a = np.ascontiguousarray(m9, dtype=np.float32).reshape(9)
             _check(self.lib.cb200_set_ccm(self._h, a.ctypes.data))
 
+    def frame_ccms(self, n):
+        """the matrices the first n frames of the last CC_FIT call were decoded with: (n, 3, 3) float32 with NaN for a frame that had
+        none (synchronises)"""
+        m = np.zeros((n, 9), dtype=np.float32)
+        act = np.zeros(n, dtype=np.uint8)
+        _check(self.lib.cb200_get_frame_ccms(self._h, n, m.ctypes.data, act.ctypes.data))
+        m[act == 0] = np.nan
+        return m.reshape(n, 3, 3)
+
     def get_ccm(self):
         """the active CCM as a 3x3 float32 array, or None"""
         a = np.zeros(9, dtype=np.float32)
@@ -577,6 +595,32 @@ class Context:
 
     def gather_chunks_wait(self, buffer):
         _check(self.lib.cb200_gather_chunks_wait(self._h, buffer))
+
+    # ---- multi-GPU CC_FIT chain (cb200_ccm_chain_*): see include/cb200.h
+    def ccm_chain_root_create(self, nranks):
+        h = (C.c_uint8 * 64)()
+        _check(self.lib.cb200_ccm_chain_root_create(self._h, nranks, C.cast(h, C.c_void_p)))
+        return bytes(h)
+
+    def ccm_chain_peer_open(self, nranks, rank, handle):
+        h = (C.c_uint8 * 64).from_buffer_copy(handle)
+        _check(self.lib.cb200_ccm_chain_peer_open(self._h, nranks, rank, C.cast(h, C.c_void_p)))
+
+    def ccm_chain_attach(self, rank, nranks):
+        _check(self.lib.cb200_ccm_chain_attach(self._h, rank, nranks))
+
+    def ccm_chain_step(self, epoch):
+        """the epoch of the next CC_FIT call (the same on every rank for the same step, increasing from step to step)"""
+        _check(self.lib.cb200_ccm_chain_step(self._h, epoch))
+
+    def ccm_chain_status(self):
+        _check(self.lib.cb200_ccm_chain_status(self._h))
+
+    def ccm_chain_link_ms(self):
+        """ms of the last chained call's link kernel (set_timing on before the call; synchronises on it)"""
+        ms = C.c_float(0)
+        _check(self.lib.cb200_ccm_chain_link_ms(self._h, C.byref(ms)))
+        return ms.value
 
     def render_frames_dev(self, d_cellvals, n, d_rgb_out):
         _check(self.lib.cb200_render_frames_dev(self._h, d_cellvals, n, d_rgb_out))

@@ -312,6 +312,16 @@ int ccm_keep_last(cb200_ctx* c, int n, const uint8_t* d_active)
     if (!d_active) c->ccm_active = true;
     return CB200_OK;
 }
+// a chained CC_FIT call keeps the step's global exit instead (the same matrix on every rank of the chain): chain_settle writes it
+// to d_carry, from there it goes to h_ccm as above
+int ccm_keep_chain(cb200_ctx* c)
+{
+    int rc = chain_settle(c, c->d_carry); if (rc) return rc;
+    CK(cudaMemcpyAsync(c->h_ccm, c->d_carry, sizeof(float) * 10, cudaMemcpyDeviceToHost, c->stream), "D2H ccm");
+    CK(cudaEventRecord(c->ccm_ev, c->stream), "record ccm");
+    c->ccm_pending = c->ccm_pending_flag = true;
+    return CB200_OK;
+}
 // color_correction == 1: one matrix per frame of n frames in d_rgb into d_ccm, computed on the device before the colour pass
 // (CimbReader.cpp:124-125); the last one becomes the context's CCM
 int ccm_simple(cb200_ctx* c, const uint8_t* d_rgb, int n)
@@ -609,6 +619,7 @@ int cb200_destroy(cb200_ctx* c)
     for (const auto& s : c->stage) if (s.ev) cudaEventDestroy(s.ev);
     if (c->ccm_ev) cudaEventDestroy(c->ccm_ev);
     gather_destroy(c->gather);
+    chain_destroy(c->chain);
     deskew_destroy(c->deskew); scan_destroy(c->scan); jpeg_destroy(c->jpeg); png_destroy(c->png);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     delete c;
@@ -674,11 +685,14 @@ int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
                   uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes = nullptr, bool enqueue_only = false)
 {
     int rc = check_n(c, n); if (rc) return rc;
-    if (n == 0) return CB200_OK;
-    if (!d_rgb || !d_chunks || !d_chunk_mask) return fail(CB200_ERR_ARG, "null buffer");
+    // a chained CC_FIT call takes part in the step even with no frames: an empty stripe publishes "no fit" and settles
+    const bool chained = chain_linked(c, flags);
+    if (n == 0 && !chained) return CB200_OK;
+    if ((flags & CB200_FLAG_CC_FIT) && (flags & CB200_FLAG_CC_SIMPLE)) return fail(CB200_ERR_ARG, "CC_SIMPLE and CC_FIT are exclusive");
+    rc = check_chain_call(c, flags); if (rc) return rc;
+    if (n > 0 && (!d_rgb || !d_chunks || !d_chunk_mask)) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
-    if ((flags & CB200_FLAG_CC_FIT) && (flags & CB200_FLAG_CC_SIMPLE)) return fail(CB200_ERR_ARG, "CC_SIMPLE and CC_FIT are exclusive");
     // init_ccm is only reached from Decoder::do_decode (not the legacy coupled layout) and needs a header from the RS stream
     const bool fit = (flags & CB200_FLAG_CC_FIT) && !m.legacy && m.ecc_bytes > 0 && m.color_bits > 0;
     bool carried = false;                      // the CCM going into frame 0 is only known on the device
@@ -687,9 +701,23 @@ int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
         if (q == cudaErrorNotReady) carried = true;
         else if (q != cudaSuccess) return fail_cuda(q, "query ccm");
     }
+    if (n == 0) {                              // chained, empty stripe
+        rc = ccm_buffers(c); if (rc) return rc;
+        CcmArg own;
+        if (carried) {
+            memset(&own, 0, sizeof(own));
+            own.per_frame = c->d_carry;
+            own.per_frame_active = reinterpret_cast<const uint8_t*>(c->d_carry + 9);
+        } else {
+            rc = ccm_arg(c, own); if (rc) return rc;
+        }
+        rc = chain_publish_link(c, 0, nullptr, nullptr, own, nullptr); if (rc) return rc;
+        c->ccm_frames = 0;
+        return ccm_keep_chain(c);
+    }
     const uint16_t* idx;
     rc = idx_for(c, flags, &idx); if (rc) return rc;
-    if (!fit && !carried) {
+    if (!fit && !carried && !chained) {
         rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen, nullptr, nullptr, d_sel_bytes); if (rc) return rc;
         mark(c);                               // ev3: (no separate pack kernel on this path: the RS kernel gathers from the cell bytes)
         CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
@@ -715,15 +743,19 @@ int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
         } else {
             CK(cudaMemsetAsync(c->d_fit_valid, 0, (size_t)n, c->stream), "memset fit flags");
         }
+        // across ranks: this stripe's fits out, the CCM entering the stripe in (from the lower ranks' fits of the same step)
+        if (chained) { rc = chain_publish_link(c, n, c->d_fit, c->d_fit_valid, initial, &initial); if (rc) return rc; }
         CK(ccm_carry_launch(n, c->d_fit, c->d_fit_valid, initial, c->d_ccm, c->d_ccm_active, c->stream), "ccm carry");
         CK(ccm_apply_launch(m, c->d_means, n, c->d_ccm, c->d_ccm_active, c->d_cellvals, c->stream), "ccm apply");
+        c->ccm_frames = n;
         if (fit) {
             CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream, m.nblocks_sym, m.nblocks - m.nblocks_sym),
                "rs launch (colours)");
-            rc = ccm_keep_last(c, n, c->d_ccm_active); if (rc) return rc;
         } else {
             CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
         }
+        if (chained) { rc = ccm_keep_chain(c); if (rc) return rc; }
+        else if (fit) { rc = ccm_keep_last(c, n, c->d_ccm_active); if (rc) return rc; }
     }
     mark(c);                                   // ev4: after RS
     CK(k2_mask_launch(m, c->d_ok, n, d_chunk_mask, c->stream), "mask launch");
@@ -768,7 +800,8 @@ int cb200_decode(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_
 {
     int rc = check_frame_flags(flags); if (rc) return rc;
     rc = check_n(c, n); if (rc) return rc;
-    if (n == 0) return CB200_OK;
+    rc = check_chain_call(c, flags); if (rc) return rc;
+    if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
     if (!rgb || !data_out) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = upload_frames(c, rgb, n); if (rc) return rc;
@@ -788,7 +821,8 @@ int decode_fountain_from_host(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t 
                               uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
     int rc = check_n(c, n); if (rc) return rc;
-    if (n == 0) return CB200_OK;
+    rc = check_chain_call(c, flags); if (rc) return rc;
+    if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
     if (!rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = upload_frames(c, rgb, n); if (rc) return rc;
@@ -801,7 +835,8 @@ int cb200::decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, ui
                                    uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
     int rc = check_n(c, n); if (rc) return rc;
-    if (n == 0) return CB200_OK;
+    rc = check_chain_call(c, flags); if (rc) return rc;
+    if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
     if (!d_rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = decode_chunks(c, d_rgb, n, flags, sharpen, c->d_data, c->d_mask, nullptr); if (rc) return rc;
@@ -932,6 +967,7 @@ int cb200_best_colors(cb200_ctx* c, const uint8_t* rgb_means, int n, uint8_t* co
 int cb200_set_ccm(cb200_ctx* c, const float* m9)
 {
     if (!c) return fail(CB200_ERR_ARG, "null context");
+    int rc = check_host_ccm(c); if (rc) return rc;
     c->ccm_pending = c->ccm_pending_flag = false;    // an explicit matrix replaces whatever the last batch left
     c->ccm_active = m9 != nullptr;
     if (m9) memcpy(c->ccm, m9, sizeof(c->ccm));
@@ -947,13 +983,25 @@ int cb200_get_ccm(cb200_ctx* c, float* m9)
     return c->ccm_active ? 1 : 0;
 }
 
+int cb200_get_frame_ccms(cb200_ctx* c, int n, float* m9n, uint8_t* active)
+{
+    if (!c || n < 0 || (n > 0 && (!m9n || !active))) return fail(CB200_ERR_ARG, "bad arguments");
+    if (n > c->ccm_frames) return fail(CB200_ERR_ARG, "the last CC_FIT call had " + std::to_string(c->ccm_frames) + " frames");
+    if (n == 0) return CB200_OK;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    CK(cudaMemcpyAsync(m9n, c->d_ccm, sizeof(float) * 9 * (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H frame ccms");
+    CK(cudaMemcpyAsync(active, c->d_ccm_active, (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H frame ccm flags");
+    CK(cudaStreamSynchronize(c->stream), "sync");
+    return CB200_OK;
+}
+
 int cb200_fit_ccm(cb200_ctx* c, const uint8_t* rgb, const uint8_t* header6, uint32_t radioactive_block_id, uint32_t flags, float* m9_out)
 {
     if (!c || !header6) return fail(CB200_ERR_ARG, "bad arguments");
+    int rc = check_host_ccm(c); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
     if (m.color_bits == 0) return 0;
-    int rc;
     if (rgb) { rc = upload_frames(c, rgb, 1); if (rc) return rc; }
     else if (!c->d_rgb) return fail(CB200_ERR_ARG, "no frame in the context's staging buffer");
     rc = ccm_buffers(c); if (rc) return rc;

@@ -17,7 +17,9 @@ struct DeskewState;      // deskew.cu
 struct ScanScratch;      // scan.cu
 struct JpegState;        // jpeg.cu
 struct PngState;         // png.cu
+struct ChainState;       // chain.cu
 void gather_destroy(GatherState* g);
+void chain_destroy(ChainState* s);
 void deskew_destroy(DeskewState* d);     // delete: its buffers free themselves
 void scan_destroy(ScanScratch* s);       // likewise
 void jpeg_destroy(JpegState* j);         // likewise
@@ -84,6 +86,19 @@ int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uin
 // the good chunks of each frame packed densely (api.cu)
 int fetch_fountain(cb200_ctx* c, int n, const int32_t* d_status, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
                    uint8_t* frame_flags, int32_t* extract_status);
+// the CCM chain across ranks (chain.cu).  chain_linked: a call with these flags on this context runs the chain (attached, CC_FIT).
+// check_chain_call: CB200_ERR_ARG for such a call without a step set; check_host_ccm: CB200_ERR_ARG for cb200_set_ccm /
+// cb200_fit_ccm on an attached context (both without CUDA calls).  chain_publish_link enqueues, after k_ccm_fit, the publish of
+// the stripe's n fits (d_fit / d_valid; n = 0: an empty stripe, no fit) and, with entry given, the link that leaves the stripe's
+// entry CCM on the device and points *entry at it; own = the CCM this context would enter the stripe with.  chain_settle enqueues
+// the global exit of the step into d_carry (9 floats + activity byte) and ends the step
+bool chain_linked(const cb200_ctx* c, uint32_t flags);
+int check_chain_call(const cb200_ctx* c, uint32_t flags);
+int check_host_ccm(const cb200_ctx* c);
+int chain_publish_link(cb200_ctx* c, int n, const float* d_fit, const uint8_t* d_valid, const CcmArg& own, CcmArg* entry);
+int chain_settle(cb200_ctx* c, float* d_carry);
+// a camera call with no pictures: on a chained CC_FIT call the empty stripe's part of the step, else nothing (scan.cu)
+int camera_empty(cb200_ctx* c, uint32_t flags);
 }  // namespace cb200
 #define CK(call, what) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cb200::fail_cuda(e__, what); } while (0)
 
@@ -144,8 +159,10 @@ struct cb200_ctx {
     cb200::DevBuf<float> d_fit;             // max_frames x 9
     cb200::DevBuf<uint8_t> d_fit_valid;     // max_frames
     cb200::DevBuf<uint8_t> d_ccm_active;    // max_frames: the frame is decoded with d_ccm[f]
+    int ccm_frames = 0;              // frames of the last call that took the fitted-CCM route (cb200_get_frame_ccms)
     cudaEvent_t ccm_ev = nullptr;    // recorded after the D2H copies of the last batch's CCM (ccm_resolve waits on it)
     cb200::GatherState* gather = nullptr;   // multi-GPU chunk-record window (gather.cu)
+    cb200::ChainState* chain = nullptr;     // multi-GPU CC_FIT chain (chain.cu)
     cb200::DeskewState* deskew = nullptr;   // extractor scratch (deskew.cu)
     cb200::ScanScratch* scan = nullptr;     // anchor-scan scratch (scan.cu)
     cb200::JpegState* jpeg = nullptr;       // JPEG decode scratch (jpeg.cu)

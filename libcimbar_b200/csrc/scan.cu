@@ -531,7 +531,14 @@ static int check_camera_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32
 {
     int rc = check_camera_dev_flags(flags); if (rc) return rc;
     rc = check_ragged(wh, d_pictures, n); if (rc) return rc;
-    return check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status);
+    rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
+    return check_chain_call(c, flags);
+}
+
+int camera_empty(cb200_ctx* c, uint32_t flags)
+{
+    if (!chain_linked(c, flags)) return CB200_OK;
+    return decode_chunks_enqueue(c, nullptr, 0, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, nullptr, nullptr, nullptr);
 }
 
 }  // namespace cb200
@@ -620,7 +627,8 @@ int cb200_scan_extract_decode_fountain(cb200_ctx* c, const uint8_t* pictures, in
     int rc = check_camera_flags(flags); if (rc) return rc;
     if (!c || !pictures || !chunks_out || !chunk_count || !extract_status || n < 0 || n > c->max_frames || w < 2 || h < 2)
         return fail(CB200_ERR_ARG, "bad arguments");
-    if (n == 0) return CB200_OK;
+    rc = check_chain_call(c, flags); if (rc) return rc;
+    if (n == 0) return camera_empty(c, flags);
     const std::vector<int32_t> wh = uniform_sizes(w, h, n);
     rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
@@ -639,7 +647,8 @@ int cb200_scan_extract_decode_fountain_ragged(cb200_ctx* c, const uint8_t* const
     if (!c) return fail(CB200_ERR_ARG, "null context");
     if (!chunks_out || !chunk_count || !extract_status) return fail(CB200_ERR_ARG, "null output");
     if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
-    if (n == 0) return CB200_OK;
+    rc = check_chain_call(c, flags); if (rc) return rc;
+    if (n == 0) return camera_empty(c, flags);
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const uint8_t* d = nullptr;
     rc = stage_pictures(c, pictures, wh, n, &d); if (rc) return rc;
@@ -650,7 +659,7 @@ int cb200_scan_extract_decode_chunks_ragged_dev(cb200_ctx* c, const uint8_t* d_p
                                                 uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
 {
     int rc = check_camera_dev(c, d_pictures, wh, n, flags, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
-    if (n == 0) return CB200_OK;
+    if (n == 0) return camera_empty(c, flags);
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     return camera_enqueue(c, d_pictures, wh, n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
 }

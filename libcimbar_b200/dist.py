@@ -114,3 +114,102 @@ class RecordExchange:
     def release(self, step):
         if self.kind in ("window", "window-direct") and self.rank == 0:
             self.ctx.gather_release(step & 1, step)
+
+
+def stripe(n_total, rank, n_per_rank):
+    """rank's contiguous stripe [start, stop) of a batch of n_total pictures, n_per_rank per rank (rank-major = batch order): the
+    last ranks of a short batch get a short or an empty stripe"""
+    start = min(n_total, rank * n_per_rank)
+    return start, min(n_total, start + n_per_rank)
+
+
+class CameraExchange:
+    """Camera batches across ranks: every step, rank r decodes the contiguous stripe of the batch that `stripe` gives it (at most
+    n_per_rank pictures) into the record window of RecordExchange ("window": local buffers + copy-engine push, "window-direct": the
+    decode stores into rank 0's window), and rank 0 collects the records, masks and extract statuses of all ranks in batch order.
+
+    With CB200_FLAG_CC_FIT in `flags` the ranks' contexts are linked to a CCM chain (cb200_ccm_chain_*), so that the colour
+    decisions, chunks and masks equal those of one context decoding the whole batch:
+
+        ex = CameraExchange(ctx, "window", n_per_rank, flags=cb.FLAG_SHARPEN_IF_NEEDED | cb.FLAG_CC_FIT)
+        for s in 1, 2, ...:
+            ex.decode(s, ("rgb", d_pictures, wh))     # or ("jpeg", files) / ("png", files): this rank's stripe (may be empty)
+            out = ex.collect(s)                      # every rank calls it; rank 0: (chunks, masks, statuses) as numpy, else None
+
+    decode() only enqueues work; collect() synchronises the context's stream."""
+
+    def __init__(self, ctx, kind, n_per_rank, flags=0, rank=None, world=None):
+        import libcimbar_b200 as cb
+        import torch
+        if kind not in ("window", "window-direct"):
+            raise ValueError("kind must be 'window' or 'window-direct'")
+        self.ctx, self.kind, self.n, self.flags = ctx, kind, n_per_rank, flags
+        self.rank = dist.get_rank() if rank is None else rank
+        self.world = dist.get_world_size() if world is None else world
+        self.records = RecordExchange(ctx, kind, n_per_rank, self.rank, self.world)
+        self.chained = bool(flags & cb.FLAG_CC_FIT)
+        if self.chained:
+            box = [ctx.ccm_chain_root_create(self.world) if self.rank == 0 else None]
+            dist.broadcast_object_list(box, src=0)
+            if self.rank != 0:
+                ctx.ccm_chain_peer_open(self.world, self.rank, box[0])
+            ctx.ccm_chain_attach(self.rank, self.world)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        self.status = [torch.zeros(max(1, n_per_rank), dtype=torch.int32, device=dev) for _ in range(2)]
+        self.counts = {}
+
+    def decode(self, step, batch):
+        """enqueue the decode of this rank's stripe for `step` (1, 2, ...): batch = ("rgb", d_pictures, wh) with wh an (n, 2) array
+        of (width, height) of the pictures packed in device memory, or ("jpeg" | "png", list of files as bytes)"""
+        kind = batch[0]
+        n = len(batch[2]) if kind == "rgb" else len(batch[1])
+        if n > self.n:
+            raise ValueError(f"{n} pictures in a stripe of {self.n}")
+        self.counts[step] = n
+        d_chunks, d_mask = self.records.begin(step)
+        d_status = self.status[step & 1].data_ptr()
+        if self.chained:
+            self.ctx.ccm_chain_step(step)
+        if kind == "rgb":
+            # (an empty stripe still makes the call -- its part of the CCM chain -- with a stand-in address that is never read)
+            self.ctx.scan_extract_decode_chunks_dev(batch[1] if n else d_status, batch[2], d_chunks, d_mask, d_status, flags=self.flags)
+        elif kind == "jpeg":
+            self.ctx.jpeg_scan_extract_decode_chunks_dev(batch[1], d_chunks, d_mask, d_status, flags=self.flags)
+        elif kind == "png":
+            self.ctx.png_scan_extract_decode_chunks_dev(batch[1], d_chunks, d_mask, d_status, flags=self.flags)
+        else:
+            raise ValueError("batch kind must be 'rgb', 'jpeg' or 'png'")
+        self.records.end(step)
+
+    def collect(self, step):
+        """collective: rank 0 returns (chunks (n, data_bytes) uint8, masks (n,) uint32, statuses (n,) int32) of the whole batch of
+        `step` in batch order, the other ranks None.  Synchronises the context's stream; raises if a rank of the exchange or of the
+        CCM chain did not arrive in time"""
+        import ctypes as C
+        import numpy as np
+        n = self.counts.pop(step)
+        b = step & 1
+        if self.rank == 0:
+            self.records.collect(step)
+        self.ctx.sync()
+        if self.chained:
+            self.ctx.ccm_chain_status()
+        mine = (n, self.status[b][:n].cpu().numpy())
+        parts = [None] * self.world if self.rank == 0 else None
+        dist.gather_object(mine, parts, dst=0)
+        if self.rank != 0:
+            return None
+        self.ctx.gather_status()
+        cudart = C.CDLL("libcudart.so.12")
+        rec = self.ctx.info.data_bytes
+        chunks, masks, statuses = [], [], []
+        for r, (nr, st) in enumerate(parts):
+            pc, pm = self.ctx.gather_slot(b, r)
+            hc = np.zeros((nr, rec), np.uint8)
+            hm = np.zeros(nr, np.uint32)
+            if nr:
+                assert cudart.cudaMemcpy(C.c_void_p(hc.ctypes.data), C.c_void_p(pc), C.c_size_t(nr * rec), 2) == 0
+                assert cudart.cudaMemcpy(C.c_void_p(hm.ctypes.data), C.c_void_p(pm), C.c_size_t(4 * nr), 2) == 0
+            chunks.append(hc); masks.append(hm); statuses.append(st)
+        self.records.release(step)
+        return np.concatenate(chunks), np.concatenate(masks), np.concatenate(statuses)
