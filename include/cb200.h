@@ -267,6 +267,34 @@ int cb200_scan_extract_decode_chunks_ragged_dev(cb200_ctx* ctx, const uint8_t* d
 /* the same for n pictures of one size w x h */
 int cb200_scan_extract_decode_chunks_dev(cb200_ctx* ctx, const uint8_t* d_pictures, int w, int h, int n, uint32_t flags, uint8_t* d_chunks,
                                          uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+/* ---- camera plans: the enqueue-only camera call captured once in a CUDA graph ----------------------------------------------
+
+   A plan is cb200_scan_extract_decode_chunks_ragged_dev for n pictures of sizes wh, with these flags and these device buffers,
+   captured once: each cb200_camera_plan_launch is one cudaGraphLaunch on the context's current stream, with no host work per batch,
+   and the graph itself (cb200_camera_plan_graph) can be embedded in a larger one.  The buffers are bound when the plan is created:
+   the caller writes each batch's pictures into d_pictures in stream order before the launch; two plans on one context double-buffer.
+   A launch gives what the direct call would give at that point of the context's call sequence: records, masks, frame flags, statuses,
+   cb200_camera_transforms, cb200_get_ccm and cb200_get_frame_ccms.  Its CCM always comes from the device (the last matrix the context
+   kept or was given, which the context keeps current there while plans exist); CC_SIMPLE's last matrix and CC_FIT's carry reach the
+   host as after an enqueue-only call, pending behind an event.
+     create: the argument checks and messages of cb200_scan_extract_decode_chunks_ragged_dev, all before any CUDA call, and
+             CB200_ERR_ARG for n == 0 and for a context attached to a CCM chain.  Every context buffer the graph uses is grown to this
+             batch's size here; with the buffers already that large, create does not wait for the device.
+     launch: outside a capture, the context's host state (pending CCM, the transforms' picture count) follows each launch as it
+             follows a direct call.  Inside a stream capture of the context's stream (torch.cuda.graph), the graph goes into that
+             capture as a child node and the host state is left alone: replays of an enclosing graph, or of one the plan's graph was
+             added to, update device memory only.  Such a graph reads the plan's buffers, so the plan must outlive it.
+   While a plan exists, the buffers its graph uses are frozen: a call on the context that would grow one fails with CB200_ERR_ARG
+   before any CUDA call, naming the buffer.  cb200_destroy destroys the context's plans; cb200_set_timing does not time launches,
+   and cb200_launch_count counts a launch as the kernels in its graph. */
+typedef struct cb200_camera_plan cb200_camera_plan;
+int cb200_camera_plan_create(cb200_ctx* ctx, const int32_t* wh, int n, uint32_t flags, const uint8_t* d_pictures, uint8_t* d_chunks,
+                             uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out);
+/* one cudaGraphLaunch on the context's current stream (or a child node in its capture) */
+int cb200_camera_plan_launch(cb200_camera_plan* plan);
+/* the plan's cudaGraph_t, owned by the plan (for cudaGraphAddChildGraphNode, which copies it) */
+int cb200_camera_plan_graph(cb200_camera_plan* plan, void** cuda_graph);
+int cb200_camera_plan_destroy(cb200_camera_plan* plan);
 /* ---- JPEG files in: the CLI's input, decoded on the device ---------------------------------------------------------------
 
    Replaces: cv::imread(file) + cv::cvtColor(BGR2RGB) (src/exe/cimbar/cimbar.cpp:132-133) for a batch of JPEG files in host memory:

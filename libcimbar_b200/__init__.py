@@ -39,6 +39,7 @@ EXPORTS = [
     "cb200_png_info", "cb200_png_decode_dev", "cb200_png_scan_extract_decode_chunks_dev",
     "cb200_ccm_chain_root_create", "cb200_ccm_chain_peer_open", "cb200_ccm_chain_attach", "cb200_ccm_chain_step", "cb200_ccm_chain_status",
     "cb200_ccm_chain_link_ms", "cb200_get_frame_ccms",
+    "cb200_camera_plan_create", "cb200_camera_plan_launch", "cb200_camera_plan_graph", "cb200_camera_plan_destroy",
 ]
 
 
@@ -152,6 +153,10 @@ def load_library():
     lib.cb200_ccm_chain_status.argtypes = [vp]
     lib.cb200_ccm_chain_link_ms.argtypes = [vp, C.POINTER(C.c_float)]
     lib.cb200_get_frame_ccms.argtypes = [vp, C.c_int, vp, vp]
+    lib.cb200_camera_plan_create.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp, C.POINTER(C.c_void_p)]
+    lib.cb200_camera_plan_launch.argtypes = [vp]
+    lib.cb200_camera_plan_graph.argtypes = [vp, C.POINTER(C.c_void_p)]
+    lib.cb200_camera_plan_destroy.argtypes = [vp]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -503,6 +508,16 @@ class Context:
         _check(self.lib.cb200_scan_extract_decode_chunks_ragged_dev(self._h, d_pictures, wh.ctypes.data, wh.shape[0], flags, d_chunks, d_mask,
                                                                     d_flags, d_status))
 
+    def camera_plan(self, wh, flags, pictures, chunks, mask, frame_flags, status):
+        """scan_extract_decode_chunks_dev for pictures of sizes wh (n x (w, h), host) with these flags, captured once in a CUDA graph
+        with its device buffers bound (device addresses; frame_flags may be None): a CameraPlan whose launch() replays it on the
+        context's stream.  Write each batch's pictures into `pictures` in stream order before its launch"""
+        wh = np.ascontiguousarray(wh, dtype=np.int32).reshape(-1, 2)
+        h = C.c_void_p()
+        _check(self.lib.cb200_camera_plan_create(self._h, wh.ctypes.data, wh.shape[0], flags, pictures, chunks, mask, frame_flags, status,
+                                                 C.byref(h)))
+        return CameraPlan(self, h)
+
     jpeg_info = staticmethod(jpeg_info)
 
     def jpeg_decode_dev(self, files, d_rgb_out, d_status=None):
@@ -624,6 +639,35 @@ class Context:
 
     def render_frames_dev(self, d_cellvals, n, d_rgb_out):
         _check(self.lib.cb200_render_frames_dev(self._h, d_cellvals, n, d_rgb_out))
+
+
+class CameraPlan:
+    """a camera plan (cb200_camera_plan_*): launch() is one graph launch on the context's stream, or a child node of the capture
+    in progress on it (torch.cuda.graph); `graph` is the cudaGraph_t as an int.  The plan belongs to its context, which must outlive
+    it (closing the context destroys its plans)"""
+
+    def __init__(self, ctx, handle):
+        self.ctx, self._h = ctx, handle
+
+    def launch(self):
+        _check(self.ctx.lib.cb200_camera_plan_launch(self._h))
+
+    @property
+    def graph(self):
+        g = C.c_void_p()
+        _check(self.ctx.lib.cb200_camera_plan_graph(self._h, C.byref(g)))
+        return g.value
+
+    def close(self):
+        if self._h and self.ctx._h:
+            self.ctx.lib.cb200_camera_plan_destroy(self._h)
+        self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class FountainSink:

@@ -466,6 +466,42 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const u
 
 }  // namespace
 
+namespace cb200 {
+// init_ccm is only reached from Decoder::do_decode (not the legacy coupled layout) and needs a header from the RS stream
+bool ccm_fits(const Mode& m, uint32_t flags) { return (flags & CB200_FLAG_CC_FIT) && !m.legacy && m.ecc_bytes > 0 && m.color_bits > 0; }
+
+int flood_reserve(cb200_ctx* c, int n)
+{
+    if (flood_workspace_fits(c->flood, n)) return CB200_OK;
+    if (!c->plans.empty()) return plan_frozen(c, "exact walk workspace", (size_t)c->flood.entry_cap, (size_t)n);
+    CK(flood_workspace_ensure(c->mode, c->flood, n), "cudaMalloc exact walk workspace");
+    return CB200_OK;
+}
+
+int decode_reserve(cb200_ctx* c, uint32_t flags)
+{
+    int rc = ccm_buffers(c); if (rc) return rc;
+    CK(c->d_means.ensure((size_t)c->max_frames * c->mode.num_cells), "cudaMalloc means");
+    CK(c->d_ccm_active.ensure((size_t)c->max_frames), "cudaMalloc ccm flags");
+    CK(c->d_sel.ensure((size_t)c->max_frames * 5), "cudaMalloc selection");
+    CK(c->d_sched.ensure(6), "cudaMalloc selection schedule");
+    const uint16_t* idx;
+    return idx_for(c, flags, &idx);
+}
+
+int carry_from_host(cb200_ctx* c)
+{
+    if (c->plans.empty()) return CB200_OK;
+    float v[10] = {};
+    if (c->ccm_active) memcpy(v, c->ccm, sizeof(c->ccm));
+    reinterpret_cast<uint8_t*>(v + 9)[0] = c->ccm_active ? 1 : 0;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    // from pageable memory: the copy is staged before the call returns
+    CK(cudaMemcpyAsync(c->d_carry, v, sizeof(v), cudaMemcpyHostToDevice, c->stream), "H2D ccm carry");
+    return CB200_OK;
+}
+}  // namespace cb200
+
 int upload_frames(cb200_ctx* c, const uint8_t* rgb, int n)
 {
     const Mode& m = c->mode;
@@ -614,6 +650,7 @@ int cb200_create(cb200_ctx** out, int device, int mode_val, int max_frames)
 int cb200_destroy(cb200_ctx* c)
 {
     if (!c) return CB200_OK;
+    while (!c->plans.empty()) cb200_camera_plan_destroy(c->plans.back());
     cudaSetDevice(c->device);          // the buffers free themselves in `delete c`, on this device
     for (int k = 0; k < cb200_ctx::kEvSets; ++k) for (int i = 0; i < 8; ++i) if (c->ev[k][i]) cudaEventDestroy(c->ev[k][i]);
     for (const auto& s : c->stage) if (s.ev) cudaEventDestroy(s.ev);
@@ -653,6 +690,7 @@ int cb200_decode_raw_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
     rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
     if (!d_rgb || !d_raw_out) return fail(CB200_ERR_ARG, "null buffer");
+    rc = check_frozen_frames(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const uint16_t* idx;
     rc = idx_for(c, flags, &idx); if (rc) return rc;
@@ -691,12 +729,13 @@ int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
     if ((flags & CB200_FLAG_CC_FIT) && (flags & CB200_FLAG_CC_SIMPLE)) return fail(CB200_ERR_ARG, "CC_SIMPLE and CC_FIT are exclusive");
     rc = check_chain_call(c, flags); if (rc) return rc;
     if (n > 0 && (!d_rgb || !d_chunks || !d_chunk_mask)) return fail(CB200_ERR_ARG, "null buffer");
+    rc = check_frozen_frames(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
-    // init_ccm is only reached from Decoder::do_decode (not the legacy coupled layout) and needs a header from the RS stream
-    const bool fit = (flags & CB200_FLAG_CC_FIT) && !m.legacy && m.ecc_bytes > 0 && m.color_bits > 0;
-    bool carried = false;                      // the CCM going into frame 0 is only known on the device
-    if (enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->ccm_pending) {
+    const bool fit = ccm_fits(m, flags);
+    // the CCM going into frame 0 is only known on the device -- always so for a camera plan, whose graph replays later
+    bool carried = enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->capturing;
+    if (enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->ccm_pending && !carried) {
         const cudaError_t q = cudaEventQuery(c->ccm_ev);
         if (q == cudaErrorNotReady) carried = true;
         else if (q != cudaSuccess) return fail_cuda(q, "query ccm");
@@ -787,6 +826,7 @@ int cb200_decode_raw(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, ui
     rc = check_n(c, n); if (rc) return rc;
     if (n == 0) return CB200_OK;
     if (!rgb || !raw_out) return fail(CB200_ERR_ARG, "null buffer");
+    rc = check_frozen_frames(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = upload_frames(c, rgb, n); if (rc) return rc;
     rc = cb200_decode_raw_dev(c, c->d_rgb, n, flags, c->d_raw, nullptr); if (rc) return rc;
@@ -803,6 +843,7 @@ int cb200_decode(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_
     rc = check_chain_call(c, flags); if (rc) return rc;
     if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
     if (!rgb || !data_out) return fail(CB200_ERR_ARG, "null buffer");
+    rc = check_frozen_frames(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = upload_frames(c, rgb, n); if (rc) return rc;
     rc = cb200_decode_chunks_dev(c, c->d_rgb, n, flags, c->d_data, c->d_mask, nullptr); if (rc) return rc;
@@ -824,6 +865,7 @@ int decode_fountain_from_host(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t 
     rc = check_chain_call(c, flags); if (rc) return rc;
     if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
     if (!rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
+    rc = check_frozen_frames(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = upload_frames(c, rgb, n); if (rc) return rc;
     return decode_fountain_to_host(c, c->d_rgb, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
@@ -838,6 +880,7 @@ int cb200::decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, ui
     rc = check_chain_call(c, flags); if (rc) return rc;
     if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
     if (!d_rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
+    rc = check_frozen_frames(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = decode_chunks(c, d_rgb, n, flags, sharpen, c->d_data, c->d_mask, nullptr); if (rc) return rc;
     return fetch_fountain(c, n, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags, nullptr);
@@ -910,6 +953,7 @@ int cb200_decode_cells_means(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t f
     if (n == 0) return CB200_OK;
     if (!rgb || !cellvals_out || !trace_out) return fail(CB200_ERR_ARG, "null buffer");
     static_assert(sizeof(cb200_cell_trace) == sizeof(CellTrace), "trace layout");
+    rc = check_frozen_frames(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = upload_frames(c, rgb, n); if (rc) return rc;
     size_t tb = (size_t)n * c->mode.num_cells * sizeof(CellTrace);
@@ -971,7 +1015,7 @@ int cb200_set_ccm(cb200_ctx* c, const float* m9)
     c->ccm_pending = c->ccm_pending_flag = false;    // an explicit matrix replaces whatever the last batch left
     c->ccm_active = m9 != nullptr;
     if (m9) memcpy(c->ccm, m9, sizeof(c->ccm));
-    return CB200_OK;
+    return carry_from_host(c);
 }
 
 int cb200_get_ccm(cb200_ctx* c, float* m9)
@@ -1020,6 +1064,7 @@ int cb200_fit_ccm(cb200_ctx* c, const uint8_t* rgb, const uint8_t* header6, uint
     c->ccm_active = true;
     memcpy(c->ccm, fitm, sizeof(fitm));
     if (m9_out) memcpy(m9_out, fitm, sizeof(fitm));
+    rc = carry_from_host(c); if (rc) return rc;
     return 1;
 }
 

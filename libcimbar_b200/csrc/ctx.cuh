@@ -99,6 +99,37 @@ int chain_publish_link(cb200_ctx* c, int n, const float* d_fit, const uint8_t* d
 int chain_settle(cb200_ctx* c, float* d_carry);
 // a camera call with no pictures: on a chained CC_FIT call the empty stripe's part of the step, else nothing (scan.cu)
 int camera_empty(cb200_ctx* c, uint32_t flags);
+// camera plans (plan.cu).  Every context buffer a plan's graph uses is grown through grow(): while plans exist a call that needs
+// more fails with CB200_ERR_ARG (plan_frozen) instead.  Called with plans, the *_reserve functions below therefore make no CUDA
+// call, and an entry point runs them first (check_frozen*) so that a frozen buffer refuses the call before any CUDA call
+int plan_frozen(const cb200_ctx* c, const char* buffer, size_t have, size_t need);
+// the camera path's buffers for n pictures of sizes wh: the scan's (scan_reserve), the transforms, the selection, the deskewed
+// frames and the exact walk's (scan.cu, deskew.cu, api.cu)
+int scan_reserve(cb200_ctx* c, const int32_t* wh, int n);
+int camera_reserve(cb200_ctx* c, const int32_t* wh, int n);
+int deskew_reserve(cb200_ctx* c, int n);
+int flood_reserve(cb200_ctx* c, int n);
+// the decode's buffers sized by max_frames, the CCM event and the slot map of these flags (api.cu): no CUDA call after the first time
+int decode_reserve(cb200_ctx* c, uint32_t flags);
+// CB200_ERR_ARG, before any CUDA call, when live plans freeze a buffer this call would grow; nothing without plans (plan.cu).
+// frames: n decoded frames (the exact walk); deskew: n deskewed frames too; camera / scan: n camera pictures of sizes wh
+int check_frozen_frames(cb200_ctx* c, int n);
+int check_frozen_deskew(cb200_ctx* c, int n);
+int check_frozen_camera(cb200_ctx* c, const int32_t* wh, int n);
+int check_frozen_scan(cb200_ctx* c, const int32_t* wh, int n);
+// the CCM a plan's graph starts from is d_carry: with plans, a matrix the host sets (cb200_set_ccm, cb200_fit_ccm, a new plan) is
+// copied there in stream order (api.cu)
+int carry_from_host(cb200_ctx* c);
+// a CC_FIT call in this mode fits matrices (init_ccm needs a header from the RS stream, not the legacy coupled layout) (api.cu)
+bool ccm_fits(const Mode& m, uint32_t flags);
+// the camera path with the picture table given in device memory (a plan's), so nothing is uploaded (scan.cu)
+int camera_enqueue_table(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
+                         uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table);
+// the pictures of the last camera call (cb200_camera_transforms reads that many) (scan.cu)
+int camera_pictures(cb200_ctx* c);
+void set_camera_pictures(cb200_ctx* c, int n);
+// the picture table of that call for n pictures of sizes wh at d_pics, built on the host (scan.cu): PicDesc n, then the order
+int camera_table(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, std::vector<uint8_t>& table);
 }  // namespace cb200
 #define CK(call, what) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cb200::fail_cuda(e__, what); } while (0)
 
@@ -167,7 +198,20 @@ struct cb200_ctx {
     cb200::ScanScratch* scan = nullptr;     // anchor-scan scratch (scan.cu)
     cb200::JpegState* jpeg = nullptr;       // JPEG decode scratch (jpeg.cu)
     cb200::PngState* png = nullptr;         // PNG decode scratch (png.cu)
+    std::vector<cb200_camera_plan*> plans;  // live camera plans (plan.cu): they freeze the buffers their graphs use
+    bool capturing = false;                 // a plan's capture is in progress: the CCM always comes from d_carry
 };
+
+namespace cb200 {
+template <typename B> int grow(cb200_ctx* c, B& b, size_t count, const char* buffer)
+{
+    if (count <= b.capacity()) return CB200_OK;
+    if (!c->plans.empty()) return plan_frozen(c, buffer, b.capacity(), count);
+    const cudaError_t e = b.ensure(count);
+    if (e != cudaSuccess) return fail_cuda(e, (std::string("cudaMalloc ") + buffer).c_str());
+    return CB200_OK;
+}
+}  // namespace cb200
 
 namespace cb200 {
 // cb200_set_timing: begin_timed_call starts the event set of a pipeline call, mark records its next event on the call's stream

@@ -151,11 +151,12 @@ static int stage_sources(cb200_ctx* c, const uint8_t* src, int w, int h, int n)
 // room for n deskewed frames in the output buffer
 static int ensure_frames(cb200_ctx* c, int n)
 {
-    CK(dstate(c)->d_dst.ensure((size_t)n * c->mode.width * c->mode.height * 3), "cudaMalloc deskew output");
-    return CB200_OK;
+    return grow(c, dstate(c)->d_dst, (size_t)n * c->mode.width * c->mode.height * 3, "deskew output");
 }
 
 }  // namespace cb200
+
+int cb200::deskew_reserve(cb200_ctx* c, int n) { return ensure_frames(c, n); }
 
 int cb200::deskew_frames(cb200_ctx* c, int n, uint8_t** frames)
 {
@@ -234,6 +235,7 @@ int cb200_deskew_dev(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, i
 {
     if (!c || !d_src || !m9 || !d_dst || n < 0 || src_w < 2 || src_h < 2) return fail(CB200_ERR_ARG, "bad arguments");
     if ((size_t)src_w * (size_t)src_h * 3 >= ((size_t)1 << 32)) return fail(CB200_ERR_ARG, "source picture of 4 GB or more");
+    int rc = check_frozen_deskew(c, n); if (rc) return rc;
     return deskew_run(c, d_src, uniform_sizes(src_w, src_h, n).data(), n, m9, d_dst);
 }
 
@@ -241,8 +243,9 @@ int cb200_deskew(cb200_ctx* c, const uint8_t* src, int src_w, int src_h, int n, 
 {
     if (!c || !src || !dst || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
     if (n == 0) return CB200_OK;
+    int rc = check_frozen_deskew(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
-    int rc = stage_sources(c, src, src_w, src_h, n); if (rc) return rc;
+    rc = stage_sources(c, src, src_w, src_h, n); if (rc) return rc;
     rc = ensure_frames(c, n); if (rc) return rc;
     const DeskewState* d = c->deskew;
     rc = cb200_deskew_dev(c, d->d_src, src_w, src_h, n, m9, d->d_dst); if (rc) return rc;
@@ -267,15 +270,16 @@ int cb200::extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, const int3
 {
     if (!c || !d_src || !corners || !chunks_out || !chunk_count || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
     if (n == 0) return CB200_OK;
+    int rc = check_frozen_deskew(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
     float outp[8];
     extract::output_points(m.width, m.height, outp);
     std::vector<double> m9((size_t)n * 9);
     for (int f = 0; f < n; ++f) {
-        int rc = cb200_perspective_transform(corners + (size_t)f * 8, outp, m9.data() + (size_t)f * 9); if (rc) return rc;
+        rc = cb200_perspective_transform(corners + (size_t)f * 8, outp, m9.data() + (size_t)f * 9); if (rc) return rc;
     }
-    int rc = ensure_frames(c, n); if (rc) return rc;
+    rc = ensure_frames(c, n); if (rc) return rc;
     rc = deskew_run(c, d_src, wh, n, m9.data(), c->deskew->d_dst); if (rc) return rc;
     // the deskewed frames never leave the device: straight into the decode
     return decode_fountain_to_host(c, c->deskew->d_dst, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
@@ -326,6 +330,7 @@ int cb200_extract_decode_fountain(cb200_ctx* c, const uint8_t* src, int src_w, i
     int rc = check_camera_flags(flags); if (rc) return rc;
     if (!c || !src || !corners || !chunks_out || !chunk_count || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
     if (n == 0) return CB200_OK;
+    rc = check_frozen_deskew(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = stage_sources(c, src, src_w, src_h, n); if (rc) return rc;
     return cb200_extract_decode_fountain_dev(c, c->deskew->d_src, src_w, src_h, n, corners, flags, chunks_out, chunk_count, chunk_mask, frame_flags);

@@ -951,8 +951,14 @@ cudaError_t flood_workspace_create(const Mode& m, int sm_count, const uint16_t* 
     return cudaSuccess;
 }
 
+bool flood_workspace_fits(const FloodWorkspace& ws, int n_frames)
+{
+    const int want = n_frames < ws.max_entries ? n_frames : ws.max_entries;
+    return ws.list.capacity() >= (size_t)n_frames && ws.counters.capacity() >= 2 + ws.list.capacity() && want <= ws.entry_cap;
+}
+
 // grows the per-batch buffers (cudaFree synchronises, so no kernel still reads the old ones)
-static cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int n_frames)
+cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int n_frames)
 {
     cudaError_t e;
     const size_t rw = raster_words16(m.width, m.height);

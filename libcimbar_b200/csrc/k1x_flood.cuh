@@ -35,6 +35,9 @@ struct FloodWorkspace {
 cudaError_t flood_init_tables(const float* adjust256, const unsigned long long* tiles_L16, uint32_t hash_mul);
 // adj_host: [num_cells][4] = AdjacentCellFinder::find for every cell (built by the caller from the cell geometry)
 cudaError_t flood_workspace_create(const Mode& m, int sm_count, const uint16_t* adj_host, FloodWorkspace* ws);
+// the per-batch buffers for n_frames frames (flood_launch grows them itself; fits: no growth needed)
+cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int n_frames);
+bool flood_workspace_fits(const FloodWorkspace& ws, int n_frames);
 // writes d_flags[f] for every frame: 0 = K1 result stands, CB200_FRAME_FALLBACK = re-decoded here,
 // CB200_FRAME_INEXACT = needed but skipped (no_fallback).  d_sharpen_of: NULL = every frame is preprocessed as `sharpen` says;
 // else one byte per frame of the batch (device memory, nonzero = sharpen) and `sharpen` is ignored

@@ -283,6 +283,7 @@ int cb200_png_scan_extract_decode_chunks_dev(cb200_ctx* c, const uint8_t* const*
     rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
     rc = check_chain_call(c, flags); if (rc) return rc;
     if (n == 0) return camera_empty(c, flags);
+    rc = check_frozen_camera(c, wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     PngState* s = pstate(c);
     uint64_t rgb = 0;

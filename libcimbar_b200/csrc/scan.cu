@@ -282,75 +282,116 @@ std::vector<int32_t> uniform_sizes(int w, int h, int n)
     return wh;
 }
 
-// blurred pictures + thresholds + anchors for n pictures of sizes wh (checked by check_picture_sizes) packed in device memory, in
-// the state's device arrays; enqueued only.  The picture table (PicDesc, in s->d_table) is this call's one upload
-static int scan_enqueue(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n)
+// rows of a scan pass for one picture: the primary pass scans h / skip rows, the bottom-right window at most 2 h / skip (half the step)
+static int scan_rows(int w, int h)
+{
+    const int skip = (w < h ? w : h) / 60;
+    return 2 * ((h + skip - 1) / skip) + 4;
+}
+
+int scan_reserve(cb200_ctx* c, const int32_t* wh, int n)
 {
     ScanScratch* s = sstate(c);
-    cudaStream_t st = c->stream;
     size_t npx = 0;
     int rows_cap = 0;
     for (int i = 0; i < n; ++i) {
-        const int w = wh[2 * i], h = wh[2 * i + 1], skip = (w < h ? w : h) / 60;
-        npx += (size_t)w * (size_t)h;
-        // rows of a pass: the primary pass scans h / skip rows, the bottom-right window at most 2 h / skip (half the step)
-        const int rc = 2 * ((h + skip - 1) / skip) + 4;
+        npx += (size_t)wh[2 * i] * (size_t)wh[2 * i + 1];
+        const int rc = scan_rows(wh[2 * i], wh[2 * i + 1]);
         if (rc > rows_cap) rows_cap = rc;
     }
-    CK(s->d_blur.ensure(npx), "cudaMalloc blurred pictures");
-    const size_t table_bytes = (sizeof(PicDesc) + sizeof(int)) * (size_t)n;
-    CK(s->d_hist.ensure(256 * (size_t)n), "cudaMalloc histograms");
-    CK(s->d_thr.ensure((size_t)n), "cudaMalloc thresholds");
-    CK(s->d_anchors.ensure(4 * (size_t)n), "cudaMalloc anchors");
-    CK(s->d_count.ensure((size_t)n), "cudaMalloc counts");
-    CK(s->d_cutoff.ensure((size_t)n), "cudaMalloc cutoffs");
-    CK(s->d_status.ensure((size_t)n), "cudaMalloc status");
-    CK(s->d_table.ensure(table_bytes), "cudaMalloc picture table");
-    CK(s->h_anchors.ensure(4 * (size_t)n), "cudaMallocHost anchors");
-    CK(s->h_count.ensure(3 * (size_t)n), "cudaMallocHost counts");
-    // the per-picture scan lists: k_scan_anchors strides them by the largest row count seen so far
-    if (n > s->ws_pics) s->ws_pics = n;
-    if (rows_cap > s->ws_rows_cap) s->ws_rows_cap = rows_cap;
-    const size_t np = (size_t)s->ws_pics, rows = (size_t)s->ws_rows_cap;
-    CK(s->d_rowbuf.ensure(np * rows * kRowCap), "cudaMalloc scan rows");
-    CK(s->d_rowcnt.ensure(np * rows), "cudaMalloc scan row counts");
-    CK(s->d_pts.ensure(np * kPtsCap), "cudaMalloc scan points");
-    CK(s->d_res.ensure(np * kPtsCap * kResCap), "cudaMalloc scan results");
-    CK(s->d_nres.ensure(np * kPtsCap), "cudaMalloc scan result counts");
-    // the descriptor table (batch order), then the pictures grouped by blur radius (batch order inside a group); the tiles of one
-    // radius are numbered across its pictures
-    int slot;
-    uint8_t* h_table;
-    int err = stage_take(c, table_bytes, &slot, &h_table); if (err) return err;
-    PicDesc* desc = reinterpret_cast<PicDesc*>(h_table);
-    int* order = reinterpret_cast<int*>(desc + n);
-    int first[5] = {}, count[5] = {};
+    int rc;
+    if ((rc = grow(c, s->d_blur, npx, "blurred pictures")) || (rc = grow(c, s->d_hist, 256 * (size_t)n, "histograms")) ||
+        (rc = grow(c, s->d_thr, (size_t)n, "thresholds")) || (rc = grow(c, s->d_anchors, 4 * (size_t)n, "anchors")) ||
+        (rc = grow(c, s->d_count, (size_t)n, "counts")) || (rc = grow(c, s->d_cutoff, (size_t)n, "cutoffs")) ||
+        (rc = grow(c, s->d_status, (size_t)n, "status")))
+        return rc;
+    // the per-picture scan lists: k_scan_anchors strides them by the largest row count seen so far (raised once they fit)
+    const size_t np = (size_t)(n > s->ws_pics ? n : s->ws_pics), rows = (size_t)(rows_cap > s->ws_rows_cap ? rows_cap : s->ws_rows_cap);
+    if ((rc = grow(c, s->d_rowbuf, np * rows * kRowCap, "scan rows")) || (rc = grow(c, s->d_rowcnt, np * rows, "scan row counts")) ||
+        (rc = grow(c, s->d_pts, np * kPtsCap, "scan points")) || (rc = grow(c, s->d_res, np * kPtsCap * kResCap, "scan results")) ||
+        (rc = grow(c, s->d_nres, np * kPtsCap, "scan result counts")))
+        return rc;
+    s->ws_pics = (int)np; s->ws_rows_cap = (int)rows;
+    return CB200_OK;
+}
+
+// the launch geometry of the blur: per radius its pictures, their first entry in the order list, their tiles, one size or not
+struct BlurGroups {
+    int count[5] = {}, group0[5] = {};
     long long tiles[5] = {};
     bool same[5] = {true, true, true, true, true};
+};
+
+// the descriptor table (batch order), then the pictures grouped by blur radius (batch order inside a group) into `table`; the tiles
+// of one radius are numbered across its pictures.  The word path depends on where d_pics and the scan's blurred buffer are
+static int pic_table(const ScanScratch* s, const uint8_t* d_pics, const int32_t* wh, int n, uint8_t* table, BlurGroups& g)
+{
+    PicDesc* desc = reinterpret_cast<PicDesc*>(table);
+    int* order = reinterpret_cast<int*>(desc + n);
+    int first[5] = {};
     for (int i = 0; i < n; ++i) {
         const int R = scan_blur_radius(wh[2 * i], wh[2 * i + 1]);
-        if (!count[R]) first[R] = i;
-        else same[R] = same[R] && wh[2 * i] == wh[2 * first[R]] && wh[2 * i + 1] == wh[2 * first[R] + 1];
-        ++count[R];
+        if (!g.count[R]) first[R] = i;
+        else g.same[R] = g.same[R] && wh[2 * i] == wh[2 * first[R]] && wh[2 * i + 1] == wh[2 * first[R] + 1];
+        ++g.count[R];
     }
     size_t off = 0;
     int next[5] = {};
-    for (int R = 1, at = 0; R <= 4; ++R) { next[R] = at; at += count[R]; }
-    int group0[5] = {};
-    for (int R = 1; R <= 4; ++R) group0[R] = next[R];
+    for (int R = 1, at = 0; R <= 4; ++R) { next[R] = at; at += g.count[R]; }
+    for (int R = 1; R <= 4; ++R) g.group0[R] = next[R];
     for (int i = 0; i < n; ++i) {
         const int w = wh[2 * i], h = wh[2 * i + 1], R = scan_blur_radius(w, h);
         PicDesc& d = desc[i];
         d.src = 3 * off; d.blur = off; d.w = w; d.h = h;
         d.words = (w % 4 == 0) && (reinterpret_cast<uintptr_t>(d_pics + d.src) % 4 == 0) && (reinterpret_cast<uintptr_t>(s->d_blur + d.blur) % 4 == 0);
-        d.tile0 = (int)tiles[R];
-        tiles[R] += (long long)((w + kBlurTW - 1) / kBlurTW) * ((h + kBlurTH - 1) / kBlurTH);
-        if (tiles[R] > 0x7FFFFFFFll) return fail(CB200_ERR_ARG, "more than 2^31 blur tiles in one batch");
+        d.tile0 = (int)g.tiles[R];
+        g.tiles[R] += (long long)((w + kBlurTW - 1) / kBlurTW) * ((h + kBlurTH - 1) / kBlurTH);
+        if (g.tiles[R] > 0x7FFFFFFFll) return fail(CB200_ERR_ARG, "more than 2^31 blur tiles in one batch");
         order[next[R]++] = i;
         off += (size_t)w * (size_t)h;
     }
-    err = stage_send(c, slot, s->d_table, table_bytes, "H2D picture table"); if (err) return err;
-    const PicDesc* d_desc = reinterpret_cast<const PicDesc*>(s->d_table.get());
+    return CB200_OK;
+}
+
+int camera_pictures(cb200_ctx* c) { return sstate(c)->camera_n; }
+void set_camera_pictures(cb200_ctx* c, int n) { sstate(c)->camera_n = n; }
+
+int camera_table(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, std::vector<uint8_t>& table)
+{
+    table.assign((sizeof(PicDesc) + sizeof(int)) * (size_t)n, 0);
+    BlurGroups g;
+    return pic_table(sstate(c), d_pics, wh, n, table.data(), g);
+}
+
+// blurred pictures + thresholds + anchors for n pictures of sizes wh (checked by check_picture_sizes) packed in device memory, in
+// the state's device arrays; enqueued only.  The picture table (PicDesc, in s->d_table) is this call's one upload -- unless
+// d_table holds it already (a camera plan's): then *d_desc = d_table and nothing is uploaded
+static int scan_enqueue(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, const PicDesc* d_table = nullptr,
+                        const PicDesc** d_desc_out = nullptr)
+{
+    ScanScratch* s = sstate(c);
+    cudaStream_t st = c->stream;
+    int err = scan_reserve(c, wh, n); if (err) return err;
+    const size_t table_bytes = (sizeof(PicDesc) + sizeof(int)) * (size_t)n;
+    BlurGroups g;
+    const PicDesc* d_desc = d_table;
+    if (d_table) {
+        std::vector<uint8_t> table(table_bytes);
+        err = pic_table(s, d_pics, wh, n, table.data(), g); if (err) return err;
+    } else {
+        CK(s->d_table.ensure(table_bytes), "cudaMalloc picture table");
+        int slot;
+        uint8_t* h_table;
+        err = stage_take(c, table_bytes, &slot, &h_table); if (err) return err;
+        err = pic_table(s, d_pics, wh, n, h_table, g); if (err) return err;
+        err = stage_send(c, slot, s->d_table, table_bytes, "H2D picture table"); if (err) return err;
+        d_desc = reinterpret_cast<const PicDesc*>(s->d_table.get());
+    }
+    if (d_desc_out) *d_desc_out = d_desc;
+    const int* count = g.count;
+    const int* group0 = g.group0;
+    const long long* tiles = g.tiles;
+    const bool* same = g.same;
     const int* d_order = reinterpret_cast<const int*>(d_desc + n);
     CK(cudaMemsetAsync(s->d_hist, 0, sizeof(unsigned) * 256 * (size_t)n, st), "memset histograms");
     // cb200_set_timing: one event set per scan -- [blur + histogram (all radii), Otsu, anchors] through cb200_get_timing
@@ -385,6 +426,8 @@ static int scan_run(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int 
     int rc = scan_enqueue(c, d_pics, wh, n); if (rc) return rc;
     ScanScratch* s = c->scan;
     cudaStream_t st = c->stream;
+    CK(s->h_anchors.ensure(4 * (size_t)n), "cudaMallocHost anchors");
+    CK(s->h_count.ensure(3 * (size_t)n), "cudaMallocHost counts");
     CK(cudaMemcpyAsync(s->h_anchors, s->d_anchors, sizeof(int4) * 4 * (size_t)n, cudaMemcpyDeviceToHost, st), "D2H anchors");
     CK(cudaMemcpyAsync(s->h_count, s->d_count, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st), "D2H counts");
     CK(cudaMemcpyAsync(s->h_count + n, s->d_cutoff, sizeof(unsigned) * (size_t)n, cudaMemcpyDeviceToHost, st), "D2H cutoffs");
@@ -456,6 +499,22 @@ __global__ void k_mask_failed(const int32_t* __restrict__ status, int n, uint32_
 int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
                    uint8_t* d_frame_flags, int32_t* d_status)
 {
+    return camera_enqueue_table(c, d, wh, n, flags, d_chunks, d_mask, d_frame_flags, d_status, nullptr);
+}
+
+int camera_reserve(cb200_ctx* c, const int32_t* wh, int n)
+{
+    ScanScratch* s = sstate(c);
+    int rc;
+    if ((rc = grow(c, s->d_minv, 9 * (size_t)n, "inverse maps")) || (rc = grow(c, s->d_fwd, 9 * (size_t)n, "transforms")) ||
+        (rc = grow(c, c->d_sel, (size_t)c->max_frames * 5, "selection")) || (rc = deskew_reserve(c, n)) || (rc = scan_reserve(c, wh, n)))
+        return rc;
+    return flood_reserve(c, n);
+}
+
+int camera_enqueue_table(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
+                         uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table)
+{
     const Mode& m = c->mode;
     size_t src_bytes = 0;
     for (int i = 0; i < n; ++i) {
@@ -464,19 +523,18 @@ int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uin
         src_bytes += b;
     }
     ScanScratch* s = sstate(c);
-    CK(s->d_minv.ensure(9 * (size_t)n), "cudaMalloc inverse maps");
-    CK(s->d_fwd.ensure(9 * (size_t)n), "cudaMalloc transforms");
-    CK(c->d_sel.ensure((size_t)c->max_frames * 5), "cudaMalloc selection");
+    int rc = camera_reserve(c, wh, n); if (rc) return rc;
     uint8_t* frames;
-    int rc = deskew_frames(c, n, &frames); if (rc) return rc;
-    rc = scan_enqueue(c, d, wh, n); if (rc) return rc;
+    rc = deskew_frames(c, n, &frames); if (rc) return rc;
+    const PicDesc* d_desc;
+    rc = scan_enqueue(c, d, wh, n, d_table, &d_desc); if (rc) return rc;
     const bool if_needed = (flags & CB200_FLAG_SHARPEN_IF_NEEDED) != 0;
     uint8_t* d_sharp = if_needed ? c->d_sel + 4 * (size_t)n : nullptr;
     k_extract<<<(n + 127) / 128, 128, 0, c->stream>>>(s->d_anchors, s->d_count, s->d_status, n, m.width, m.height, d_status, s->d_minv, s->d_fwd, d_sharp);
     count_launch();
     CK(cudaGetLastError(), "extract launch");
     s->camera_n = n;
-    rc = deskew_launch(c, d, src_bytes, s->d_minv, reinterpret_cast<const PicDesc*>(s->d_table.get()), n, frames); if (rc) return rc;
+    rc = deskew_launch(c, d, src_bytes, s->d_minv, d_desc, n, frames); if (rc) return rc;
     rc = decode_chunks_enqueue(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, d_sharp, d_chunks, d_mask, d_frame_flags); if (rc) return rc;
     k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
     count_launch();
@@ -532,7 +590,8 @@ static int check_camera_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32
     int rc = check_camera_dev_flags(flags); if (rc) return rc;
     rc = check_ragged(wh, d_pictures, n); if (rc) return rc;
     rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
-    return check_chain_call(c, flags);
+    rc = check_chain_call(c, flags); if (rc) return rc;
+    return check_frozen_camera(c, wh, n);
 }
 
 int camera_empty(cb200_ctx* c, uint32_t flags)
@@ -553,6 +612,7 @@ int cb200_scan_dev(cb200_ctx* c, const uint8_t* d_pictures, int w, int h, int n,
     if (n == 0) return CB200_OK;
     const std::vector<int32_t> wh = uniform_sizes(w, h, n);
     int rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
+    rc = check_frozen_scan(c, wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = scan_run(c, d_pictures, wh.data(), n); if (rc) return rc;
     return scan_results(c, n, anchors, count, cutoff);
@@ -564,6 +624,7 @@ int cb200_scan(cb200_ctx* c, const uint8_t* pictures, int w, int h, int n, int32
     if (n == 0) return CB200_OK;
     const std::vector<int32_t> wh = uniform_sizes(w, h, n);
     int rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
+    rc = check_frozen_scan(c, wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const uint8_t* d = nullptr;
     rc = stage_pictures(c, uniform_pointers(pictures, w, h, n).data(), wh.data(), n, &d); if (rc) return rc;
@@ -576,6 +637,7 @@ int cb200_scan_ragged_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32_t
     int rc = check_ragged(wh, d_pictures, n); if (rc) return rc;
     if (!c || !count) return fail(CB200_ERR_ARG, !c ? "null context" : "null count");
     if (n == 0) return CB200_OK;
+    rc = check_frozen_scan(c, wh, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = scan_run(c, d_pictures, wh, n); if (rc) return rc;
     return scan_results(c, n, anchors, count, cutoff);
@@ -587,6 +649,7 @@ int cb200_scan_ragged(cb200_ctx* c, const uint8_t* const* pictures, const int32_
     rc = check_host_pictures(pictures, n); if (rc) return rc;
     if (!c || !count) return fail(CB200_ERR_ARG, !c ? "null context" : "null count");
     if (n == 0) return CB200_OK;
+    rc = check_frozen_scan(c, wh, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const uint8_t* d = nullptr;
     rc = stage_pictures(c, pictures, wh, n, &d); if (rc) return rc;
@@ -631,6 +694,7 @@ int cb200_scan_extract_decode_fountain(cb200_ctx* c, const uint8_t* pictures, in
     if (n == 0) return camera_empty(c, flags);
     const std::vector<int32_t> wh = uniform_sizes(w, h, n);
     rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
+    rc = check_frozen_camera(c, wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const uint8_t* d = nullptr;
     rc = stage_pictures(c, uniform_pointers(pictures, w, h, n).data(), wh.data(), n, &d); if (rc) return rc;
@@ -649,6 +713,7 @@ int cb200_scan_extract_decode_fountain_ragged(cb200_ctx* c, const uint8_t* const
     if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
     rc = check_chain_call(c, flags); if (rc) return rc;
     if (n == 0) return camera_empty(c, flags);
+    rc = check_frozen_camera(c, wh, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const uint8_t* d = nullptr;
     rc = stage_pictures(c, pictures, wh, n, &d); if (rc) return rc;
