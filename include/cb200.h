@@ -295,6 +295,33 @@ int cb200_camera_plan_launch(cb200_camera_plan* plan);
 /* the plan's cudaGraph_t, owned by the plan (for cudaGraphAddChildGraphNode, which copies it) */
 int cb200_camera_plan_graph(cb200_camera_plan* plan, void** cuda_graph);
 int cb200_camera_plan_destroy(cb200_camera_plan* plan);
+/* ---- auto mode: the sender's mode detected by decoding ----------------------------------------------------------------------
+
+   The receiver's auto mode (the reference's web receiver tries 66, 68, 67 and 4 and keeps the first mode under which a frame gives
+   a chunk): the camera path of cb200_scan_extract_decode_chunks_ragged_dev under several candidate modes in one enqueue-only call.
+     ctxs, n_modes: 1 .. 5 contexts the caller created, one per mode, in priority order.  Each keeps its own CCM
+                 (cb200_get_ccm / cb200_set_ccm / cb200_get_frame_ccms work on it as before).
+     d_pictures, wh, n, flags: as on cb200_scan_extract_decode_chunks_ragged_dev; the call runs on the contexts' stream.
+     d_mode:     n int32: the index into ctxs of the first context whose decode of picture i accepted a chunk (mask != 0), or -1 when
+                 no mode did (a picture that fails extraction included).
+     d_chunks:   n fixed slots of the largest data_bytes of the set (8750 with mode 8, 7500 with 68 or 4): slot i holds picture
+                 i's record under its detected mode in that mode's fixed-slot layout, zeros after it and in the whole slot for -1.
+     d_chunk_mask: that mode's mask (0 for -1); d_extract_status: the extract status under the detected mode, under ctxs[0] for -1.
+     d_mode_masks: NULL, or n x n_modes uint32: every mode's mask of every picture (picture-major).
+   Exactness: every context is left where cb200_scan_extract_decode_chunks_ragged_dev on it with these pictures and flags would
+   leave it -- records, masks, statuses, transforms, CCM carry (a wrong-mode decode moves that mode's CCM as a direct call would).
+   The output only selects among those results.
+   Sharing: the anchor scan runs once (on ctxs[0]'s scratch); each frame geometry (68 / 4 / 8: 1024 x 1024; 67; 66) is deskewed and
+   walked once, on the group's first context, and the other modes of the geometry colour that walk's positions with their own
+   palette and CCM.  K1, colours, RS and the masks run per mode.  With more than one geometry the geometries run on side streams
+   forked from the contexts' stream and joined back into it before the selection, so their walks overlap on the device.
+   CB200_ERR_ARG before any CUDA call, naming the violation: n_modes outside 1 .. 5, a null context, two contexts of one mode, contexts
+   on different devices or streams, a context attached to a CCM chain or with live camera plans, n above a context's max_frames, a
+   null output other than d_mode_masks, and the flag and picture checks of cb200_scan_extract_decode_chunks_ragged_dev.  Waits for
+   the device as that call does (a buffer that grows, the upload ring of ctxs[0]).  Not capturable in a camera plan. */
+int cb200_detect_scan_extract_decode_chunks_dev(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d_pictures, const int32_t* wh, int n,
+                                                uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
+                                                int32_t* d_mode, uint32_t* d_mode_masks);
 /* ---- JPEG files in: the CLI's input, decoded on the device ---------------------------------------------------------------
 
    Replaces: cv::imread(file) + cv::cvtColor(BGR2RGB) (src/exe/cimbar/cimbar.cpp:132-133) for a batch of JPEG files in host memory:

@@ -40,6 +40,7 @@ EXPORTS = [
     "cb200_ccm_chain_root_create", "cb200_ccm_chain_peer_open", "cb200_ccm_chain_attach", "cb200_ccm_chain_step", "cb200_ccm_chain_status",
     "cb200_ccm_chain_link_ms", "cb200_get_frame_ccms",
     "cb200_camera_plan_create", "cb200_camera_plan_launch", "cb200_camera_plan_graph", "cb200_camera_plan_destroy",
+    "cb200_detect_scan_extract_decode_chunks_dev",
 ]
 
 
@@ -157,6 +158,7 @@ def load_library():
     lib.cb200_camera_plan_launch.argtypes = [vp]
     lib.cb200_camera_plan_graph.argtypes = [vp, C.POINTER(C.c_void_p)]
     lib.cb200_camera_plan_destroy.argtypes = [vp]
+    lib.cb200_detect_scan_extract_decode_chunks_dev.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -201,6 +203,19 @@ def interleave_indices(mode_val=68):
     idx = np.zeros(info.total_cells, dtype=np.uint16)
     _check(load_library().cb200_interleave_indices(mode_val, idx.ctypes.data))
     return idx
+
+
+def detect_scan_extract_decode_chunks_dev(ctxs, d_pictures, wh, d_chunks, d_mask, d_status, d_mode, d_mode_masks=None, flags=0):
+    """The receiver's auto mode, enqueue-only: Context.scan_extract_decode_chunks_dev of one ragged batch under every context of
+    `ctxs` (one per candidate mode, in priority order, all on one device and stream), with the scan done once and one exact walk per
+    frame geometry.  d_mode: n int32, the index into ctxs of the first mode whose decode of the picture gave a chunk, or -1;
+    d_chunks: n slots of the largest data_bytes of the set with that mode's record; d_mask / d_status: that mode's mask and extract
+    status (ctxs[0]'s status for -1); d_mode_masks (optional): n x len(ctxs) uint32, every mode's mask.  Each context is left as a
+    direct scan_extract_decode_chunks_dev on it would leave it (CCM carry included)"""
+    wh = np.ascontiguousarray(wh, dtype=np.int32).reshape(-1, 2)
+    hs = (C.c_void_p * max(len(ctxs), 1))(*[c._h.value for c in ctxs])
+    _check(load_library().cb200_detect_scan_extract_decode_chunks_dev(hs, len(ctxs), d_pictures, wh.ctypes.data, wh.shape[0], flags,
+                                                                      d_chunks, d_mask, d_status, d_mode, d_mode_masks))
 
 
 def _hptr(a):

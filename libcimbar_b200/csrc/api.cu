@@ -458,8 +458,15 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const u
     }
     mark(c);                                   // ev1: after K1
     // frames K1 flagged (or all of them when exact_only) are re-done by the exact walk on the same preprocessing (sharpen or not)
-    CK(flood_launch(m, c->flood, d_rgb, n, (flags & CB200_FLAG_NO_FALLBACK) != 0, exact_only, sharpen, d_sharp,
-                    c->d_cellvals, c->d_dirty, c->d_flags, d_trace, cc, st), "flood launch");
+    const SharedWalk* sw = c->shared_walk;
+    if (sw && sw->lead != c) {                 // a detect call: this geometry's walk has run on the lead context (detect.cu)
+        CK(cudaMemcpyAsync(c->d_flags, sw->lead->d_flags, (size_t)n, cudaMemcpyDeviceToDevice, st), "copy frame flags");
+        if (!(flags & CB200_FLAG_NO_FALLBACK))
+            CK(flood_colour_launch(m, sw->lead->flood, d_rgb, n, sw->kept, c->d_cellvals, cc, st), "flood colour launch");
+    } else {
+        CK(flood_launch(m, c->flood, d_rgb, n, (flags & CB200_FLAG_NO_FALLBACK) != 0, exact_only, sharpen, d_sharp,
+                        c->d_cellvals, c->d_dirty, c->d_flags, d_trace, cc, st, sw ? sw->kept : nullptr), "flood launch");
+    }
     mark(c);                                   // ev2: after K1x
     return CB200_OK;
 }
@@ -657,6 +664,7 @@ int cb200_destroy(cb200_ctx* c)
     if (c->ccm_ev) cudaEventDestroy(c->ccm_ev);
     gather_destroy(c->gather);
     chain_destroy(c->chain);
+    detect_destroy(c->detect);
     deskew_destroy(c->deskew); scan_destroy(c->scan); jpeg_destroy(c->jpeg); png_destroy(c->png);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     delete c;

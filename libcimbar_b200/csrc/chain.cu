@@ -176,6 +176,8 @@ void chain_destroy(ChainState* s)
     delete s;
 }
 
+bool chain_attached(const cb200_ctx* c) { return c && c->chain && c->chain->attached; }
+
 bool chain_linked(const cb200_ctx* c, uint32_t flags)
 {
     return c && c->chain && c->chain->attached && (flags & CB200_FLAG_CC_FIT);

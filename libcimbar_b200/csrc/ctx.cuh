@@ -18,8 +18,15 @@ struct ScanScratch;      // scan.cu
 struct JpegState;        // jpeg.cu
 struct PngState;         // png.cu
 struct ChainState;       // chain.cu
+struct DetectState;      // detect.cu
 void gather_destroy(GatherState* g);
 void chain_destroy(ChainState* s);
+void detect_destroy(DetectState* d);
+// the exact walk of a detect call (detect.cu), shared by the modes of one frame geometry: `lead` walks (flood_launch, the walk's
+// records kept in `kept`), every other context of the geometry takes its frame flags and colours that walk's positions in its own
+// palette and CCM (flood_colour_launch).  The walk reads only the geometry, the frames and their sharpen bytes, and K1's dirty
+// flag is a symbol decision, so each mode's cells equal what its own walk would give
+struct SharedWalk { cb200_ctx* lead; uint32_t* kept; };
 void deskew_destroy(DeskewState* d);     // delete: its buffers free themselves
 void scan_destroy(ScanScratch* s);       // likewise
 void jpeg_destroy(JpegState* j);         // likewise
@@ -130,6 +137,18 @@ int camera_pictures(cb200_ctx* c);
 void set_camera_pictures(cb200_ctx* c, int n);
 // the picture table of that call for n pictures of sizes wh at d_pics, built on the host (scan.cu): PicDesc n, then the order
 int camera_table(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, std::vector<uint8_t>& table);
+// the stages of the camera path, for the detect call (scan.cu).  camera_source_bytes: the packed batch's size, CB200_ERR_ARG for a
+// picture of 4 GB or more (no CUDA call).  camera_reserve_for: camera_reserve without the scan's buffers (scans = false) or the
+// deskewed frames' and the walk's (walks = false).  camera_scan: the scan of n pictures on this context's scratch, *d_desc = its
+// picture table.  camera_after_scan: k_extract on `scanned`'s anchors into this context's transforms and d_status, the deskew into
+// `frames` (deskew = false: `frames` holds them already, deskewed for this geometry), the decode and the failed pictures' masks
+int camera_source_bytes(const int32_t* wh, int n, size_t* bytes);
+int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks);
+int camera_scan(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, const PicDesc* d_table, const PicDesc** d_desc);
+int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const uint8_t* d, size_t src_bytes, const PicDesc* d_desc, int n, uint32_t flags,
+                      uint8_t* frames, bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status);
+// the context is attached to a CCM chain (chain.cu)
+bool chain_attached(const cb200_ctx* c);
 }  // namespace cb200
 #define CK(call, what) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cb200::fail_cuda(e__, what); } while (0)
 
@@ -194,6 +213,8 @@ struct cb200_ctx {
     cudaEvent_t ccm_ev = nullptr;    // recorded after the D2H copies of the last batch's CCM (ccm_resolve waits on it)
     cb200::GatherState* gather = nullptr;   // multi-GPU chunk-record window (gather.cu)
     cb200::ChainState* chain = nullptr;     // multi-GPU CC_FIT chain (chain.cu)
+    cb200::DetectState* detect = nullptr;   // side streams and buffers of detect calls led by this context (detect.cu)
+    const cb200::SharedWalk* shared_walk = nullptr;   // set only while a detect call decodes this context's mode
     cb200::DeskewState* deskew = nullptr;   // extractor scratch (deskew.cu)
     cb200::ScanScratch* scan = nullptr;     // anchor-scan scratch (scan.cu)
     cb200::JpegState* jpeg = nullptr;       // JPEG decode scratch (jpeg.cu)

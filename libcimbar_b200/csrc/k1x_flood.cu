@@ -982,7 +982,7 @@ cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int n_fram
 
 cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb, int n_frames, bool no_fallback,
                          bool force_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
-                         uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st)
+                         uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st, uint32_t* keep)
 {
     if (n_frames <= 0) return cudaSuccess;
     cudaError_t e = flood_workspace_ensure(m, ws, n_frames);
@@ -1000,14 +1000,33 @@ cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb
         if (d_sharpen_of || sharpen) { k_flood_raster_fast_sharpen<<<rgrid, kFastThreads, 0, st>>>(m, d_rgb, ws.list, ws.counters, base, cap, d_sharpen_of, ws.raster); count_launch(); }
         int wgrid = cap < ws.slots ? cap : ws.slots;
         const bool few = cap <= ws.few_frames;              // at most one wave of big-heap walks: latency over occupancy
+        uint32_t* result = keep ? keep + (size_t)base * m.num_cells : ws.result.get();
         k_flood_walk<<<wgrid, 32, few ? ws.walk_smem_few : ws.walk_smem, st>>>(m, ws.list, ws.counters, base, cap, ws.counters + 1 + c,
-                                                      few ? ws.heap_smem_few : ws.heap_smem, ws.raster, ws.result,
+                                                      few ? ws.heap_smem_few : ws.heap_smem, ws.raster, result,
                                                       ws.spill, ws.spill_cap, ws.prio, ws.cinfo, d_trace, ws.serial_above,
                                                       1.0f / (float)(m.cells_x - 2 * m.corner), 1.0f / (float)m.cells_x); count_launch();
         long long cthreads = (long long)cap * m.num_cells;
         long long cblocks = (cthreads + 255) / 256;
         int cgrid = (int)(cblocks < (long long)ws.sm_count * 8 ? cblocks : (long long)ws.sm_count * 8);
-        k_flood_colour<<<cgrid, 256, 0, st>>>(m, d_rgb, ws.list, ws.counters, base, cap, ws.result, d_cellvals, cc); count_launch();
+        k_flood_colour<<<cgrid, 256, 0, st>>>(m, d_rgb, ws.list, ws.counters, base, cap, result, d_cellvals, cc); count_launch();
+    }
+    return cudaGetLastError();
+}
+
+// the colours of another context's walk (flood_launch with `keep`), in its chunks: the work list and its counters are `walked`'s
+cudaError_t flood_colour_launch(const Mode& m, const FloodWorkspace& walked, const uint8_t* d_rgb, int n_frames, const uint32_t* kept,
+                                uint8_t* d_cellvals, const CcmArg& cc, cudaStream_t st)
+{
+    if (n_frames <= 0) return cudaSuccess;
+    const int nchunks = (n_frames + walked.entry_cap - 1) / walked.entry_cap;
+    for (int c = 0; c < nchunks; ++c) {
+        const int base = c * walked.entry_cap;
+        const int cap = n_frames - base < walked.entry_cap ? n_frames - base : walked.entry_cap;
+        long long cthreads = (long long)cap * m.num_cells;
+        long long cblocks = (cthreads + 255) / 256;
+        int cgrid = (int)(cblocks < (long long)walked.sm_count * 8 ? cblocks : (long long)walked.sm_count * 8);
+        k_flood_colour<<<cgrid, 256, 0, st>>>(m, d_rgb, walked.list, walked.counters, base, cap, kept + (size_t)base * m.num_cells, d_cellvals, cc);
+        count_launch();
     }
     return cudaGetLastError();
 }

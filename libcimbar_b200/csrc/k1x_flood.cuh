@@ -40,9 +40,15 @@ cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int n_fram
 bool flood_workspace_fits(const FloodWorkspace& ws, int n_frames);
 // writes d_flags[f] for every frame: 0 = K1 result stands, CB200_FRAME_FALLBACK = re-decoded here,
 // CB200_FRAME_INEXACT = needed but skipped (no_fallback).  d_sharpen_of: NULL = every frame is preprocessed as `sharpen` says;
-// else one byte per frame of the batch (device memory, nonzero = sharpen) and `sharpen` is ignored
+// else one byte per frame of the batch (device memory, nonzero = sharpen) and `sharpen` is ignored.
+// keep != NULL: the walk's per-cell records (x | y << 11 | sym << 22) of all n_frames listed frames stay there, in list order
+// (n_frames x num_cells words), instead of one chunk at a time in the workspace
 cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb, int n_frames, bool no_fallback,
                          bool force_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
-                         uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st);
+                         uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st, uint32_t* keep = nullptr);
+// the colour pass of a walk that flood_launch ran on `walked` with `keep` = kept, for another mode of the same frame geometry: the
+// frames it listed get their colours (or, with cc.means, their mean colours) at the walk's positions and its symbols in d_cellvals
+cudaError_t flood_colour_launch(const Mode& m, const FloodWorkspace& walked, const uint8_t* d_rgb, int n_frames, const uint32_t* kept,
+                                uint8_t* d_cellvals, const CcmArg& cc, cudaStream_t st);
 
 }  // namespace cb200

@@ -502,44 +502,67 @@ int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uin
     return camera_enqueue_table(c, d, wh, n, flags, d_chunks, d_mask, d_frame_flags, d_status, nullptr);
 }
 
-int camera_reserve(cb200_ctx* c, const int32_t* wh, int n)
+int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks)
 {
     ScanScratch* s = sstate(c);
     int rc;
     if ((rc = grow(c, s->d_minv, 9 * (size_t)n, "inverse maps")) || (rc = grow(c, s->d_fwd, 9 * (size_t)n, "transforms")) ||
-        (rc = grow(c, c->d_sel, (size_t)c->max_frames * 5, "selection")) || (rc = deskew_reserve(c, n)) || (rc = scan_reserve(c, wh, n)))
+        (rc = grow(c, c->d_sel, (size_t)c->max_frames * 5, "selection")) || (walks && (rc = deskew_reserve(c, n))) ||
+        (scans && (rc = scan_reserve(c, wh, n))))
         return rc;
-    return flood_reserve(c, n);
+    return walks ? flood_reserve(c, n) : CB200_OK;
 }
 
-int camera_enqueue_table(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
-                         uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table)
+int camera_reserve(cb200_ctx* c, const int32_t* wh, int n) { return camera_reserve_for(c, wh, n, true, true); }
+
+int camera_source_bytes(const int32_t* wh, int n, size_t* bytes)
 {
-    const Mode& m = c->mode;
-    size_t src_bytes = 0;
+    *bytes = 0;
     for (int i = 0; i < n; ++i) {
         const size_t b = (size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3;
         if (b >= ((size_t)1 << 32)) return fail(CB200_ERR_ARG, "source picture " + std::to_string(i) + " of 4 GB or more");   // k_deskew's offsets
-        src_bytes += b;
+        *bytes += b;
     }
+    return CB200_OK;
+}
+
+int camera_scan(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, const PicDesc* d_table, const PicDesc** d_desc)
+{
+    return scan_enqueue(c, d, wh, n, d_table, d_desc);
+}
+
+int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const uint8_t* d, size_t src_bytes, const PicDesc* d_desc, int n, uint32_t flags,
+                      uint8_t* frames, bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status)
+{
+    const Mode& m = c->mode;
     ScanScratch* s = sstate(c);
-    int rc = camera_reserve(c, wh, n); if (rc) return rc;
-    uint8_t* frames;
-    rc = deskew_frames(c, n, &frames); if (rc) return rc;
-    const PicDesc* d_desc;
-    rc = scan_enqueue(c, d, wh, n, d_table, &d_desc); if (rc) return rc;
+    const ScanScratch* s0 = scanned->scan;
     const bool if_needed = (flags & CB200_FLAG_SHARPEN_IF_NEEDED) != 0;
     uint8_t* d_sharp = if_needed ? c->d_sel + 4 * (size_t)n : nullptr;
-    k_extract<<<(n + 127) / 128, 128, 0, c->stream>>>(s->d_anchors, s->d_count, s->d_status, n, m.width, m.height, d_status, s->d_minv, s->d_fwd, d_sharp);
+    k_extract<<<(n + 127) / 128, 128, 0, c->stream>>>(s0->d_anchors, s0->d_count, s0->d_status, n, m.width, m.height, d_status, s->d_minv, s->d_fwd, d_sharp);
     count_launch();
     CK(cudaGetLastError(), "extract launch");
     s->camera_n = n;
-    rc = deskew_launch(c, d, src_bytes, s->d_minv, d_desc, n, frames); if (rc) return rc;
+    int rc;
+    if (deskew) { rc = deskew_launch(c, d, src_bytes, s->d_minv, d_desc, n, frames); if (rc) return rc; }
     rc = decode_chunks_enqueue(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, d_sharp, d_chunks, d_mask, d_frame_flags); if (rc) return rc;
     k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
     count_launch();
     CK(cudaGetLastError(), "mask launch");
     return CB200_OK;
+}
+
+int camera_enqueue_table(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
+                         uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table)
+{
+    size_t src_bytes;
+    int rc = camera_source_bytes(wh, n, &src_bytes); if (rc) return rc;
+    rc = camera_reserve(c, wh, n); if (rc) return rc;
+    uint8_t* frames;
+    rc = deskew_frames(c, n, &frames); if (rc) return rc;
+    const PicDesc* d_desc;
+    rc = scan_enqueue(c, d, wh, n, d_table, &d_desc); if (rc) return rc;
+    return camera_after_scan(c, c, d, src_bytes, d_desc, n, flags, frames, true, d_chunks, d_mask, d_frame_flags, d_status);
 }
 
 // the synchronous camera entry points: the enqueue-only path into the context's buffers, one copy back, one synchronise
