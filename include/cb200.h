@@ -267,6 +267,34 @@ int cb200_scan_extract_decode_chunks_ragged_dev(cb200_ctx* ctx, const uint8_t* d
 /* the same for n pictures of one size w x h */
 int cb200_scan_extract_decode_chunks_dev(cb200_ctx* ctx, const uint8_t* d_pictures, int w, int h, int n, uint32_t flags, uint8_t* d_chunks,
                                          uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+
+/* ---- camera pictures in the caller's layout ----------------------------------------------------------------------------------
+
+   One descriptor per picture, so a batch needs no packing: each picture may sit in its own allocation, at any byte address, with
+   padding at the end of its rows.  Pixel (x, y) of an interleaved layout starts at data + y * row_pitch + x * channels; in the
+   planar layout its R, G and B bytes are at data + y * row_pitch + x, plus 0, 1 and 2 plane_pitch.  A picture decodes exactly as its
+   packed RGB copy (cvtColor's BGR2RGB, RGBA2RGB or BGRA2RGB) does: alpha is ignored. */
+#define CB200_LAYOUT_RGB        0     /* R G B, 3 bytes per pixel (OpenCV after cvtColor(BGR2RGB), numpy / torch HWC) */
+#define CB200_LAYOUT_BGR        1     /* B G R, 3 bytes per pixel (an OpenCV Mat as imread gives it) */
+#define CB200_LAYOUT_RGBA       2     /* R G B A, 4 bytes per pixel (browser ImageData, Android RGBA_8888) */
+#define CB200_LAYOUT_BGRA       3     /* B G R A, 4 bytes per pixel (capture and interop surfaces) */
+#define CB200_LAYOUT_RGB_PLANAR 4     /* three planes R, G, B of 1 byte per pixel (torch CHW, torchvision.io.decode_jpeg) */
+typedef struct cb200_picture {
+    const uint8_t* data;              /* device address of pixel (0, 0) (of the R plane for CB200_LAYOUT_RGB_PLANAR) */
+    int32_t w, h;
+    int64_t row_pitch;                /* bytes from one row to the next: >= w x channels (3, 4, or 1 per plane) */
+    int64_t plane_pitch;              /* CB200_LAYOUT_RGB_PLANAR: bytes from one plane to the next, >= h x row_pitch; otherwise ignored */
+    int32_t layout;                   /* CB200_LAYOUT_* */
+} cb200_picture;
+/* cb200_scan_extract_decode_chunks_ragged_dev for n pictures described by pics[0 .. n) (HOST memory, read before the call returns):
+   the outputs, the flags, the CCM carry, cb200_camera_transforms, the sharpen selection and the statuses are exactly those of that
+   call on the packed RGB batch, and it waits for the device only as that call does (one picture table through the upload ring).
+   The pictures belong to the stream until it passes the call.  CB200_ERR_ARG, before any CUDA call, naming the picture: n < 0 or
+   n > max_frames, a null pics or data pointer, an unknown layout, a size the scan does not take (short side 60 .. 4499), a negative
+   pitch, a row pitch below w x channels, planes that overlap (plane pitch below h x row pitch), a picture that spans 4 GB or more,
+   and the flags and outputs cb200_scan_extract_decode_chunks_ragged_dev refuses. */
+int cb200_scan_extract_decode_chunks_pictures_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags, uint8_t* d_chunks,
+                                                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
 /* ---- camera plans: the enqueue-only camera call captured once in a CUDA graph ----------------------------------------------
 
    A plan is cb200_scan_extract_decode_chunks_ragged_dev for n pictures of sizes wh, with these flags and these device buffers,

@@ -40,7 +40,7 @@ EXPORTS = [
     "cb200_ccm_chain_root_create", "cb200_ccm_chain_peer_open", "cb200_ccm_chain_attach", "cb200_ccm_chain_step", "cb200_ccm_chain_status",
     "cb200_ccm_chain_link_ms", "cb200_get_frame_ccms",
     "cb200_camera_plan_create", "cb200_camera_plan_launch", "cb200_camera_plan_graph", "cb200_camera_plan_destroy",
-    "cb200_detect_scan_extract_decode_chunks_dev",
+    "cb200_detect_scan_extract_decode_chunks_dev", "cb200_scan_extract_decode_chunks_pictures_dev",
 ]
 
 
@@ -49,6 +49,16 @@ class Info(C.Structure):
         "mode_val", "image_size_x", "image_size_y", "frame_bytes", "total_cells", "symbol_bits", "color_bits",
         "raw_bytes", "raw_symbol_bytes", "ecc_bytes", "ecc_block_size", "rs_blocks", "data_bytes", "chunk_size",
         "chunks_per_frame", "legacy_mode", "max_frames", "sm_count")]
+
+
+# picture layouts of Context.scan_extract_decode_chunks_pictures_dev (cb200_picture.layout)
+LAYOUT_RGB, LAYOUT_BGR, LAYOUT_RGBA, LAYOUT_BGRA, LAYOUT_RGB_PLANAR = 0, 1, 2, 3, 4
+
+
+class Picture(C.Structure):
+    """cb200_picture: one camera picture in device memory in the caller's layout"""
+    _fields_ = [("data", C.c_void_p), ("w", C.c_int32), ("h", C.c_int32), ("row_pitch", C.c_int64), ("plane_pitch", C.c_int64),
+                ("layout", C.c_int32)]
 
 
 TRACE_DTYPE = np.dtype([("order", "<u2"), ("x", "<i2"), ("y", "<i2"), ("drift_offset", "u1"), ("distance", "u1")])
@@ -159,6 +169,7 @@ def load_library():
     lib.cb200_camera_plan_graph.argtypes = [vp, C.POINTER(C.c_void_p)]
     lib.cb200_camera_plan_destroy.argtypes = [vp]
     lib.cb200_detect_scan_extract_decode_chunks_dev.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp]
+    lib.cb200_scan_extract_decode_chunks_pictures_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -169,6 +180,40 @@ def load_library():
 def _check(rc):
     if rc != 0:
         raise Cb200Error(f"cb200 error {rc}: {load_library().cb200_last_error().decode()}")
+
+
+_LAYOUTS = {("rgb", 3): LAYOUT_RGB, ("bgr", 3): LAYOUT_BGR, ("rgb", 4): LAYOUT_RGBA, ("bgr", 4): LAYOUT_BGRA,
+            ("rgba", 4): LAYOUT_RGBA, ("bgra", 4): LAYOUT_BGRA}
+
+
+def picture(t, order="rgb"):
+    """the cb200_picture of a uint8 CUDA tensor: (h, w, 3 | 4) with stride(1) == channels and stride(2) == 1, in channel order
+    `order` ("rgb" / "bgr"; 4 channels: the alpha last, "rgba" / "bgra" also accepted), or (3, h, w) R, G, B planes with
+    stride(2) == 1.  The pitches are the tensor's strides; a tensor whose strides do not fit is refused, never copied"""
+    import torch
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.dim() != 3:
+        raise Cb200Error("a picture is a 3-dimensional uint8 tensor")
+    s = t.stride()
+    if t.shape[2] in (3, 4):
+        h, w, ch = t.shape
+        if s[2] != 1 or s[1] != ch:
+            raise Cb200Error(f"an (h, w, {ch}) picture needs stride(1) == {ch} and stride(2) == 1, not {s}")
+        lay = _LAYOUTS.get((order, ch))
+        if lay is None:
+            raise Cb200Error(f"order {order!r} does not name a layout of {ch} channels")
+        row, plane = s[0], 0
+    elif t.shape[0] == 3:
+        _, h, w = t.shape
+        if s[2] != 1:
+            raise Cb200Error(f"a (3, h, w) picture needs stride(2) == 1, not {s}")
+        if order != "rgb":
+            raise Cb200Error("the planes of a (3, h, w) picture are R, G, B: order must be 'rgb'")
+        lay, row, plane = LAYOUT_RGB_PLANAR, s[1], s[0]
+    else:
+        raise Cb200Error(f"a picture is (h, w, 3 | 4) or (3, h, w), not {tuple(t.shape)}")
+    if not t.is_cuda:
+        raise Cb200Error("a picture must be in device memory (a CUDA tensor)")
+    return Picture(t.data_ptr(), w, h, row, plane, lay)
 
 
 def launch_count():
@@ -522,6 +567,17 @@ class Context:
         wh = np.ascontiguousarray(wh, dtype=np.int32).reshape(-1, 2)
         _check(self.lib.cb200_scan_extract_decode_chunks_ragged_dev(self._h, d_pictures, wh.ctypes.data, wh.shape[0], flags, d_chunks, d_mask,
                                                                     d_flags, d_status))
+
+    def scan_extract_decode_chunks_pictures_dev(self, pictures, d_chunks, d_mask, d_status, d_flags=None, flags=0, order="rgb"):
+        """scan_extract_decode_chunks_dev on a list of uint8 CUDA tensors, each in its own layout and allocation (see picture()):
+        order is one string for every picture or one per picture.  Enqueue-only; keep the tensors alive until the stream has
+        passed the call"""
+        orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+        if len(orders) != len(pictures):
+            raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+        descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+        _check(self.lib.cb200_scan_extract_decode_chunks_pictures_dev(self._h, C.cast(descs, C.c_void_p), len(pictures), flags, d_chunks,
+                                                                      d_mask, d_flags, d_status))
 
     def camera_plan(self, wh, flags, pictures, chunks, mask, frame_flags, status):
         """scan_extract_decode_chunks_dev for pictures of sizes wh (n x (w, h), host) with these flags, captured once in a CUDA graph

@@ -54,14 +54,20 @@ int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t 
 // CB200_ERR_ARG for CB200_FLAG_SHARPEN together with CB200_FLAG_SHARPEN_IF_NEEDED (deskew.cu)
 int check_camera_flags(uint32_t flags);
 // one camera picture of a batch as the extractor kernels (scan.cu, deskew.cu) read it.  The host builds the table per call, for
-// uniform batches too: picture i of a packed batch starts at byte 3 * sum_{j<i} w_j h_j, its blurred gray at sum_{j<i} w_j h_j
+// uniform batches too: picture i of a packed batch starts at byte 3 * sum_{j<i} w_j h_j of the buffer (layout RGB, row pitch
+// 3 w), its blurred gray at sum_{j<i} w_j h_j
 struct PicDesc {
-    uint64_t src;        // byte offset of the RGB8 picture in the source buffer
+    uint64_t src;        // device address of the picture's pixel (0, 0) (of its R plane when planar): layout_core.cuh reads it
     uint64_t blur;       // byte offset of its blurred gray picture in the scan's buffer (k_scan_blur4 / k_scan_anchors)
     int w, h;
-    int words;           // k_scan_blur4's word path: w % 4 == 0 and both bases 4-byte aligned
+    int words;           // k_scan_blur4's word path: w % 4 == 0, the source's base and pitches and the blurred base 4-byte aligned
     int tile0;           // first tile of the picture in the blur launch of its radius
+    uint64_t pitch;      // bytes from one row to the next
+    uint64_t plane;      // bytes from one plane to the next (CB200_LAYOUT_RGB_PLANAR)
+    int layout;          // CB200_LAYOUT_*
 };
+// the packed RGB batch of the _ragged_dev entry points (n pictures of sizes wh back to back from d) as picture descriptors
+std::vector<cb200_picture> packed_pictures(const uint8_t* d, const int32_t* wh, int n);
 // wh: n x (w, h) on the host.  CB200_ERR_ARG naming the picture if a size is outside what the scan restates (short side 60 ..
 // 4499) (scan.cu); no CUDA call
 int check_picture_sizes(const int32_t* wh, int n);
@@ -74,8 +80,9 @@ int extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh
 std::vector<uint8_t> sharpen_from_corners(const cb200_ctx* c, const float* corners, int n);
 // room for n deskewed frames in the context's frame buffer, *frames = its base (deskew.cu)
 int deskew_frames(cb200_ctx* c, int n, uint8_t** frames);
-// k_deskew over n pictures described by d_desc (src, w, h; src_bytes in all) with the inverse maps d_minv (n x 9) into d_dst (deskew.cu)
-int deskew_launch(cb200_ctx* c, const uint8_t* d_src, size_t src_bytes, const double* d_minv, const PicDesc* d_desc, int n, uint8_t* d_dst);
+// k_deskew over n pictures described by d_desc (src, w, h; with `layouts` also the pitches and the layout, else packed RGB rows)
+// with the inverse maps d_minv (n x 9) into d_dst (deskew.cu)
+int deskew_launch(cb200_ctx* c, const double* d_minv, const PicDesc* d_desc, bool layouts, int n, uint8_t* d_dst);
 // the enqueue-only decode of n extracted frames (api.cu): cb200_decode_chunks_dev, but the sharpen selection, if any, is n bytes in
 // device memory (d_sharp, at c->d_sel + 4 n: k_select builds the frame lists there; NULL = as the flags say) and a CCM that an earlier call still in flight may
 // change is taken from the device (c->d_carry) instead of waiting for it
@@ -145,8 +152,8 @@ int camera_table(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, 
 int camera_source_bytes(const int32_t* wh, int n, size_t* bytes);
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks);
 int camera_scan(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, const PicDesc* d_table, const PicDesc** d_desc);
-int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const uint8_t* d, size_t src_bytes, const PicDesc* d_desc, int n, uint32_t flags,
-                      uint8_t* frames, bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status);
+int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const PicDesc* d_desc, bool layouts, int n, uint32_t flags, uint8_t* frames,
+                      bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status);
 // the context is attached to a CCM chain (chain.cu)
 bool chain_attached(const cb200_ctx* c);
 }  // namespace cb200

@@ -17,6 +17,7 @@
 // returns to the host before its chunks do.
 #include "ctx.cuh"
 #include "extract_core.cuh"
+#include "layout_core.cuh"
 
 #include <cfloat>
 #include <cmath>
@@ -41,26 +42,13 @@ void deskew_destroy(DeskewState* d) { delete d; }
 // words and realigned by funnel shifts: a source that lies rotated in the photograph makes every lane hit its own sector, and the
 // kernel is then bound by L1 sector look-ups (ncu: 27 sectors per request), so fewer, wider requests are what counts.
 // A tap outside the source gets weight 0 (== BORDER_CONSTANT 0); its bytes come from a clamped, valid address.
-__device__ __forceinline__ void load_row_pair(const uint8_t* __restrict__ p, const uint8_t* __restrict__ end, uint32_t& lo, uint32_t& hi)
-{   // bytes p[0..5] -> lo = p[0..3], hi = p[4..5] (upper half unspecified); `end` = one past the last readable byte
-    const uintptr_t addr = reinterpret_cast<uintptr_t>(p);
-    const uint32_t a = (uint32_t)(addr & 3u);
-    const uint8_t* base = p - a;
-    if (base + 12 <= end) {
-        const uint32_t* w = reinterpret_cast<const uint32_t*>(base);
-        const uint32_t w0 = __ldg(w), w1 = __ldg(w + 1);
-        const uint32_t w2 = (a == 3u) ? __ldg(w + 2) : 0u;           // six bytes from offset 3 reach into the third word
-        lo = __funnelshift_r(w0, w1, 8u * a);
-        hi = __funnelshift_r(w1, w2, 8u * a);
-    } else {                                                        // the last few bytes of the buffer: byte loads
-        lo = (uint32_t)__ldg(p) | ((uint32_t)__ldg(p + 1) << 8) | ((uint32_t)__ldg(p + 2) << 16) | ((uint32_t)__ldg(p + 3) << 24);
-        hi = (uint32_t)__ldg(p + 4) | ((uint32_t)__ldg(p + 5) << 8);
-    }
-}
-
+// The taps are fetched per the picture's layout (layout_core.cuh): the six bytes of a packed 3-byte pair or the eight of a 4-byte
+// pair as above, two bytes from each plane of a planar picture, and reordered into the packed RGB pair the blend below reads; the
+// frames are packed RGB whatever the pictures' layout.  Word loads stop short of the end of the picture (of each plane).  Without
+// kLayouts every picture is packed RGB (row pitch 3 w) and the layout is not read: the packed batches' code, in fewer registers.
+template <bool kLayouts>
 __global__ void __launch_bounds__(256)
-k_deskew(const uint8_t* __restrict__ src, size_t src_bytes, const double* __restrict__ minv, const PicDesc* __restrict__ desc, int n,
-         int dst_w, int dst_h, int bw0, uint8_t* __restrict__ dst)
+k_deskew(const double* __restrict__ minv, const PicDesc* __restrict__ desc, int n, int dst_w, int dst_h, int bw0, uint8_t* __restrict__ dst)
 {
     const int quads = dst_w >> 2;
     const int per_frame = dst_h * quads;
@@ -68,11 +56,13 @@ k_deskew(const uint8_t* __restrict__ src, size_t src_bytes, const double* __rest
     if (i >= per_frame) return;
     const int y = i / quads, q = i - y * quads;
     const int x = 4 * q, bx = (x / bw0) * bw0;
-    const uint8_t* const end = src + src_bytes;
     for (int f = (int)blockIdx.y; f < n; f += (int)gridDim.y) {
         const double* M = minv + (size_t)f * 9;
-        const uint8_t* s = src + __ldg(&desc[f].src);
-        const int src_w = __ldg(&desc[f].w), src_h = __ldg(&desc[f].h);
+        const uint8_t* s = reinterpret_cast<const uint8_t*>(__ldg(&desc[f].src));
+        const int src_w = __ldg(&desc[f].w), src_h = __ldg(&desc[f].h), lay = kLayouts ? __ldg(&desc[f].layout) : CB200_LAYOUT_RGB;
+        const uint32_t pitch = kLayouts ? (uint32_t)__ldg(&desc[f].pitch) : 3u * (uint32_t)src_w, cpp = (uint32_t)layout::channels(lay);
+        const uint64_t plane = kLayouts ? __ldg(&desc[f].plane) : 0;
+        const uint8_t* const end = s + (size_t)(src_h - 1) * pitch + (size_t)src_w * cpp;
         const double M0 = __ldg(M), M1 = __ldg(M + 1), M2 = __ldg(M + 2), M3 = __ldg(M + 3), M4 = __ldg(M + 4), M5 = __ldg(M + 5),
                      M6 = __ldg(M + 6), M7 = __ldg(M + 7), M8 = __ldg(M + 8);
         // no FMA contraction: OpenCV's x86-64 code rounds after every multiply and add
@@ -103,12 +93,28 @@ k_deskew(const uint8_t* __restrict__ src, size_t src_bytes, const double* __rest
             const int c = sx < 0 ? 0 : (sx > src_w - 2 ? src_w - 2 : sx);
             left[u] = sx < c; right[u] = sx > c;
             const int cy0 = sy < 0 ? 0 : (sy >= src_h ? src_h - 1 : sy), cy1 = sy + 1 < 0 ? 0 : (sy + 1 >= src_h ? src_h - 1 : sy + 1);
-            off[u][0] = 3u * ((uint32_t)cy0 * (uint32_t)src_w + (uint32_t)c);
-            off[u][1] = 3u * ((uint32_t)cy1 * (uint32_t)src_w + (uint32_t)c);
+            off[u][0] = (uint32_t)cy0 * pitch + cpp * (uint32_t)c;
+            off[u][1] = (uint32_t)cy1 * pitch + cpp * (uint32_t)c;
         }
         uint32_t lo[4][2], hi[4][2];
+        if (lay == CB200_LAYOUT_RGB_PLANAR) {
 #pragma unroll
-        for (int u = 0; u < 4; ++u) { load_row_pair(s + off[u][0], end, lo[u][0], hi[u][0]); load_row_pair(s + off[u][1], end, lo[u][1], hi[u][1]); }
+            for (int u = 0; u < 4; ++u) {
+                layout::planar_pair(s + off[u][0], plane, end, lo[u][0], hi[u][0]);
+                layout::planar_pair(s + off[u][1], plane, end, lo[u][1], hi[u][1]);
+            }
+        } else {
+            const uint32_t nb = 2u * cpp;
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                layout::load_bytes(s + off[u][0], end, nb, lo[u][0], hi[u][0]);
+                layout::load_bytes(s + off[u][1], end, nb, lo[u][1], hi[u][1]);
+            }
+            if (lay != CB200_LAYOUT_RGB) {
+#pragma unroll
+                for (int u = 0; u < 4; ++u) { layout::pair_rgb(lay, lo[u][0], hi[u][0]); layout::pair_rgb(lay, lo[u][1], hi[u][1]); }
+            }
+        }
         uint32_t px[4][3];
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
@@ -167,15 +173,13 @@ int cb200::deskew_frames(cb200_ctx* c, int n, uint8_t** frames)
 
 namespace cb200 {
 
-// warpPerspective of n source pictures of sizes wh (n x (w, h), host) packed in d_src, one frame each
+// warpPerspective of n source pictures of sizes wh (n x (w, h), host) packed in d_src (RGB), one frame each
 static int deskew_run(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int n, const double* m9, uint8_t* d_dst)
 {
-    size_t src_bytes = 0;
     for (int f = 0; f < n; ++f) {
         if (wh[2 * f] < 2 || wh[2 * f + 1] < 2) return fail(CB200_ERR_ARG, "bad arguments");
         const size_t b = (size_t)wh[2 * f] * (size_t)wh[2 * f + 1] * 3;
         if (b >= ((size_t)1 << 32)) return fail(CB200_ERR_ARG, "source picture " + std::to_string(f) + " of 4 GB or more");
-        src_bytes += b;
     }
     if (n == 0) return CB200_OK;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
@@ -189,20 +193,20 @@ static int deskew_run(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int
     int rc = stage_take(c, table_bytes, &slot, &table); if (rc) return rc;
     double* inv = reinterpret_cast<double*>(table);
     PicDesc* desc = reinterpret_cast<PicDesc*>(inv + 9 * (size_t)n);
-    size_t off = 0;
+    const std::vector<cb200_picture> pics = packed_pictures(d_src, wh, n);
     for (int f = 0; f < n; ++f) {
         if (!extract::invert3(m9 + (size_t)f * 9, inv + (size_t)f * 9)) return fail(CB200_ERR_ARG, "singular perspective transform");
-        desc[f] = PicDesc{off, 0, wh[2 * f], wh[2 * f + 1], 0, 0};
-        off += (size_t)wh[2 * f] * (size_t)wh[2 * f + 1] * 3;
+        const cb200_picture& p = pics[(size_t)f];
+        desc[f] = PicDesc{reinterpret_cast<uint64_t>(p.data), 0, p.w, p.h, 0, 0, (uint64_t)p.row_pitch, 0, p.layout};
     }
     rc = stage_send(c, slot, d->d_table, table_bytes, "H2D transforms"); if (rc) return rc;
     const double* d_inv = reinterpret_cast<const double*>(d->d_table.get());
-    return deskew_launch(c, d_src, src_bytes, d_inv, reinterpret_cast<const PicDesc*>(d_inv + 9 * (size_t)n), n, d_dst);
+    return deskew_launch(c, d_inv, reinterpret_cast<const PicDesc*>(d_inv + 9 * (size_t)n), false, n, d_dst);
 }
 
 }  // namespace cb200
 
-int cb200::deskew_launch(cb200_ctx* c, const uint8_t* d_src, size_t src_bytes, const double* d_minv, const PicDesc* d_desc, int n, uint8_t* d_dst)
+int cb200::deskew_launch(cb200_ctx* c, const double* d_minv, const PicDesc* d_desc, bool layouts, int n, uint8_t* d_dst)
 {
     const Mode& m = c->mode;
     // OpenCV's block geometry (WarpPerspectiveInvoker): bh0 = min(16, H); bw0 = min(1024 / bh0, W)
@@ -210,7 +214,8 @@ int cb200::deskew_launch(cb200_ctx* c, const uint8_t* d_src, size_t src_bytes, c
     int bw0 = 1024 / bh0; if (bw0 > m.width) bw0 = m.width;
     const int per_frame = m.height * (m.width / 4);
     const dim3 grid((unsigned)((per_frame + 255) / 256), (unsigned)(n < 32768 ? n : 32768));
-    k_deskew<<<grid, 256, 0, c->stream>>>(d_src, src_bytes, d_minv, d_desc, n, m.width, m.height, bw0, d_dst);
+    if (layouts) k_deskew<true><<<grid, 256, 0, c->stream>>>(d_minv, d_desc, n, m.width, m.height, bw0, d_dst);
+    else k_deskew<false><<<grid, 256, 0, c->stream>>>(d_minv, d_desc, n, m.width, m.height, bw0, d_dst);
     count_launch();
     CK(cudaGetLastError(), "deskew launch");
     return CB200_OK;

@@ -119,8 +119,7 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d,
                           uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks)
 {
     cb200_ctx* c0 = ctxs[0];
-    size_t src_bytes;
-    int rc = camera_source_bytes(wh, n, &src_bytes); if (rc) return rc;
+    int rc;
     // geometries: lead[g] = the first context of geometry g in priority order
     int group[kDetectModes], lead[kDetectModes], ng = 0;
     for (int k = 0; k < n_modes; ++k) {
@@ -160,7 +159,7 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d,
             if (group[k] != g) continue;
             cb200_ctx* c = ctxs[k];
             StreamSwap on(c, ng > 1 ? ds->side[g] : main, &sw);
-            rc = camera_after_scan(c, c0, d, src_bytes, d_desc, n, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr,
+            rc = camera_after_scan(c, c0, d_desc, false, n, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr,
                                    ds->status + (size_t)k * n);
         }
     }

@@ -21,6 +21,7 @@
 #include "ctx.cuh"
 #include "scan_core.cuh"
 #include "extract_core.cuh"
+#include "layout_core.cuh"
 
 #include <string>
 #include <vector>
@@ -68,9 +69,11 @@ constexpr int kBlurTW = 128, kBlurTH = 32, kBlurThreads = 256;
 // as three aligned words and are converted with K1's IDP.2A form (8 instructions per four pixels), the horizontal taps are IDP.4A dot
 // products of realigned gray words with the packed coefficients, the vertical pass reads four 16-bit sums per 64-bit load, and a warp
 // owns a tile row (no divisions).
-// The word path needs 4-byte aligned rows: a picture width that is a multiple of four and aligned source and blurred bases (decided
-// per picture by the host: in a packed batch a picture that follows one of odd area starts unaligned); otherwise, and in tiles that
-// cross the right edge, pixels are fetched one by one.
+// The word path needs 4-byte aligned rows: a picture width that is a multiple of four, aligned source and blurred bases and an
+// aligned row (and plane) pitch (decided per picture by the host: in a packed batch a picture that follows one of odd area starts
+// unaligned); otherwise, and in tiles that cross the right edge, pixels are fetched one by one.  The gray comes from the picture's
+// layout (layout_core.cuh): the IDP.2A form with the coefficients in the channel order for 3-byte pixels, one word per 4-byte
+// pixel, one word per plane for planar pictures.
 template <int R> struct BlurKW {     // the 2R+1 coefficients as bytes of up to three words (IDP.4A operands)
     __device__ static constexpr uint32_t w(int i)
     {
@@ -79,18 +82,15 @@ template <int R> struct BlurKW {     // the 2R+1 coefficients as bytes of up to 
     }
 };
 
-__device__ __forceinline__ uint32_t gray_scalar(const uint8_t* p)
-{
-    return (9798u * p[0] + 19235u * p[1] + 3735u * p[2] + 16384u) >> 15;
-}
-
 // One launch per radius over the flattened tiles of that radius' pictures: order[0 .. npics) lists them (batch indices into the
 // descriptor table, in batch order), their tiles are numbered consecutively from desc[order[k]].tile0, row-major inside a picture.
 // A CTA finds its picture by division when all listed pictures have one size (uniform_tiles tiles each), else by binary search.
-template <int R>
+// kLayouts: the pictures' layouts and pitches come from the table; without it every picture is packed RGB (row pitch 3 w), the
+// code the packed batches have always run (fewer registers)
+template <int R, bool kLayouts>
 __global__ void __launch_bounds__(kBlurThreads)
-k_scan_blur4(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out, const PicDesc* __restrict__ desc, const int* __restrict__ order,
-             int npics, int uniform_tiles, unsigned* __restrict__ hist)
+k_scan_blur4(uint8_t* __restrict__ out, const PicDesc* __restrict__ desc, const int* __restrict__ order, int npics, int uniform_tiles,
+             unsigned* __restrict__ hist)
 {
     constexpr int GH = kBlurTH + 2 * R, GP = kBlurTW + 8, NW = (2 * R + 1 + 3) / 4;      // gray pitch: interior at byte 4
     __shared__ __align__(16) uint8_t g[GH][GP];
@@ -111,33 +111,29 @@ k_scan_blur4(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out, const P
     const int w = __ldg(&d->w), h = __ldg(&d->h), words_ok = __ldg(&d->words);
     const int tiles_x = (w + kBlurTW - 1) / kBlurTW, tl = t - __ldg(&d->tile0), tyi = tl / tiles_x;
     const int tx0 = (tl - tyi * tiles_x) * kBlurTW, ty0 = tyi * kBlurTH;
-    const uint8_t* src = rgb + __ldg(&d->src);
+    const uint8_t* src = reinterpret_cast<const uint8_t*>(__ldg(&d->src));
+    const size_t pitch = kLayouts ? __ldg(&d->pitch) : 3 * (size_t)w;
+    const uint64_t plane = kLayouts ? __ldg(&d->plane) : 0;
+    const int lay = kLayouts ? __ldg(&d->layout) : CB200_LAYOUT_RGB;
+    const layout::Fetch fx = layout::fetch_of(lay, plane);
     lh[tid] = 0;
     // ---- gray of the tile and its halo
     const int x = tx0 + 4 * lane;
     for (int r = warp; r < GH; r += kBlurThreads / 32) {
         const int y = reflect101_clamped(ty0 - R + r, h);
-        const uint8_t* row = src + (size_t)y * (size_t)w * 3;
+        const uint8_t* row = src + (size_t)y * pitch;
         uint32_t g4;
         if (words_ok && x + 3 < w) {
-            const uint32_t* p = reinterpret_cast<const uint32_t*>(row + 3 * (size_t)x);
-            const uint32_t q0 = __ldg(p), q1 = __ldg(p + 1), q2 = __ldg(p + 2);          // R0 G0 B0 R1 | G1 B1 R2 G2 | B2 R3 G3 B3
-            const uint32_t cRG = 19596u | (38470u << 16), cB0 = 7470u, c0R = 19596u << 16, cGB = 38470u | (7470u << 16);
-            uint32_t n0, n1, n2, n3;                     // (19596 R + 38470 G + 7470 B + 2^15): gray is byte 2 (== (9798 R + 19235 G + 3735 B + 2^14) >> 15)
-            n0 = __dp2a_lo(cRG, q0, 32768u); n0 = __dp2a_hi(cB0, q0, n0);
-            n1 = __dp2a_hi(c0R, q0, 32768u); n1 = __dp2a_lo(cGB, q1, n1);
-            n2 = __dp2a_hi(cRG, q1, 32768u); n2 = __dp2a_lo(cB0, q2, n2);
-            n3 = __dp2a_lo(c0R, q2, 32768u); n3 = __dp2a_hi(cGB, q2, n3);
-            g4 = __byte_perm(__byte_perm(n0, n1, 0x0062), __byte_perm(n2, n3, 0x6200), 0x7610);
+            g4 = layout::gray4_words(row, x, plane, lay);
         } else {
             g4 = 0;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) g4 |= gray_scalar(row + 3 * (size_t)reflect101_clamped(x + k, w)) << (8 * k);
+            for (int k = 0; k < 4; ++k) g4 |= layout::gray_px(row, reflect101_clamped(x + k, w), fx) << (8 * k);
         }
         *reinterpret_cast<uint32_t*>(&g[r][4 + 4 * lane]) = g4;
         if (lane < 2 * R) {                               // halo columns: R to the left of the tile, R to the right
             const int xx = lane < R ? tx0 - R + lane : tx0 + kBlurTW + (lane - R);
-            g[r][lane < R ? 4 - R + lane : 4 + kBlurTW + (lane - R)] = (uint8_t)gray_scalar(row + 3 * (size_t)reflect101_clamped(xx, w));
+            g[r][lane < R ? 4 - R + lane : 4 + kBlurTW + (lane - R)] = (uint8_t)layout::gray_px(row, reflect101_clamped(xx, w), fx);
         }
     }
     __syncthreads();
@@ -323,8 +319,8 @@ struct BlurGroups {
 };
 
 // the descriptor table (batch order), then the pictures grouped by blur radius (batch order inside a group) into `table`; the tiles
-// of one radius are numbered across its pictures.  The word path depends on where d_pics and the scan's blurred buffer are
-static int pic_table(const ScanScratch* s, const uint8_t* d_pics, const int32_t* wh, int n, uint8_t* table, BlurGroups& g)
+// of one radius are numbered across its pictures.  The word path depends on where the pictures and the scan's blurred buffer are
+static int pic_table(const ScanScratch* s, const cb200_picture* pics, const int32_t* wh, int n, uint8_t* table, BlurGroups& g)
 {
     PicDesc* desc = reinterpret_cast<PicDesc*>(table);
     int* order = reinterpret_cast<int*>(desc + n);
@@ -341,9 +337,13 @@ static int pic_table(const ScanScratch* s, const uint8_t* d_pics, const int32_t*
     for (int R = 1; R <= 4; ++R) g.group0[R] = next[R];
     for (int i = 0; i < n; ++i) {
         const int w = wh[2 * i], h = wh[2 * i + 1], R = scan_blur_radius(w, h);
+        const cb200_picture& p = pics[i];
+        const bool planar = p.layout == CB200_LAYOUT_RGB_PLANAR;
         PicDesc& d = desc[i];
-        d.src = 3 * off; d.blur = off; d.w = w; d.h = h;
-        d.words = (w % 4 == 0) && (reinterpret_cast<uintptr_t>(d_pics + d.src) % 4 == 0) && (reinterpret_cast<uintptr_t>(s->d_blur + d.blur) % 4 == 0);
+        d.src = reinterpret_cast<uint64_t>(p.data); d.blur = off; d.w = w; d.h = h;
+        d.pitch = (uint64_t)p.row_pitch; d.plane = planar ? (uint64_t)p.plane_pitch : 0; d.layout = p.layout;
+        d.words = (w % 4 == 0) && (d.src % 4 == 0) && (d.pitch % 4 == 0) && (d.plane % 4 == 0) &&
+                  (reinterpret_cast<uintptr_t>(s->d_blur + d.blur) % 4 == 0);
         d.tile0 = (int)g.tiles[R];
         g.tiles[R] += (long long)((w + kBlurTW - 1) / kBlurTW) * ((h + kBlurTH - 1) / kBlurTH);
         if (g.tiles[R] > 0x7FFFFFFFll) return fail(CB200_ERR_ARG, "more than 2^31 blur tiles in one batch");
@@ -356,17 +356,37 @@ static int pic_table(const ScanScratch* s, const uint8_t* d_pics, const int32_t*
 int camera_pictures(cb200_ctx* c) { return sstate(c)->camera_n; }
 void set_camera_pictures(cb200_ctx* c, int n) { sstate(c)->camera_n = n; }
 
+std::vector<cb200_picture> packed_pictures(const uint8_t* d, const int32_t* wh, int n)
+{
+    std::vector<cb200_picture> p((size_t)(n > 0 ? n : 0));
+    size_t off = 0;
+    for (int i = 0; i < n; ++i) {
+        const int w = wh[2 * i], h = wh[2 * i + 1];
+        p[(size_t)i] = cb200_picture{d + off, w, h, 3 * (int64_t)w, 0, CB200_LAYOUT_RGB};
+        off += 3 * (size_t)w * (size_t)h;
+    }
+    return p;
+}
+
+// every picture in packed RGB rows (layout RGB, row pitch 3 w): the kernels' packed instantiations take the batch
+static bool packed_rgb(const cb200_picture* pics, int n)
+{
+    for (int i = 0; i < n; ++i)
+        if (pics[i].layout != CB200_LAYOUT_RGB || pics[i].row_pitch != 3 * (int64_t)pics[i].w) return false;
+    return true;
+}
+
 int camera_table(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, std::vector<uint8_t>& table)
 {
     table.assign((sizeof(PicDesc) + sizeof(int)) * (size_t)n, 0);
     BlurGroups g;
-    return pic_table(sstate(c), d_pics, wh, n, table.data(), g);
+    return pic_table(sstate(c), packed_pictures(d_pics, wh, n).data(), wh, n, table.data(), g);
 }
 
-// blurred pictures + thresholds + anchors for n pictures of sizes wh (checked by check_picture_sizes) packed in device memory, in
-// the state's device arrays; enqueued only.  The picture table (PicDesc, in s->d_table) is this call's one upload -- unless
-// d_table holds it already (a camera plan's): then *d_desc = d_table and nothing is uploaded
-static int scan_enqueue(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, const PicDesc* d_table = nullptr,
+// blurred pictures + thresholds + anchors for n pictures of sizes wh (checked by check_picture_sizes) described by pics, in the
+// state's device arrays; enqueued only.  The picture table (PicDesc, in s->d_table) is this call's one upload -- unless d_table
+// holds it already (a camera plan's): then *d_desc = d_table and nothing is uploaded
+static int scan_enqueue(cb200_ctx* c, const cb200_picture* pics, const int32_t* wh, int n, const PicDesc* d_table = nullptr,
                         const PicDesc** d_desc_out = nullptr)
 {
     ScanScratch* s = sstate(c);
@@ -377,13 +397,13 @@ static int scan_enqueue(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, 
     const PicDesc* d_desc = d_table;
     if (d_table) {
         std::vector<uint8_t> table(table_bytes);
-        err = pic_table(s, d_pics, wh, n, table.data(), g); if (err) return err;
+        err = pic_table(s, pics, wh, n, table.data(), g); if (err) return err;
     } else {
         CK(s->d_table.ensure(table_bytes), "cudaMalloc picture table");
         int slot;
         uint8_t* h_table;
         err = stage_take(c, table_bytes, &slot, &h_table); if (err) return err;
-        err = pic_table(s, d_pics, wh, n, h_table, g); if (err) return err;
+        err = pic_table(s, pics, wh, n, h_table, g); if (err) return err;
         err = stage_send(c, slot, s->d_table, table_bytes, "H2D picture table"); if (err) return err;
         d_desc = reinterpret_cast<const PicDesc*>(s->d_table.get());
     }
@@ -392,6 +412,7 @@ static int scan_enqueue(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, 
     const int* group0 = g.group0;
     const long long* tiles = g.tiles;
     const bool* same = g.same;
+    const bool layouts = !packed_rgb(pics, n);
     const int* d_order = reinterpret_cast<const int*>(d_desc + n);
     CK(cudaMemsetAsync(s->d_hist, 0, sizeof(unsigned) * 256 * (size_t)n, st), "memset histograms");
     // cb200_set_timing: one event set per scan -- [blur + histogram (all radii), Otsu, anchors] through cb200_get_timing
@@ -403,10 +424,14 @@ static int scan_enqueue(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, 
         const unsigned grid = (unsigned)tiles[R];
         const int* ord = d_order + group0[R];
         switch (R) {
-        case 1: k_scan_blur4<1><<<grid, kBlurThreads, 0, st>>>(d_pics, s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
-        case 2: k_scan_blur4<2><<<grid, kBlurThreads, 0, st>>>(d_pics, s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
-        case 3: k_scan_blur4<3><<<grid, kBlurThreads, 0, st>>>(d_pics, s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
-        default: k_scan_blur4<4><<<grid, kBlurThreads, 0, st>>>(d_pics, s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
+        case 1: if (layouts) k_scan_blur4<1, true><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, count[R], uniform, s->d_hist);
+                 else k_scan_blur4<1, false><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
+        case 2: if (layouts) k_scan_blur4<2, true><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, count[R], uniform, s->d_hist);
+                 else k_scan_blur4<2, false><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
+        case 3: if (layouts) k_scan_blur4<3, true><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, count[R], uniform, s->d_hist);
+                 else k_scan_blur4<3, false><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
+        default: if (layouts) k_scan_blur4<4, true><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, count[R], uniform, s->d_hist);
+                 else k_scan_blur4<4, false><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, count[R], uniform, s->d_hist); break;
         }
         count_launch();
     }
@@ -423,7 +448,7 @@ static int scan_enqueue(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, 
 // scan_enqueue, then its results into the pinned host arrays of the state
 static int scan_run(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n)
 {
-    int rc = scan_enqueue(c, d_pics, wh, n); if (rc) return rc;
+    int rc = scan_enqueue(c, packed_pictures(d_pics, wh, n).data(), wh, n); if (rc) return rc;
     ScanScratch* s = c->scan;
     cudaStream_t st = c->stream;
     CK(s->h_anchors.ensure(4 * (size_t)n), "cudaMallocHost anchors");
@@ -528,11 +553,11 @@ int camera_source_bytes(const int32_t* wh, int n, size_t* bytes)
 
 int camera_scan(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, const PicDesc* d_table, const PicDesc** d_desc)
 {
-    return scan_enqueue(c, d, wh, n, d_table, d_desc);
+    return scan_enqueue(c, packed_pictures(d, wh, n).data(), wh, n, d_table, d_desc);
 }
 
-int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const uint8_t* d, size_t src_bytes, const PicDesc* d_desc, int n, uint32_t flags,
-                      uint8_t* frames, bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status)
+int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const PicDesc* d_desc, bool layouts, int n, uint32_t flags, uint8_t* frames,
+                      bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status)
 {
     const Mode& m = c->mode;
     ScanScratch* s = sstate(c);
@@ -544,7 +569,7 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const uint8_t* d, 
     CK(cudaGetLastError(), "extract launch");
     s->camera_n = n;
     int rc;
-    if (deskew) { rc = deskew_launch(c, d, src_bytes, s->d_minv, d_desc, n, frames); if (rc) return rc; }
+    if (deskew) { rc = deskew_launch(c, s->d_minv, d_desc, layouts, n, frames); if (rc) return rc; }
     rc = decode_chunks_enqueue(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, d_sharp, d_chunks, d_mask, d_frame_flags); if (rc) return rc;
     k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
     count_launch();
@@ -552,17 +577,24 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const uint8_t* d, 
     return CB200_OK;
 }
 
+// the camera path for n pictures of sizes wh described by pics, arguments checked
+static int camera_enqueue_pictures(cb200_ctx* c, const cb200_picture* pics, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks,
+                                   uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table)
+{
+    int rc = camera_reserve(c, wh, n); if (rc) return rc;
+    uint8_t* frames;
+    rc = deskew_frames(c, n, &frames); if (rc) return rc;
+    const PicDesc* d_desc;
+    rc = scan_enqueue(c, pics, wh, n, d_table, &d_desc); if (rc) return rc;
+    return camera_after_scan(c, c, d_desc, !packed_rgb(pics, n), n, flags, frames, true, d_chunks, d_mask, d_frame_flags, d_status);
+}
+
 int camera_enqueue_table(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
                          uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table)
 {
     size_t src_bytes;
     int rc = camera_source_bytes(wh, n, &src_bytes); if (rc) return rc;
-    rc = camera_reserve(c, wh, n); if (rc) return rc;
-    uint8_t* frames;
-    rc = deskew_frames(c, n, &frames); if (rc) return rc;
-    const PicDesc* d_desc;
-    rc = scan_enqueue(c, d, wh, n, d_table, &d_desc); if (rc) return rc;
-    return camera_after_scan(c, c, d, src_bytes, d_desc, n, flags, frames, true, d_chunks, d_mask, d_frame_flags, d_status);
+    return camera_enqueue_pictures(c, packed_pictures(d, wh, n).data(), wh, n, flags, d_chunks, d_mask, d_frame_flags, d_status, d_table);
 }
 
 // the synchronous camera entry points: the enqueue-only path into the context's buffers, one copy back, one synchronise
@@ -615,6 +647,41 @@ static int check_camera_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32
     rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
     rc = check_chain_call(c, flags); if (rc) return rc;
     return check_frozen_camera(c, wh, n);
+}
+
+// the picture descriptors of cb200_scan_extract_decode_chunks_pictures_dev, all before any CUDA call; wh = their sizes
+static int check_pictures(const cb200_picture* pics, int n, std::vector<int32_t>& wh)
+{
+    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
+    if (!pics) return fail(CB200_ERR_ARG, "null pictures");
+    wh.assign(2 * (size_t)n, 0);
+    for (int i = 0; i < n; ++i) {
+        const cb200_picture& p = pics[i];
+        const std::string name = "picture " + std::to_string(i);
+        if (!p.data) return fail(CB200_ERR_ARG, name + " has a null data pointer");
+        if (!layout::known(p.layout)) return fail(CB200_ERR_ARG, name + " has an unknown layout " + std::to_string(p.layout));
+        if (p.row_pitch < 0 || p.plane_pitch < 0)
+            return fail(CB200_ERR_ARG, name + " has a negative " + (p.row_pitch < 0 ? "row" : "plane") + " pitch");
+        wh[2 * (size_t)i] = p.w; wh[2 * (size_t)i + 1] = p.h;
+    }
+    int rc = check_picture_sizes(wh.data(), n); if (rc) return rc;
+    for (int i = 0; i < n; ++i) {
+        const cb200_picture& p = pics[i];
+        const std::string name = "picture " + std::to_string(i);
+        const bool planar = p.layout == CB200_LAYOUT_RGB_PLANAR;
+        const int64_t row = (int64_t)p.w * layout::channels(p.layout);
+        if (p.row_pitch < row)
+            return fail(CB200_ERR_ARG, name + " has a row pitch of " + std::to_string(p.row_pitch) + " bytes, below w x channels = " + std::to_string(row));
+        if (planar && p.plane_pitch < (int64_t)p.h * p.row_pitch)
+            return fail(CB200_ERR_ARG, name + " has overlapping planes: a plane pitch of " + std::to_string(p.plane_pitch) + " bytes, below h x row pitch = " +
+                                           std::to_string((int64_t)p.h * p.row_pitch));
+        // k_deskew's offsets inside a picture are 32-bit
+        const int64_t lim = (int64_t)1 << 32;
+        if (p.row_pitch >= lim || (planar && p.plane_pitch >= lim) ||
+            (planar ? 2 * p.plane_pitch : 0) + (int64_t)(p.h - 1) * p.row_pitch + row >= lim)
+            return fail(CB200_ERR_ARG, name + " spans 4 GB or more");
+    }
+    return CB200_OK;
 }
 
 int camera_empty(cb200_ctx* c, uint32_t flags)
@@ -758,6 +825,21 @@ int cb200_scan_extract_decode_chunks_dev(cb200_ctx* c, const uint8_t* d_pictures
     if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
     const std::vector<int32_t> wh = uniform_sizes(w, h, n);
     return cb200_scan_extract_decode_chunks_ragged_dev(c, d_pictures, wh.data(), n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+}
+
+int cb200_scan_extract_decode_chunks_pictures_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, uint8_t* d_chunks,
+                                                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
+{
+    // the checks of cb200_scan_extract_decode_chunks_ragged_dev, in its order, with the descriptors' in place of wh and the pictures
+    int rc = check_camera_dev_flags(flags); if (rc) return rc;
+    std::vector<int32_t> wh;
+    rc = check_pictures(pics, n, wh); if (rc) return rc;
+    rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
+    rc = check_chain_call(c, flags); if (rc) return rc;
+    rc = check_frozen_camera(c, wh.data(), n); if (rc) return rc;
+    if (n == 0) return camera_empty(c, flags);
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    return camera_enqueue_pictures(c, pics, wh.data(), n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr);
 }
 
 int cb200_camera_transforms(cb200_ctx* c, double* m9_out, int n)
