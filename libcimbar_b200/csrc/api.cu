@@ -205,25 +205,6 @@ bool adjacency_consistent(const Mode& m, const std::vector<uint16_t>& adj)
 
 namespace cb200 {
 void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
-
-int stage_take(cb200_ctx* c, size_t bytes, int* slot, uint8_t** h)
-{
-    *slot = c->stage_next;
-    c->stage_next = (*slot + 1) % cb200_ctx::kStageSlots;
-    cb200_ctx::StageSlot& s = c->stage[*slot];
-    if (!s.ev) CK(cudaEventCreateWithFlags(&s.ev, cudaEventDisableTiming), "cudaEventCreate upload slot");
-    CK(cudaEventSynchronize(s.ev), "sync (upload slot)");      // the slot may only grow once its last copy has run
-    CK(s.h.ensure(bytes), "cudaMallocHost upload slot");
-    *h = s.h;
-    return CB200_OK;
-}
-
-int stage_send(cb200_ctx* c, int slot, void* d_dst, size_t bytes, const char* what)
-{
-    CK(cudaMemcpyAsync(d_dst, c->stage[slot].h, bytes, cudaMemcpyHostToDevice, c->stream), what);
-    CK(cudaEventRecord(c->stage[slot].ev, c->stream), "record upload slot");
-    return CB200_OK;
-}
 }  // namespace cb200
 
 namespace {
@@ -380,7 +361,7 @@ int build_selection(cb200_ctx* c, int n)
     return CB200_OK;
 }
 
-// a mixed sharpen selection from the host: its n bytes go up through the context's pinned slots (stage_take), k_select builds the
+// a mixed sharpen selection from the host: its n bytes go up through the context's upload ring, k_select builds the
 // batch indices of the plain frames (d_list[0], nl[0] of them) and of the sharpened ones (d_list[1]), both in batch order, and
 // one 0 / 1 byte per frame (d_sharp)
 int upload_selection(cb200_ctx* c, const uint8_t* sel, int n, const int nl[2], const uint32_t* d_list[2], const uint8_t** d_sharp)
@@ -388,9 +369,9 @@ int upload_selection(cb200_ctx* c, const uint8_t* sel, int n, const int nl[2], c
     CK(c->d_sel.ensure((size_t)c->max_frames * 5), "cudaMalloc selection");
     int slot;
     uint8_t* h;
-    int rc = stage_take(c, (size_t)n, &slot, &h); if (rc) return rc;
+    int rc = c->upload.take((size_t)n, &slot, &h); if (rc) return rc;
     memcpy(h, sel, (size_t)n);
-    rc = stage_send(c, slot, c->d_sel + (size_t)n * 4, (size_t)n, "H2D selection"); if (rc) return rc;
+    rc = c->upload.send(c->stream, slot, c->d_sel + (size_t)n * 4, (size_t)n); if (rc) return rc;
     rc = build_selection(c, n); if (rc) return rc;
     d_list[0] = reinterpret_cast<const uint32_t*>(c->d_sel.get());
     d_list[1] = d_list[0] + nl[0];
@@ -660,7 +641,6 @@ int cb200_destroy(cb200_ctx* c)
     while (!c->plans.empty()) cb200_camera_plan_destroy(c->plans.back());
     cudaSetDevice(c->device);          // the buffers free themselves in `delete c`, on this device
     for (int k = 0; k < cb200_ctx::kEvSets; ++k) for (int i = 0; i < 8; ++i) if (c->ev[k][i]) cudaEventDestroy(c->ev[k][i]);
-    for (const auto& s : c->stage) if (s.ev) cudaEventDestroy(s.ev);
     if (c->ccm_ev) cudaEventDestroy(c->ccm_ev);
     gather_destroy(c->gather);
     chain_destroy(c->chain);

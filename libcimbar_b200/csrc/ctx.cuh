@@ -31,27 +31,28 @@ void deskew_destroy(DeskewState* d);     // delete: its buffers free themselves
 void scan_destroy(ScanScratch* s);       // likewise
 void jpeg_destroy(JpegState* j);         // likewise
 void png_destroy(PngState* p);           // likewise
-// the uploads of the file calls (descriptors + compressed data, jpeg.cu / png.cu): a ring of pinned buffers, each reused once the
-// copy enqueued from it has run -- one per call, so, as on the RGB camera call, a fourth call in flight waits until the first
-// one's upload has run.  take() hands out the next slot with room for `bytes`; send() enqueues the copy of its first `bytes` to
-// d_dst and records the slot's event
-struct FileUpload {
+// host-built data of a call on its way to the device: a ring of pinned buffers, each reused once the copy enqueued from it has run.
+// take() hands out the next slot with room for `bytes` (after the copy last enqueued from it has run); the caller fills *host, and
+// send() enqueues the copy of its first `bytes` to d_dst on stream st and records the slot's event.  The caller's own host inputs
+// are free again when the call returns.  Instances: the context's (cb200_ctx::upload), the JPEG calls' and the PNG calls'
+struct UploadRing {
     static constexpr int kSlots = 3;
     PinnedBuf<uint8_t> h[kSlots];
     cudaEvent_t ev[kSlots] = {};
     int next = 0;
-    ~FileUpload() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+    ~UploadRing() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
     int take(size_t bytes, int* slot, uint8_t** host);
     int send(cudaStream_t st, int slot, void* d_dst, size_t bytes);
 };
 // status -2 (and, when d_mask is given, mask 0) for every picture whose flag in d_bad is set: the corrupt files of a file call
-// (files.cu, like FileUpload's members)
+// (files.cu, like UploadRing's members)
 int file_status(cb200_ctx* c, const int* d_bad, int n, int32_t* d_status, uint32_t* d_mask);
 // cb200_decode_fountain_from_dev with an optional per-frame sharpen selection: `sharpen` = n host bytes (nonzero =
 // should_preprocess) or NULL (the batch-wide CB200_FLAG_SHARPEN decides).  The flags are checked by the caller (api.cu)
 int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
                             uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
-// CB200_ERR_ARG for CB200_FLAG_SHARPEN together with CB200_FLAG_SHARPEN_IF_NEEDED (deskew.cu)
+// CB200_ERR_ARG for CB200_FLAG_SHARPEN together with CB200_FLAG_SHARPEN_IF_NEEDED, or CB200_FLAG_CC_SIMPLE with CB200_FLAG_CC_FIT
+// (scan.cu)
 int check_camera_flags(uint32_t flags);
 // one camera picture of a batch as the extractor kernels (scan.cu, deskew.cu) read it.  The host builds the table per call, for
 // uniform batches too: picture i of a packed batch starts at byte 3 * sum_{j<i} w_j h_j of the buffer (layout RGB, row pitch
@@ -66,36 +67,48 @@ struct PicDesc {
     uint64_t plane;      // bytes from one plane to the next (CB200_LAYOUT_RGB_PLANAR)
     int layout;          // CB200_LAYOUT_*
 };
-// the packed RGB batch of the _ragged_dev entry points (n pictures of sizes wh back to back from d) as picture descriptors
-std::vector<cb200_picture> packed_pictures(const uint8_t* d, const int32_t* wh, int n);
+// The pictures of one camera, corner or deskew call, whatever the caller passed in (scan.cu): one descriptor per picture, their
+// sizes n x (w, h) (what scan_reserve and check_frozen_* take), and `packed`: every picture is RGB with row pitch 3 w, so the
+// kernels run their packed (kLayouts = false) instantiations.  `host`: the pictures are still in host memory, stage_batch takes
+// them to the device.  One builder per kind of input applies that kind's per-picture rules, all before any CUDA call
+struct CameraBatch {
+    std::vector<cb200_picture> pics;
+    std::vector<int32_t> wh;
+    bool packed = true, host = false;
+    int n() const { return (int)(wh.size() / 2); }
+    void pack(const uint8_t* d);       // the pictures of sizes wh back to back from d in packed RGB
+};
 // wh: n x (w, h) on the host.  CB200_ERR_ARG naming the picture if a size is outside what the scan restates (short side 60 ..
 // 4499) (scan.cu); no CUDA call
 int check_picture_sizes(const int32_t* wh, int n);
 // the uniform batch as a ragged one: n x (w, h)
 std::vector<int32_t> uniform_sizes(int w, int h, int n);
-// cb200_extract_decode_fountain_dev with the same selection, for pictures of sizes wh (n x (w, h)) packed in d_src (deskew.cu)
-int extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int n, const float* corners, uint32_t flags,
-                           const uint8_t* sharpen, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
-// CB200_FLAG_SHARPEN_IF_NEEDED on given corners: sharpen[i] = 1 iff picture i's corners fail Corners::is_granular_scale (deskew.cu)
-std::vector<uint8_t> sharpen_from_corners(const cb200_ctx* c, const float* corners, int n);
+// the builders (scan.cu): n packed pictures of sizes wh from the device buffer d (the _dev entry points, plans, detect; a file
+// call's decoded pictures are packed this way too, with the sizes parse_files gives); n packed pictures of w x h from d (host or
+// device: the uniform entry points, which then take the ragged path); n host pointers, packed when staged; n picture descriptors
+// in the caller's layouts.  The scan's size rule (check_picture_sizes) applies to all four
+int packed_batch(const uint8_t* d, const int32_t* wh, int n, CameraBatch& b);
+int uniform_batch(const uint8_t* d, int w, int h, int n, CameraBatch& b);
+int host_batch(const uint8_t* const* pictures, const int32_t* wh, int n, CameraBatch& b);
+int picture_batch(const cb200_picture* pics, int n, CameraBatch& b);
+// CB200_ERR_ARG naming the first picture that spans 4 GB or more: k_deskew's offsets inside a picture are 32-bit (scan.cu)
+int check_spans(const CameraBatch& b);
+// a host batch packed into the context's one staging buffer for host pictures, with one copy per run of adjacent pictures; the
+// batch then describes the staged pictures.  Nothing for a device batch (scan.cu)
+int stage_batch(cb200_ctx* c, CameraBatch& b);
 // room for n deskewed frames in the context's frame buffer, *frames = its base (deskew.cu)
 int deskew_frames(cb200_ctx* c, int n, uint8_t** frames);
-// k_deskew over n pictures described by d_desc (src, w, h; with `layouts` also the pitches and the layout, else packed RGB rows)
-// with the inverse maps d_minv (n x 9) into d_dst (deskew.cu)
-int deskew_launch(cb200_ctx* c, const double* d_minv, const PicDesc* d_desc, bool layouts, int n, uint8_t* d_dst);
+// k_deskew over the pictures of b described by d_desc, with the inverse maps d_minv (n x 9), into d_dst (deskew.cu)
+int deskew_launch(cb200_ctx* c, const CameraBatch& b, const double* d_minv, const PicDesc* d_desc, uint8_t* d_dst);
 // the enqueue-only decode of n extracted frames (api.cu): cb200_decode_chunks_dev, but the sharpen selection, if any, is n bytes in
 // device memory (d_sharp, at c->d_sel + 4 n: k_select builds the frame lists there; NULL = as the flags say) and a CCM that an earlier call still in flight may
 // change is taken from the device (c->d_carry) instead of waiting for it
 int decode_chunks_enqueue(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* d_sharp, uint8_t* d_chunks,
                           uint32_t* d_chunk_mask, uint8_t* d_frame_flags);
-// the argument checks of cb200_scan_extract_decode_chunks_ragged_dev beyond its pictures, all before any CUDA call (scan.cu): the
-// flags (both sharpen flags, CC_SIMPLE with CC_FIT), then the context, the outputs and n against max_frames
-int check_camera_dev_flags(uint32_t flags);
-int check_camera_dev_outputs(cb200_ctx* c, int n, const uint8_t* d_chunks, const uint32_t* d_chunk_mask, const int32_t* d_extract_status);
-// the enqueue-only camera path (scan, k_extract, deskew, decode, failed pictures' masks cleared) for n pictures of sizes wh packed
-// in device memory, arguments checked (scan.cu)
-int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
-                   uint8_t* d_frame_flags, int32_t* d_status);
+// the enqueue-only camera path (reserve, scan, k_extract, deskew, decode, failed pictures' masks cleared) for a device batch,
+// arguments checked (scan.cu).  The picture table is this call's one upload, unless d_table holds it already (a camera plan's)
+int camera_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags,
+                   int32_t* d_status, const PicDesc* d_table = nullptr);
 // the results of the last decode (c->d_data, c->d_mask, c->d_flags, and d_status when given) to host memory with one synchronise,
 // the good chunks of each frame packed densely (api.cu)
 int fetch_fountain(cb200_ctx* c, int n, const int32_t* d_status, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
@@ -136,23 +149,20 @@ int check_frozen_scan(cb200_ctx* c, const int32_t* wh, int n);
 int carry_from_host(cb200_ctx* c);
 // a CC_FIT call in this mode fits matrices (init_ccm needs a header from the RS stream, not the legacy coupled layout) (api.cu)
 bool ccm_fits(const Mode& m, uint32_t flags);
-// the camera path with the picture table given in device memory (a plan's), so nothing is uploaded (scan.cu)
-int camera_enqueue_table(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
-                         uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table);
 // the pictures of the last camera call (cb200_camera_transforms reads that many) (scan.cu)
 int camera_pictures(cb200_ctx* c);
 void set_camera_pictures(cb200_ctx* c, int n);
-// the picture table of that call for n pictures of sizes wh at d_pics, built on the host (scan.cu): PicDesc n, then the order
-int camera_table(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, std::vector<uint8_t>& table);
-// the stages of the camera path, for the detect call (scan.cu).  camera_source_bytes: the packed batch's size, CB200_ERR_ARG for a
-// picture of 4 GB or more (no CUDA call).  camera_reserve_for: camera_reserve without the scan's buffers (scans = false) or the
-// deskewed frames' and the walk's (walks = false).  camera_scan: the scan of n pictures on this context's scratch, *d_desc = its
-// picture table.  camera_after_scan: k_extract on `scanned`'s anchors into this context's transforms and d_status, the deskew into
-// `frames` (deskew = false: `frames` holds them already, deskewed for this geometry), the decode and the failed pictures' masks
-int camera_source_bytes(const int32_t* wh, int n, size_t* bytes);
+// the picture table of a batch as the scan reads it, built on the host (scan.cu): n PicDesc, then the pictures grouped by blur
+// radius (n int); a camera plan builds its own with it
+int pic_table(cb200_ctx* c, const CameraBatch& b, std::vector<uint8_t>& table);
+// the stages of camera_enqueue, for the detect call (scan.cu).  camera_reserve_for: camera_reserve without the scan's buffers
+// (scans = false) or the deskewed frames' and the walk's (walks = false).  camera_scan: the scan of the batch on this context's
+// scratch (the table from d_table, else uploaded), *d_desc = its picture table.  camera_after_scan: k_extract on `scanned`'s
+// anchors into this context's transforms and d_status, the deskew into `frames` (deskew = false: `frames` holds them already,
+// deskewed for this geometry), the decode and the failed pictures' masks
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks);
-int camera_scan(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, const PicDesc* d_table, const PicDesc** d_desc);
-int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const PicDesc* d_desc, bool layouts, int n, uint32_t flags, uint8_t* frames,
+int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc);
+int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
                       bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status);
 // the context is attached to a CCM chain (chain.cu)
 bool chain_attached(const cb200_ctx* c);
@@ -190,14 +200,10 @@ struct cb200_ctx {
     cb200::DevBuf<uint8_t> d_scratch;
     // pinned host staging for results of the host-pointer entry points
     cb200::PinnedBuf<uint8_t> h_pinned;
-    // host-built tables of a call (sharpen selections, picture tables, inverse maps) on their way to the device: a ring of pinned
-    // slots, each reused once the copy enqueued from it has run (stage_take / stage_send).  A call uploads at most two tables
-    // (cb200_deskew_dev: its table; a frame call with a mixed selection: the selection), so no call waits for a copy it enqueued
-    // itself; a camera call uploads one (its picture table), so three camera calls can be in flight before the fourth waits
-    struct StageSlot { cb200::PinnedBuf<uint8_t> h; cudaEvent_t ev = nullptr; };
-    static constexpr int kStageSlots = 3;
-    StageSlot stage[kStageSlots];
-    int stage_next = 0;
+    // host-built tables of a call (sharpen selections, picture tables, inverse maps) on their way to the device.  A call uploads at
+    // most two tables (a corner call: its table; a frame call with a mixed selection: the selection), so no call waits for a copy it
+    // enqueued itself; a camera call uploads one (its picture table), so three camera calls can be in flight before the fourth waits
+    cb200::UploadRing upload;
     // a sharpen selection of n frames: the plain frames' batch indices, then the sharpened ones' (both in batch order, 4 n bytes),
     // then one sharpen byte per frame (n bytes); built from the bytes by k_select (api.cu), which also leaves the launch schedule
     // of each list in d_sched: {count, K1 bands, first entry} for the plain and for the sharpened frames
@@ -245,9 +251,19 @@ namespace cb200 {
 // cb200_set_timing: begin_timed_call starts the event set of a pipeline call, mark records its next event on the call's stream
 inline void begin_timed_call(cb200_ctx* c) { if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; } }
 inline void mark(cb200_ctx* c) { if (c->timing && c->ev_count[c->cur] < 8) cudaEventRecord(c->ev[c->cur][c->ev_count[c->cur]++], c->stream); }
-// a host-built table for this call: stage_take hands out the next pinned slot with room for `bytes` (after the copy last
-// enqueued from it has run); the caller fills *h, and stage_send enqueues the copy of its first `bytes` to d_dst on the call's
-// stream and records the slot's event.  The caller's own host inputs are free again when the call returns
-int stage_take(cb200_ctx* c, size_t bytes, int* slot, uint8_t** h);
-int stage_send(cb200_ctx* c, int slot, void* d_dst, size_t bytes, const char* what);
+
+// the checks every camera and corner call shares, in this order and before any CUDA call: the flags; the batch, from the call's
+// builder `build` (which may add the call's own checks that come before the context), and the 4 GB span rule of the deskew; the
+// context; `missing` (the message for a null output, or nullptr); n against max_frames; the CCM chain.  The frozen buffers the
+// call would grow are checked by the caller (check_frozen_*), which knows which ones it uses
+template <class Build>
+int check_camera_call(cb200_ctx* c, uint32_t flags, Build&& build, CameraBatch& b, const char* missing)
+{
+    int rc = check_camera_flags(flags); if (rc) return rc;
+    if ((rc = build(b)) || (rc = check_spans(b))) return rc;
+    if (!c) return fail(CB200_ERR_ARG, "null context");
+    if (missing) return fail(CB200_ERR_ARG, missing);
+    if (b.n() > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(b.n()) + " > max_frames = " + std::to_string(c->max_frames));
+    return check_chain_call(c, flags);
+}
 }  // namespace cb200

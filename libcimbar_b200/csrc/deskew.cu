@@ -29,7 +29,6 @@ namespace cb200 {
 
 struct DeskewState {
     DevBuf<uint8_t> d_table;       // n x 9 inverse maps (destination -> source) in double, then n PicDesc (the sources)
-    DevBuf<uint8_t> d_src;         // staging for the host-pointer entry point
     DevBuf<uint8_t> d_dst;         // deskewed frames of the host-pointer entry points
 };
 
@@ -144,20 +143,87 @@ static DeskewState* dstate(cb200_ctx* c)
     return c->deskew;
 }
 
-// the host-pointer entry points: n source pictures of w x h into the staging buffer
-static int stage_sources(cb200_ctx* c, const uint8_t* src, int w, int h, int n)
-{
-    DeskewState* d = dstate(c);
-    const size_t sb = (size_t)n * w * h * 3;
-    CK(d->d_src.ensure(sb), "cudaMalloc deskew source");
-    CK(cudaMemcpyAsync(d->d_src, src, sb, cudaMemcpyHostToDevice, c->stream), "H2D camera frames");
-    return CB200_OK;
-}
-
 // room for n deskewed frames in the output buffer
 static int ensure_frames(cb200_ctx* c, int n)
 {
     return grow(c, dstate(c)->d_dst, (size_t)n * c->mode.width * c->mode.height * 3, "deskew output");
+}
+
+// the batch of the uniform deskew and corner calls: n pictures of w x h packed from d (in host memory when `host`).  The deskew
+// reads any picture of 2 x 2 or more: the scan's size rule is not theirs
+static int deskew_batch(const uint8_t* d, int w, int h, int n, bool host, CameraBatch& b)
+{
+    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
+    if (!d) return fail(CB200_ERR_ARG, "null pictures");
+    if (n > 0 && (w < 2 || h < 2))
+        return fail(CB200_ERR_ARG, "pictures of " + std::to_string(w) + " x " + std::to_string(h) + ": the deskew needs 2 x 2 or more");
+    b.wh = uniform_sizes(w, h, n);
+    b.pack(d);
+    b.host = host;
+    return CB200_OK;
+}
+
+// warpPerspective of the pictures of a device batch with the transforms m9 (n x 9, host), one frame each into d_dst
+static int deskew_run(cb200_ctx* c, const CameraBatch& b, const double* m9, uint8_t* d_dst)
+{
+    const int n = b.n();
+    DeskewState* d = dstate(c);
+    const size_t table_bytes = (sizeof(double) * 9 + sizeof(PicDesc)) * (size_t)n;
+    CK(d->d_table.ensure(table_bytes), "cudaMalloc transforms");
+    // warpPerspective inverts the transform it is given (no WARP_INVERSE_MAP): cv::invert, DECOMP_LU; a singular matrix maps
+    // everything to (0, 0) there (invert leaves zeros) -- reported here instead
+    int slot;
+    uint8_t* table;
+    int rc = c->upload.take(table_bytes, &slot, &table); if (rc) return rc;
+    double* inv = reinterpret_cast<double*>(table);
+    PicDesc* desc = reinterpret_cast<PicDesc*>(inv + 9 * (size_t)n);
+    for (int f = 0; f < n; ++f) {
+        if (!extract::invert3(m9 + (size_t)f * 9, inv + (size_t)f * 9)) return fail(CB200_ERR_ARG, "singular perspective transform");
+        const cb200_picture& p = b.pics[(size_t)f];
+        desc[f] = PicDesc{reinterpret_cast<uint64_t>(p.data), 0, p.w, p.h, 0, 0, (uint64_t)p.row_pitch, 0, p.layout};
+    }
+    rc = c->upload.send(c->stream, slot, d->d_table, table_bytes); if (rc) return rc;
+    const double* d_inv = reinterpret_cast<const double*>(d->d_table.get());
+    return deskew_launch(c, b, d_inv, reinterpret_cast<const PicDesc*>(d_inv + 9 * (size_t)n), d_dst);
+}
+
+// Extractor::extract (Extractor.h:30-46): NEEDS_SHARPEN unless every side of the corner quadrilateral spans more than the frame in x
+// or in y (Corners::is_granular_scale, Corners.h:57-75)
+static std::vector<uint8_t> sharpen_from_corners(const cb200_ctx* c, const float* corners, int n)
+{
+    std::vector<uint8_t> sharpen((size_t)n);
+    for (int i = 0; i < n; ++i) sharpen[(size_t)i] = extract::is_granular_scale(corners + 8 * (size_t)i, c->mode.width, c->mode.height) ? 0 : 1;
+    return sharpen;
+}
+
+// the corner calls: the batch checked and staged, deskewed on the caller's corners and decoded, the results copied out.  With
+// CB200_FLAG_SHARPEN_IF_NEEDED the corners decide which frames are sharpened
+template <class Build>
+static int extract_decode(cb200_ctx* c, Build&& build, const float* corners, uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count,
+                          uint32_t* chunk_mask, uint8_t* frame_flags)
+{
+    CameraBatch b;
+    int rc = check_camera_call(c, flags, build, b, !corners ? "null corners" : chunks_out && chunk_count ? nullptr : "null output");
+    if (rc) return rc;
+    const int n = b.n();
+    if (n == 0) return CB200_OK;
+    rc = check_frozen_deskew(c, n); if (rc) return rc;
+    const Mode& m = c->mode;
+    float outp[8];
+    extract::output_points(m.width, m.height, outp);
+    std::vector<double> m9((size_t)n * 9);
+    for (int f = 0; f < n; ++f) {
+        rc = cb200_perspective_transform(corners + (size_t)f * 8, outp, m9.data() + (size_t)f * 9); if (rc) return rc;
+    }
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    rc = stage_batch(c, b); if (rc) return rc;
+    rc = ensure_frames(c, n); if (rc) return rc;
+    rc = deskew_run(c, b, m9.data(), c->deskew->d_dst); if (rc) return rc;
+    // the deskewed frames never leave the device: straight into the decode
+    const bool if_needed = (flags & CB200_FLAG_SHARPEN_IF_NEEDED) != 0;
+    const std::vector<uint8_t> sharpen = if_needed ? sharpen_from_corners(c, corners, n) : std::vector<uint8_t>();
+    return decode_fountain_to_host(c, c->deskew->d_dst, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, if_needed ? sharpen.data() : nullptr,
+                                   chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
 }  // namespace cb200
@@ -171,59 +237,21 @@ int cb200::deskew_frames(cb200_ctx* c, int n, uint8_t** frames)
     return CB200_OK;
 }
 
-namespace cb200 {
-
-// warpPerspective of n source pictures of sizes wh (n x (w, h), host) packed in d_src (RGB), one frame each
-static int deskew_run(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int n, const double* m9, uint8_t* d_dst)
-{
-    for (int f = 0; f < n; ++f) {
-        if (wh[2 * f] < 2 || wh[2 * f + 1] < 2) return fail(CB200_ERR_ARG, "bad arguments");
-        const size_t b = (size_t)wh[2 * f] * (size_t)wh[2 * f + 1] * 3;
-        if (b >= ((size_t)1 << 32)) return fail(CB200_ERR_ARG, "source picture " + std::to_string(f) + " of 4 GB or more");
-    }
-    if (n == 0) return CB200_OK;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    DeskewState* d = dstate(c);
-    const size_t table_bytes = (sizeof(double) * 9 + sizeof(PicDesc)) * (size_t)n;
-    CK(d->d_table.ensure(table_bytes), "cudaMalloc transforms");
-    // warpPerspective inverts the transform it is given (no WARP_INVERSE_MAP): cv::invert, DECOMP_LU; a singular matrix maps
-    // everything to (0, 0) there (invert leaves zeros) -- reported here instead
-    int slot;
-    uint8_t* table;
-    int rc = stage_take(c, table_bytes, &slot, &table); if (rc) return rc;
-    double* inv = reinterpret_cast<double*>(table);
-    PicDesc* desc = reinterpret_cast<PicDesc*>(inv + 9 * (size_t)n);
-    const std::vector<cb200_picture> pics = packed_pictures(d_src, wh, n);
-    for (int f = 0; f < n; ++f) {
-        if (!extract::invert3(m9 + (size_t)f * 9, inv + (size_t)f * 9)) return fail(CB200_ERR_ARG, "singular perspective transform");
-        const cb200_picture& p = pics[(size_t)f];
-        desc[f] = PicDesc{reinterpret_cast<uint64_t>(p.data), 0, p.w, p.h, 0, 0, (uint64_t)p.row_pitch, 0, p.layout};
-    }
-    rc = stage_send(c, slot, d->d_table, table_bytes, "H2D transforms"); if (rc) return rc;
-    const double* d_inv = reinterpret_cast<const double*>(d->d_table.get());
-    return deskew_launch(c, d_inv, reinterpret_cast<const PicDesc*>(d_inv + 9 * (size_t)n), false, n, d_dst);
-}
-
-}  // namespace cb200
-
-int cb200::deskew_launch(cb200_ctx* c, const double* d_minv, const PicDesc* d_desc, bool layouts, int n, uint8_t* d_dst)
+int cb200::deskew_launch(cb200_ctx* c, const CameraBatch& b, const double* d_minv, const PicDesc* d_desc, uint8_t* d_dst)
 {
     const Mode& m = c->mode;
+    const int n = b.n();
     // OpenCV's block geometry (WarpPerspectiveInvoker): bh0 = min(16, H); bw0 = min(1024 / bh0, W)
     const int bh0 = m.height < 16 ? m.height : 16;
     int bw0 = 1024 / bh0; if (bw0 > m.width) bw0 = m.width;
     const int per_frame = m.height * (m.width / 4);
     const dim3 grid((unsigned)((per_frame + 255) / 256), (unsigned)(n < 32768 ? n : 32768));
-    if (layouts) k_deskew<true><<<grid, 256, 0, c->stream>>>(d_minv, d_desc, n, m.width, m.height, bw0, d_dst);
+    if (!b.packed) k_deskew<true><<<grid, 256, 0, c->stream>>>(d_minv, d_desc, n, m.width, m.height, bw0, d_dst);
     else k_deskew<false><<<grid, 256, 0, c->stream>>>(d_minv, d_desc, n, m.width, m.height, bw0, d_dst);
     count_launch();
     CK(cudaGetLastError(), "deskew launch");
     return CB200_OK;
 }
-
-namespace cb200 {
-
-}  // namespace cb200
 
 using namespace cb200;
 
@@ -238,107 +266,54 @@ int cb200_perspective_transform(const float* src_xy, const float* dst_xy, double
 
 int cb200_deskew_dev(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, int n, const double* m9, uint8_t* d_dst)
 {
-    if (!c || !d_src || !m9 || !d_dst || n < 0 || src_w < 2 || src_h < 2) return fail(CB200_ERR_ARG, "bad arguments");
-    if ((size_t)src_w * (size_t)src_h * 3 >= ((size_t)1 << 32)) return fail(CB200_ERR_ARG, "source picture of 4 GB or more");
-    int rc = check_frozen_deskew(c, n); if (rc) return rc;
-    return deskew_run(c, d_src, uniform_sizes(src_w, src_h, n).data(), n, m9, d_dst);
+    CameraBatch b;
+    int rc = deskew_batch(d_src, src_w, src_h, n, false, b);
+    if (rc || (rc = check_spans(b))) return rc;
+    if (!c || !m9 || !d_dst) return fail(CB200_ERR_ARG, !c ? "null context" : "null argument");
+    rc = check_frozen_deskew(c, n); if (rc) return rc;
+    if (n == 0) return CB200_OK;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    return deskew_run(c, b, m9, d_dst);
 }
 
 int cb200_deskew(cb200_ctx* c, const uint8_t* src, int src_w, int src_h, int n, const double* m9, uint8_t* dst)
 {
-    if (!c || !src || !dst || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
+    CameraBatch b;
+    int rc = deskew_batch(src, src_w, src_h, n, true, b);
+    if (rc || (rc = check_spans(b))) return rc;
+    if (!c || !dst) return fail(CB200_ERR_ARG, !c ? "null context" : "null output");
+    if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
     if (n == 0) return CB200_OK;
-    int rc = check_frozen_deskew(c, n); if (rc) return rc;
+    if (!m9) return fail(CB200_ERR_ARG, "null argument");
+    rc = check_frozen_deskew(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
-    rc = stage_sources(c, src, src_w, src_h, n); if (rc) return rc;
+    rc = stage_batch(c, b); if (rc) return rc;
     rc = ensure_frames(c, n); if (rc) return rc;
-    const DeskewState* d = c->deskew;
-    rc = cb200_deskew_dev(c, d->d_src, src_w, src_h, n, m9, d->d_dst); if (rc) return rc;
-    CK(cudaMemcpyAsync(dst, d->d_dst, (size_t)n * c->mode.width * c->mode.height * 3, cudaMemcpyDeviceToHost, c->stream), "D2H frames");
+    rc = deskew_run(c, b, m9, c->deskew->d_dst); if (rc) return rc;
+    CK(cudaMemcpyAsync(dst, c->deskew->d_dst, (size_t)n * c->mode.width * c->mode.height * 3, cudaMemcpyDeviceToHost, c->stream), "D2H frames");
     CK(cudaStreamSynchronize(c->stream), "sync");
     return CB200_OK;
 }
 
-}  // extern "C"
-
-// both sharpen flags together are a contradiction (CB200_FLAG_SHARPEN_IF_NEEDED is the CLI's --preprocess -1, SHARPEN its 1)
-int cb200::check_camera_flags(uint32_t flags)
-{
-    if ((flags & CB200_FLAG_SHARPEN) && (flags & CB200_FLAG_SHARPEN_IF_NEEDED))
-        return fail(CB200_ERR_ARG, "CB200_FLAG_SHARPEN and CB200_FLAG_SHARPEN_IF_NEEDED are exclusive");
-    return CB200_OK;
-}
-
-// the pictures are already in device memory (the scan entry points stage them once for scan + deskew)
-int cb200::extract_decode_to_host(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int n, const float* corners, uint32_t flags,
-                                  const uint8_t* sharpen, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
-{
-    if (!c || !d_src || !corners || !chunks_out || !chunk_count || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
-    if (n == 0) return CB200_OK;
-    int rc = check_frozen_deskew(c, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    const Mode& m = c->mode;
-    float outp[8];
-    extract::output_points(m.width, m.height, outp);
-    std::vector<double> m9((size_t)n * 9);
-    for (int f = 0; f < n; ++f) {
-        rc = cb200_perspective_transform(corners + (size_t)f * 8, outp, m9.data() + (size_t)f * 9); if (rc) return rc;
-    }
-    rc = ensure_frames(c, n); if (rc) return rc;
-    rc = deskew_run(c, d_src, wh, n, m9.data(), c->deskew->d_dst); if (rc) return rc;
-    // the deskewed frames never leave the device: straight into the decode
-    return decode_fountain_to_host(c, c->deskew->d_dst, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
-}
-
-// Extractor::extract (Extractor.h:30-46): NEEDS_SHARPEN unless every side of the corner quadrilateral spans more than the frame in x
-// or in y (Corners::is_granular_scale, Corners.h:57-75)
-std::vector<uint8_t> cb200::sharpen_from_corners(const cb200_ctx* c, const float* corners, int n)
-{
-    std::vector<uint8_t> sharpen((size_t)n);
-    for (int i = 0; i < n; ++i) sharpen[(size_t)i] = extract::is_granular_scale(corners + 8 * (size_t)i, c->mode.width, c->mode.height) ? 0 : 1;
-    return sharpen;
-}
-
-extern "C" {
-
 int cb200_extract_decode_fountain_dev(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
                                       uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
-    int rc = check_camera_flags(flags); if (rc) return rc;
-    const std::vector<int32_t> wh = uniform_sizes(src_w, src_h, n);
-    if (!(flags & CB200_FLAG_SHARPEN_IF_NEEDED) || !c || !corners || n < 0 || n > c->max_frames)
-        return extract_decode_to_host(c, d_src, wh.data(), n, corners, flags, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags);
-    return extract_decode_to_host(c, d_src, wh.data(), n, corners, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, sharpen_from_corners(c, corners, n).data(),
-                                  chunks_out, chunk_count, chunk_mask, frame_flags);
+    auto build = [&](CameraBatch& b) { return deskew_batch(d_src, src_w, src_h, n, false, b); };
+    return extract_decode(c, build, corners, flags, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
 int cb200_extract_decode_fountain_ragged_dev(cb200_ctx* c, const uint8_t* d_src, const int32_t* wh, int n, const float* corners, uint32_t flags,
                                              uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
-    int rc = check_camera_flags(flags); if (rc) return rc;
-    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
-    if (!wh) return fail(CB200_ERR_ARG, "null wh");
-    if (!d_src) return fail(CB200_ERR_ARG, "null pictures");
-    rc = check_picture_sizes(wh, n); if (rc) return rc;
-    if (!c) return fail(CB200_ERR_ARG, "null context");
-    if (!corners || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, !corners ? "null corners" : "null output");
-    if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
-    if (!(flags & CB200_FLAG_SHARPEN_IF_NEEDED))
-        return extract_decode_to_host(c, d_src, wh, n, corners, flags, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags);
-    return extract_decode_to_host(c, d_src, wh, n, corners, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, sharpen_from_corners(c, corners, n).data(),
-                                  chunks_out, chunk_count, chunk_mask, frame_flags);
+    auto build = [&](CameraBatch& b) { return packed_batch(d_src, wh, n, b); };
+    return extract_decode(c, build, corners, flags, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
 int cb200_extract_decode_fountain(cb200_ctx* c, const uint8_t* src, int src_w, int src_h, int n, const float* corners, uint32_t flags,
                                   uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
-    int rc = check_camera_flags(flags); if (rc) return rc;
-    if (!c || !src || !corners || !chunks_out || !chunk_count || n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "bad arguments");
-    if (n == 0) return CB200_OK;
-    rc = check_frozen_deskew(c, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    rc = stage_sources(c, src, src_w, src_h, n); if (rc) return rc;
-    return cb200_extract_decode_fountain_dev(c, c->deskew->d_src, src_w, src_h, n, corners, flags, chunks_out, chunk_count, chunk_mask, frame_flags);
+    auto build = [&](CameraBatch& b) { return deskew_batch(src, src_w, src_h, n, true, b); };
+    return extract_decode(c, build, corners, flags, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
 }  // extern "C"

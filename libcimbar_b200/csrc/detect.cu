@@ -75,17 +75,13 @@ static std::string ctx_name(int k) { return "context " + std::to_string(k); }
 
 // every argument check, before any CUDA call: the ones that need no context first
 static int check_detect(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d_pictures, const int32_t* wh, int n, uint32_t flags,
-                        const uint8_t* d_chunks, const uint32_t* d_chunk_mask, const int32_t* d_extract_status, const int32_t* d_mode)
+                        const uint8_t* d_chunks, const uint32_t* d_chunk_mask, const int32_t* d_extract_status, const int32_t* d_mode,
+                        CameraBatch& b)
 {
     if (n_modes < 1 || n_modes > kDetectModes)
         return fail(CB200_ERR_ARG, "n_modes = " + std::to_string(n_modes) + ": between 1 and " + std::to_string(kDetectModes) + " candidate modes");
-    int rc = check_camera_dev_flags(flags); if (rc) return rc;
-    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
-    if (!wh) return fail(CB200_ERR_ARG, "null wh");
-    if (!d_pictures) return fail(CB200_ERR_ARG, "null pictures");
-    rc = check_picture_sizes(wh, n); if (rc) return rc;
-    size_t src_bytes;
-    rc = camera_source_bytes(wh, n, &src_bytes); if (rc) return rc;
+    int rc = check_camera_flags(flags); if (rc) return rc;
+    if ((rc = packed_batch(d_pictures, wh, n, b)) || (rc = check_spans(b))) return rc;
     if (!d_chunks || !d_chunk_mask || !d_extract_status || !d_mode) return fail(CB200_ERR_ARG, "null output");
     if (!ctxs) return fail(CB200_ERR_ARG, "null context list");
     for (int k = 0; k < n_modes; ++k)
@@ -115,10 +111,11 @@ struct StreamSwap {
     ~StreamSwap() { c->stream = was; c->shared_walk = nullptr; }
 };
 
-static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d, const int32_t* wh, int n, uint32_t flags,
-                          uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks)
+static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                          int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks)
 {
     cb200_ctx* c0 = ctxs[0];
+    const int n = b.n();
     int rc;
     // geometries: lead[g] = the first context of geometry g in priority order
     int group[kDetectModes], lead[kDetectModes], ng = 0;
@@ -130,7 +127,7 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d,
     }
     if (!c0->detect) c0->detect = new DetectState();
     DetectState* ds = c0->detect;
-    for (int k = 0; k < n_modes; ++k) { rc = camera_reserve_for(ctxs[k], wh, n, k == 0, lead[group[k]] == k); if (rc) return rc; }
+    for (int k = 0; k < n_modes; ++k) { rc = camera_reserve_for(ctxs[k], b.wh.data(), n, k == 0, lead[group[k]] == k); if (rc) return rc; }
     CK(ds->status.ensure((size_t)n_modes * n), "cudaMalloc detect statuses");
     uint8_t* frames[kDetectModes];
     for (int g = 0; g < ng; ++g) {
@@ -146,7 +143,7 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d,
         }
     }
     const PicDesc* d_desc;
-    rc = camera_scan(c0, d, wh, n, nullptr, &d_desc); if (rc) return rc;
+    rc = camera_scan(c0, b, nullptr, &d_desc); if (rc) return rc;
     cudaStream_t main = c0->stream;
     if (ng > 1) {
         CK(cudaEventRecord(ds->fork, main), "record detect fork");
@@ -159,8 +156,7 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d,
             if (group[k] != g) continue;
             cb200_ctx* c = ctxs[k];
             StreamSwap on(c, ng > 1 ? ds->side[g] : main, &sw);
-            rc = camera_after_scan(c, c0, d_desc, false, n, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr,
-                                   ds->status + (size_t)k * n);
+            rc = camera_after_scan(c, c0, b, d_desc, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr, ds->status + (size_t)k * n);
         }
     }
     if (ng > 1) {
@@ -192,8 +188,9 @@ extern "C" int cb200_detect_scan_extract_decode_chunks_dev(cb200_ctx* const* ctx
                                                            int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
                                                            int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks)
 {
-    int rc = check_detect(ctxs, n_modes, d_pictures, wh, n, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode); if (rc) return rc;
+    CameraBatch b;
+    int rc = check_detect(ctxs, n_modes, d_pictures, wh, n, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, b); if (rc) return rc;
     if (n == 0) return CB200_OK;
     CK(cudaSetDevice(ctxs[0]->device), "cudaSetDevice");
-    return detect_enqueue(ctxs, n_modes, d_pictures, wh, n, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
+    return detect_enqueue(ctxs, n_modes, b, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
 }

@@ -1,5 +1,5 @@
-// files.cu -- the plumbing both file decoders (jpeg.cu, png.cu) share: the pinned upload ring of a file call (ctx.cuh FileUpload)
-// and the status of its corrupt files (k_file_status)
+// files.cu -- the pinned upload ring (ctx.cuh UploadRing: the context's and each file decoder's) and the status of the corrupt
+// files of a file call (k_file_status), which both file decoders (jpeg.cu, png.cu) share
 #include "ctx.cuh"
 
 namespace cb200 {
@@ -19,21 +19,21 @@ int file_status(cb200_ctx* c, const int* d_bad, int n, int32_t* d_status, uint32
     return CB200_OK;
 }
 
-int FileUpload::take(size_t bytes, int* slot, uint8_t** host)
+int UploadRing::take(size_t bytes, int* slot, uint8_t** host)
 {
     *slot = next;
     next = (next + 1) % kSlots;
-    if (!ev[*slot]) CK(cudaEventCreateWithFlags(&ev[*slot], cudaEventDisableTiming), "cudaEventCreate file upload");
-    CK(cudaEventSynchronize(ev[*slot]), "sync (file upload slot)");   // the slot's last copy has run
-    CK(h[*slot].ensure(bytes), "cudaMallocHost file upload");
+    if (!ev[*slot]) CK(cudaEventCreateWithFlags(&ev[*slot], cudaEventDisableTiming), "cudaEventCreate upload slot");
+    CK(cudaEventSynchronize(ev[*slot]), "sync (upload slot)");   // the slot's last copy has run
+    CK(h[*slot].ensure(bytes), "cudaMallocHost upload slot");
     *host = h[*slot];
     return CB200_OK;
 }
 
-int FileUpload::send(cudaStream_t st, int slot, void* d_dst, size_t bytes)
+int UploadRing::send(cudaStream_t st, int slot, void* d_dst, size_t bytes)
 {
-    CK(cudaMemcpyAsync(d_dst, h[slot], bytes, cudaMemcpyHostToDevice, st), "H2D files");
-    CK(cudaEventRecord(ev[slot], st), "record file upload");
+    CK(cudaMemcpyAsync(d_dst, h[slot], bytes, cudaMemcpyHostToDevice, st), "H2D upload");
+    CK(cudaEventRecord(ev[slot], st), "record upload slot");
     return CB200_OK;
 }
 

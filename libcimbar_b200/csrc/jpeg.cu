@@ -4,7 +4,7 @@
 //
 // The host parses the markers (jpeg_core.cuh parse: tables, scans, restart intervals, EXIF orientation) and uploads the picture,
 // scan, segment and table descriptors together with the compressed files in one copy from a pinned ring of its own (ctx.cuh
-// FileUpload, the type the PNG calls use too).  Then,
+// UploadRing; the PNG calls have one too).  Then,
 // enqueued on the context's stream:
 //   k_jpeg_init     the per-picture corrupt flag from the parse (a file that ends inside its data)
 //   k_jpeg_unstuff  one CTA per segment (restart interval, or whole scan): FF 00 stuffing out by a flag + block-wide prefix sum
@@ -32,7 +32,7 @@ using namespace jpeg;
 constexpr int kSegThreads = 512;       // threads per segment in k_jpeg_unstuff / k_jpeg_decode
 
 struct JpegState {
-    FileUpload up;                     // the calls' uploads (descriptors + files)
+    UploadRing up;                     // the calls' uploads (descriptors + files)
     DevBuf<uint8_t> d_blob;            // the call's upload (descriptors + files)
     DevBuf<uint8_t> d_unstuffed;       // the segments' bytes without FF 00 stuffing, at their offsets in the data section
     DevBuf<uint32_t> d_ulen;           // per segment: its unstuffed bytes
@@ -304,21 +304,25 @@ int cb200_jpeg_decode_dev(cb200_ctx* c, const uint8_t* const* files, const uint6
 int cb200_jpeg_scan_extract_decode_chunks_dev(cb200_ctx* c, const uint8_t* const* files, const uint64_t* sizes, int n, uint32_t flags,
                                               uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
 {
+    // the decoded pictures are a packed batch of the sizes in the files' headers; where they go is known once they are decoded
     std::vector<Parsed> ps;
-    std::vector<int32_t> wh;
-    int rc = parse_files(files, sizes, n, ps, wh); if (rc) return rc;
-    rc = check_camera_dev_flags(flags); if (rc) return rc;
-    rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
-    rc = check_chain_call(c, flags); if (rc) return rc;
+    auto build = [&](CameraBatch& b) {
+        int rc = parse_files(files, sizes, n, ps, b.wh); if (rc) return rc;
+        b.pack(nullptr);
+        return CB200_OK;
+    };
+    CameraBatch b;
+    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
     if (n == 0) return camera_empty(c, flags);
-    rc = check_frozen_camera(c, wh.data(), n); if (rc) return rc;
+    rc = check_frozen_camera(c, b.wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     JpegState* j = jstate(c);
     uint64_t rgb = 0;
-    for (int i = 0; i < n; ++i) rgb += 3 * (uint64_t)wh[2 * (size_t)i] * (uint64_t)wh[2 * (size_t)i + 1];
+    for (int i = 0; i < n; ++i) rgb += 3 * (uint64_t)b.wh[2 * (size_t)i] * (uint64_t)b.wh[2 * (size_t)i + 1];
     CK(j->d_rgb.ensure(rgb), "cudaMalloc JPEG pictures");
     rc = jpeg_enqueue(c, ps, files, sizes, j->d_rgb); if (rc) return rc;
-    rc = camera_enqueue(c, j->d_rgb, wh.data(), n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status); if (rc) return rc;
+    b.pack(j->d_rgb);
+    rc = camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status); if (rc) return rc;
     return file_status(c, j->d_bad, n, d_extract_status, d_chunk_mask);
 }
 

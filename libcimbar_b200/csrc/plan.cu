@@ -70,8 +70,8 @@ int count_kernel_nodes(cudaGraph_t g, int* kernels)
 
 // camera_enqueue on the private stream `cap`, captured into p->graph.  The context's stream, timing and host CCM state are set aside
 // for the duration and restored: a capture runs nothing, so it changes nothing the host can observe
-int capture(cb200_camera_plan* p, cudaStream_t cap, const uint8_t* d_pictures, const int32_t* wh, uint8_t* d_chunks, uint32_t* d_mask,
-            uint8_t* d_frame_flags, int32_t* d_status)
+int capture(cb200_camera_plan* p, cudaStream_t cap, const CameraBatch& b, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags,
+            int32_t* d_status)
 {
     cb200_ctx* c = p->ctx;
     cudaEvent_t scratch_ev;                 // ccm_keep_last records c->ccm_ev: inside a capture that record joins the graph
@@ -89,8 +89,7 @@ int capture(cb200_camera_plan* p, cudaStream_t cap, const uint8_t* d_pictures, c
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) rc = fail_cuda(e, "cudaStreamBeginCapture");
     if (!rc) {
-        rc = camera_enqueue_table(c, d_pictures, wh, p->n, p->flags, d_chunks, d_mask, d_frame_flags, d_status,
-                                  reinterpret_cast<const PicDesc*>(p->d_table.get()));
+        rc = camera_enqueue(c, b, p->flags, d_chunks, d_mask, d_frame_flags, d_status, reinterpret_cast<const PicDesc*>(p->d_table.get()));
         cudaGraph_t g = nullptr;
         e = cudaStreamEndCapture(cap, &g);
         if (!rc && e != cudaSuccess) rc = fail_cuda(e, "cudaStreamEndCapture");
@@ -116,21 +115,18 @@ extern "C" {
 int cb200_camera_plan_create(cb200_ctx* c, const int32_t* wh, int n, uint32_t flags, const uint8_t* d_pictures, uint8_t* d_chunks,
                              uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out)
 {
-    // the checks of cb200_scan_extract_decode_chunks_ragged_dev, in its order, then the plan's own
-    int rc = check_camera_dev_flags(flags); if (rc) return rc;
-    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
-    if (!wh) return fail(CB200_ERR_ARG, "null wh");
-    if (!d_pictures) return fail(CB200_ERR_ARG, "null pictures");
-    rc = check_picture_sizes(wh, n); if (rc) return rc;
-    if (n == 0) return fail(CB200_ERR_ARG, "n = 0: a camera plan needs at least one picture");
-    if (!out) return fail(CB200_ERR_ARG, "null plan");
-    *out = nullptr;
-    rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
+    // the checks of cb200_scan_extract_decode_chunks_ragged_dev, with the plan's own after the batch's and after the CCM chain's
+    auto build = [&](CameraBatch& b) {
+        int rc = packed_batch(d_pictures, wh, n, b); if (rc) return rc;
+        if (n == 0) return fail(CB200_ERR_ARG, "n = 0: a camera plan needs at least one picture");
+        if (!out) return fail(CB200_ERR_ARG, "null plan");
+        *out = nullptr;
+        return CB200_OK;
+    };
+    CameraBatch b;
+    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
     if (check_host_ccm(c))
         return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
-    for (int i = 0; i < n; ++i)
-        if ((size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3 >= ((size_t)1 << 32))
-            return fail(CB200_ERR_ARG, "source picture " + std::to_string(i) + " of 4 GB or more");
     rc = check_frozen_camera(c, wh, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     // every buffer the graph uses, at this batch's size (with plans already there, the freeze check above guarantees this grows nothing)
@@ -141,7 +137,7 @@ int cb200_camera_plan_create(cb200_ctx* c, const int32_t* wh, int n, uint32_t fl
     p->keeps_ccm = (flags & CB200_FLAG_CC_SIMPLE) || ccm_fits(c->mode, flags);
     std::vector<uint8_t> table;
     cudaStream_t cap = nullptr;
-    rc = camera_table(c, d_pictures, wh, n, table);
+    rc = pic_table(c, b, table);
     if (!rc) { const cudaError_t e = p->d_table.ensure(table.size()); if (e != cudaSuccess) rc = fail_cuda(e, "cudaMalloc plan picture table"); }
     if (!rc) { const cudaError_t e = cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking); if (e != cudaSuccess) rc = fail_cuda(e, "cudaStreamCreate"); }
     if (!rc) {   // the table goes up once, on the private stream, before anything can replay
@@ -149,7 +145,7 @@ int cb200_camera_plan_create(cb200_ctx* c, const int32_t* wh, int n, uint32_t fl
         if (e == cudaSuccess) e = cudaStreamSynchronize(cap);
         if (e != cudaSuccess) rc = fail_cuda(e, "H2D plan picture table");
     }
-    if (!rc) rc = capture(p, cap, d_pictures, wh, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    if (!rc) rc = capture(p, cap, b, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
     if (cap) cudaStreamDestroy(cap);
     if (!rc) rc = count_kernel_nodes(p->graph, &p->kernels);
     if (!rc) { const cudaError_t e = cudaGraphInstantiate(&p->exec, p->graph, 0); if (e != cudaSuccess) rc = fail_cuda(e, "cudaGraphInstantiate"); }

@@ -5,7 +5,7 @@
 //
 // The host walks the chunks (png_core.cuh parse: IHDR, PLTE, eXIf, the IDAT chunks, the zlib header) and uploads the picture and
 // IDAT chunk descriptors, the palettes and each file's IDAT payloads back to back (its zlib stream) in one copy from the file
-// calls' pinned ring (ctx.cuh FileUpload).  Then, enqueued on the context's stream:
+// calls' pinned ring (ctx.cuh UploadRing).  Then, enqueued on the context's stream:
 //   k_png_crc       one warp per IDAT chunk: CRC-32 of 32 pieces, combined (png_core.cuh crc_piece / chunk_crc); a mismatch sets
 //                   the picture's corrupt flag
 //   k_png_inflate   one warp per file: lane 0 reads block headers and decodes batches of up to 32 tokens from a 64-bit bit buffer;
@@ -30,7 +30,7 @@ namespace cb200 {
 using namespace png;
 
 struct PngState {
-    FileUpload up;                     // the calls' uploads (descriptors + IDAT payloads)
+    UploadRing up;                     // the calls' uploads (descriptors + IDAT payloads)
     DevBuf<uint8_t> d_blob;            // the call's upload
     DevBuf<uint8_t> d_raw;             // filtered, then unfiltered, scanlines of every file
     DevBuf<int> d_bad;                 // per picture: corrupt data
@@ -276,21 +276,25 @@ int cb200_png_decode_dev(cb200_ctx* c, const uint8_t* const* files, const uint64
 int cb200_png_scan_extract_decode_chunks_dev(cb200_ctx* c, const uint8_t* const* files, const uint64_t* sizes, int n, uint32_t flags,
                                              uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
 {
+    // the decoded pictures are a packed batch of the sizes in the files' headers; where they go is known once they are decoded
     std::vector<Parsed> ps;
-    std::vector<int32_t> wh;
-    int rc = parse_files(files, sizes, n, ps, wh); if (rc) return rc;
-    rc = check_camera_dev_flags(flags); if (rc) return rc;
-    rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
-    rc = check_chain_call(c, flags); if (rc) return rc;
+    auto build = [&](CameraBatch& b) {
+        int rc = parse_files(files, sizes, n, ps, b.wh); if (rc) return rc;
+        b.pack(nullptr);
+        return CB200_OK;
+    };
+    CameraBatch b;
+    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
     if (n == 0) return camera_empty(c, flags);
-    rc = check_frozen_camera(c, wh.data(), n); if (rc) return rc;
+    rc = check_frozen_camera(c, b.wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     PngState* s = pstate(c);
     uint64_t rgb = 0;
-    for (int i = 0; i < n; ++i) rgb += 3 * (uint64_t)wh[2 * (size_t)i] * (uint64_t)wh[2 * (size_t)i + 1];
+    for (int i = 0; i < n; ++i) rgb += 3 * (uint64_t)b.wh[2 * (size_t)i] * (uint64_t)b.wh[2 * (size_t)i + 1];
     CK(s->d_rgb.ensure(rgb), "cudaMalloc PNG pictures");
     rc = png_enqueue(c, ps, files, s->d_rgb); if (rc) return rc;
-    rc = camera_enqueue(c, s->d_rgb, wh.data(), n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status); if (rc) return rc;
+    b.pack(s->d_rgb);
+    rc = camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status); if (rc) return rc;
     return file_status(c, s->d_bad, n, d_extract_status, d_chunk_mask);
 }
 

@@ -31,7 +31,7 @@ namespace cb200 {
 using namespace scan;
 
 struct ScanScratch {                 // per-context scratch of the scan entry points
-    DevBuf<uint8_t> d_pics;                                 // staging of host pictures
+    DevBuf<uint8_t> d_pics;                                 // host pictures of any call, staged (stage_batch)
     DevBuf<uint8_t> d_blur;                                 // blurred gray, n x h x w
     DevBuf<unsigned> d_hist; DevBuf<int> d_thr;
     DevBuf<Anchor> d_rowbuf; DevBuf<int> d_rowcnt; DevBuf<Anchor> d_pts; DevBuf<Anchor> d_res; DevBuf<int> d_nres;
@@ -278,6 +278,123 @@ std::vector<int32_t> uniform_sizes(int w, int h, int n)
     return wh;
 }
 
+void CameraBatch::pack(const uint8_t* d)
+{
+    pics.resize((size_t)n());
+    size_t off = 0;
+    for (int i = 0; i < n(); ++i) {
+        const int w = wh[2 * (size_t)i], h = wh[2 * (size_t)i + 1];
+        pics[(size_t)i] = cb200_picture{d ? d + off : nullptr, w, h, 3 * (int64_t)w, 0, CB200_LAYOUT_RGB};
+        off += 3 * (size_t)w * (size_t)h;
+    }
+    packed = true;
+}
+
+// the checks every builder of a packed or host batch starts with; b.wh = the sizes
+static int sized_batch(const void* pictures, const int32_t* wh, int n, CameraBatch& b)
+{
+    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
+    if (!wh) return fail(CB200_ERR_ARG, "null wh");
+    if (!pictures) return fail(CB200_ERR_ARG, "null pictures");
+    int rc = check_picture_sizes(wh, n); if (rc) return rc;
+    b.wh.assign(wh, wh + 2 * (size_t)n);
+    return CB200_OK;
+}
+
+int packed_batch(const uint8_t* d, const int32_t* wh, int n, CameraBatch& b)
+{
+    int rc = sized_batch(d, wh, n, b); if (rc) return rc;
+    b.pack(d);
+    return CB200_OK;
+}
+
+int uniform_batch(const uint8_t* d, int w, int h, int n, CameraBatch& b)
+{
+    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
+    if (!d) return fail(CB200_ERR_ARG, "null pictures");
+    b.wh = uniform_sizes(w, h, n);
+    int rc = check_picture_sizes(b.wh.data(), n); if (rc) return rc;
+    b.pack(d);
+    return CB200_OK;
+}
+
+int host_batch(const uint8_t* const* pictures, const int32_t* wh, int n, CameraBatch& b)
+{
+    int rc = sized_batch(pictures, wh, n, b); if (rc) return rc;
+    b.pack(nullptr);
+    for (int i = 0; i < n; ++i) {
+        if (!pictures[i]) return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " is a null pointer");
+        b.pics[(size_t)i].data = pictures[i];
+    }
+    b.host = true;
+    return CB200_OK;
+}
+
+int picture_batch(const cb200_picture* pics, int n, CameraBatch& b)
+{
+    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
+    if (!pics) return fail(CB200_ERR_ARG, "null pictures");
+    b.wh.assign(2 * (size_t)n, 0);
+    for (int i = 0; i < n; ++i) {
+        const cb200_picture& p = pics[i];
+        const std::string name = "picture " + std::to_string(i);
+        if (!p.data) return fail(CB200_ERR_ARG, name + " has a null data pointer");
+        if (!layout::known(p.layout)) return fail(CB200_ERR_ARG, name + " has an unknown layout " + std::to_string(p.layout));
+        if (p.row_pitch < 0 || p.plane_pitch < 0)
+            return fail(CB200_ERR_ARG, name + " has a negative " + (p.row_pitch < 0 ? "row" : "plane") + " pitch");
+        b.wh[2 * (size_t)i] = p.w; b.wh[2 * (size_t)i + 1] = p.h;
+    }
+    int rc = check_picture_sizes(b.wh.data(), n); if (rc) return rc;
+    b.packed = true;
+    for (int i = 0; i < n; ++i) {
+        const cb200_picture& p = pics[i];
+        const int64_t row = (int64_t)p.w * layout::channels(p.layout);
+        if (p.row_pitch < row)
+            return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " has a row pitch of " + std::to_string(p.row_pitch) +
+                                           " bytes, below w x channels = " + std::to_string(row));
+        if (p.layout == CB200_LAYOUT_RGB_PLANAR && p.plane_pitch < (int64_t)p.h * p.row_pitch)
+            return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " has overlapping planes: a plane pitch of " + std::to_string(p.plane_pitch) +
+                                           " bytes, below h x row pitch = " + std::to_string((int64_t)p.h * p.row_pitch));
+        b.packed = b.packed && p.layout == CB200_LAYOUT_RGB && p.row_pitch == row;
+    }
+    b.pics.assign(pics, pics + n);
+    return CB200_OK;
+}
+
+int check_spans(const CameraBatch& b)
+{
+    const int64_t lim = (int64_t)1 << 32;
+    for (int i = 0; i < b.n(); ++i) {
+        const cb200_picture& p = b.pics[(size_t)i];
+        const bool planar = p.layout == CB200_LAYOUT_RGB_PLANAR;
+        if (p.row_pitch >= lim || (planar && p.plane_pitch >= lim) ||
+            (planar ? 2 * p.plane_pitch : 0) + (int64_t)(p.h - 1) * p.row_pitch + (int64_t)p.w * layout::channels(p.layout) >= lim)
+            return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " spans 4 GB or more");
+    }
+    return CB200_OK;
+}
+
+int stage_batch(cb200_ctx* c, CameraBatch& b)
+{
+    if (!b.host) return CB200_OK;
+    ScanScratch* s = sstate(c);
+    size_t bytes = 0;
+    for (int i = 0; i < b.n(); ++i) bytes += 3 * (size_t)b.pics[(size_t)i].w * (size_t)b.pics[(size_t)i].h;
+    CK(s->d_pics.ensure(bytes), "cudaMalloc picture staging");
+    size_t off = 0;
+    for (int i = 0; i < b.n();) {
+        const uint8_t* src = b.pics[(size_t)i].data;
+        size_t run = 0;
+        do run += 3 * (size_t)b.pics[(size_t)i].w * (size_t)b.pics[(size_t)i].h;
+        while (++i < b.n() && b.pics[(size_t)i].data == src + run);
+        CK(cudaMemcpyAsync(s->d_pics + off, src, run, cudaMemcpyHostToDevice, c->stream), "H2D pictures");
+        off += run;
+    }
+    b.pack(s->d_pics);
+    b.host = false;
+    return CB200_OK;
+}
+
 // rows of a scan pass for one picture: the primary pass scans h / skip rows, the bottom-right window at most 2 h / skip (half the step)
 static int scan_rows(int w, int h)
 {
@@ -320,8 +437,11 @@ struct BlurGroups {
 
 // the descriptor table (batch order), then the pictures grouped by blur radius (batch order inside a group) into `table`; the tiles
 // of one radius are numbered across its pictures.  The word path depends on where the pictures and the scan's blurred buffer are
-static int pic_table(const ScanScratch* s, const cb200_picture* pics, const int32_t* wh, int n, uint8_t* table, BlurGroups& g)
+static int pic_table(const ScanScratch* s, const CameraBatch& b, uint8_t* table, BlurGroups& g)
 {
+    const int n = b.n();
+    const int32_t* wh = b.wh.data();
+    const cb200_picture* pics = b.pics.data();
     PicDesc* desc = reinterpret_cast<PicDesc*>(table);
     int* order = reinterpret_cast<int*>(desc + n);
     int first[5] = {};
@@ -356,55 +476,35 @@ static int pic_table(const ScanScratch* s, const cb200_picture* pics, const int3
 int camera_pictures(cb200_ctx* c) { return sstate(c)->camera_n; }
 void set_camera_pictures(cb200_ctx* c, int n) { sstate(c)->camera_n = n; }
 
-std::vector<cb200_picture> packed_pictures(const uint8_t* d, const int32_t* wh, int n)
+int pic_table(cb200_ctx* c, const CameraBatch& b, std::vector<uint8_t>& table)
 {
-    std::vector<cb200_picture> p((size_t)(n > 0 ? n : 0));
-    size_t off = 0;
-    for (int i = 0; i < n; ++i) {
-        const int w = wh[2 * i], h = wh[2 * i + 1];
-        p[(size_t)i] = cb200_picture{d + off, w, h, 3 * (int64_t)w, 0, CB200_LAYOUT_RGB};
-        off += 3 * (size_t)w * (size_t)h;
-    }
-    return p;
-}
-
-// every picture in packed RGB rows (layout RGB, row pitch 3 w): the kernels' packed instantiations take the batch
-static bool packed_rgb(const cb200_picture* pics, int n)
-{
-    for (int i = 0; i < n; ++i)
-        if (pics[i].layout != CB200_LAYOUT_RGB || pics[i].row_pitch != 3 * (int64_t)pics[i].w) return false;
-    return true;
-}
-
-int camera_table(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n, std::vector<uint8_t>& table)
-{
-    table.assign((sizeof(PicDesc) + sizeof(int)) * (size_t)n, 0);
+    table.assign((sizeof(PicDesc) + sizeof(int)) * (size_t)b.n(), 0);
     BlurGroups g;
-    return pic_table(sstate(c), packed_pictures(d_pics, wh, n).data(), wh, n, table.data(), g);
+    return pic_table(sstate(c), b, table.data(), g);
 }
 
-// blurred pictures + thresholds + anchors for n pictures of sizes wh (checked by check_picture_sizes) described by pics, in the
-// state's device arrays; enqueued only.  The picture table (PicDesc, in s->d_table) is this call's one upload -- unless d_table
-// holds it already (a camera plan's): then *d_desc = d_table and nothing is uploaded
-static int scan_enqueue(cb200_ctx* c, const cb200_picture* pics, const int32_t* wh, int n, const PicDesc* d_table = nullptr,
-                        const PicDesc** d_desc_out = nullptr)
+// blurred pictures + thresholds + anchors for a device batch, in the state's device arrays; enqueued only.  The picture table
+// (PicDesc, in s->d_table) is this call's one upload -- unless d_table holds it already (a camera plan's): then *d_desc = d_table
+// and nothing is uploaded
+int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc_out)
 {
     ScanScratch* s = sstate(c);
     cudaStream_t st = c->stream;
-    int err = scan_reserve(c, wh, n); if (err) return err;
+    const int n = b.n();
+    int err = scan_reserve(c, b.wh.data(), n); if (err) return err;
     const size_t table_bytes = (sizeof(PicDesc) + sizeof(int)) * (size_t)n;
     BlurGroups g;
     const PicDesc* d_desc = d_table;
     if (d_table) {
         std::vector<uint8_t> table(table_bytes);
-        err = pic_table(s, pics, wh, n, table.data(), g); if (err) return err;
+        err = pic_table(s, b, table.data(), g); if (err) return err;
     } else {
         CK(s->d_table.ensure(table_bytes), "cudaMalloc picture table");
         int slot;
         uint8_t* h_table;
-        err = stage_take(c, table_bytes, &slot, &h_table); if (err) return err;
-        err = pic_table(s, pics, wh, n, h_table, g); if (err) return err;
-        err = stage_send(c, slot, s->d_table, table_bytes, "H2D picture table"); if (err) return err;
+        err = c->upload.take(table_bytes, &slot, &h_table); if (err) return err;
+        err = pic_table(s, b, h_table, g); if (err) return err;
+        err = c->upload.send(st, slot, s->d_table, table_bytes); if (err) return err;
         d_desc = reinterpret_cast<const PicDesc*>(s->d_table.get());
     }
     if (d_desc_out) *d_desc_out = d_desc;
@@ -412,7 +512,7 @@ static int scan_enqueue(cb200_ctx* c, const cb200_picture* pics, const int32_t* 
     const int* group0 = g.group0;
     const long long* tiles = g.tiles;
     const bool* same = g.same;
-    const bool layouts = !packed_rgb(pics, n);
+    const bool layouts = !b.packed;
     const int* d_order = reinterpret_cast<const int*>(d_desc + n);
     CK(cudaMemsetAsync(s->d_hist, 0, sizeof(unsigned) * 256 * (size_t)n, st), "memset histograms");
     // cb200_set_timing: one event set per scan -- [blur + histogram (all radii), Otsu, anchors] through cb200_get_timing
@@ -445,10 +545,11 @@ static int scan_enqueue(cb200_ctx* c, const cb200_picture* pics, const int32_t* 
     return CB200_OK;
 }
 
-// scan_enqueue, then its results into the pinned host arrays of the state
-static int scan_run(cb200_ctx* c, const uint8_t* d_pics, const int32_t* wh, int n)
+// camera_scan, then its results into the pinned host arrays of the state
+static int scan_run(cb200_ctx* c, const CameraBatch& b)
 {
-    int rc = scan_enqueue(c, packed_pictures(d_pics, wh, n).data(), wh, n); if (rc) return rc;
+    const int n = b.n();
+    int rc = camera_scan(c, b, nullptr, nullptr); if (rc) return rc;
     ScanScratch* s = c->scan;
     cudaStream_t st = c->stream;
     CK(s->h_anchors.ensure(4 * (size_t)n), "cudaMallocHost anchors");
@@ -473,31 +574,6 @@ static int scan_results(cb200_ctx* c, int n, int32_t* anchors, int32_t* count, u
     return CB200_OK;
 }
 
-// the host pictures, packed into the staging buffer with one copy each
-static int stage_pictures(cb200_ctx* c, const uint8_t* const* pics, const int32_t* wh, int n, const uint8_t** d_out)
-{
-    ScanScratch* s = sstate(c);
-    size_t bytes = 0;
-    for (int i = 0; i < n; ++i) bytes += (size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3;
-    CK(s->d_pics.ensure(bytes), "cudaMalloc picture staging");
-    size_t off = 0;
-    for (int i = 0; i < n; ++i) {
-        const size_t b = (size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3;
-        CK(cudaMemcpyAsync(s->d_pics + off, pics[i], b, cudaMemcpyHostToDevice, c->stream), "H2D pictures");
-        off += b;
-    }
-    *d_out = s->d_pics;
-    return CB200_OK;
-}
-
-// the host pointers of a uniform batch (picture i at pics + i w h 3)
-static std::vector<const uint8_t*> uniform_pointers(const uint8_t* pics, int w, int h, int n)
-{
-    std::vector<const uint8_t*> p((size_t)n);
-    for (int i = 0; i < n; ++i) p[(size_t)i] = pics + (size_t)i * w * h * 3;
-    return p;
-}
-
 // Extractor::extract (Extractor.h:30-46) of every picture of a scan, on the device: one thread per picture
 __global__ void k_extract(const int4* __restrict__ anchors, const int* __restrict__ count, const int* __restrict__ scan_status, int n,
                           int width, int height, int32_t* __restrict__ status, double* __restrict__ minv, double* __restrict__ fwd,
@@ -518,15 +594,6 @@ __global__ void k_mask_failed(const int32_t* __restrict__ status, int n, uint32_
     if (i < n && status[i] <= 0) mask[i] = 0;
 }
 
-// Extractor::extract + Decoder::decode_fountain for n pictures of sizes wh packed in device memory, enqueued on the context's stream
-// without a host round trip: scan, k_extract, deskew with the scan's picture table, decode (with CB200_FLAG_SHARPEN_IF_NEEDED the
-// frame lists are built on the device), masks of failed pictures cleared.  The arguments are checked by the caller
-int camera_enqueue(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
-                   uint8_t* d_frame_flags, int32_t* d_status)
-{
-    return camera_enqueue_table(c, d, wh, n, flags, d_chunks, d_mask, d_frame_flags, d_status, nullptr);
-}
-
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks)
 {
     ScanScratch* s = sstate(c);
@@ -540,26 +607,11 @@ int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool 
 
 int camera_reserve(cb200_ctx* c, const int32_t* wh, int n) { return camera_reserve_for(c, wh, n, true, true); }
 
-int camera_source_bytes(const int32_t* wh, int n, size_t* bytes)
-{
-    *bytes = 0;
-    for (int i = 0; i < n; ++i) {
-        const size_t b = (size_t)wh[2 * i] * (size_t)wh[2 * i + 1] * 3;
-        if (b >= ((size_t)1 << 32)) return fail(CB200_ERR_ARG, "source picture " + std::to_string(i) + " of 4 GB or more");   // k_deskew's offsets
-        *bytes += b;
-    }
-    return CB200_OK;
-}
-
-int camera_scan(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, const PicDesc* d_table, const PicDesc** d_desc)
-{
-    return scan_enqueue(c, packed_pictures(d, wh, n).data(), wh, n, d_table, d_desc);
-}
-
-int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const PicDesc* d_desc, bool layouts, int n, uint32_t flags, uint8_t* frames,
+int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
                       bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status)
 {
     const Mode& m = c->mode;
+    const int n = b.n();
     ScanScratch* s = sstate(c);
     const ScanScratch* s0 = scanned->scan;
     const bool if_needed = (flags & CB200_FLAG_SHARPEN_IF_NEEDED) != 0;
@@ -569,7 +621,7 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const PicDesc* d_d
     CK(cudaGetLastError(), "extract launch");
     s->camera_n = n;
     int rc;
-    if (deskew) { rc = deskew_launch(c, s->d_minv, d_desc, layouts, n, frames); if (rc) return rc; }
+    if (deskew) { rc = deskew_launch(c, b, s->d_minv, d_desc, frames); if (rc) return rc; }
     rc = decode_chunks_enqueue(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, d_sharp, d_chunks, d_mask, d_frame_flags); if (rc) return rc;
     k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
     count_launch();
@@ -577,111 +629,73 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const PicDesc* d_d
     return CB200_OK;
 }
 
-// the camera path for n pictures of sizes wh described by pics, arguments checked
-static int camera_enqueue_pictures(cb200_ctx* c, const cb200_picture* pics, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks,
-                                   uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table)
+// Extractor::extract + Decoder::decode_fountain for a device batch, enqueued on the context's stream without a host round trip:
+// scan, k_extract, deskew with the scan's picture table, decode (with CB200_FLAG_SHARPEN_IF_NEEDED the frame lists are built on
+// the device), masks of failed pictures cleared
+int camera_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags,
+                   int32_t* d_status, const PicDesc* d_table)
 {
-    int rc = camera_reserve(c, wh, n); if (rc) return rc;
+    int rc = camera_reserve(c, b.wh.data(), b.n()); if (rc) return rc;
     uint8_t* frames;
-    rc = deskew_frames(c, n, &frames); if (rc) return rc;
+    rc = deskew_frames(c, b.n(), &frames); if (rc) return rc;
     const PicDesc* d_desc;
-    rc = scan_enqueue(c, pics, wh, n, d_table, &d_desc); if (rc) return rc;
-    return camera_after_scan(c, c, d_desc, !packed_rgb(pics, n), n, flags, frames, true, d_chunks, d_mask, d_frame_flags, d_status);
+    rc = camera_scan(c, b, d_table, &d_desc); if (rc) return rc;
+    return camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_mask, d_frame_flags, d_status);
 }
 
-int camera_enqueue_table(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask,
-                         uint8_t* d_frame_flags, int32_t* d_status, const PicDesc* d_table)
+int check_camera_flags(uint32_t flags)
 {
-    size_t src_bytes;
-    int rc = camera_source_bytes(wh, n, &src_bytes); if (rc) return rc;
-    return camera_enqueue_pictures(c, packed_pictures(d, wh, n).data(), wh, n, flags, d_chunks, d_mask, d_frame_flags, d_status, d_table);
-}
-
-// the synchronous camera entry points: the enqueue-only path into the context's buffers, one copy back, one synchronise
-static int scan_extract_decode(cb200_ctx* c, const uint8_t* d, const int32_t* wh, int n, uint32_t flags, uint8_t* chunks_out,
-                               uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags, int32_t* extract_status)
-{
-    ScanScratch* s = sstate(c);
-    CK(s->d_ext_status.ensure((size_t)n), "cudaMalloc extract status");
-    int rc = camera_enqueue(c, d, wh, n, flags, c->d_data, c->d_mask, nullptr, s->d_ext_status); if (rc) return rc;
-    return fetch_fountain(c, n, s->d_ext_status, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
-}
-
-// the argument checks of the ragged entry points, all before any CUDA call
-static int check_ragged(const int32_t* wh, const void* pictures, int n)
-{
-    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
-    if (!wh) return fail(CB200_ERR_ARG, "null wh");
-    if (!pictures) return fail(CB200_ERR_ARG, "null pictures");
-    return check_picture_sizes(wh, n);
-}
-
-static int check_host_pictures(const uint8_t* const* pictures, int n)
-{
-    for (int i = 0; i < n; ++i)
-        if (!pictures[i]) return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " is a null pointer");
-    return CB200_OK;
-}
-
-int check_camera_dev_flags(uint32_t flags)
-{
-    int rc = check_camera_flags(flags); if (rc) return rc;
+    // both sharpen flags together are a contradiction (CB200_FLAG_SHARPEN_IF_NEEDED is the CLI's --preprocess -1, SHARPEN its 1)
+    if ((flags & CB200_FLAG_SHARPEN) && (flags & CB200_FLAG_SHARPEN_IF_NEEDED))
+        return fail(CB200_ERR_ARG, "CB200_FLAG_SHARPEN and CB200_FLAG_SHARPEN_IF_NEEDED are exclusive");
     if ((flags & CB200_FLAG_CC_FIT) && (flags & CB200_FLAG_CC_SIMPLE)) return fail(CB200_ERR_ARG, "CC_SIMPLE and CC_FIT are exclusive");
     return CB200_OK;
 }
 
-int check_camera_dev_outputs(cb200_ctx* c, int n, const uint8_t* d_chunks, const uint32_t* d_chunk_mask, const int32_t* d_extract_status)
+// the synchronous camera entry points: the batch checked and staged, the enqueue-only path into the context's buffers, one copy
+// back, one synchronise
+template <class Build>
+static int scan_extract_decode(cb200_ctx* c, Build&& build, uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
+                               uint8_t* frame_flags, int32_t* extract_status)
 {
-    if (!c) return fail(CB200_ERR_ARG, "null context");
-    if (!d_chunks || !d_chunk_mask || !d_extract_status) return fail(CB200_ERR_ARG, "null output");
-    if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
-    return CB200_OK;
+    CameraBatch b;
+    int rc = check_camera_call(c, flags, build, b, chunks_out && chunk_count && extract_status ? nullptr : "null output"); if (rc) return rc;
+    const int n = b.n();
+    if (n == 0) return camera_empty(c, flags);
+    rc = check_frozen_camera(c, b.wh.data(), n); if (rc) return rc;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    rc = stage_batch(c, b); if (rc) return rc;
+    ScanScratch* s = sstate(c);
+    CK(s->d_ext_status.ensure((size_t)n), "cudaMalloc extract status");
+    rc = camera_enqueue(c, b, flags, c->d_data, c->d_mask, nullptr, s->d_ext_status); if (rc) return rc;
+    return fetch_fountain(c, n, s->d_ext_status, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
 }
 
-// the argument checks of the enqueue-only camera entry point, all before any CUDA call
-static int check_camera_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32_t* wh, int n, uint32_t flags, const uint8_t* d_chunks,
-                            const uint32_t* d_chunk_mask, const int32_t* d_extract_status)
+// the enqueue-only camera entry points on device pictures
+template <class Build>
+static int scan_extract_decode_dev(cb200_ctx* c, Build&& build, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                                   int32_t* d_extract_status)
 {
-    int rc = check_camera_dev_flags(flags); if (rc) return rc;
-    rc = check_ragged(wh, d_pictures, n); if (rc) return rc;
-    rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
-    rc = check_chain_call(c, flags); if (rc) return rc;
-    return check_frozen_camera(c, wh, n);
+    CameraBatch b;
+    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
+    if (b.n() == 0) return camera_empty(c, flags);
+    rc = check_frozen_camera(c, b.wh.data(), b.n()); if (rc) return rc;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
 }
 
-// the picture descriptors of cb200_scan_extract_decode_chunks_pictures_dev, all before any CUDA call; wh = their sizes
-static int check_pictures(const cb200_picture* pics, int n, std::vector<int32_t>& wh)
+// the scan entry points: the batch, the context and the count output checked, the batch staged and scanned, the results copied out
+static int scan_call(cb200_ctx* c, int built, CameraBatch& b, int32_t* anchors, int32_t* count, uint32_t* cutoff)
 {
-    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
-    if (!pics) return fail(CB200_ERR_ARG, "null pictures");
-    wh.assign(2 * (size_t)n, 0);
-    for (int i = 0; i < n; ++i) {
-        const cb200_picture& p = pics[i];
-        const std::string name = "picture " + std::to_string(i);
-        if (!p.data) return fail(CB200_ERR_ARG, name + " has a null data pointer");
-        if (!layout::known(p.layout)) return fail(CB200_ERR_ARG, name + " has an unknown layout " + std::to_string(p.layout));
-        if (p.row_pitch < 0 || p.plane_pitch < 0)
-            return fail(CB200_ERR_ARG, name + " has a negative " + (p.row_pitch < 0 ? "row" : "plane") + " pitch");
-        wh[2 * (size_t)i] = p.w; wh[2 * (size_t)i + 1] = p.h;
-    }
-    int rc = check_picture_sizes(wh.data(), n); if (rc) return rc;
-    for (int i = 0; i < n; ++i) {
-        const cb200_picture& p = pics[i];
-        const std::string name = "picture " + std::to_string(i);
-        const bool planar = p.layout == CB200_LAYOUT_RGB_PLANAR;
-        const int64_t row = (int64_t)p.w * layout::channels(p.layout);
-        if (p.row_pitch < row)
-            return fail(CB200_ERR_ARG, name + " has a row pitch of " + std::to_string(p.row_pitch) + " bytes, below w x channels = " + std::to_string(row));
-        if (planar && p.plane_pitch < (int64_t)p.h * p.row_pitch)
-            return fail(CB200_ERR_ARG, name + " has overlapping planes: a plane pitch of " + std::to_string(p.plane_pitch) + " bytes, below h x row pitch = " +
-                                           std::to_string((int64_t)p.h * p.row_pitch));
-        // k_deskew's offsets inside a picture are 32-bit
-        const int64_t lim = (int64_t)1 << 32;
-        if (p.row_pitch >= lim || (planar && p.plane_pitch >= lim) ||
-            (planar ? 2 * p.plane_pitch : 0) + (int64_t)(p.h - 1) * p.row_pitch + row >= lim)
-            return fail(CB200_ERR_ARG, name + " spans 4 GB or more");
-    }
-    return CB200_OK;
+    if (built) return built;
+    if (!c || !count) return fail(CB200_ERR_ARG, !c ? "null context" : "null count");
+    const int n = b.n();
+    if (n == 0) return CB200_OK;
+    int rc = check_frozen_scan(c, b.wh.data(), n); if (rc) return rc;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    rc = stage_batch(c, b); if (rc) return rc;
+    rc = scan_run(c, b); if (rc) return rc;
+    return scan_results(c, n, anchors, count, cutoff);
 }
 
 int camera_empty(cb200_ctx* c, uint32_t flags)
@@ -698,53 +712,31 @@ extern "C" {
 
 int cb200_scan_dev(cb200_ctx* c, const uint8_t* d_pictures, int w, int h, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
 {
-    if (!c || !d_pictures || !count || n < 0 || w < 1 || h < 1) return fail(CB200_ERR_ARG, "bad arguments");
-    if (n == 0) return CB200_OK;
-    const std::vector<int32_t> wh = uniform_sizes(w, h, n);
-    int rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
-    rc = check_frozen_scan(c, wh.data(), n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    rc = scan_run(c, d_pictures, wh.data(), n); if (rc) return rc;
-    return scan_results(c, n, anchors, count, cutoff);
+    CameraBatch b;
+    const int rc = uniform_batch(d_pictures, w, h, n, b);
+    return scan_call(c, rc, b, anchors, count, cutoff);
 }
 
 int cb200_scan(cb200_ctx* c, const uint8_t* pictures, int w, int h, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
 {
-    if (!c || !pictures || !count || n < 0 || w < 1 || h < 1) return fail(CB200_ERR_ARG, "bad arguments");
-    if (n == 0) return CB200_OK;
-    const std::vector<int32_t> wh = uniform_sizes(w, h, n);
-    int rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
-    rc = check_frozen_scan(c, wh.data(), n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    const uint8_t* d = nullptr;
-    rc = stage_pictures(c, uniform_pointers(pictures, w, h, n).data(), wh.data(), n, &d); if (rc) return rc;
-    rc = scan_run(c, d, wh.data(), n); if (rc) return rc;
-    return scan_results(c, n, anchors, count, cutoff);
+    CameraBatch b;
+    const int rc = uniform_batch(pictures, w, h, n, b);
+    b.host = true;
+    return scan_call(c, rc, b, anchors, count, cutoff);
 }
 
 int cb200_scan_ragged_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32_t* wh, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
 {
-    int rc = check_ragged(wh, d_pictures, n); if (rc) return rc;
-    if (!c || !count) return fail(CB200_ERR_ARG, !c ? "null context" : "null count");
-    if (n == 0) return CB200_OK;
-    rc = check_frozen_scan(c, wh, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    rc = scan_run(c, d_pictures, wh, n); if (rc) return rc;
-    return scan_results(c, n, anchors, count, cutoff);
+    CameraBatch b;
+    const int rc = packed_batch(d_pictures, wh, n, b);
+    return scan_call(c, rc, b, anchors, count, cutoff);
 }
 
 int cb200_scan_ragged(cb200_ctx* c, const uint8_t* const* pictures, const int32_t* wh, int n, int32_t* anchors, int32_t* count, uint32_t* cutoff)
 {
-    int rc = check_ragged(wh, pictures, n); if (rc) return rc;
-    rc = check_host_pictures(pictures, n); if (rc) return rc;
-    if (!c || !count) return fail(CB200_ERR_ARG, !c ? "null context" : "null count");
-    if (n == 0) return CB200_OK;
-    rc = check_frozen_scan(c, wh, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    const uint8_t* d = nullptr;
-    rc = stage_pictures(c, pictures, wh, n, &d); if (rc) return rc;
-    rc = scan_run(c, d, wh, n); if (rc) return rc;
-    return scan_results(c, n, anchors, count, cutoff);
+    CameraBatch b;
+    const int rc = host_batch(pictures, wh, n, b);
+    return scan_call(c, rc, b, anchors, count, cutoff);
 }
 
 // the first npx blurred bytes and n thresholds of the last scan
@@ -777,69 +769,41 @@ int cb200_scan_extract_decode_fountain(cb200_ctx* c, const uint8_t* pictures, in
                                        uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
                                        int32_t* extract_status)
 {
-    int rc = check_camera_flags(flags); if (rc) return rc;
-    if (!c || !pictures || !chunks_out || !chunk_count || !extract_status || n < 0 || n > c->max_frames || w < 2 || h < 2)
-        return fail(CB200_ERR_ARG, "bad arguments");
-    rc = check_chain_call(c, flags); if (rc) return rc;
-    if (n == 0) return camera_empty(c, flags);
-    const std::vector<int32_t> wh = uniform_sizes(w, h, n);
-    rc = check_picture_sizes(wh.data(), 1); if (rc) return rc;
-    rc = check_frozen_camera(c, wh.data(), n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    const uint8_t* d = nullptr;
-    rc = stage_pictures(c, uniform_pointers(pictures, w, h, n).data(), wh.data(), n, &d); if (rc) return rc;
-    return scan_extract_decode(c, d, wh.data(), n, flags, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
+    auto build = [&](CameraBatch& b) {
+        const int rc = uniform_batch(pictures, w, h, n, b);
+        b.host = true;
+        return rc;
+    };
+    return scan_extract_decode(c, build, flags, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
 }
 
 int cb200_scan_extract_decode_fountain_ragged(cb200_ctx* c, const uint8_t* const* pictures, const int32_t* wh, int n, uint32_t flags,
                                               uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags,
                                               int32_t* extract_status)
 {
-    int rc = check_camera_flags(flags); if (rc) return rc;
-    rc = check_ragged(wh, pictures, n); if (rc) return rc;
-    rc = check_host_pictures(pictures, n); if (rc) return rc;
-    if (!c) return fail(CB200_ERR_ARG, "null context");
-    if (!chunks_out || !chunk_count || !extract_status) return fail(CB200_ERR_ARG, "null output");
-    if (n > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames));
-    rc = check_chain_call(c, flags); if (rc) return rc;
-    if (n == 0) return camera_empty(c, flags);
-    rc = check_frozen_camera(c, wh, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    const uint8_t* d = nullptr;
-    rc = stage_pictures(c, pictures, wh, n, &d); if (rc) return rc;
-    return scan_extract_decode(c, d, wh, n, flags, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
+    auto build = [&](CameraBatch& b) { return host_batch(pictures, wh, n, b); };
+    return scan_extract_decode(c, build, flags, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
 }
 
 int cb200_scan_extract_decode_chunks_ragged_dev(cb200_ctx* c, const uint8_t* d_pictures, const int32_t* wh, int n, uint32_t flags,
                                                 uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
 {
-    int rc = check_camera_dev(c, d_pictures, wh, n, flags, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
-    if (n == 0) return camera_empty(c, flags);
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    return camera_enqueue(c, d_pictures, wh, n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    auto build = [&](CameraBatch& b) { return packed_batch(d_pictures, wh, n, b); };
+    return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
 }
 
 int cb200_scan_extract_decode_chunks_dev(cb200_ctx* c, const uint8_t* d_pictures, int w, int h, int n, uint32_t flags, uint8_t* d_chunks,
                                          uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
 {
-    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
-    const std::vector<int32_t> wh = uniform_sizes(w, h, n);
-    return cb200_scan_extract_decode_chunks_ragged_dev(c, d_pictures, wh.data(), n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    auto build = [&](CameraBatch& b) { return uniform_batch(d_pictures, w, h, n, b); };
+    return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
 }
 
 int cb200_scan_extract_decode_chunks_pictures_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, uint8_t* d_chunks,
                                                   uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
 {
-    // the checks of cb200_scan_extract_decode_chunks_ragged_dev, in its order, with the descriptors' in place of wh and the pictures
-    int rc = check_camera_dev_flags(flags); if (rc) return rc;
-    std::vector<int32_t> wh;
-    rc = check_pictures(pics, n, wh); if (rc) return rc;
-    rc = check_camera_dev_outputs(c, n, d_chunks, d_chunk_mask, d_extract_status); if (rc) return rc;
-    rc = check_chain_call(c, flags); if (rc) return rc;
-    rc = check_frozen_camera(c, wh.data(), n); if (rc) return rc;
-    if (n == 0) return camera_empty(c, flags);
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    return camera_enqueue_pictures(c, pics, wh.data(), n, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr);
+    auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
+    return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
 }
 
 int cb200_camera_transforms(cb200_ctx* c, double* m9_out, int n)
