@@ -51,7 +51,9 @@ extern "C" {
                                          and the frame's colours are decided with it.  A frame without a usable header keeps
                                          the CCM of the frame before it (frame 0: the context's), exactly like the
                                          reference's thread-local decoder state when frames are decoded in order; the
-                                         context's CCM afterwards is the last frame's.  Mutually exclusive with CC_SIMPLE. */
+                                         context's CCM afterwards is the last frame's.  Mutually exclusive with CC_SIMPLE:
+                                         every entry point that honours CC_FIT refuses the pair with CB200_ERR_ARG before
+                                         any CUDA call, whatever n is. */
 
 #define CB200_FLAG_NO_INTERLEAVE 0x10u /* Decoder(use_ecc, interleave=false): cells map to stream slots in linear order
                                          (Interleave::interleave_indices with num_chunks == 0, Interleave.h:10-16; Decoder.h:68) */

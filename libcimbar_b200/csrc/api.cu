@@ -209,19 +209,30 @@ void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memo
 
 namespace {
 
-// CB200_FLAG_SHARPEN_IF_NEEDED is a decision about camera pictures: the entry points that take extracted frames refuse it
-int check_frame_flags(uint32_t flags)
+// the frame entry points by what they take: the raw and cell calls ignore CC_FIT (cb200.h), the chunk calls honour it, and the
+// selection calls are chunk calls with a per-frame sharpen selection
+enum class Frames { cells, chunks, selection };
+
+// the checks every frame call shares, in this order and before any CUDA call: the flags (SHARPEN_IF_NEEDED is about camera pictures;
+// CC_SIMPLE with CC_FIT where CC_FIT is honoured), the selection, the context, n; then, unless n = 0 on a call that is not a chained
+// CC_FIT call (empty_stripe), `buffers` (the call's required pointers are non-null), the chain step and the frozen walk workspace
+int check_frame_call(cb200_ctx* c, int n, uint32_t flags, Frames kind, const uint8_t* sharpen, bool buffers)
 {
     if (flags & CB200_FLAG_SHARPEN_IF_NEEDED) return fail(CB200_ERR_ARG, "CB200_FLAG_SHARPEN_IF_NEEDED applies to camera pictures, not to frames");
-    return CB200_OK;
-}
-// the frame entry points with a per-frame selection
-int check_selection_args(uint32_t flags, const uint8_t* sharpen)
-{
-    int rc = check_frame_flags(flags); if (rc) return rc;
-    if (flags & CB200_FLAG_SHARPEN) return fail(CB200_ERR_ARG, "CB200_FLAG_SHARPEN with a per-frame sharpen selection");
-    if (!sharpen) return fail(CB200_ERR_ARG, "null sharpen selection");
-    return CB200_OK;
+    const bool fits = kind != Frames::cells;
+    int rc = fits ? check_camera_flags(flags) : CB200_OK;           // SHARPEN_IF_NEEDED refused, only its CC pair rule is left
+    if (rc) return rc;
+    if (kind == Frames::selection) {
+        if (flags & CB200_FLAG_SHARPEN) return fail(CB200_ERR_ARG, "CB200_FLAG_SHARPEN with a per-frame sharpen selection");
+        if (!sharpen) return fail(CB200_ERR_ARG, "null sharpen selection");
+    }
+    if (!c) return fail(CB200_ERR_ARG, "null context");
+    if (n < 0 || n > c->max_frames) return fail(CB200_ERR_ARG, "n exceeds the context's max_frames");
+    const bool chained = fits && chain_linked(c, flags);
+    if (n == 0 && !chained) return CB200_OK;
+    if (n > 0 && !buffers) return fail(CB200_ERR_ARG, "null buffer");
+    if (chained && (rc = check_chain_call(c, flags))) return rc;
+    return check_frozen_frames(c, n);
 }
 
 int check_n(const cb200_ctx* c, int n)
@@ -266,15 +277,27 @@ int idx_for(cb200_ctx* c, uint32_t flags, const uint16_t** out)
     return CB200_OK;
 }
 
-// the colour-correction buffers: the per-frame matrices and fits, and the last frame's matrix on its way to the host
-int ccm_buffers(cb200_ctx* c)
+// the decode's own buffers (sized by max_frames) by part: kCcm the per-frame CCMs and fits and the carry, kFitted the fitted-CCM
+// route's mean colours and CCM flags, kLists a mixed host selection's lists, kSchedule k_select's schedule.  A decode grows its
+// route's parts here once, before it enqueues anything: nothing else allocates them
+enum : unsigned { kCcm = 1, kFitted = 2, kLists = 4, kSchedule = 8 };
+int decode_buffers(cb200_ctx* c, unsigned parts)
 {
-    CK(c->d_ccm.ensure(9 * (size_t)c->max_frames), "cudaMalloc ccm");
-    CK(c->d_carry.ensure(12), "cudaMalloc ccm carry");
-    CK(c->h_ccm.ensure(12), "cudaMallocHost ccm");
-    if (!c->ccm_ev) CK(cudaEventCreateWithFlags(&c->ccm_ev, cudaEventDisableTiming), "cudaEventCreate ccm");
-    CK(c->d_fit.ensure(9 * (size_t)c->max_frames), "cudaMalloc fit");
-    CK(c->d_fit_valid.ensure((size_t)c->max_frames), "cudaMalloc fit flags");
+    const size_t frames = (size_t)c->max_frames;
+    if (parts & kCcm) {
+        CK(c->d_ccm.ensure(9 * frames), "cudaMalloc ccm");
+        CK(c->d_carry.ensure(12), "cudaMalloc ccm carry");
+        CK(c->h_ccm.ensure(12), "cudaMallocHost ccm");
+        if (!c->ccm_ev) CK(cudaEventCreateWithFlags(&c->ccm_ev, cudaEventDisableTiming), "cudaEventCreate ccm");
+        CK(c->d_fit.ensure(9 * frames), "cudaMalloc fit");
+        CK(c->d_fit_valid.ensure(frames), "cudaMalloc fit flags");
+    }
+    if (parts & kFitted) {
+        CK(c->d_means.ensure(frames * c->mode.num_cells), "cudaMalloc means");
+        CK(c->d_ccm_active.ensure(frames), "cudaMalloc ccm flags");
+    }
+    if (parts & kLists) CK(c->d_sel.ensure(frames * 5), "cudaMalloc selection");
+    if (parts & kSchedule) CK(c->d_sched.ensure(6), "cudaMalloc selection schedule");
     return CB200_OK;
 }
 
@@ -307,7 +330,6 @@ int ccm_keep_chain(cb200_ctx* c)
 // (CimbReader.cpp:124-125); the last one becomes the context's CCM
 int ccm_simple(cb200_ctx* c, const uint8_t* d_rgb, int n)
 {
-    int rc = ccm_buffers(c); if (rc) return rc;
     CK(ccm_simple_launch(c->mode, d_rgb, n, c->d_ccm, c->stream), "ccm launch");
     return ccm_keep_last(c, n, nullptr);
 }
@@ -355,10 +377,17 @@ int k1_grid(const cb200_ctx* c, int k) { return c->sm_count * k1_ctas_per_sm(k =
 // the frame lists of a selection whose n bytes (nonzero = sharpen) are in c->d_sel + 4 n, built there by k_select
 int build_selection(cb200_ctx* c, int n)
 {
-    CK(c->d_sched.ensure(6), "cudaMalloc selection schedule");
     k_select<<<1, 1024, 0, c->stream>>>(c->d_sel, n, k1_grid(c, 0), k1_grid(c, 1), c->mode.cells_y / 4, c->d_sched); count_launch();
     CK(cudaGetLastError(), "selection launch");
     return CB200_OK;
+}
+
+// n host selection bytes that sharpen some frames but not all (run_cells lists such a selection on the device)
+bool mixed_selection(const uint8_t* sel, int n)
+{
+    int k = 0;
+    for (int f = 0; sel && f < n; ++f) k += sel[f] != 0;
+    return k > 0 && k < n;
 }
 
 // a mixed sharpen selection from the host: its n bytes go up through the context's upload ring, k_select builds the
@@ -366,7 +395,6 @@ int build_selection(cb200_ctx* c, int n)
 // one 0 / 1 byte per frame (d_sharp)
 int upload_selection(cb200_ctx* c, const uint8_t* sel, int n, const int nl[2], const uint32_t* d_list[2], const uint8_t** d_sharp)
 {
-    CK(c->d_sel.ensure((size_t)c->max_frames * 5), "cudaMalloc selection");
     int slot;
     uint8_t* h;
     int rc = c->upload.take((size_t)n, &slot, &h); if (rc) return rc;
@@ -452,6 +480,41 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const u
     return CB200_OK;
 }
 
+// a host-pointer call's n frames into the context's one staging buffer, which cb200_fit_ccm(ctx, NULL, ...) reads later: so only
+// once every check of the call has passed
+int upload_frames(cb200_ctx* c, const uint8_t* rgb, int n)
+{
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    const Mode& m = c->mode;
+    size_t fb = (size_t)m.width * m.height * 3;
+    CK(c->d_rgb.ensure(fb * (size_t)c->max_frames), "cudaMalloc rgb staging");
+    CK(cudaMemcpyAsync(c->d_rgb, rgb, fb * (size_t)n, cudaMemcpyHostToDevice, c->stream), "H2D frames");
+    return CB200_OK;
+}
+
+// the decoder's CCM going into frame 0: with `carried`, the one an earlier batch leaves in c->d_carry, read on the device
+// (k_ccm_carry); else the context's
+int entry_ccm(cb200_ctx* c, bool carried, CcmArg& cc)
+{
+    if (!carried) return ccm_arg(c, cc);
+    memset(&cc, 0, sizeof(cc));
+    cc.per_frame = c->d_carry;
+    cc.per_frame_active = reinterpret_cast<const uint8_t*>(c->d_carry + 9);
+    return CB200_OK;
+}
+
+// K1 and the exact walk of n frames on the device, their raw stream packed into d_raw_out
+int decode_raw(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* d_raw_out)
+{
+    const uint16_t* idx;
+    int rc = decode_buffers(c, (flags & CB200_FLAG_CC_SIMPLE) ? kCcm : 0u); if (rc) return rc;
+    rc = idx_for(c, flags, &idx); if (rc) return rc;
+    rc = run_cells(c, d_rgb, n, flags, nullptr); if (rc) return rc;
+    CK(k2_pack_launch(c->mode, c->d_cellvals, idx, n, d_raw_out, c->stream), "pack launch");
+    mark(c);                                   // ev3: after pack
+    return CB200_OK;
+}
+
 }  // namespace
 
 namespace cb200 {
@@ -468,11 +531,7 @@ int flood_reserve(cb200_ctx* c, int n)
 
 int decode_reserve(cb200_ctx* c, uint32_t flags)
 {
-    int rc = ccm_buffers(c); if (rc) return rc;
-    CK(c->d_means.ensure((size_t)c->max_frames * c->mode.num_cells), "cudaMalloc means");
-    CK(c->d_ccm_active.ensure((size_t)c->max_frames), "cudaMalloc ccm flags");
-    CK(c->d_sel.ensure((size_t)c->max_frames * 5), "cudaMalloc selection");
-    CK(c->d_sched.ensure(6), "cudaMalloc selection schedule");
+    int rc = decode_buffers(c, kCcm | kFitted | kLists | kSchedule); if (rc) return rc;
     const uint16_t* idx;
     return idx_for(c, flags, &idx);
 }
@@ -489,16 +548,6 @@ int carry_from_host(cb200_ctx* c)
     return CB200_OK;
 }
 }  // namespace cb200
-
-int upload_frames(cb200_ctx* c, const uint8_t* rgb, int n)
-{
-    const Mode& m = c->mode;
-    size_t fb = (size_t)m.width * m.height * 3;
-    CK(c->d_rgb.ensure(fb * (size_t)c->max_frames), "cudaMalloc rgb staging");
-    CK(cudaMemcpyAsync(c->d_rgb, rgb, fb * (size_t)n, cudaMemcpyHostToDevice, c->stream), "H2D frames");
-    return CB200_OK;
-}
-
 
 extern "C" {
 
@@ -674,17 +723,10 @@ int cb200_sync(cb200_ctx* c)
 
 int cb200_decode_raw_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* d_raw_out, uint8_t* d_frame_flags)
 {
-    int rc = check_frame_flags(flags); if (rc) return rc;
-    rc = check_n(c, n); if (rc) return rc;
-    if (n == 0) return CB200_OK;
-    if (!d_rgb || !d_raw_out) return fail(CB200_ERR_ARG, "null buffer");
-    rc = check_frozen_frames(c, n); if (rc) return rc;
+    int rc = check_frame_call(c, n, flags, Frames::cells, nullptr, d_rgb && d_raw_out);
+    if (rc || n == 0) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
-    const uint16_t* idx;
-    rc = idx_for(c, flags, &idx); if (rc) return rc;
-    rc = run_cells(c, d_rgb, n, flags, nullptr); if (rc) return rc;
-    CK(k2_pack_launch(c->mode, c->d_cellvals, idx, n, d_raw_out, c->stream), "pack launch");
-    mark(c);                                   // ev3: after pack
+    rc = decode_raw(c, d_rgb, n, flags, d_raw_out); if (rc) return rc;
     if (d_frame_flags) CK(cudaMemcpyAsync(d_frame_flags, c->d_flags, (size_t)n, cudaMemcpyDeviceToDevice, c->stream), "copy flags");
     return CB200_OK;
 }
@@ -702,25 +744,12 @@ int cb200_rs_correct_dev(cb200_ctx* c, const uint8_t* d_raw, int n, uint8_t* d_d
 
 }  // extern "C"
 
-namespace {
-// cb200_decode_chunks_dev with an optional per-frame selection (run_cells: sharpen on the host, or d_sel_bytes on the device).
-// enqueue_only: a CCM still on its way from an earlier batch (ccm_keep_last) is not waited for but read
-// from c->d_carry on the device -- through k_ccm_carry, so a batch without a fit then takes the fitted-CCM route with no fits
-// (mean colours, carry, colour decisions), which decides every colour as K1 would with that matrix or without one
-int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
-                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes = nullptr, bool enqueue_only = false)
+int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
+                         uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes, bool enqueue_only)
 {
-    int rc = check_n(c, n); if (rc) return rc;
-    // a chained CC_FIT call takes part in the step even with no frames: an empty stripe publishes "no fit" and settles
-    const bool chained = chain_linked(c, flags);
-    if (n == 0 && !chained) return CB200_OK;
-    if ((flags & CB200_FLAG_CC_FIT) && (flags & CB200_FLAG_CC_SIMPLE)) return fail(CB200_ERR_ARG, "CC_SIMPLE and CC_FIT are exclusive");
-    rc = check_chain_call(c, flags); if (rc) return rc;
-    if (n > 0 && (!d_rgb || !d_chunks || !d_chunk_mask)) return fail(CB200_ERR_ARG, "null buffer");
-    rc = check_frozen_frames(c, n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
-    const bool fit = ccm_fits(m, flags);
+    const bool fit = ccm_fits(m, flags), chained = chain_linked(c, flags);
     // the CCM going into frame 0 is only known on the device -- always so for a camera plan, whose graph replays later
     bool carried = enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->capturing;
     if (enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->ccm_pending && !carried) {
@@ -728,40 +757,28 @@ int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
         if (q == cudaErrorNotReady) carried = true;
         else if (q != cudaSuccess) return fail_cuda(q, "query ccm");
     }
-    if (n == 0) {                              // chained, empty stripe
-        rc = ccm_buffers(c); if (rc) return rc;
-        CcmArg own;
-        if (carried) {
-            memset(&own, 0, sizeof(own));
-            own.per_frame = c->d_carry;
-            own.per_frame_active = reinterpret_cast<const uint8_t*>(c->d_carry + 9);
-        } else {
-            rc = ccm_arg(c, own); if (rc) return rc;
-        }
-        rc = chain_publish_link(c, 0, nullptr, nullptr, own, nullptr); if (rc) return rc;
+    const bool fitted = fit || carried || chained;                 // the fitted-CCM route
+    unsigned parts = fitted ? kCcm | (n > 0 ? kFitted : 0u) : (flags & CB200_FLAG_CC_SIMPLE) ? kCcm : 0u;
+    if (d_sel_bytes) parts |= kSchedule;
+    else if (mixed_selection(sharpen, n)) parts |= kLists | kSchedule;
+    int rc = decode_buffers(c, parts); if (rc) return rc;
+    CcmArg initial;                            // the decoder's CCM going into frame 0
+    if (n == 0) {                              // chained, empty stripe: publishes "no fit" and settles
+        rc = entry_ccm(c, carried, initial); if (rc) return rc;
+        rc = chain_publish_link(c, 0, nullptr, nullptr, initial, nullptr); if (rc) return rc;
         c->ccm_frames = 0;
         return ccm_keep_chain(c);
     }
     const uint16_t* idx;
     rc = idx_for(c, flags, &idx); if (rc) return rc;
-    if (!fit && !carried && !chained) {
+    if (!fitted) {
         rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen, nullptr, nullptr, d_sel_bytes); if (rc) return rc;
         mark(c);                               // ev3: (no separate pack kernel on this path: the RS kernel gathers from the cell bytes)
         CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
     } else {
         // color_correction == 2: symbols (+ mean colours) -> RS of the symbol stream -> header -> CCM fit -> colours -> RS of
         // the colour stream (Decoder.h:83-117)
-        rc = ccm_buffers(c); if (rc) return rc;
-        CK(c->d_means.ensure((size_t)c->max_frames * m.num_cells), "cudaMalloc means");
-        CK(c->d_ccm_active.ensure((size_t)c->max_frames), "cudaMalloc ccm flags");
-        CcmArg initial;                        // the decoder's CCM going into frame 0
-        if (carried) {
-            memset(&initial, 0, sizeof(initial));
-            initial.per_frame = c->d_carry;
-            initial.per_frame_active = reinterpret_cast<const uint8_t*>(c->d_carry + 9);
-        } else {
-            rc = ccm_arg(c, initial); if (rc) return rc;
-        }
+        rc = entry_ccm(c, carried, initial); if (rc) return rc;
         rc = run_cells(c, d_rgb, n, flags & ~(CB200_FLAG_CC_FIT | CB200_FLAG_CC_SIMPLE), sharpen, nullptr, c->d_means, d_sel_bytes); if (rc) return rc;
         mark(c);                               // ev3
         if (fit) {
@@ -790,34 +807,43 @@ int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
     if (d_frame_flags) CK(cudaMemcpyAsync(d_frame_flags, c->d_flags, (size_t)n, cudaMemcpyDeviceToDevice, c->stream), "copy flags");
     return CB200_OK;
 }
-}  // namespace
+
+int cb200::empty_stripe(cb200_ctx* c, uint32_t flags, bool enqueue_only)
+{
+    if (!chain_linked(c, flags)) return CB200_OK;
+    return decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr, nullptr, enqueue_only);
+}
+
+int cb200::decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
+                                   uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
+{
+    int rc = decode_chunks(c, d_rgb, n, flags, sharpen, c->d_data, c->d_mask, nullptr); if (rc) return rc;
+    return fetch_fountain(c, n, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags, nullptr);
+}
 
 extern "C" {
 
 int cb200_decode_chunks_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
 {
-    int rc = check_frame_flags(flags); if (rc) return rc;
+    int rc = check_frame_call(c, n, flags, Frames::chunks, nullptr, d_rgb && d_chunks && d_chunk_mask); if (rc) return rc;
+    if (n == 0) return empty_stripe(c, flags, false);
     return decode_chunks(c, d_rgb, n, flags, nullptr, d_chunks, d_chunk_mask, d_frame_flags);
 }
 
 int cb200_decode_chunks_sharpen_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
                                     uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
 {
-    int rc = check_selection_args(flags, sharpen); if (rc) return rc;
+    int rc = check_frame_call(c, n, flags, Frames::selection, sharpen, d_rgb && d_chunks && d_chunk_mask); if (rc) return rc;
+    if (n == 0) return empty_stripe(c, flags, false);
     return decode_chunks(c, d_rgb, n, flags, sharpen, d_chunks, d_chunk_mask, d_frame_flags);
 }
 
 // ---- host-pointer entry points
 int cb200_decode_raw(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* raw_out, uint8_t* frame_flags)
 {
-    int rc = check_frame_flags(flags); if (rc) return rc;
-    rc = check_n(c, n); if (rc) return rc;
-    if (n == 0) return CB200_OK;
-    if (!rgb || !raw_out) return fail(CB200_ERR_ARG, "null buffer");
-    rc = check_frozen_frames(c, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    rc = upload_frames(c, rgb, n); if (rc) return rc;
-    rc = cb200_decode_raw_dev(c, c->d_rgb, n, flags, c->d_raw, nullptr); if (rc) return rc;
+    int rc = check_frame_call(c, n, flags, Frames::cells, nullptr, rgb && raw_out);
+    if (rc || n == 0) return rc;
+    if ((rc = upload_frames(c, rgb, n)) || (rc = decode_raw(c, c->d_rgb, n, flags, c->d_raw))) return rc;
     CK(cudaMemcpyAsync(raw_out, c->d_raw, (size_t)n * c->mode.cap_all, cudaMemcpyDeviceToHost, c->stream), "D2H raw");
     if (frame_flags) CK(cudaMemcpyAsync(frame_flags, c->d_flags, (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H flags");
     CK(cudaStreamSynchronize(c->stream), "sync");
@@ -826,15 +852,9 @@ int cb200_decode_raw(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, ui
 
 int cb200_decode(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* data_out, uint8_t* block_ok, uint8_t* frame_flags)
 {
-    int rc = check_frame_flags(flags); if (rc) return rc;
-    rc = check_n(c, n); if (rc) return rc;
-    rc = check_chain_call(c, flags); if (rc) return rc;
-    if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
-    if (!rgb || !data_out) return fail(CB200_ERR_ARG, "null buffer");
-    rc = check_frozen_frames(c, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    rc = upload_frames(c, rgb, n); if (rc) return rc;
-    rc = cb200_decode_chunks_dev(c, c->d_rgb, n, flags, c->d_data, c->d_mask, nullptr); if (rc) return rc;
+    int rc = check_frame_call(c, n, flags, Frames::chunks, nullptr, rgb && data_out); if (rc) return rc;
+    if (n == 0) return empty_stripe(c, flags, false);
+    if ((rc = upload_frames(c, rgb, n)) || (rc = decode_chunks(c, c->d_rgb, n, flags, nullptr, c->d_data, c->d_mask, nullptr))) return rc;
     CK(cudaMemcpyAsync(data_out, c->d_data, (size_t)n * c->mode.data_bytes, cudaMemcpyDeviceToHost, c->stream), "D2H data");
     if (block_ok) CK(cudaMemcpyAsync(block_ok, c->d_ok, (size_t)n * c->mode.nblocks, cudaMemcpyDeviceToHost, c->stream), "D2H ok");
     if (frame_flags) CK(cudaMemcpyAsync(frame_flags, c->d_flags, (size_t)n, cudaMemcpyDeviceToHost, c->stream), "D2H flags");
@@ -843,42 +863,6 @@ int cb200_decode(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_
 }
 
 }  // extern "C"
-
-namespace {
-// the host-pointer fountain entry points: H2D of the frames, then the device-frame path
-int decode_fountain_from_host(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
-                              uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
-{
-    int rc = check_n(c, n); if (rc) return rc;
-    rc = check_chain_call(c, flags); if (rc) return rc;
-    if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
-    if (!rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
-    rc = check_frozen_frames(c, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    rc = upload_frames(c, rgb, n); if (rc) return rc;
-    return decode_fountain_to_host(c, c->d_rgb, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
-}
-}  // namespace
-
-// frames already on the device (the staging buffer, or the deskew kernel's output), results to host memory
-int cb200::decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
-                                   uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
-{
-    int rc = check_n(c, n); if (rc) return rc;
-    rc = check_chain_call(c, flags); if (rc) return rc;
-    if (n == 0) return chain_linked(c, flags) ? decode_chunks(c, nullptr, 0, flags, nullptr, nullptr, nullptr, nullptr) : CB200_OK;
-    if (!d_rgb || !chunks_out || !chunk_count) return fail(CB200_ERR_ARG, "null buffer");
-    rc = check_frozen_frames(c, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
-    rc = decode_chunks(c, d_rgb, n, flags, sharpen, c->d_data, c->d_mask, nullptr); if (rc) return rc;
-    return fetch_fountain(c, n, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags, nullptr);
-}
-
-int cb200::decode_chunks_enqueue(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* d_sharp, uint8_t* d_chunks,
-                                 uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
-{
-    return decode_chunks(c, d_rgb, n, flags, nullptr, d_chunks, d_chunk_mask, d_frame_flags, d_sharp, true);
-}
 
 int cb200::fetch_fountain(cb200_ctx* c, int n, const int32_t* d_status, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
                           uint8_t* frame_flags, int32_t* extract_status)
@@ -910,40 +894,38 @@ extern "C" {
 int cb200_decode_fountain(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count,
                           uint32_t* chunk_mask, uint8_t* frame_flags)
 {
-    int rc = check_frame_flags(flags); if (rc) return rc;
-    return decode_fountain_from_host(c, rgb, n, flags, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags);
+    int rc = check_frame_call(c, n, flags, Frames::chunks, nullptr, rgb && chunks_out && chunk_count); if (rc) return rc;
+    if (n == 0) return empty_stripe(c, flags, false);
+    rc = upload_frames(c, rgb, n); if (rc) return rc;
+    return decode_fountain_to_host(c, c->d_rgb, n, flags, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
 int cb200_decode_fountain_sharpen(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
                                   uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags)
 {
-    int rc = check_selection_args(flags, sharpen); if (rc) return rc;
-    return decode_fountain_from_host(c, rgb, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
+    int rc = check_frame_call(c, n, flags, Frames::selection, sharpen, rgb && chunks_out && chunk_count); if (rc) return rc;
+    if (n == 0) return empty_stripe(c, flags, false);
+    rc = upload_frames(c, rgb, n); if (rc) return rc;
+    return decode_fountain_to_host(c, c->d_rgb, n, flags, sharpen, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
 int cb200_decode_fountain_from_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* chunks_out, uint32_t* chunk_count,
                                    uint32_t* chunk_mask, uint8_t* frame_flags)
 {
-    int rc = check_frame_flags(flags); if (rc) return rc;
+    int rc = check_frame_call(c, n, flags, Frames::chunks, nullptr, d_rgb && chunks_out && chunk_count); if (rc) return rc;
+    if (n == 0) return empty_stripe(c, flags, false);
     return decode_fountain_to_host(c, d_rgb, n, flags, nullptr, chunks_out, chunk_count, chunk_mask, frame_flags);
 }
 
-int cb200_decode_cells(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* cellvals_out, cb200_cell_trace* trace_out)
+// the cell calls: K1 and the exact walk of every cell of n host frames (no fallback skipped), with its trace, and the mean colours
+// instead of the colours when means_out is given
+static int decode_cells(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* cellvals_out, cb200_cell_trace* trace_out, uint32_t* means_out)
 {
-    return cb200_decode_cells_means(c, rgb, n, flags, cellvals_out, trace_out, nullptr);
-}
-
-int cb200_decode_cells_means(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* cellvals_out, cb200_cell_trace* trace_out,
-                             uint32_t* means_out)
-{
-    int rc = check_frame_flags(flags); if (rc) return rc;
-    rc = check_n(c, n); if (rc) return rc;
-    if (n == 0) return CB200_OK;
-    if (!rgb || !cellvals_out || !trace_out) return fail(CB200_ERR_ARG, "null buffer");
+    int rc = check_frame_call(c, n, flags, Frames::cells, nullptr, rgb && cellvals_out && trace_out);
+    if (rc || n == 0) return rc;
     static_assert(sizeof(cb200_cell_trace) == sizeof(CellTrace), "trace layout");
-    rc = check_frozen_frames(c, n); if (rc) return rc;
-    CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = upload_frames(c, rgb, n); if (rc) return rc;
+    rc = decode_buffers(c, (flags & CB200_FLAG_CC_SIMPLE) ? kCcm : 0u); if (rc) return rc;
     size_t tb = (size_t)n * c->mode.num_cells * sizeof(CellTrace);
     size_t mb = means_out ? (size_t)n * c->mode.num_cells * sizeof(uint32_t) : 0;
     CK(c->d_scratch.ensure(tb + mb), "cudaMalloc scratch");
@@ -958,6 +940,17 @@ int cb200_decode_cells_means(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t f
     CK(cudaMemcpyAsync(trace_out, d_trace, tb, cudaMemcpyDeviceToHost, c->stream), "D2H trace");
     CK(cudaStreamSynchronize(c->stream), "sync");
     return CB200_OK;
+}
+
+int cb200_decode_cells(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* cellvals_out, cb200_cell_trace* trace_out)
+{
+    return decode_cells(c, rgb, n, flags, cellvals_out, trace_out, nullptr);
+}
+
+int cb200_decode_cells_means(cb200_ctx* c, const uint8_t* rgb, int n, uint32_t flags, uint8_t* cellvals_out, cb200_cell_trace* trace_out,
+                             uint32_t* means_out)
+{
+    return decode_cells(c, rgb, n, flags, cellvals_out, trace_out, means_out);
 }
 
 int cb200_decode_symbols(cb200_ctx* c, const uint16_t* windows, const uint8_t* cooldown, int n, uint8_t* symbol, uint8_t* drift_offset, uint8_t* distance)
@@ -1036,7 +1029,7 @@ int cb200_fit_ccm(cb200_ctx* c, const uint8_t* rgb, const uint8_t* header6, uint
     if (m.color_bits == 0) return 0;
     if (rgb) { rc = upload_frames(c, rgb, 1); if (rc) return rc; }
     else if (!c->d_rgb) return fail(CB200_ERR_ARG, "no frame in the context's staging buffer");
-    rc = ccm_buffers(c); if (rc) return rc;
+    rc = decode_buffers(c, kCcm); if (rc) return rc;
     const uint16_t* idx;
     rc = idx_for(c, flags, &idx); if (rc) return rc;
     GivenHeader g;

@@ -47,8 +47,14 @@ struct UploadRing {
 // status -2 (and, when d_mask is given, mask 0) for every picture whose flag in d_bad is set: the corrupt files of a file call
 // (files.cu, like UploadRing's members)
 int file_status(cb200_ctx* c, const int* d_bad, int n, int32_t* d_status, uint32_t* d_mask);
-// cb200_decode_fountain_from_dev with an optional per-frame sharpen selection: `sharpen` = n host bytes (nonzero =
-// should_preprocess) or NULL (the batch-wide CB200_FLAG_SHARPEN decides).  The flags are checked by the caller (api.cu)
+// the decode of n extracted frames (n = 0: a chained call's empty stripe) that every frame, corner, camera and detect call runs
+// once, after its own checks (n <= max_frames, chain step, frozen walk workspace, non-null buffers): it checks nothing (api.cu).
+// Selection: n host bytes (sharpen), n device bytes at c->d_sel + 4 n (d_sel_bytes), or neither (CB200_FLAG_SHARPEN decides).
+// enqueue_only: a CCM still on its way from an earlier batch is not waited for but read from c->d_carry on the device (k_ccm_carry:
+// a batch without a fit then takes the fitted-CCM route with no fits, deciding every colour as K1 would with that matrix)
+int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
+                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes = nullptr, bool enqueue_only = false);
+// decode_chunks into the context's buffers, then fetch_fountain (api.cu)
 int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
                             uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
 // CB200_ERR_ARG for CB200_FLAG_SHARPEN together with CB200_FLAG_SHARPEN_IF_NEEDED, or CB200_FLAG_CC_SIMPLE with CB200_FLAG_CC_FIT
@@ -100,11 +106,6 @@ int stage_batch(cb200_ctx* c, CameraBatch& b);
 int deskew_frames(cb200_ctx* c, int n, uint8_t** frames);
 // k_deskew over the pictures of b described by d_desc, with the inverse maps d_minv (n x 9), into d_dst (deskew.cu)
 int deskew_launch(cb200_ctx* c, const CameraBatch& b, const double* d_minv, const PicDesc* d_desc, uint8_t* d_dst);
-// the enqueue-only decode of n extracted frames (api.cu): cb200_decode_chunks_dev, but the sharpen selection, if any, is n bytes in
-// device memory (d_sharp, at c->d_sel + 4 n: k_select builds the frame lists there; NULL = as the flags say) and a CCM that an earlier call still in flight may
-// change is taken from the device (c->d_carry) instead of waiting for it
-int decode_chunks_enqueue(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* d_sharp, uint8_t* d_chunks,
-                          uint32_t* d_chunk_mask, uint8_t* d_frame_flags);
 // the enqueue-only camera path (reserve, scan, k_extract, deskew, decode, failed pictures' masks cleared) for a device batch,
 // arguments checked (scan.cu).  The picture table is this call's one upload, unless d_table holds it already (a camera plan's)
 int camera_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags,
@@ -124,8 +125,9 @@ int check_chain_call(const cb200_ctx* c, uint32_t flags);
 int check_host_ccm(const cb200_ctx* c);
 int chain_publish_link(cb200_ctx* c, int n, const float* d_fit, const uint8_t* d_valid, const CcmArg& own, CcmArg* entry);
 int chain_settle(cb200_ctx* c, float* d_carry);
-// a camera call with no pictures: on a chained CC_FIT call the empty stripe's part of the step, else nothing (scan.cu)
-int camera_empty(cb200_ctx* c, uint32_t flags);
+// a frame or camera call with no frames, checked: on a chained CC_FIT call the empty stripe's part of the step (it publishes "no fit"
+// and settles), else nothing.  enqueue_only as for decode_chunks (the camera calls) (api.cu)
+int empty_stripe(cb200_ctx* c, uint32_t flags, bool enqueue_only);
 // camera plans (plan.cu).  Every context buffer a plan's graph uses is grown through grow(): while plans exist a call that needs
 // more fails with CB200_ERR_ARG (plan_frozen) instead.  Called with plans, the *_reserve functions below therefore make no CUDA
 // call, and an entry point runs them first (check_frozen*) so that a frozen buffer refuses the call before any CUDA call

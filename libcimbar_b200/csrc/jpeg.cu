@@ -313,7 +313,7 @@ int cb200_jpeg_scan_extract_decode_chunks_dev(cb200_ctx* c, const uint8_t* const
     };
     CameraBatch b;
     int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
-    if (n == 0) return camera_empty(c, flags);
+    if (n == 0) return empty_stripe(c, flags, true);
     rc = check_frozen_camera(c, b.wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     JpegState* j = jstate(c);

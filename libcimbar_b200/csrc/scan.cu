@@ -622,7 +622,7 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     s->camera_n = n;
     int rc;
     if (deskew) { rc = deskew_launch(c, b, s->d_minv, d_desc, frames); if (rc) return rc; }
-    rc = decode_chunks_enqueue(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, d_sharp, d_chunks, d_mask, d_frame_flags); if (rc) return rc;
+    rc = decode_chunks(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, d_chunks, d_mask, d_frame_flags, d_sharp, true); if (rc) return rc;
     k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
     count_launch();
     CK(cudaGetLastError(), "mask launch");
@@ -661,7 +661,7 @@ static int scan_extract_decode(cb200_ctx* c, Build&& build, uint32_t flags, uint
     CameraBatch b;
     int rc = check_camera_call(c, flags, build, b, chunks_out && chunk_count && extract_status ? nullptr : "null output"); if (rc) return rc;
     const int n = b.n();
-    if (n == 0) return camera_empty(c, flags);
+    if (n == 0) return empty_stripe(c, flags, true);
     rc = check_frozen_camera(c, b.wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     rc = stage_batch(c, b); if (rc) return rc;
@@ -678,7 +678,7 @@ static int scan_extract_decode_dev(cb200_ctx* c, Build&& build, uint32_t flags, 
 {
     CameraBatch b;
     int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
-    if (b.n() == 0) return camera_empty(c, flags);
+    if (b.n() == 0) return empty_stripe(c, flags, true);
     rc = check_frozen_camera(c, b.wh.data(), b.n()); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
@@ -696,12 +696,6 @@ static int scan_call(cb200_ctx* c, int built, CameraBatch& b, int32_t* anchors, 
     rc = stage_batch(c, b); if (rc) return rc;
     rc = scan_run(c, b); if (rc) return rc;
     return scan_results(c, n, anchors, count, cutoff);
-}
-
-int camera_empty(cb200_ctx* c, uint32_t flags)
-{
-    if (!chain_linked(c, flags)) return CB200_OK;
-    return decode_chunks_enqueue(c, nullptr, 0, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, nullptr, nullptr, nullptr);
 }
 
 }  // namespace cb200
