@@ -297,6 +297,39 @@ typedef struct cb200_picture {
    and the flags and outputs cb200_scan_extract_decode_chunks_ragged_dev refuses. */
 int cb200_scan_extract_decode_chunks_pictures_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags, uint8_t* d_chunks,
                                                   uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+/* ---- receivers: pictures of many decoders in one batch ------------------------------------------------------------------------
+
+   A batch of the calls above is one decoder: under CC_FIT a picture without a usable header takes the matrix of the picture before
+   it, and CC_SIMPLE leaves the last picture's matrix as the context's CCM.  The _receivers_dev calls decode pictures of many
+   independent decoders ("receivers", e.g. the users of a decode service) in one batch, each with its own colour-correction state.
+   cb200_receiver_state is the state one decoder carries from picture to picture (its CimbDecoder's CCM, CimbDecoder.cpp:69-85): the
+   matrix, row-major, and whether it is active.  The caller keeps one per receiver in device memory. */
+typedef struct cb200_receiver_state {
+    float ccm[9];
+    uint32_t active;                  /* nonzero: the matrix is used; 0: no CCM (cb200_set_ccm(NULL)) */
+} cb200_receiver_state;               /* 40 bytes */
+/* Picture i belongs to receiver receiver_of[i] (HOST memory, n entries, read before the call returns).  For every receiver r, the
+   outputs for r's pictures equal, bit for bit, those of the matching direct call on a context whose CCM was set to d_states[r]
+   (cb200_set_ccm(ccm), or NULL when active == 0) run on r's pictures alone, in batch order: cb200_decode_chunks_dev for the frame
+   call, cb200_scan_extract_decode_chunks_pictures_dev for the camera call (records, masks, frame flags, extract statuses,
+   cb200_camera_transforms).  After the call d_states[r] holds what cb200_get_ccm of that context would return:
+     CC_FIT (a mode that fits): r's last fit in this call, else its entry matrix, with the activity of r's last picture;
+     CC_SIMPLE: the matrix of r's last picture, active;
+     no CC flag, or CC_FIT in a legacy mode (which never fits): unchanged.
+   Receivers without a picture in the call are neither read nor written.  The call neither reads nor changes the context's own CCM
+   (cb200_get_ccm and the next direct call are as if it had not run); cb200_get_frame_ccms reports the matrix each picture was decoded
+   with.  Enqueue-only like the calls they mirror: the camera call makes one upload (the receiver map travels with the picture table),
+   the frame call one (the map).  d_states belongs to the stream until it passes the call.
+   CB200_ERR_ARG, before any CUDA call: a null receiver_of, a null d_states or one not 4-byte aligned, n_receivers < 1, a receiver
+   index outside [0, n_receivers) (naming the picture), a context linked to a CCM chain (the chain carries one decoder's CCM across
+   ranks), and everything the mirrored call refuses.  Several modes in one call: use one context per mode. */
+int cb200_decode_chunks_receivers_dev(cb200_ctx* ctx, const uint8_t* d_rgb, int n, uint32_t flags, const int32_t* receiver_of,
+                                      int n_receivers, cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                      uint8_t* d_frame_flags);
+int cb200_scan_extract_decode_chunks_receivers_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags,
+                                                   const int32_t* receiver_of, int n_receivers, cb200_receiver_state* d_states,
+                                                   uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                                                   int32_t* d_extract_status);
 /* ---- camera plans: the enqueue-only camera call captured once in a CUDA graph ----------------------------------------------
 
    A plan is cb200_scan_extract_decode_chunks_ragged_dev for n pictures of sizes wh, with these flags and these device buffers,

@@ -41,6 +41,7 @@ EXPORTS = [
     "cb200_ccm_chain_link_ms", "cb200_get_frame_ccms",
     "cb200_camera_plan_create", "cb200_camera_plan_launch", "cb200_camera_plan_graph", "cb200_camera_plan_destroy",
     "cb200_detect_scan_extract_decode_chunks_dev", "cb200_scan_extract_decode_chunks_pictures_dev",
+    "cb200_decode_chunks_receivers_dev", "cb200_scan_extract_decode_chunks_receivers_dev",
 ]
 
 
@@ -59,6 +60,11 @@ class Picture(C.Structure):
     """cb200_picture: one camera picture in device memory in the caller's layout"""
     _fields_ = [("data", C.c_void_p), ("w", C.c_int32), ("h", C.c_int32), ("row_pitch", C.c_int64), ("plane_pitch", C.c_int64),
                 ("layout", C.c_int32)]
+
+
+class ReceiverState(C.Structure):
+    """cb200_receiver_state: one receiver's CCM, row-major, and whether it is active (40 bytes, device memory)"""
+    _fields_ = [("ccm", C.c_float * 9), ("active", C.c_uint32)]
 
 
 TRACE_DTYPE = np.dtype([("order", "<u2"), ("x", "<i2"), ("y", "<i2"), ("drift_offset", "u1"), ("distance", "u1")])
@@ -170,6 +176,8 @@ def load_library():
     lib.cb200_camera_plan_destroy.argtypes = [vp]
     lib.cb200_detect_scan_extract_decode_chunks_dev.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_pictures_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
+    lib.cb200_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp]
+    lib.cb200_scan_extract_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -214,6 +222,40 @@ def picture(t, order="rgb"):
     if not t.is_cuda:
         raise Cb200Error("a picture must be in device memory (a CUDA tensor)")
     return Picture(t.data_ptr(), w, h, row, plane, lay)
+
+
+def receiver_states(ccms, device=None):
+    """a CUDA tensor of receiver states (cb200_receiver_state, 40 bytes each, as int32 words) from one host matrix per receiver:
+    a 3x3 (or 9) float matrix, or None for a receiver without a CCM"""
+    import torch
+    a = np.zeros((len(ccms), 10), np.float32)
+    words = a.view(np.uint32)
+    for r, m in enumerate(ccms):
+        if m is not None:
+            a[r, :9] = np.asarray(m, np.float32).reshape(9)
+            words[r, 9] = 1
+    return torch.from_numpy(a.view(np.int32)).to("cuda" if device is None else device)
+
+
+def read_receiver_states(states):
+    """the host matrices of a receiver-state tensor (synchronises): a 3x3 float32 array per receiver, None where inactive"""
+    a = states.detach().cpu().numpy().reshape(-1, 10)
+    m = a.view(np.float32)[:, :9].reshape(-1, 3, 3).copy()
+    return [m[r] if a[r, 9] != 0 else None for r in range(a.shape[0])]
+
+
+def _receiver_map(receiver_of, n):
+    of = np.ascontiguousarray(receiver_of, dtype=np.int32).reshape(-1)
+    if of.shape[0] != n:
+        raise Cb200Error(f"{of.shape[0]} receiver indices for {n} pictures")
+    return of
+
+
+def _states_ptr(states):
+    import torch
+    if not isinstance(states, torch.Tensor) or not states.is_cuda or not states.is_contiguous() or states.numel() * states.element_size() % 40:
+        raise Cb200Error("receiver states are a contiguous CUDA tensor of 40-byte entries (see receiver_states)")
+    return states.data_ptr(), states.numel() * states.element_size() // 40
 
 
 def launch_count():
@@ -578,6 +620,26 @@ class Context:
         descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
         _check(self.lib.cb200_scan_extract_decode_chunks_pictures_dev(self._h, C.cast(descs, C.c_void_p), len(pictures), flags, d_chunks,
                                                                       d_mask, d_flags, d_status))
+
+    def decode_chunks_receivers_dev(self, d_rgb, n, receiver_of, states, d_chunks, d_mask, d_flags=None, flags=0):
+        """decode_chunks_dev for frames of several receivers: frame i belongs to receiver receiver_of[i] (host), each receiver decodes
+        with its own state in `states` (receiver_states) and leaves its new one there.  Enqueue-only"""
+        of = _receiver_map(receiver_of, n)
+        ptr, count = _states_ptr(states)
+        _check(self.lib.cb200_decode_chunks_receivers_dev(self._h, d_rgb, n, flags, of.ctypes.data, count, ptr, d_chunks, d_mask, d_flags))
+
+    def scan_extract_decode_chunks_receivers_dev(self, pictures, receiver_of, states, d_chunks, d_mask, d_status, d_flags=None, flags=0,
+                                                 order="rgb"):
+        """scan_extract_decode_chunks_pictures_dev for pictures of several receivers: picture i belongs to receiver receiver_of[i]
+        (host), each receiver decodes with its own state in `states` (receiver_states) and leaves its new one there.  Enqueue-only"""
+        orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+        if len(orders) != len(pictures):
+            raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+        of = _receiver_map(receiver_of, len(pictures))
+        ptr, count = _states_ptr(states)
+        descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+        _check(self.lib.cb200_scan_extract_decode_chunks_receivers_dev(self._h, C.cast(descs, C.c_void_p), len(pictures), flags, of.ctypes.data,
+                                                                       count, ptr, d_chunks, d_mask, d_flags, d_status))
 
     def camera_plan(self, wh, flags, pictures, chunks, mask, frame_flags, status):
         """scan_extract_decode_chunks_dev for pictures of sizes wh (n x (w, h), host) with these flags, captured once in a CUDA graph

@@ -6,6 +6,7 @@
 #include "k2_rs.cuh"
 #include "render.cuh"
 #include "encode.cuh"
+#include "receivers_core.cuh"
 
 #include <atomic>
 #include <cmath>
@@ -278,9 +279,9 @@ int idx_for(cb200_ctx* c, uint32_t flags, const uint16_t** out)
 }
 
 // the decode's own buffers (sized by max_frames) by part: kCcm the per-frame CCMs and fits and the carry, kFitted the fitted-CCM
-// route's mean colours and CCM flags, kLists a mixed host selection's lists, kSchedule k_select's schedule.  A decode grows its
-// route's parts here once, before it enqueues anything: nothing else allocates them
-enum : unsigned { kCcm = 1, kFitted = 2, kLists = 4, kSchedule = 8 };
+// route's mean colours and CCM flags, kLists a mixed host selection's lists, kSchedule k_select's schedule, kReceivers a receivers
+// call's CCM flags and map.  A decode grows its route's parts here once, before it enqueues anything: nothing else allocates them
+enum : unsigned { kCcm = 1, kFitted = 2, kLists = 4, kSchedule = 8, kReceivers = 16 };
 int decode_buffers(cb200_ctx* c, unsigned parts)
 {
     const size_t frames = (size_t)c->max_frames;
@@ -298,6 +299,10 @@ int decode_buffers(cb200_ctx* c, unsigned parts)
     }
     if (parts & kLists) CK(c->d_sel.ensure(frames * 5), "cudaMalloc selection");
     if (parts & kSchedule) CK(c->d_sched.ensure(6), "cudaMalloc selection schedule");
+    if (parts & kReceivers) {
+        CK(c->d_ccm_active.ensure(frames), "cudaMalloc ccm flags");
+        CK(c->d_recv.ensure(2 * frames), "cudaMalloc receiver map");
+    }
     return CB200_OK;
 }
 
@@ -412,14 +417,17 @@ int upload_selection(cb200_ctx* c, const uint8_t* sel, int n, const int nl[2], c
 // sel: NULL = every frame is preprocessed as CB200_FLAG_SHARPEN says; else n host bytes, nonzero = sharpen that frame (flags
 // must not carry CB200_FLAG_SHARPEN then).  A selection of one kind only takes the list-less path of that kind.
 // d_sel_bytes (instead of sel): the selection is n bytes at c->d_sel + 4 n on the device; the lists are built there and K1 takes
-// their lengths from the device (both kinds are launched, one may be empty)
+// their lengths from the device (both kinds are launched, one may be empty).  given: the CCM of the colour decisions, instead of
+// the one the flags and the context give
 int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sel, CellTrace* d_trace = nullptr,
-              uint32_t* d_means = nullptr, const uint8_t* d_sel_bytes = nullptr)
+              uint32_t* d_means = nullptr, const uint8_t* d_sel_bytes = nullptr, const CcmArg* given = nullptr)
 {
     const Mode& m = c->mode;
     cudaStream_t st = c->stream;
     CcmArg cc;
-    if (d_means) {
+    if (given) {
+        cc = *given;
+    } else if (d_means) {
         memset(&cc, 0, sizeof(cc));
         cc.means = d_means;
     } else if ((flags & CB200_FLAG_CC_SIMPLE) && n > 0) {
@@ -503,6 +511,24 @@ int entry_ccm(cb200_ctx* c, bool carried, CcmArg& cc)
     return CB200_OK;
 }
 
+// the matrices of a receivers call outside the fitted-CCM route, per picture in d_ccm / d_ccm_active (cb200_get_frame_ccms reads
+// them), and the CCM argument that decodes each picture with its own: CC_SIMPLE each picture's von Kries matrix, each receiver then
+// keeping its last picture's; otherwise each picture's receiver state
+int receivers_ccm(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const Receivers& r, CcmArg& cc)
+{
+    const int32_t* d_of = r.d_map;
+    if (flags & CB200_FLAG_CC_SIMPLE) {
+        CK(ccm_simple_launch(c->mode, d_rgb, n, c->d_ccm, c->stream), "ccm launch");
+        CK(cudaMemsetAsync(c->d_ccm_active, 1, (size_t)n, c->stream), "set ccm flags");
+        CK(receivers_keep_launch(n, d_of, d_of + n, c->d_ccm, r.d_states, c->stream), "receivers keep launch");
+    } else {
+        CK(receivers_gather_launch(n, d_of, r.d_states, c->d_ccm, c->d_ccm_active, c->stream), "receivers gather launch");
+    }
+    memset(&cc, 0, sizeof(cc));
+    cc.per_frame = c->d_ccm; cc.active = 1;
+    return CB200_OK;
+}
+
 // K1 and the exact walk of n frames on the device, their raw stream packed into d_raw_out
 int decode_raw(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, uint8_t* d_raw_out)
 {
@@ -534,6 +560,27 @@ int decode_reserve(cb200_ctx* c, uint32_t flags)
     int rc = decode_buffers(c, kCcm | kFitted | kLists | kSchedule); if (rc) return rc;
     const uint16_t* idx;
     return idx_for(c, flags, &idx);
+}
+
+int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states)
+{
+    if (!receiver_of) return fail(CB200_ERR_ARG, "null receiver_of");
+    if (!d_states) return fail(CB200_ERR_ARG, "null d_states");
+    if (reinterpret_cast<uintptr_t>(d_states) % 4) return fail(CB200_ERR_ARG, "d_states is not 4-byte aligned");
+    if (n_receivers < 1) return fail(CB200_ERR_ARG, "n_receivers < 1");
+    for (int i = 0; i < n; ++i)
+        if (receiver_of[i] < 0 || receiver_of[i] >= n_receivers)
+            return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + ": receiver " + std::to_string(receiver_of[i]) + " outside [0, " +
+                                       std::to_string(n_receivers) + ")");
+    if (chain_attached(c)) return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, which carries one decoder's CCM: a receivers call decodes many");
+    return CB200_OK;
+}
+
+Receivers::Receivers(const int32_t* receiver_of, int n, int n_receivers, cb200_receiver_state* states)
+    : map(2 * (size_t)n), d_states(states)
+{
+    memcpy(map.data(), receiver_of, sizeof(int32_t) * (size_t)n);
+    receivers::make_order(receiver_of, n, n_receivers, map.data() + n);
 }
 
 int carry_from_host(cb200_ctx* c)
@@ -745,20 +792,21 @@ int cb200_rs_correct_dev(cb200_ctx* c, const uint8_t* d_raw, int n, uint8_t* d_d
 }  // extern "C"
 
 int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
-                         uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes, bool enqueue_only)
+                         uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes, bool enqueue_only, Receivers* recv)
 {
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
     const bool fit = ccm_fits(m, flags), chained = chain_linked(c, flags);
     // the CCM going into frame 0 is only known on the device -- always so for a camera plan, whose graph replays later
     bool carried = enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->capturing;
-    if (enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->ccm_pending && !carried) {
+    if (enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->ccm_pending && !carried && !recv) {
         const cudaError_t q = cudaEventQuery(c->ccm_ev);
         if (q == cudaErrorNotReady) carried = true;
         else if (q != cudaSuccess) return fail_cuda(q, "query ccm");
     }
     const bool fitted = fit || carried || chained;                 // the fitted-CCM route
-    unsigned parts = fitted ? kCcm | (n > 0 ? kFitted : 0u) : (flags & CB200_FLAG_CC_SIMPLE) ? kCcm : 0u;
+    unsigned parts = fitted ? kCcm | (n > 0 ? kFitted : 0u) : (recv || (flags & CB200_FLAG_CC_SIMPLE)) ? kCcm : 0u;
+    if (recv) parts |= kReceivers;
     if (d_sel_bytes) parts |= kSchedule;
     else if (mixed_selection(sharpen, n)) parts |= kLists | kSchedule;
     int rc = decode_buffers(c, parts); if (rc) return rc;
@@ -771,14 +819,24 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
     }
     const uint16_t* idx;
     rc = idx_for(c, flags, &idx); if (rc) return rc;
+    if (recv && !recv->d_map) {                // the frame call's one upload
+        int slot;
+        uint8_t* h;
+        if ((rc = c->upload.take(recv->bytes(), &slot, &h))) return rc;
+        memcpy(h, recv->map.data(), recv->bytes());
+        if ((rc = c->upload.send(c->stream, slot, c->d_recv, recv->bytes()))) return rc;
+        recv->d_map = c->d_recv;
+    }
     if (!fitted) {
-        rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen, nullptr, nullptr, d_sel_bytes); if (rc) return rc;
+        CcmArg own;
+        if (recv) { rc = receivers_ccm(c, d_rgb, n, flags, *recv, own); if (rc) return rc; c->ccm_frames = n; }
+        rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen, nullptr, nullptr, d_sel_bytes, recv ? &own : nullptr); if (rc) return rc;
         mark(c);                               // ev3: (no separate pack kernel on this path: the RS kernel gathers from the cell bytes)
         CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
     } else {
         // color_correction == 2: symbols (+ mean colours) -> RS of the symbol stream -> header -> CCM fit -> colours -> RS of
         // the colour stream (Decoder.h:83-117)
-        rc = entry_ccm(c, carried, initial); if (rc) return rc;
+        if (!recv) { rc = entry_ccm(c, carried, initial); if (rc) return rc; }
         rc = run_cells(c, d_rgb, n, flags & ~(CB200_FLAG_CC_FIT | CB200_FLAG_CC_SIMPLE), sharpen, nullptr, c->d_means, d_sel_bytes); if (rc) return rc;
         mark(c);                               // ev3
         if (fit) {
@@ -789,7 +847,9 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
         }
         // across ranks: this stripe's fits out, the CCM entering the stripe in (from the lower ranks' fits of the same step)
         if (chained) { rc = chain_publish_link(c, n, c->d_fit, c->d_fit_valid, initial, &initial); if (rc) return rc; }
-        CK(ccm_carry_launch(n, c->d_fit, c->d_fit_valid, initial, c->d_ccm, c->d_ccm_active, c->stream), "ccm carry");
+        if (recv) CK(ccm_carry_receivers_launch(n, recv->d_map, recv->d_map + n, c->d_fit, c->d_fit_valid, recv->d_states, c->d_ccm,
+                                                c->d_ccm_active, c->stream), "ccm carry");
+        else CK(ccm_carry_launch(n, c->d_fit, c->d_fit_valid, initial, c->d_ccm, c->d_ccm_active, c->stream), "ccm carry");
         CK(ccm_apply_launch(m, c->d_means, n, c->d_ccm, c->d_ccm_active, c->d_cellvals, c->stream), "ccm apply");
         c->ccm_frames = n;
         if (fit) {
@@ -799,7 +859,7 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
             CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
         }
         if (chained) { rc = ccm_keep_chain(c); if (rc) return rc; }
-        else if (fit) { rc = ccm_keep_last(c, n, c->d_ccm_active); if (rc) return rc; }
+        else if (fit && !recv) { rc = ccm_keep_last(c, n, c->d_ccm_active); if (rc) return rc; }
     }
     mark(c);                                   // ev4: after RS
     CK(k2_mask_launch(m, c->d_ok, n, d_chunk_mask, c->stream), "mask launch");
@@ -836,6 +896,16 @@ int cb200_decode_chunks_sharpen_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, u
     int rc = check_frame_call(c, n, flags, Frames::selection, sharpen, d_rgb && d_chunks && d_chunk_mask); if (rc) return rc;
     if (n == 0) return empty_stripe(c, flags, false);
     return decode_chunks(c, d_rgb, n, flags, sharpen, d_chunks, d_chunk_mask, d_frame_flags);
+}
+
+int cb200_decode_chunks_receivers_dev(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const int32_t* receiver_of, int n_receivers,
+                                      cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags)
+{
+    int rc = check_receivers(c, receiver_of, n, n_receivers, d_states); if (rc) return rc;
+    rc = check_frame_call(c, n, flags, Frames::chunks, nullptr, d_rgb && d_chunks && d_chunk_mask);
+    if (rc || n == 0) return rc;
+    Receivers r(receiver_of, n, n_receivers, d_states);
+    return decode_chunks(c, d_rgb, n, flags, nullptr, d_chunks, d_chunk_mask, d_frame_flags, nullptr, false, &r);
 }
 
 // ---- host-pointer entry points

@@ -1,5 +1,6 @@
 // ccm.cu -- color_correction == 1: one von Kries adaptation matrix per frame from the anchors' white (see ccm.cuh)
 #include "ccm.cuh"
+#include "receivers_core.cuh"
 #include <cstring>
 
 namespace cb200 {
@@ -367,6 +368,70 @@ k_ccm_carry(int n_frames, const float* __restrict__ fit, const uint8_t* __restri
     }
 }
 
+// k_ccm_carry for a batch of several receivers: the same two-level max scan, over the receiver-major order and with the segment
+// starts scanned alongside (receivers_core.cuh), so each picture takes its own receiver's last fit or entry state.  used and
+// used_active are written in batch order; each receiver's last picture writes its exit state, after every entry state is read
+__global__ void __launch_bounds__(1024)
+k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ fit,
+                      const uint8_t* __restrict__ valid, cb200_receiver_state* __restrict__ states, float* __restrict__ used,
+                      uint8_t* __restrict__ used_active)
+{
+    __shared__ int seg_fit[1024], seg_start[1024];
+    const int t = threadIdx.x;
+    const int seg = (n_frames + 1023) / 1024, j0 = min(t * seg, n_frames), j1 = min(j0 + seg, n_frames);
+    receivers::Carry c = receivers::range(of, order, valid, j0, j1);
+    seg_fit[t] = c.fit; seg_start[t] = c.start;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {
+        const int vf = t >= o ? seg_fit[t - o] : -1, vs = t >= o ? seg_start[t - o] : 0;
+        __syncthreads();
+        if (vf > seg_fit[t]) seg_fit[t] = vf;
+        if (vs > seg_start[t]) seg_start[t] = vs;
+        __syncthreads();
+    }
+    c = t > 0 ? receivers::Carry{seg_fit[t - 1], seg_start[t - 1]} : receivers::Carry{-1, 0};
+    for (int j = j0; j < j1; ++j) {
+        const int f = order[j], g = receivers::step(of, order, valid, j, c);
+        const cb200_receiver_state& e = states[of[f]];
+        for (int i = 0; i < 9; ++i) used[(size_t)f * 9 + i] = g >= 0 ? fit[(size_t)g * 9 + i] : e.ccm[i];
+        used_active[f] = (g >= 0 || e.active != 0) ? 1 : 0;
+    }
+    __syncthreads();
+    for (int j = j0; j < j1; ++j) {
+        if (!receivers::closes(of, order, n_frames, j)) continue;
+        const int f = order[j];
+        cb200_receiver_state& x = states[of[f]];
+        for (int i = 0; i < 9; ++i) x.ccm[i] = used[(size_t)f * 9 + i];
+        x.active = used_active[f];
+    }
+}
+
+// without a CC flag every picture decodes with its receiver's matrix.  An inactive receiver's pictures get the identity: the colour
+// decision on integer means through the identity is exactly the decision without a CCM (see k_ccm_apply), so one K1 instantiation
+// serves the whole batch
+__global__ void k_receivers_gather(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
+                                   float* __restrict__ ccm, uint8_t* __restrict__ active)
+{
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n_frames) return;
+    const cb200_receiver_state& s = states[of[f]];
+    const bool a = s.active != 0;
+    for (int i = 0; i < 9; ++i) ccm[(size_t)f * 9 + i] = a ? s.ccm[i] : (i % 4 == 0 ? 1.0f : 0.0f);
+    active[f] = a ? 1 : 0;
+}
+
+// CC_SIMPLE: each receiver keeps the matrix of its last picture
+__global__ void k_receivers_keep(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ ccm,
+                                 cb200_receiver_state* __restrict__ states)
+{
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n_frames || !receivers::closes(of, order, n_frames, j)) return;
+    const int f = order[j];
+    cb200_receiver_state& x = states[of[f]];
+    for (int i = 0; i < 9; ++i) x.ccm[i] = ccm[(size_t)f * 9 + i];
+    x.active = 1;
+}
+
 // CimbDecoder::get_best_color for every cell from the mean colours the first pass stored.  blockIdx.y walks the frames (the
 // frame's matrix sits in shared memory), blockIdx.x the cells.
 __global__ void __launch_bounds__(256)
@@ -428,6 +493,24 @@ cudaError_t ccm_apply_launch(const Mode& m, const uint32_t* d_means, int n_frame
 {
     dim3 grid((unsigned)((m.num_cells + 255) / 256), (unsigned)(n_frames < 2048 ? n_frames : 2048));
     k_ccm_apply<<<grid, 256, 0, st>>>(m, d_means, n_frames, d_used, d_used_active, d_cellvals); count_launch();
+    return cudaGetLastError();
+}
+cudaError_t ccm_carry_receivers_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_fit, const uint8_t* d_valid,
+                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st)
+{
+    k_ccm_carry_receivers<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active); count_launch();
+    return cudaGetLastError();
+}
+cudaError_t receivers_gather_launch(int n_frames, const int32_t* d_of, const cb200_receiver_state* d_states, float* d_ccm, uint8_t* d_active,
+                                    cudaStream_t st)
+{
+    k_receivers_gather<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_states, d_ccm, d_active); count_launch();
+    return cudaGetLastError();
+}
+cudaError_t receivers_keep_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_ccm, cb200_receiver_state* d_states,
+                                  cudaStream_t st)
+{
+    k_receivers_keep<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_order, d_ccm, d_states); count_launch();
     return cudaGetLastError();
 }
 

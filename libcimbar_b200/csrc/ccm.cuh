@@ -10,6 +10,7 @@
 // which the reference's x86-64 build does not have.  Pinned by the matrix string and colours of the reference's own tests
 // (tests/golden/manifest.json: adaptation_golden, ccm_goldens).
 #pragma once
+#include "../../include/cb200.h"
 #include "cb200_common.cuh"
 
 namespace cb200 {
@@ -81,5 +82,16 @@ cudaError_t ccm_carry_launch(int n_frames, const float* d_fit, const uint8_t* d_
                              uint8_t* d_used_active, cudaStream_t st);
 cudaError_t ccm_apply_launch(const Mode& m, const uint32_t* d_means, int n_frames, const float* d_used, const uint8_t* d_used_active,
                              uint8_t* d_cellvals, cudaStream_t st);
+// a batch of several receivers (include/cb200.h, _receivers_dev; receivers_core.cuh): d_of = receiver of each of the n pictures,
+// d_order = the stable receiver-major order, d_states = the receivers' states.  ccm_carry_receivers_launch: the CC_FIT carry of each
+// receiver over its own pictures, from its entry state, its exit state written back by its last picture.  receivers_gather_launch:
+// each picture's receiver matrix into d_ccm / d_active.  receivers_keep_launch: the matrix d_ccm holds for each receiver's last
+// picture into its state, active
+cudaError_t ccm_carry_receivers_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_fit, const uint8_t* d_valid,
+                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st);
+cudaError_t receivers_gather_launch(int n_frames, const int32_t* d_of, const cb200_receiver_state* d_states, float* d_ccm, uint8_t* d_active,
+                                    cudaStream_t st);
+cudaError_t receivers_keep_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_ccm, cb200_receiver_state* d_states,
+                                  cudaStream_t st);
 
 }  // namespace cb200

@@ -52,8 +52,11 @@ int file_status(cb200_ctx* c, const int* d_bad, int n, int32_t* d_status, uint32
 // Selection: n host bytes (sharpen), n device bytes at c->d_sel + 4 n (d_sel_bytes), or neither (CB200_FLAG_SHARPEN decides).
 // enqueue_only: a CCM still on its way from an earlier batch is not waited for but read from c->d_carry on the device (k_ccm_carry:
 // a batch without a fit then takes the fitted-CCM route with no fits, deciding every colour as K1 would with that matrix)
+// recv: a _receivers_dev call's receivers (the CCM of each picture is its receiver's; the context's CCM is neither read nor changed)
+struct Receivers;
 int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
-                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes = nullptr, bool enqueue_only = false);
+                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes = nullptr, bool enqueue_only = false,
+                  Receivers* recv = nullptr);
 // decode_chunks into the context's buffers, then fetch_fountain (api.cu)
 int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
                             uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
@@ -107,9 +110,10 @@ int deskew_frames(cb200_ctx* c, int n, uint8_t** frames);
 // k_deskew over the pictures of b described by d_desc, with the inverse maps d_minv (n x 9), into d_dst (deskew.cu)
 int deskew_launch(cb200_ctx* c, const CameraBatch& b, const double* d_minv, const PicDesc* d_desc, uint8_t* d_dst);
 // the enqueue-only camera path (reserve, scan, k_extract, deskew, decode, failed pictures' masks cleared) for a device batch,
-// arguments checked (scan.cu).  The picture table is this call's one upload, unless d_table holds it already (a camera plan's)
+// arguments checked (scan.cu).  The picture table is this call's one upload, unless d_table holds it already (a camera plan's); a
+// receivers call's map goes up with it
 int camera_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags,
-                   int32_t* d_status, const PicDesc* d_table = nullptr);
+                   int32_t* d_status, const PicDesc* d_table = nullptr, Receivers* recv = nullptr);
 // the results of the last decode (c->d_data, c->d_mask, c->d_flags, and d_status when given) to host memory with one synchronise,
 // the good chunks of each frame packed densely (api.cu)
 int fetch_fountain(cb200_ctx* c, int n, const int32_t* d_status, uint8_t* chunks_out, uint32_t* chunk_count, uint32_t* chunk_mask,
@@ -163,9 +167,22 @@ int pic_table(cb200_ctx* c, const CameraBatch& b, std::vector<uint8_t>& table);
 // anchors into this context's transforms and d_status, the deskew into `frames` (deskew = false: `frames` holds them already,
 // deskewed for this geometry), the decode and the failed pictures' masks
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks);
-int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc);
+int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc, Receivers* recv = nullptr);
 int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
-                      bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status);
+                      bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status,
+                      Receivers* recv = nullptr);
+// the receivers of a _receivers_dev call (include/cb200.h).  check_receivers: CB200_ERR_ARG, before any CUDA call, for a null
+// receiver map, null or misaligned states, n_receivers < 1, a receiver index out of range, a context linked to a CCM chain (api.cu).
+// Receivers(...) then builds `map` on the host: the n receiver indices, then the receiver-major order (receivers_core.cuh); d_map is
+// its device copy once uploaded (the camera calls: behind the picture table; the frame call: in cb200_ctx::d_recv)
+int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states);
+struct Receivers {
+    std::vector<int32_t> map;
+    const int32_t* d_map = nullptr;
+    cb200_receiver_state* d_states = nullptr;
+    Receivers(const int32_t* receiver_of, int n, int n_receivers, cb200_receiver_state* states);
+    size_t bytes() const { return map.size() * sizeof(int32_t); }
+};
 // the context is attached to a CCM chain (chain.cu)
 bool chain_attached(const cb200_ctx* c);
 }  // namespace cb200
@@ -224,6 +241,7 @@ struct cb200_ctx {
     cb200::DevBuf<float> d_fit;             // max_frames x 9
     cb200::DevBuf<uint8_t> d_fit_valid;     // max_frames
     cb200::DevBuf<uint8_t> d_ccm_active;    // max_frames: the frame is decoded with d_ccm[f]
+    cb200::DevBuf<int32_t> d_recv;          // a receivers frame call's map (Receivers::map): max_frames x 2
     int ccm_frames = 0;              // frames of the last call that took the fitted-CCM route (cb200_get_frame_ccms)
     cudaEvent_t ccm_ev = nullptr;    // recorded after the D2H copies of the last batch's CCM (ccm_resolve waits on it)
     cb200::GatherState* gather = nullptr;   // multi-GPU chunk-record window (gather.cu)

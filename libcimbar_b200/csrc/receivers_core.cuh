@@ -1,0 +1,59 @@
+// receivers_core.cuh -- the CCM carry of a batch whose pictures belong to several receivers (include/cb200.h, the _receivers_dev
+// calls): each receiver is one reference Decoder, whose CimbDecoder keeps the CCM of its last fit (CimbDecoder.cpp:69-85).  So
+// picture f takes the fit of the last picture g <= f of the same receiver that has one, else that receiver's entry state.
+//
+// The host lists the batch receiver-major (`order`: a stable counting sort of the receiver map, so each receiver's pictures stay in
+// batch order and form one segment).  Over that order, "the last position with a fit" and "the last segment start" are both
+// running maxima: a position takes the fit at the first one when it is not before the second, else its receiver's entry state.
+// k_ccm_carry_receivers (ccm.cu) splits the order into one contiguous range per thread, combines the ranges' maxima with a block
+// scan and replays each range from its prefix.  Every function is __host__ __device__ so that tests/cpp/receivers_core_host.cpp
+// runs the same rule on the CPU.
+#pragma once
+#include <stdint.h>
+#include <vector>
+
+#include "scan_core.cuh"            // CB_HD
+
+namespace cb200 {
+namespace receivers {
+
+// over a range of the order: the last position with a fit (-1: none) and the last segment start (0: none, position 0 starts one)
+struct Carry { int fit, start; };
+
+CB_HD Carry combine(Carry a, Carry b) { return {a.fit > b.fit ? a.fit : b.fit, a.start > b.start ? a.start : b.start}; }
+
+// position j of the order opens its receiver's segment / closes it
+CB_HD bool opens(const int32_t* of, const int32_t* order, int j) { return j == 0 || of[order[j]] != of[order[j - 1]]; }
+CB_HD bool closes(const int32_t* of, const int32_t* order, int n, int j) { return j == n - 1 || of[order[j + 1]] != of[order[j]]; }
+
+// positions [j0, j1) on their own
+CB_HD Carry range(const int32_t* of, const int32_t* order, const uint8_t* valid, int j0, int j1)
+{
+    Carry c = {-1, 0};
+    for (int j = j0; j < j1; ++j) {
+        if (opens(of, order, j)) c.start = j;
+        if (valid[order[j]]) c.fit = j;
+    }
+    return c;
+}
+
+// position j after the positions before it (c: their carry, updated): the picture whose fit picture order[j] is decoded with, or
+// -1 for its receiver's entry state
+CB_HD int step(const int32_t* of, const int32_t* order, const uint8_t* valid, int j, Carry& c)
+{
+    if (opens(of, order, j)) c.start = j;
+    if (valid[order[j]]) c.fit = j;
+    return c.fit >= c.start ? order[c.fit] : -1;
+}
+
+// the host side: the stable receiver-major order of n pictures of receivers [0, receivers) (every of[i] in range)
+inline void make_order(const int32_t* of, int n, int receivers, int32_t* order)
+{
+    std::vector<int32_t> first((size_t)receivers + 1, 0);
+    for (int i = 0; i < n; ++i) ++first[(size_t)of[i] + 1];
+    for (int r = 0; r < receivers; ++r) first[(size_t)r + 1] += first[(size_t)r];
+    for (int i = 0; i < n; ++i) order[first[(size_t)of[i]]++] = i;
+}
+
+}  // namespace receivers
+}  // namespace cb200

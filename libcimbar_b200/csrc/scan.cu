@@ -485,8 +485,8 @@ int pic_table(cb200_ctx* c, const CameraBatch& b, std::vector<uint8_t>& table)
 
 // blurred pictures + thresholds + anchors for a device batch, in the state's device arrays; enqueued only.  The picture table
 // (PicDesc, in s->d_table) is this call's one upload -- unless d_table holds it already (a camera plan's): then *d_desc = d_table
-// and nothing is uploaded
-int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc_out)
+// and nothing is uploaded.  A receivers call's map travels behind the table, in the same slot
+int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc_out, Receivers* recv)
 {
     ScanScratch* s = sstate(c);
     cudaStream_t st = c->stream;
@@ -499,13 +499,16 @@ int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, cons
         std::vector<uint8_t> table(table_bytes);
         err = pic_table(s, b, table.data(), g); if (err) return err;
     } else {
-        CK(s->d_table.ensure(table_bytes), "cudaMalloc picture table");
+        const size_t map_bytes = recv ? recv->bytes() : 0;
+        CK(s->d_table.ensure(table_bytes + map_bytes), "cudaMalloc picture table");
         int slot;
         uint8_t* h_table;
-        err = c->upload.take(table_bytes, &slot, &h_table); if (err) return err;
+        err = c->upload.take(table_bytes + map_bytes, &slot, &h_table); if (err) return err;
         err = pic_table(s, b, h_table, g); if (err) return err;
-        err = c->upload.send(st, slot, s->d_table, table_bytes); if (err) return err;
+        if (recv) memcpy(h_table + table_bytes, recv->map.data(), map_bytes);
+        err = c->upload.send(st, slot, s->d_table, table_bytes + map_bytes); if (err) return err;
         d_desc = reinterpret_cast<const PicDesc*>(s->d_table.get());
+        if (recv) recv->d_map = reinterpret_cast<const int32_t*>(s->d_table + table_bytes);
     }
     if (d_desc_out) *d_desc_out = d_desc;
     const int* count = g.count;
@@ -608,7 +611,7 @@ int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool 
 int camera_reserve(cb200_ctx* c, const int32_t* wh, int n) { return camera_reserve_for(c, wh, n, true, true); }
 
 int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
-                      bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status)
+                      bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status, Receivers* recv)
 {
     const Mode& m = c->mode;
     const int n = b.n();
@@ -622,7 +625,8 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     s->camera_n = n;
     int rc;
     if (deskew) { rc = deskew_launch(c, b, s->d_minv, d_desc, frames); if (rc) return rc; }
-    rc = decode_chunks(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, d_chunks, d_mask, d_frame_flags, d_sharp, true); if (rc) return rc;
+    rc = decode_chunks(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, d_chunks, d_mask, d_frame_flags, d_sharp, true, recv);
+    if (rc) return rc;
     k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
     count_launch();
     CK(cudaGetLastError(), "mask launch");
@@ -633,14 +637,14 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
 // scan, k_extract, deskew with the scan's picture table, decode (with CB200_FLAG_SHARPEN_IF_NEEDED the frame lists are built on
 // the device), masks of failed pictures cleared
 int camera_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags,
-                   int32_t* d_status, const PicDesc* d_table)
+                   int32_t* d_status, const PicDesc* d_table, Receivers* recv)
 {
     int rc = camera_reserve(c, b.wh.data(), b.n()); if (rc) return rc;
     uint8_t* frames;
     rc = deskew_frames(c, b.n(), &frames); if (rc) return rc;
     const PicDesc* d_desc;
-    rc = camera_scan(c, b, d_table, &d_desc); if (rc) return rc;
-    return camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_mask, d_frame_flags, d_status);
+    rc = camera_scan(c, b, d_table, &d_desc, recv); if (rc) return rc;
+    return camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_mask, d_frame_flags, d_status, recv);
 }
 
 int check_camera_flags(uint32_t flags)
@@ -671,17 +675,24 @@ static int scan_extract_decode(cb200_ctx* c, Build&& build, uint32_t flags, uint
     return fetch_fountain(c, n, s->d_ext_status, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
 }
 
-// the enqueue-only camera entry points on device pictures
+// the receiver arguments of cb200_scan_extract_decode_chunks_receivers_dev
+struct ReceiverArgs { const int32_t* of; int n, count; cb200_receiver_state* d_states; };
+
+// the enqueue-only camera entry points on device pictures.  A receivers call (ra) checks its receivers first; it is never chained,
+// so with no pictures it does nothing
 template <class Build>
 static int scan_extract_decode_dev(cb200_ctx* c, Build&& build, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
-                                   int32_t* d_extract_status)
+                                   int32_t* d_extract_status, const ReceiverArgs* ra = nullptr)
 {
     CameraBatch b;
-    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
+    int rc = ra ? check_receivers(c, ra->of, ra->n, ra->count, ra->d_states) : CB200_OK; if (rc) return rc;
+    rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
     if (b.n() == 0) return empty_stripe(c, flags, true);
     rc = check_frozen_camera(c, b.wh.data(), b.n()); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
-    return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    if (!ra) return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    Receivers r(ra->of, b.n(), ra->count, ra->d_states);
+    return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, &r);
 }
 
 // the scan entry points: the batch, the context and the count output checked, the batch staged and scanned, the results copied out
@@ -798,6 +809,15 @@ int cb200_scan_extract_decode_chunks_pictures_dev(cb200_ctx* c, const cb200_pict
 {
     auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
     return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+}
+
+int cb200_scan_extract_decode_chunks_receivers_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, const int32_t* receiver_of,
+                                                   int n_receivers, cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                                   uint8_t* d_frame_flags, int32_t* d_extract_status)
+{
+    auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
+    const ReceiverArgs ra = {receiver_of, n, n_receivers, d_states};
+    return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &ra);
 }
 
 int cb200_camera_transforms(cb200_ctx* c, double* m9_out, int n)
