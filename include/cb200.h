@@ -358,6 +358,31 @@ int cb200_camera_plan_launch(cb200_camera_plan* plan);
 /* the plan's cudaGraph_t, owned by the plan (for cudaGraphAddChildGraphNode, which copies it) */
 int cb200_camera_plan_graph(cb200_camera_plan* plan, void** cuda_graph);
 int cb200_camera_plan_destroy(cb200_camera_plan* plan);
+/* ---- receivers camera plans: cb200_scan_extract_decode_chunks_receivers_dev captured once ---------------------------------------
+
+   A camera plan (above) over pictures of many receivers, for a decode service that replays fixed-size batches.  The pictures are
+   bound as descriptors (pics, HOST memory, read at create: any layout and pitch, one allocation per picture; the caller writes each
+   batch's pixels into them in stream order before the launch).  d_receiver_of: n int32 in DEVICE memory, bound at create and read
+   when each launch runs, so the caller rewrites it per batch (a copy on the stream, or a kernel in the same capture).  d_states
+   (n_receivers entries, cb200_receiver_state) and n_receivers are bound at create.
+   At each launch, let P be the slots whose d_receiver_of lies in [0, n_receivers).  Every output for P, and every receiver's state
+   afterwards, equals bit for bit what cb200_scan_extract_decode_chunks_receivers_dev gives on the pictures of P alone, in batch
+   order, with the same receivers and states: records, masks, frame flags, extract statuses, cb200_camera_transforms and
+   cb200_get_frame_ccms.  A slot whose receiver lies outside [0, n_receivers) (-1 by convention) is EMPTY: it is still scanned and
+   decoded (it costs GPU time), but it reads and writes no state, its mask is 0 and its extract status CB200_EXTRACT_EMPTY.  So a
+   plan of n slots runs part-full batches, and an index that is out of range at replay time -- which no check at create can see --
+   leaves its slot empty instead of touching memory outside d_states.  The map is grouped by receiver on the device at each launch:
+   one kernel more than the direct call, with work and memory that depend on n, not on n_receivers.
+   Like the receivers calls, a launch neither reads nor changes the context's own CCM (the plan keeps no CCM); it sets the
+   transforms' picture count and cb200_get_frame_ccms's frame count as the direct call does.  Launched, embedded, frozen, counted
+   and destroyed as every camera plan.
+   CB200_ERR_ARG, before any CUDA call: a null d_receiver_of or one not 4-byte aligned, a null d_states or one not 4-byte aligned,
+   n_receivers < 1, everything else cb200_scan_extract_decode_chunks_receivers_dev refuses, n == 0 and a context attached to a CCM
+   chain. */
+#define CB200_EXTRACT_EMPTY (-3)      /* extract status of an empty slot of a receivers plan */
+int cb200_camera_plan_create_receivers(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags, const int32_t* d_receiver_of,
+                                       int n_receivers, cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                       uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out);
 /* ---- auto mode: the sender's mode detected by decoding ----------------------------------------------------------------------
 
    The receiver's auto mode (the reference's web receiver tries 66, 68, 67 and 4 and keeps the first mode under which a frame gives

@@ -19,6 +19,7 @@ FLAG_NO_INTERLEAVE = 0x10
 FLAG_SHARPEN_IF_NEEDED = 0x20     # camera entry points only: sharpen the pictures Extractor::extract calls NEEDS_SHARPEN
 FRAME_FALLBACK = 0x1
 FRAME_INEXACT = 0x2
+EXTRACT_EMPTY = -3                # extract status of an empty slot of a receivers camera plan
 
 EXPORTS = [
     "cb200_last_error", "cb200_version", "cb200_create", "cb200_destroy", "cb200_get_info", "cb200_set_stream",
@@ -41,7 +42,7 @@ EXPORTS = [
     "cb200_ccm_chain_link_ms", "cb200_get_frame_ccms",
     "cb200_camera_plan_create", "cb200_camera_plan_launch", "cb200_camera_plan_graph", "cb200_camera_plan_destroy",
     "cb200_detect_scan_extract_decode_chunks_dev", "cb200_scan_extract_decode_chunks_pictures_dev",
-    "cb200_decode_chunks_receivers_dev", "cb200_scan_extract_decode_chunks_receivers_dev",
+    "cb200_decode_chunks_receivers_dev", "cb200_scan_extract_decode_chunks_receivers_dev", "cb200_camera_plan_create_receivers",
 ]
 
 
@@ -178,6 +179,7 @@ def load_library():
     lib.cb200_scan_extract_decode_chunks_pictures_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp]
+    lib.cb200_camera_plan_create_receivers.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp, vp]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -651,6 +653,27 @@ class Context:
                                                  C.byref(h)))
         return CameraPlan(self, h)
 
+    def receivers_camera_plan(self, pictures, receiver_of, states, chunks, mask, status, frame_flags=None, flags=0, order="rgb"):
+        """scan_extract_decode_chunks_receivers_dev captured once (cb200_camera_plan_create_receivers): a CameraPlan over the
+        pictures (uint8 CUDA tensors, as for scan_extract_decode_chunks_receivers_dev) whose receivers are read at each launch from
+        receiver_of (an int32 CUDA tensor of n values; one outside [0, n_receivers) leaves its slot empty: mask 0, status
+        EXTRACT_EMPTY).  states: a receiver_states tensor, one row per receiver.  chunks, mask, status, frame_flags: device
+        addresses, as for camera_plan.  Write each batch's pixels and map in stream order before its launch; the plan keeps the
+        tensors it binds alive"""
+        import torch
+        orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+        if len(orders) != len(pictures):
+            raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+        if not isinstance(receiver_of, torch.Tensor) or not receiver_of.is_cuda or receiver_of.dtype != torch.int32 or \
+                not receiver_of.is_contiguous() or receiver_of.numel() != len(pictures):
+            raise Cb200Error(f"receiver_of is a contiguous int32 CUDA tensor of {len(pictures)} values")
+        ptr, count = _states_ptr(states)
+        descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+        h = C.c_void_p()
+        _check(self.lib.cb200_camera_plan_create_receivers(self._h, C.cast(descs, C.c_void_p), len(pictures), flags, receiver_of.data_ptr(),
+                                                           count, ptr, chunks, mask, frame_flags, status, C.byref(h)))
+        return CameraPlan(self, h, keep=(list(pictures), receiver_of, states))
+
     jpeg_info = staticmethod(jpeg_info)
 
     def jpeg_decode_dev(self, files, d_rgb_out, d_status=None):
@@ -779,8 +802,9 @@ class CameraPlan:
     in progress on it (torch.cuda.graph); `graph` is the cudaGraph_t as an int.  The plan belongs to its context, which must outlive
     it (closing the context destroys its plans)"""
 
-    def __init__(self, ctx, handle):
+    def __init__(self, ctx, handle, keep=()):
         self.ctx, self._h = ctx, handle
+        self._keep = keep                  # the tensors a receivers plan binds
 
     def launch(self):
         _check(self.ctx.lib.cb200_camera_plan_launch(self._h))

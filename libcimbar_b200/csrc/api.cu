@@ -520,9 +520,9 @@ int receivers_ccm(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
     if (flags & CB200_FLAG_CC_SIMPLE) {
         CK(ccm_simple_launch(c->mode, d_rgb, n, c->d_ccm, c->stream), "ccm launch");
         CK(cudaMemsetAsync(c->d_ccm_active, 1, (size_t)n, c->stream), "set ccm flags");
-        CK(receivers_keep_launch(n, d_of, d_of + n, c->d_ccm, r.d_states, c->stream), "receivers keep launch");
+        CK(receivers_keep_launch(n, d_of, d_of + n, c->d_ccm, r.d_states, c->stream, r.empty_slots), "receivers keep launch");
     } else {
-        CK(receivers_gather_launch(n, d_of, r.d_states, c->d_ccm, c->d_ccm_active, c->stream), "receivers gather launch");
+        CK(receivers_gather_launch(n, d_of, r.d_states, c->d_ccm, c->d_ccm_active, c->stream, r.empty_slots), "receivers gather launch");
     }
     memset(&cc, 0, sizeof(cc));
     cc.per_frame = c->d_ccm; cc.active = 1;
@@ -555,24 +555,28 @@ int flood_reserve(cb200_ctx* c, int n)
     return CB200_OK;
 }
 
-int decode_reserve(cb200_ctx* c, uint32_t flags)
+int decode_reserve(cb200_ctx* c, uint32_t flags, bool receivers)
 {
-    int rc = decode_buffers(c, kCcm | kFitted | kLists | kSchedule); if (rc) return rc;
+    int rc = decode_buffers(c, kCcm | kFitted | kLists | kSchedule | (receivers ? kReceivers : 0u)); if (rc) return rc;
     const uint16_t* idx;
     return idx_for(c, flags, &idx);
 }
 
-int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states)
+int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states,
+                    bool on_device)
 {
-    if (!receiver_of) return fail(CB200_ERR_ARG, "null receiver_of");
+    if (!receiver_of) return fail(CB200_ERR_ARG, on_device ? "null d_receiver_of" : "null receiver_of");
+    if (on_device && reinterpret_cast<uintptr_t>(receiver_of) % 4) return fail(CB200_ERR_ARG, "d_receiver_of is not 4-byte aligned");
     if (!d_states) return fail(CB200_ERR_ARG, "null d_states");
     if (reinterpret_cast<uintptr_t>(d_states) % 4) return fail(CB200_ERR_ARG, "d_states is not 4-byte aligned");
     if (n_receivers < 1) return fail(CB200_ERR_ARG, "n_receivers < 1");
-    for (int i = 0; i < n; ++i)
+    for (int i = 0; i < n && !on_device; ++i)
         if (receiver_of[i] < 0 || receiver_of[i] >= n_receivers)
             return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + ": receiver " + std::to_string(receiver_of[i]) + " outside [0, " +
                                        std::to_string(n_receivers) + ")");
-    if (chain_attached(c)) return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, which carries one decoder's CCM: a receivers call decodes many");
+    // (a plan refuses a chained context after the batch's checks, as every camera plan does)
+    if (!on_device && chain_attached(c))
+        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, which carries one decoder's CCM: a receivers call decodes many");
     return CB200_OK;
 }
 
@@ -797,8 +801,9 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
     const bool fit = ccm_fits(m, flags), chained = chain_linked(c, flags);
-    // the CCM going into frame 0 is only known on the device -- always so for a camera plan, whose graph replays later
-    bool carried = enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->capturing;
+    // the CCM going into frame 0 is only known on the device -- always so for a camera plan, whose graph replays later.  A receivers
+    // call reads no context CCM, so a receivers plan takes the direct receivers call's route
+    bool carried = enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->capturing && !recv;
     if (enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->ccm_pending && !carried && !recv) {
         const cudaError_t q = cudaEventQuery(c->ccm_ev);
         if (q == cudaErrorNotReady) carried = true;
@@ -848,7 +853,7 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
         // across ranks: this stripe's fits out, the CCM entering the stripe in (from the lower ranks' fits of the same step)
         if (chained) { rc = chain_publish_link(c, n, c->d_fit, c->d_fit_valid, initial, &initial); if (rc) return rc; }
         if (recv) CK(ccm_carry_receivers_launch(n, recv->d_map, recv->d_map + n, c->d_fit, c->d_fit_valid, recv->d_states, c->d_ccm,
-                                                c->d_ccm_active, c->stream), "ccm carry");
+                                                c->d_ccm_active, c->stream, recv->empty_slots), "ccm carry");
         else CK(ccm_carry_launch(n, c->d_fit, c->d_fit_valid, initial, c->d_ccm, c->d_ccm_active, c->stream), "ccm carry");
         CK(ccm_apply_launch(m, c->d_means, n, c->d_ccm, c->d_ccm_active, c->d_cellvals, c->stream), "ccm apply");
         c->ccm_frames = n;

@@ -370,11 +370,14 @@ k_ccm_carry(int n_frames, const float* __restrict__ fit, const uint8_t* __restri
 
 // k_ccm_carry for a batch of several receivers: the same two-level max scan, over the receiver-major order and with the segment
 // starts scanned alongside (receivers_core.cuh), so each picture takes its own receiver's last fit or entry state.  used and
-// used_active are written in batch order; each receiver's last picture writes its exit state, after every entry state is read
-__global__ void __launch_bounds__(1024)
-k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ fit,
-                      const uint8_t* __restrict__ valid, cb200_receiver_state* __restrict__ states, float* __restrict__ used,
-                      uint8_t* __restrict__ used_active)
+// used_active are written in batch order; each receiver's last picture writes its exit state, after every entry state is read.
+// kEmpty (a receivers plan's map): slots of receiver -1 are empty, the last run of the order; they read and write no state and
+// decode without a CCM
+template <bool kEmpty>
+__device__ __forceinline__ void ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order,
+                                                    const float* __restrict__ fit, const uint8_t* __restrict__ valid,
+                                                    cb200_receiver_state* __restrict__ states, float* __restrict__ used,
+                                                    uint8_t* __restrict__ used_active)
 {
     __shared__ int seg_fit[1024], seg_start[1024];
     const int t = threadIdx.x;
@@ -392,6 +395,11 @@ k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_
     c = t > 0 ? receivers::Carry{seg_fit[t - 1], seg_start[t - 1]} : receivers::Carry{-1, 0};
     for (int j = j0; j < j1; ++j) {
         const int f = order[j], g = receivers::step(of, order, valid, j, c);
+        if (kEmpty && of[f] < 0) {
+            for (int i = 0; i < 9; ++i) used[(size_t)f * 9 + i] = 0.0f;
+            used_active[f] = 0;
+            continue;
+        }
         const cb200_receiver_state& e = states[of[f]];
         for (int i = 0; i < 9; ++i) used[(size_t)f * 9 + i] = g >= 0 ? fit[(size_t)g * 9 + i] : e.ccm[i];
         used_active[f] = (g >= 0 || e.active != 0) ? 1 : 0;
@@ -400,36 +408,104 @@ k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_
     for (int j = j0; j < j1; ++j) {
         if (!receivers::closes(of, order, n_frames, j)) continue;
         const int f = order[j];
+        if (kEmpty && of[f] < 0) continue;
         cb200_receiver_state& x = states[of[f]];
         for (int i = 0; i < 9; ++i) x.ccm[i] = used[(size_t)f * 9 + i];
         x.active = used_active[f];
     }
 }
 
+__global__ void __launch_bounds__(1024)
+k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ fit,
+                      const uint8_t* __restrict__ valid, cb200_receiver_state* __restrict__ states, float* __restrict__ used,
+                      uint8_t* __restrict__ used_active)
+{
+    ccm_carry_receivers<false>(n_frames, of, order, fit, valid, states, used, used_active);
+}
+
+__global__ void __launch_bounds__(1024)
+k_ccm_carry_receivers_empty(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ fit,
+                            const uint8_t* __restrict__ valid, cb200_receiver_state* __restrict__ states, float* __restrict__ used,
+                            uint8_t* __restrict__ used_active)
+{
+    ccm_carry_receivers<true>(n_frames, of, order, fit, valid, states, used, used_active);
+}
+
 // without a CC flag every picture decodes with its receiver's matrix.  An inactive receiver's pictures get the identity: the colour
 // decision on integer means through the identity is exactly the decision without a CCM (see k_ccm_apply), so one K1 instantiation
-// serves the whole batch
-__global__ void k_receivers_gather(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
-                                   float* __restrict__ ccm, uint8_t* __restrict__ active)
+// serves the whole batch.  kEmpty: an empty slot (receiver -1) gets the identity too
+template <bool kEmpty>
+__device__ __forceinline__ void receivers_gather(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
+                                                 float* __restrict__ ccm, uint8_t* __restrict__ active)
 {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_frames) return;
+    if (kEmpty && of[f] < 0) {
+        for (int i = 0; i < 9; ++i) ccm[(size_t)f * 9 + i] = i % 4 == 0 ? 1.0f : 0.0f;
+        active[f] = 0;
+        return;
+    }
     const cb200_receiver_state& s = states[of[f]];
     const bool a = s.active != 0;
     for (int i = 0; i < 9; ++i) ccm[(size_t)f * 9 + i] = a ? s.ccm[i] : (i % 4 == 0 ? 1.0f : 0.0f);
     active[f] = a ? 1 : 0;
 }
 
-// CC_SIMPLE: each receiver keeps the matrix of its last picture
-__global__ void k_receivers_keep(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ ccm,
-                                 cb200_receiver_state* __restrict__ states)
+__global__ void k_receivers_gather(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
+                                   float* __restrict__ ccm, uint8_t* __restrict__ active)
+{
+    receivers_gather<false>(n_frames, of, states, ccm, active);
+}
+
+__global__ void k_receivers_gather_empty(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
+                                         float* __restrict__ ccm, uint8_t* __restrict__ active)
+{
+    receivers_gather<true>(n_frames, of, states, ccm, active);
+}
+
+// CC_SIMPLE: each receiver keeps the matrix of its last picture (kEmpty: the run of empty slots keeps nothing)
+template <bool kEmpty>
+__device__ __forceinline__ void receivers_keep(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order,
+                                               const float* __restrict__ ccm, cb200_receiver_state* __restrict__ states)
 {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n_frames || !receivers::closes(of, order, n_frames, j)) return;
     const int f = order[j];
+    if (kEmpty && of[f] < 0) return;
     cb200_receiver_state& x = states[of[f]];
     for (int i = 0; i < 9; ++i) x.ccm[i] = ccm[(size_t)f * 9 + i];
     x.active = 1;
+}
+
+__global__ void k_receivers_keep(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ ccm,
+                                 cb200_receiver_state* __restrict__ states)
+{
+    receivers_keep<false>(n_frames, of, order, ccm, states);
+}
+
+__global__ void k_receivers_keep_empty(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order,
+                                       const float* __restrict__ ccm, cb200_receiver_state* __restrict__ states)
+{
+    receivers_keep<true>(n_frames, of, order, ccm, states);
+}
+
+// a receivers plan's map from the receiver indices the caller wrote for this launch (receivers_core.cuh): of[i] = slot i's
+// receiver, -1 for an empty slot, and order[rank of slot i] = i.  32 slots per block; its 8 warps split each slot's n key
+// comparisons, all lanes of a warp reading the same slot j at a time
+constexpr int kOrderSlots = 32, kOrderParts = 8;
+__global__ void __launch_bounds__(kOrderSlots * kOrderParts)
+k_receivers_order(int n, const int32_t* __restrict__ receiver_of, int receivers, int32_t* __restrict__ of, int32_t* __restrict__ order)
+{
+    __shared__ int part[kOrderParts][kOrderSlots];
+    const int lane = threadIdx.x % kOrderSlots, w = threadIdx.x / kOrderSlots, i = blockIdx.x * kOrderSlots + lane;
+    const int32_t r = i < n ? receiver_of[i] : -1;
+    part[w][lane] = i < n ? receivers::rank_part(receiver_of, n, receivers, receivers::slot_key(r, receivers, i), w, kOrderParts) : 0;
+    __syncthreads();
+    if (w != 0 || i >= n) return;
+    int rank = 0;
+    for (int q = 0; q < kOrderParts; ++q) rank += part[q][lane];
+    of[i] = receivers::slot_receiver(r, receivers);
+    order[rank] = i;
 }
 
 // CimbDecoder::get_best_color for every cell from the mean colours the first pass stored.  blockIdx.y walks the frames (the
@@ -496,21 +572,33 @@ cudaError_t ccm_apply_launch(const Mode& m, const uint32_t* d_means, int n_frame
     return cudaGetLastError();
 }
 cudaError_t ccm_carry_receivers_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_fit, const uint8_t* d_valid,
-                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st)
+                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st, bool empty_slots)
 {
-    k_ccm_carry_receivers<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active); count_launch();
+    if (empty_slots) k_ccm_carry_receivers_empty<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active);
+    else k_ccm_carry_receivers<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active);
+    count_launch();
     return cudaGetLastError();
 }
 cudaError_t receivers_gather_launch(int n_frames, const int32_t* d_of, const cb200_receiver_state* d_states, float* d_ccm, uint8_t* d_active,
-                                    cudaStream_t st)
+                                    cudaStream_t st, bool empty_slots)
 {
-    k_receivers_gather<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_states, d_ccm, d_active); count_launch();
+    if (empty_slots) k_receivers_gather_empty<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_states, d_ccm, d_active);
+    else k_receivers_gather<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_states, d_ccm, d_active);
+    count_launch();
     return cudaGetLastError();
 }
 cudaError_t receivers_keep_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_ccm, cb200_receiver_state* d_states,
-                                  cudaStream_t st)
+                                  cudaStream_t st, bool empty_slots)
 {
-    k_receivers_keep<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_order, d_ccm, d_states); count_launch();
+    if (empty_slots) k_receivers_keep_empty<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_order, d_ccm, d_states);
+    else k_receivers_keep<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_order, d_ccm, d_states);
+    count_launch();
+    return cudaGetLastError();
+}
+cudaError_t receivers_order_launch(int n, const int32_t* d_receiver_of, int receivers, int32_t* d_map, cudaStream_t st)
+{
+    k_receivers_order<<<(n + kOrderSlots - 1) / kOrderSlots, kOrderSlots * kOrderParts, 0, st>>>(n, d_receiver_of, receivers, d_map, d_map + n);
+    count_launch();
     return cudaGetLastError();
 }
 

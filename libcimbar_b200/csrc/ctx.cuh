@@ -142,8 +142,9 @@ int scan_reserve(cb200_ctx* c, const int32_t* wh, int n);
 int camera_reserve(cb200_ctx* c, const int32_t* wh, int n);
 int deskew_reserve(cb200_ctx* c, int n);
 int flood_reserve(cb200_ctx* c, int n);
-// the decode's buffers sized by max_frames, the CCM event and the slot map of these flags (api.cu): no CUDA call after the first time
-int decode_reserve(cb200_ctx* c, uint32_t flags);
+// the decode's buffers sized by max_frames, the CCM event and the slot map of these flags, and with `receivers` a receivers call's
+// (api.cu): no CUDA call after the first time
+int decode_reserve(cb200_ctx* c, uint32_t flags, bool receivers = false);
 // CB200_ERR_ARG, before any CUDA call, when live plans freeze a buffer this call would grow; nothing without plans (plan.cu).
 // frames: n decoded frames (the exact walk); deskew: n deskewed frames too; camera / scan: n camera pictures of sizes wh
 int check_frozen_frames(cb200_ctx* c, int n);
@@ -174,13 +175,19 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
 // the receivers of a _receivers_dev call (include/cb200.h).  check_receivers: CB200_ERR_ARG, before any CUDA call, for a null
 // receiver map, null or misaligned states, n_receivers < 1, a receiver index out of range, a context linked to a CCM chain (api.cu).
 // Receivers(...) then builds `map` on the host: the n receiver indices, then the receiver-major order (receivers_core.cuh); d_map is
-// its device copy once uploaded (the camera calls: behind the picture table; the frame call: in cb200_ctx::d_recv)
-int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states);
+// its device copy once uploaded (the camera calls: behind the picture table; the frame call: in cb200_ctx::d_recv).
+// A receivers camera plan reads its map on the device: check_receivers with on_device checks the pointer (null, 4-byte alignment)
+// instead of the indices, and Receivers(d_map, states) has no host map -- d_map is the plan's, built by k_receivers_order at each
+// launch, where receiver -1 marks an empty slot (empty_slots: the kernels' variants that skip those)
+int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states,
+                    bool on_device = false);
 struct Receivers {
     std::vector<int32_t> map;
     const int32_t* d_map = nullptr;
     cb200_receiver_state* d_states = nullptr;
+    bool empty_slots = false;
     Receivers(const int32_t* receiver_of, int n, int n_receivers, cb200_receiver_state* states);
+    Receivers(const int32_t* d_plan_map, cb200_receiver_state* states) : d_map(d_plan_map), d_states(states), empty_slots(true) {}
     size_t bytes() const { return map.size() * sizeof(int32_t); }
 };
 // the context is attached to a CCM chain (chain.cu)

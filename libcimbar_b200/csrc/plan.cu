@@ -9,6 +9,10 @@
 //   - the CCM always comes from the device (c->d_carry, which carry_from_host keeps current while plans exist) instead of
 //     cudaEventQuery choosing between the host matrix and the carry, a choice a graph would freeze at capture time.
 // The kernels are the direct call's, launched by the same code on a private capture stream.
+//
+// A receivers plan (cb200_camera_plan_create_receivers) is the receivers camera call captured so.  Its receiver map is the one
+// input the direct call builds on the host per batch: here k_receivers_order, captured at the head of the graph, builds it at each
+// launch from the caller's d_receiver_of into the plan's own d_map, and the rest of the graph reads it from there.
 #include "ctx.cuh"
 
 #include <string>
@@ -21,6 +25,11 @@ struct cb200_camera_plan {
     int n = 0;
     uint32_t flags = 0;
     DevBuf<uint8_t> d_table;                // n PicDesc, then the pictures grouped by blur radius
+    // a receivers plan: the caller's map and states, and the map the graph builds from it (n receivers, -1 = empty, then the order)
+    const int32_t* d_receiver_of = nullptr;
+    int n_receivers = 0;
+    cb200_receiver_state* d_states = nullptr;
+    DevBuf<int32_t> d_map;
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     int kernels = 0;                        // kernel nodes of the graph (cb200_launch_count)
@@ -89,7 +98,15 @@ int capture(cb200_camera_plan* p, cudaStream_t cap, const CameraBatch& b, uint8_
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) rc = fail_cuda(e, "cudaStreamBeginCapture");
     if (!rc) {
-        rc = camera_enqueue(c, b, p->flags, d_chunks, d_mask, d_frame_flags, d_status, reinterpret_cast<const PicDesc*>(p->d_table.get()));
+        const PicDesc* table = reinterpret_cast<const PicDesc*>(p->d_table.get());
+        if (!p->d_receiver_of) {
+            rc = camera_enqueue(c, b, p->flags, d_chunks, d_mask, d_frame_flags, d_status, table);
+        } else {
+            Receivers r(p->d_map.get(), p->d_states);
+            e = receivers_order_launch(p->n, p->d_receiver_of, p->n_receivers, p->d_map, cap);
+            rc = e != cudaSuccess ? fail_cuda(e, "receivers order launch")
+                                  : camera_enqueue(c, b, p->flags, d_chunks, d_mask, d_frame_flags, d_status, table, &r);
+        }
         cudaGraph_t g = nullptr;
         e = cudaStreamEndCapture(cap, &g);
         if (!rc && e != cudaSuccess) rc = fail_cuda(e, "cudaStreamEndCapture");
@@ -108,36 +125,39 @@ int capture(cb200_camera_plan* p, cudaStream_t cap, const CameraBatch& b, uint8_
     return rc;
 }
 
-}  // namespace
-
-extern "C" {
-
-int cb200_camera_plan_create(cb200_ctx* c, const int32_t* wh, int n, uint32_t flags, const uint8_t* d_pictures, uint8_t* d_chunks,
-                             uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out)
+// a plan's own rules, checked after its batch's
+int plan_rules(int n, cb200_camera_plan** out)
 {
-    // the checks of cb200_scan_extract_decode_chunks_ragged_dev, with the plan's own after the batch's and after the CCM chain's
-    auto build = [&](CameraBatch& b) {
-        int rc = packed_batch(d_pictures, wh, n, b); if (rc) return rc;
-        if (n == 0) return fail(CB200_ERR_ARG, "n = 0: a camera plan needs at least one picture");
-        if (!out) return fail(CB200_ERR_ARG, "null plan");
-        *out = nullptr;
-        return CB200_OK;
-    };
-    CameraBatch b;
-    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
-    if (check_host_ccm(c))
-        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
-    rc = check_frozen_camera(c, wh, n); if (rc) return rc;
+    if (n == 0) return fail(CB200_ERR_ARG, "n = 0: a camera plan needs at least one picture");
+    if (!out) return fail(CB200_ERR_ARG, "null plan");
+    *out = nullptr;
+    return CB200_OK;
+}
+
+// a plan for the checked batch b (after every argument check): the buffers grown, the table uploaded, the capture, the graph
+// instantiated.  recv: a receivers plan's bound map and states (its d_map is allocated here)
+struct PlanReceivers { const int32_t* d_receiver_of; int n_receivers; cb200_receiver_state* d_states; };
+
+int make_plan(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+              int32_t* d_extract_status, const PlanReceivers* recv, cb200_camera_plan** out)
+{
+    const int n = b.n();
+    int rc = check_frozen_camera(c, b.wh.data(), n); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     // every buffer the graph uses, at this batch's size (with plans already there, the freeze check above guarantees this grows nothing)
-    rc = camera_reserve(c, wh, n); if (rc) return rc;
-    rc = decode_reserve(c, flags); if (rc) return rc;
+    rc = camera_reserve(c, b.wh.data(), n); if (rc) return rc;
+    rc = decode_reserve(c, flags, recv != nullptr); if (rc) return rc;
     cb200_camera_plan* p = new cb200_camera_plan();
     p->ctx = c; p->n = n; p->flags = flags;
-    p->keeps_ccm = (flags & CB200_FLAG_CC_SIMPLE) || ccm_fits(c->mode, flags);
+    p->keeps_ccm = !recv && ((flags & CB200_FLAG_CC_SIMPLE) || ccm_fits(c->mode, flags));
+    if (recv) {
+        p->d_receiver_of = recv->d_receiver_of; p->n_receivers = recv->n_receivers; p->d_states = recv->d_states;
+        const cudaError_t e = p->d_map.ensure(2 * (size_t)n);
+        if (e != cudaSuccess) rc = fail_cuda(e, "cudaMalloc plan receiver map");
+    }
     std::vector<uint8_t> table;
     cudaStream_t cap = nullptr;
-    rc = pic_table(c, b, table);
+    if (!rc) rc = pic_table(c, b, table);
     if (!rc) { const cudaError_t e = p->d_table.ensure(table.size()); if (e != cudaSuccess) rc = fail_cuda(e, "cudaMalloc plan picture table"); }
     if (!rc) { const cudaError_t e = cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking); if (e != cudaSuccess) rc = fail_cuda(e, "cudaStreamCreate"); }
     if (!rc) {   // the table goes up once, on the private stream, before anything can replay
@@ -155,11 +175,44 @@ int cb200_camera_plan_create(cb200_ctx* c, const int32_t* wh, int n, uint32_t fl
         delete p;
         return fail(rc, why);
     }
-    // the graph starts from d_carry: unless a CCM is on its way there from the device, the host's goes there now
+    // the graph starts from d_carry: unless a CCM is on its way there from the device, the host's goes there now (a receivers plan
+    // reads no context CCM, but while plans exist d_carry mirrors the host's matrix for every plain one)
     c->plans.push_back(p);
     if (!c->ccm_pending && (rc = carry_from_host(c)) != CB200_OK) { cb200_camera_plan_destroy(p); return rc; }
     *out = p;
     return CB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cb200_camera_plan_create(cb200_ctx* c, const int32_t* wh, int n, uint32_t flags, const uint8_t* d_pictures, uint8_t* d_chunks,
+                             uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out)
+{
+    // the checks of cb200_scan_extract_decode_chunks_ragged_dev, with the plan's own after the batch's and after the CCM chain's
+    auto build = [&](CameraBatch& b) { const int rc = packed_batch(d_pictures, wh, n, b); return rc ? rc : plan_rules(n, out); };
+    CameraBatch b;
+    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
+    if (check_host_ccm(c))
+        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
+    return make_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, out);
+}
+
+int cb200_camera_plan_create_receivers(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, const int32_t* d_receiver_of,
+                                       int n_receivers, cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                       uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out)
+{
+    // the checks of cb200_scan_extract_decode_chunks_receivers_dev (the map's pointer in place of its indices, which only a launch
+    // reads), then the plan's own as cb200_camera_plan_create makes them
+    int rc = check_receivers(c, d_receiver_of, n, n_receivers, d_states, true); if (rc) return rc;
+    auto build = [&](CameraBatch& b) { const int rc = picture_batch(pics, n, b); return rc ? rc : plan_rules(n, out); };
+    CameraBatch b;
+    rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
+    if (check_host_ccm(c))
+        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
+    const PlanReceivers recv = {d_receiver_of, n_receivers, d_states};
+    return make_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
 }
 
 int cb200_camera_plan_launch(cb200_camera_plan* p)
@@ -180,9 +233,9 @@ int cb200_camera_plan_launch(cb200_camera_plan* p)
     }
     CK(cudaGraphLaunch(p->exec, c->stream), "cudaGraphLaunch");
     count_launch(p->kernels);
-    // the host state the direct call leaves behind
+    // the host state the direct call leaves behind (a receivers call reports every picture's matrix, CC_SIMPLE too)
     set_camera_pictures(c, p->n);
-    if (!(p->flags & CB200_FLAG_CC_SIMPLE)) c->ccm_frames = p->n;
+    if (p->d_receiver_of || !(p->flags & CB200_FLAG_CC_SIMPLE)) c->ccm_frames = p->n;
     if (p->keeps_ccm) {
         CK(cudaEventRecord(c->ccm_ev, c->stream), "record ccm");
         c->ccm_pending = true;

@@ -55,5 +55,25 @@ inline void make_order(const int32_t* of, int n, int receivers, int32_t* order)
     for (int i = 0; i < n; ++i) order[first[(size_t)of[i]]++] = i;
 }
 
+// The device side (a receivers camera plan, whose map is read at replay time, k_receivers_order in ccm.cu): the same order, built
+// without a pass over the receivers, and with "empty" slots -- a receiver outside [0, receivers) -- after every other slot.  Slot i
+// sorts by key(i) = (receiver, i), an empty slot's receiver counting as 2^32 - 1; the keys are distinct, and the position of slot i
+// is its rank, the number of slots with a smaller key.  On the non-empty slots that is make_order's stable counting sort.  Work
+// and memory depend on n only: a service may bind 10^6 receivers.
+CB_HD bool empty_slot(int32_t r, int receivers) { return r < 0 || r >= receivers; }
+// the receiver a kernel reads for a slot: -1 for an empty one, so that the empty slots form one run at the end of the order
+CB_HD int32_t slot_receiver(int32_t r, int receivers) { return empty_slot(r, receivers) ? -1 : r; }
+CB_HD uint64_t slot_key(int32_t r, int receivers, int i)
+{
+    return ((uint64_t)(empty_slot(r, receivers) ? 0xFFFFFFFFu : (uint32_t)r) << 32) | (uint32_t)i;
+}
+// the slots j = j0, j0 + stride, ... < n whose key is below k: one lane's part of a rank
+CB_HD int rank_part(const int32_t* of, int n, int receivers, uint64_t k, int j0, int stride)
+{
+    int below = 0;
+    for (int j = j0; j < n; j += stride) below += slot_key(of[j], receivers, j) < k;
+    return below;
+}
+
 }  // namespace receivers
 }  // namespace cb200

@@ -597,6 +597,16 @@ __global__ void k_mask_failed(const int32_t* __restrict__ status, int n, uint32_
     if (i < n && status[i] <= 0) mask[i] = 0;
 }
 
+// k_mask_failed in a receivers plan: an empty slot (receiver -1 in the plan's map, of) yields no chunks either, and its status,
+// which k_extract wrote before, becomes CB200_EXTRACT_EMPTY
+__global__ void k_mask_failed_empty(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (of[i] < 0) status[i] = CB200_EXTRACT_EMPTY;
+    if (status[i] <= 0) mask[i] = 0;
+}
+
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks)
 {
     ScanScratch* s = sstate(c);
@@ -627,7 +637,8 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     if (deskew) { rc = deskew_launch(c, b, s->d_minv, d_desc, frames); if (rc) return rc; }
     rc = decode_chunks(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, d_chunks, d_mask, d_frame_flags, d_sharp, true, recv);
     if (rc) return rc;
-    k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
+    if (recv && recv->empty_slots) k_mask_failed_empty<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv->d_map);
+    else k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
     count_launch();
     CK(cudaGetLastError(), "mask launch");
     return CB200_OK;
