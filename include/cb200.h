@@ -410,6 +410,41 @@ int cb200_camera_plan_create_receivers(cb200_ctx* ctx, const cb200_picture* pics
 int cb200_detect_scan_extract_decode_chunks_dev(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d_pictures, const int32_t* wh, int n,
                                                 uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
                                                 int32_t* d_mode, uint32_t* d_mode_masks);
+/* ---- auto mode for receivers: each picture under its receiver's candidate modes ------------------------------------------------
+
+   The auto-mode call for a batch of many receivers (a decode service's sessions, some still detecting their sender's mode, others
+   locked to one), in one enqueue-only call.
+     ctxs, n_modes: as on cb200_detect_scan_extract_decode_chunks_dev (1 .. 5 contexts, one per mode, priority order).
+     pics, n, flags: as on cb200_scan_extract_decode_chunks_receivers_dev (descriptors in any layout and pitch).
+     candidates: HOST, n entries, read before the call returns: picture i is decoded under ctxs[k] when bit k is set.  NULL: every
+                 picture under every mode.
+     receiver_of, n_receivers: HOST, n entries in [0, n_receivers), as on the receivers calls.
+     d_states:   a HOST array of n_modes pointers, each to a DEVICE table of n_receivers cb200_receiver_state: mode k's state of every
+                 receiver.  The n_modes tables must not overlap.
+     d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks: as on the detect call.
+   Contract.  Let P_k be the pictures whose candidates have bit k set, in batch order.  For every k, every output for the pictures of
+   P_k, and d_states[k] afterwards, equals bit for bit what cb200_scan_extract_decode_chunks_receivers_dev(ctxs[k], P_k's
+   descriptors, P_k's receivers, d_states[k]) gives: records, masks, frame flags, extract statuses, states.  d_mode[i] is the first k
+   in priority order with i in P_k and a nonzero mask, or -1; d_chunks slot i holds that mode's record as on the detect call;
+   d_extract_status[i] is the status under d_mode[i], or under picture i's first candidate for -1; d_mode_masks[i][k] is 0 when i is
+   not in P_k.  As on the receivers calls, no context's own CCM is read or changed; as on the detect call, a wrong-mode decode moves
+   that mode's receiver state (a receiver with every candidate bit advances every mode's table).  cb200_camera_transforms and
+   cb200_get_frame_ccms on the contexts are not part of the contract after this call.
+   Sharing: one anchor scan over all n pictures; each frame geometry extracts, deskews and walks only the pictures that some of its
+   modes decode, once, on side streams as in the detect call, and a geometry none of whose modes has pictures launches nothing.  So a
+   batch locked to one mode pays for that mode's geometry only.  K1, colours, CCM, RS and masks run per mode with that mode's receiver
+   table; a picture of the geometry's sub-batch that the mode does not decode is an empty slot of that table, as in a receivers plan.
+   The lists travel in the one upload of the picture table.
+   CB200_ERR_ARG before any CUDA call, naming the violation: everything the detect call refuses (n_modes, flags, null outputs and the
+   context checks); everything cb200_scan_extract_decode_chunks_receivers_dev refuses on the pictures and receivers (descriptors,
+   sizes, spans, a null receiver_of, n_receivers < 1, a receiver out of range, naming the picture); a candidates entry that is 0 or
+   has a bit at or above n_modes (naming the picture); a null d_states, a null or not 4-byte aligned table (naming it); two tables
+   whose n_receivers-entry ranges overlap (their modes may run on different streams).  Not capturable in a camera plan. */
+int cb200_detect_scan_extract_decode_chunks_receivers_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n,
+                                                          uint32_t flags, const uint32_t* candidates, const int32_t* receiver_of,
+                                                          int n_receivers, cb200_receiver_state* const* d_states, uint8_t* d_chunks,
+                                                          uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode,
+                                                          uint32_t* d_mode_masks);
 /* ---- JPEG files in: the CLI's input, decoded on the device ---------------------------------------------------------------
 
    Replaces: cv::imread(file) + cv::cvtColor(BGR2RGB) (src/exe/cimbar/cimbar.cpp:132-133) for a batch of JPEG files in host memory:

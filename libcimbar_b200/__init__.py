@@ -43,6 +43,7 @@ EXPORTS = [
     "cb200_camera_plan_create", "cb200_camera_plan_launch", "cb200_camera_plan_graph", "cb200_camera_plan_destroy",
     "cb200_detect_scan_extract_decode_chunks_dev", "cb200_scan_extract_decode_chunks_pictures_dev",
     "cb200_decode_chunks_receivers_dev", "cb200_scan_extract_decode_chunks_receivers_dev", "cb200_camera_plan_create_receivers",
+    "cb200_detect_scan_extract_decode_chunks_receivers_dev",
 ]
 
 
@@ -180,6 +181,8 @@ def load_library():
     lib.cb200_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp]
     lib.cb200_camera_plan_create_receivers.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp, vp]
+    lib.cb200_detect_scan_extract_decode_chunks_receivers_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, C.c_int, vp, vp, vp,
+                                                                          vp, vp, vp]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -305,6 +308,36 @@ def detect_scan_extract_decode_chunks_dev(ctxs, d_pictures, wh, d_chunks, d_mask
     hs = (C.c_void_p * max(len(ctxs), 1))(*[c._h.value for c in ctxs])
     _check(load_library().cb200_detect_scan_extract_decode_chunks_dev(hs, len(ctxs), d_pictures, wh.ctypes.data, wh.shape[0], flags,
                                                                       d_chunks, d_mask, d_status, d_mode, d_mode_masks))
+
+
+def detect_scan_extract_decode_chunks_receivers_dev(ctxs, pictures, receiver_of, states, d_chunks, d_mask, d_status, d_mode, candidates=None,
+                                                    d_mode_masks=None, flags=0, order="rgb"):
+    """The auto mode for pictures of many receivers, enqueue-only (cb200_detect_scan_extract_decode_chunks_receivers_dev): picture i
+    (a uint8 CUDA tensor, as for Context.scan_extract_decode_chunks_receivers_dev) belongs to receiver receiver_of[i] and is decoded
+    under ctxs[k] when bit k of candidates[i] is set (candidates: n bitmasks, or None for every mode).  states: one receiver_states
+    tensor per context, each receiver's state under that mode.  For every k, the pictures with bit k get what
+    Context.scan_extract_decode_chunks_receivers_dev on ctxs[k] gives on those pictures alone with states[k]; the outputs select among
+    them as detect_scan_extract_decode_chunks_dev does (d_mode: the index into ctxs, or -1)"""
+    orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+    if len(orders) != len(pictures):
+        raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+    if len(states) != len(ctxs):
+        raise Cb200Error(f"{len(states)} state tables for {len(ctxs)} contexts")
+    of = _receiver_map(receiver_of, len(pictures))
+    tables = [_states_ptr(s) for s in states]
+    if len({count for _, count in tables}) > 1:
+        raise Cb200Error("every state table holds the same receivers: " + ", ".join(str(count) for _, count in tables) + " entries")
+    cand = None
+    if candidates is not None:
+        cand = np.ascontiguousarray(candidates, dtype=np.uint32).reshape(-1)
+        if cand.shape[0] != len(pictures):
+            raise Cb200Error(f"{cand.shape[0]} candidate masks for {len(pictures)} pictures")
+    hs = (C.c_void_p * max(len(ctxs), 1))(*[c._h.value for c in ctxs])
+    ptrs = (C.c_void_p * max(len(tables), 1))(*[p for p, _ in tables])
+    descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+    _check(load_library().cb200_detect_scan_extract_decode_chunks_receivers_dev(
+        hs, len(ctxs), C.cast(descs, C.c_void_p), len(pictures), flags, _hptr(cand), of.ctypes.data, tables[0][1] if tables else 0, ptrs,
+        d_chunks, d_mask, d_status, d_mode, d_mode_masks))
 
 
 def _hptr(a):

@@ -166,12 +166,15 @@ int pic_table(cb200_ctx* c, const CameraBatch& b, std::vector<uint8_t>& table);
 // (scans = false) or the deskewed frames' and the walk's (walks = false).  camera_scan: the scan of the batch on this context's
 // scratch (the table from d_table, else uploaded), *d_desc = its picture table.  camera_after_scan: k_extract on `scanned`'s
 // anchors into this context's transforms and d_status, the deskew into `frames` (deskew = false: `frames` holds them already,
-// deskewed for this geometry), the decode and the failed pictures' masks
+// deskewed for this geometry), the decode and the failed pictures' masks.  A detect receivers call's geometry runs camera_after_scan
+// on a sub-batch: b and d_desc describe its pictures, and d_slots (device) names each one's picture in the scanned batch; its host
+// lists (tail) travel with camera_scan's upload
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks);
-int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc, Receivers* recv = nullptr);
+int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc, Receivers* recv = nullptr,
+                const std::vector<uint8_t>* tail = nullptr, const uint8_t** d_tail = nullptr);
 int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
                       bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status,
-                      Receivers* recv = nullptr);
+                      Receivers* recv = nullptr, const int32_t* d_slots = nullptr);
 // the receivers of a _receivers_dev call (include/cb200.h).  check_receivers: CB200_ERR_ARG, before any CUDA call, for a null
 // receiver map, null or misaligned states, n_receivers < 1, a receiver index out of range, a context linked to a CCM chain (api.cu).
 // Receivers(...) then builds `map` on the host: the n receiver indices, then the receiver-major order (receivers_core.cuh); d_map is

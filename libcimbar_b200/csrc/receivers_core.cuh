@@ -46,13 +46,50 @@ CB_HD int step(const int32_t* of, const int32_t* order, const uint8_t* valid, in
     return c.fit >= c.start ? order[c.fit] : -1;
 }
 
-// the host side: the stable receiver-major order of n pictures of receivers [0, receivers) (every of[i] in range)
+// the host side: the stable receiver-major order of n pictures of receivers [0, receivers), every of[i] in range or -1 for an empty
+// slot (a detect receivers call's, below), which goes after every other
 inline void make_order(const int32_t* of, int n, int receivers, int32_t* order)
 {
-    std::vector<int32_t> first((size_t)receivers + 1, 0);
-    for (int i = 0; i < n; ++i) ++first[(size_t)of[i] + 1];
+    std::vector<int32_t> first((size_t)receivers + 2, 0);
+    auto bucket = [&](int i) { return (size_t)(of[i] < 0 ? receivers : of[i]); };
+    for (int i = 0; i < n; ++i) ++first[bucket(i) + 1];
     for (int r = 0; r < receivers; ++r) first[(size_t)r + 1] += first[(size_t)r];
-    for (int i = 0; i < n; ++i) order[first[(size_t)of[i]]++] = i;
+    for (int i = 0; i < n; ++i) order[first[bucket(i)]++] = i;
+}
+
+// The host side of a detect receivers call (cb200_detect_scan_extract_decode_chunks_receivers_dev, detect.cu).  Picture i is decoded
+// under mode k when bit k of cand[i] is set; P_k: those pictures in batch order.  The modes of one frame geometry (group[k]) share
+// one sub-batch U_g, the batch-ordered union of their P_k: it is extracted, deskewed and walked once.  For mode k, a position of U_g
+// outside P_k is an empty slot -- receiver -1, after every other position in the order -- as in a receivers plan's map
+constexpr int kMaxModes = 5;                 // detect.cu's kDetectModes
+struct DetectLists {
+    std::vector<int32_t> slots[kMaxModes];   // per geometry: U_g's batch indices
+    std::vector<int32_t> map[kMaxModes];     // per mode with P_k nonempty: |U_g| receivers (-1: empty), then the order
+    std::vector<int32_t> pos;                // n_modes x n: picture i's position in U_{group[k]} when i is in P_k, else -1
+    int count[kMaxModes] = {};               // |P_k|
+};
+inline void detect_lists(const uint32_t* cand, const int32_t* of, int n, int receivers, int n_modes, const int* group, DetectLists& l)
+{
+    uint32_t modes_of[kMaxModes] = {};       // per geometry: its modes' bits
+    for (int k = 0; k < n_modes; ++k) { modes_of[group[k]] |= 1u << k; l.count[k] = 0; l.map[k].clear(); }
+    for (int g = 0; g < kMaxModes; ++g) l.slots[g].clear();
+    l.pos.assign((size_t)n_modes * (size_t)n, -1);
+    for (int i = 0; i < n; ++i)
+        for (int g = 0; g < n_modes; ++g) {
+            if (!(cand[i] & modes_of[g])) continue;
+            const int at = (int)l.slots[g].size();
+            l.slots[g].push_back(i);
+            for (int k = 0; k < n_modes; ++k)
+                if (group[k] == g && (cand[i] >> k & 1u)) { l.pos[(size_t)k * n + i] = at; ++l.count[k]; }
+        }
+    for (int k = 0; k < n_modes; ++k) {
+        if (!l.count[k]) continue;
+        const std::vector<int32_t>& u = l.slots[group[k]];
+        const int m = (int)u.size();
+        l.map[k].resize(2 * (size_t)m);
+        for (int j = 0; j < m; ++j) l.map[k][(size_t)j] = (cand[u[(size_t)j]] >> k & 1u) ? of[u[(size_t)j]] : -1;
+        make_order(l.map[k].data(), m, receivers, l.map[k].data() + m);
+    }
 }
 
 // The device side (a receivers camera plan, whose map is read at replay time, k_receivers_order in ccm.cu): the same order, built

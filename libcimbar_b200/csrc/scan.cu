@@ -485,8 +485,10 @@ int pic_table(cb200_ctx* c, const CameraBatch& b, std::vector<uint8_t>& table)
 
 // blurred pictures + thresholds + anchors for a device batch, in the state's device arrays; enqueued only.  The picture table
 // (PicDesc, in s->d_table) is this call's one upload -- unless d_table holds it already (a camera plan's): then *d_desc = d_table
-// and nothing is uploaded.  A receivers call's map travels behind the table, in the same slot
-int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc_out, Receivers* recv)
+// and nothing is uploaded.  A receivers call's map travels behind the table, in the same slot, and so do a detect receivers call's
+// lists (`tail`, 8-byte aligned on the device at *d_tail)
+int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, const PicDesc** d_desc_out, Receivers* recv,
+                const std::vector<uint8_t>* tail, const uint8_t** d_tail)
 {
     ScanScratch* s = sstate(c);
     cudaStream_t st = c->stream;
@@ -499,16 +501,19 @@ int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, cons
         std::vector<uint8_t> table(table_bytes);
         err = pic_table(s, b, table.data(), g); if (err) return err;
     } else {
-        const size_t map_bytes = recv ? recv->bytes() : 0;
-        CK(s->d_table.ensure(table_bytes + map_bytes), "cudaMalloc picture table");
+        const size_t map_bytes = recv ? recv->bytes() : 0, tail_at = (table_bytes + map_bytes + 7) & ~(size_t)7;
+        const size_t bytes = tail ? tail_at + tail->size() : table_bytes + map_bytes;
+        CK(s->d_table.ensure(bytes), "cudaMalloc picture table");
         int slot;
         uint8_t* h_table;
-        err = c->upload.take(table_bytes + map_bytes, &slot, &h_table); if (err) return err;
+        err = c->upload.take(bytes, &slot, &h_table); if (err) return err;
         err = pic_table(s, b, h_table, g); if (err) return err;
         if (recv) memcpy(h_table + table_bytes, recv->map.data(), map_bytes);
-        err = c->upload.send(st, slot, s->d_table, table_bytes + map_bytes); if (err) return err;
+        if (tail) memcpy(h_table + tail_at, tail->data(), tail->size());
+        err = c->upload.send(st, slot, s->d_table, bytes); if (err) return err;
         d_desc = reinterpret_cast<const PicDesc*>(s->d_table.get());
         if (recv) recv->d_map = reinterpret_cast<const int32_t*>(s->d_table + table_bytes);
+        if (tail) *d_tail = s->d_table + tail_at;
     }
     if (d_desc_out) *d_desc_out = d_desc;
     const int* count = g.count;
@@ -577,14 +582,16 @@ static int scan_results(cb200_ctx* c, int n, int32_t* anchors, int32_t* count, u
     return CB200_OK;
 }
 
-// Extractor::extract (Extractor.h:30-46) of every picture of a scan, on the device: one thread per picture
+// Extractor::extract (Extractor.h:30-46) of every picture of a scan, on the device: one thread per picture.  slots: NULL, or picture
+// i of a sub-batch is the scan's picture slots[i] (a detect receivers call's geometry)
 __global__ void k_extract(const int4* __restrict__ anchors, const int* __restrict__ count, const int* __restrict__ scan_status, int n,
                           int width, int height, int32_t* __restrict__ status, double* __restrict__ minv, double* __restrict__ fwd,
-                          uint8_t* __restrict__ sharpen)
+                          uint8_t* __restrict__ sharpen, const int32_t* __restrict__ slots)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int st = extract::extract_picture(reinterpret_cast<const Anchor*>(anchors + 4 * (size_t)i), count[i], (scan_status[i] & kScanOverflow) != 0,
+    const int s = slots ? slots[i] : i;
+    const int st = extract::extract_picture(reinterpret_cast<const Anchor*>(anchors + 4 * (size_t)s), count[s], (scan_status[s] & kScanOverflow) != 0,
                                             width, height, fwd + 9 * (size_t)i, minv + 9 * (size_t)i);
     status[i] = st;
     if (sharpen) sharpen[i] = st == 2;             // CB200_FLAG_SHARPEN_IF_NEEDED: the CLI sharpens exactly the NEEDS_SHARPEN pictures
@@ -621,7 +628,8 @@ int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool 
 int camera_reserve(cb200_ctx* c, const int32_t* wh, int n) { return camera_reserve_for(c, wh, n, true, true); }
 
 int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
-                      bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status, Receivers* recv)
+                      bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status, Receivers* recv,
+                      const int32_t* d_slots)
 {
     const Mode& m = c->mode;
     const int n = b.n();
@@ -629,7 +637,8 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     const ScanScratch* s0 = scanned->scan;
     const bool if_needed = (flags & CB200_FLAG_SHARPEN_IF_NEEDED) != 0;
     uint8_t* d_sharp = if_needed ? c->d_sel + 4 * (size_t)n : nullptr;
-    k_extract<<<(n + 127) / 128, 128, 0, c->stream>>>(s0->d_anchors, s0->d_count, s0->d_status, n, m.width, m.height, d_status, s->d_minv, s->d_fwd, d_sharp);
+    k_extract<<<(n + 127) / 128, 128, 0, c->stream>>>(s0->d_anchors, s0->d_count, s0->d_status, n, m.width, m.height, d_status, s->d_minv, s->d_fwd, d_sharp,
+                                                      d_slots);
     count_launch();
     CK(cudaGetLastError(), "extract launch");
     s->camera_n = n;
