@@ -406,7 +406,8 @@ int cb200_camera_plan_create_receivers(cb200_ctx* ctx, const cb200_picture* pics
    CB200_ERR_ARG before any CUDA call, naming the violation: n_modes outside 1 .. 5, a null context, two contexts of one mode, contexts
    on different devices or streams, a context attached to a CCM chain or with live camera plans, n above a context's max_frames, a
    null output other than d_mode_masks, and the flag and picture checks of cb200_scan_extract_decode_chunks_ragged_dev.  Waits for
-   the device as that call does (a buffer that grows, the upload ring of ctxs[0]).  Not capturable in a camera plan. */
+   the device as that call does (a buffer that grows, the upload ring of ctxs[0]).  Not capturable in a camera plan; graph replay
+   of auto mode is cb200_camera_plan_create_detect_receivers, over receiver tables instead of the contexts' own CCM. */
 int cb200_detect_scan_extract_decode_chunks_dev(cb200_ctx* const* ctxs, int n_modes, const uint8_t* d_pictures, const int32_t* wh, int n,
                                                 uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
                                                 int32_t* d_mode, uint32_t* d_mode_masks);
@@ -439,12 +440,46 @@ int cb200_detect_scan_extract_decode_chunks_dev(cb200_ctx* const* ctxs, int n_mo
    context checks); everything cb200_scan_extract_decode_chunks_receivers_dev refuses on the pictures and receivers (descriptors,
    sizes, spans, a null receiver_of, n_receivers < 1, a receiver out of range, naming the picture); a candidates entry that is 0 or
    has a bit at or above n_modes (naming the picture); a null d_states, a null or not 4-byte aligned table (naming it); two tables
-   whose n_receivers-entry ranges overlap (their modes may run on different streams).  Not capturable in a camera plan. */
+   whose n_receivers-entry ranges overlap (their modes may run on different streams).  Not capturable in a camera plan itself: its
+   plan is cb200_camera_plan_create_detect_receivers, below. */
 int cb200_detect_scan_extract_decode_chunks_receivers_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n,
                                                           uint32_t flags, const uint32_t* candidates, const int32_t* receiver_of,
                                                           int n_receivers, cb200_receiver_state* const* d_states, uint8_t* d_chunks,
                                                           uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode,
                                                           uint32_t* d_mode_masks);
+/* ---- detect receivers camera plans: the auto mode for receivers captured once ---------------------------------------------------
+
+   cb200_detect_scan_extract_decode_chunks_receivers_dev captured once over n fixed slots, for a decode service whose sessions are
+   partly in auto mode and which replays its batches from a graph.
+     bound at create: ctxs, n_modes, the picture descriptors (pics, HOST, read at create; the caller writes each batch's pixels into
+                 them in stream order before the launch), flags, n_receivers, the n_modes state tables (d_states: a HOST array of
+                 DEVICE pointers, read at create) and the outputs.
+     d_candidates: n uint32 in DEVICE memory, or NULL for every mode; d_receiver_of: n int32 in DEVICE memory.  Both are read when
+                 each launch runs, so the caller rewrites them per batch (a copy on the stream, or a kernel in the same capture).
+   At a launch, slot i is EMPTY when its receiver lies outside [0, n_receivers) or its candidates have no bit below n_modes (higher
+   bits are ignored).  For every mode k let P_k be the non-empty slots with bit k set, in slot order.  Every output for the non-empty
+   slots, and every mode's state table afterwards, equals bit for bit what the direct call gives on the non-empty slots alone, in
+   order: records, masks, extract statuses, d_mode, d_mode_masks.  An empty slot gets mode -1, mask 0, a zeroed record slot, a
+   d_mode_masks row of zeros and status CB200_EXTRACT_EMPTY, and reads and writes no state: an index that is out of range at replay
+   time never reaches memory outside a table.  A launch neither reads nor changes any context's own CCM or host CCM state.
+   How: a kernel at the head of the graph builds every list of the direct call from the two device arrays, over all n slots (slot i is
+   picture i in every geometry, and a slot a mode does not decode is an empty slot of that mode's receiver map).  A slot that no mode
+   of a geometry decodes is skipped by that geometry's exact walk, so a batch locked to one geometry walks that geometry only; its
+   K1, RS and list kernels still run on the absent slots (deskew included), which costs little next to a walk.  The geometries are
+   parallel branches of the graph.
+   The plan is registered with every one of its contexts: each freezes the buffers the graph uses (the detect call's own included),
+   cb200_destroy on any of them destroys the plan, and cb200_camera_plan_destroy unregisters it from all.  Launched (on ctxs[0]'s
+   stream), embedded, counted and destroyed as every camera plan; cb200_launch_count counts a launch as the kernels of its graph, the
+   same for every map and every candidate pattern.
+   CB200_ERR_ARG, before any CUDA call, naming the cause: everything the direct call refuses except the contents of the candidates
+   and of the map; a null d_receiver_of or one not 4-byte aligned; a d_candidates not 4-byte aligned; n == 0 and a null out; any
+   context attached to a CCM chain.  Unlike the direct call, contexts with live camera plans are accepted when no buffer has to grow
+   (so two plans on the same contexts double-buffer the pixel uploads); a buffer that would grow is refused, naming it. */
+int cb200_camera_plan_create_detect_receivers(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags,
+                                              const uint32_t* d_candidates, const int32_t* d_receiver_of, int n_receivers,
+                                              cb200_receiver_state* const* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                              int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks,
+                                              cb200_camera_plan** out);
 /* ---- JPEG files in: the CLI's input, decoded on the device ---------------------------------------------------------------
 
    Replaces: cv::imread(file) + cv::cvtColor(BGR2RGB) (src/exe/cimbar/cimbar.cpp:132-133) for a batch of JPEG files in host memory:

@@ -43,7 +43,7 @@ EXPORTS = [
     "cb200_camera_plan_create", "cb200_camera_plan_launch", "cb200_camera_plan_graph", "cb200_camera_plan_destroy",
     "cb200_detect_scan_extract_decode_chunks_dev", "cb200_scan_extract_decode_chunks_pictures_dev",
     "cb200_decode_chunks_receivers_dev", "cb200_scan_extract_decode_chunks_receivers_dev", "cb200_camera_plan_create_receivers",
-    "cb200_detect_scan_extract_decode_chunks_receivers_dev",
+    "cb200_detect_scan_extract_decode_chunks_receivers_dev", "cb200_camera_plan_create_detect_receivers",
 ]
 
 
@@ -183,6 +183,8 @@ def load_library():
     lib.cb200_camera_plan_create_receivers.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp, vp]
     lib.cb200_detect_scan_extract_decode_chunks_receivers_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, C.c_int, vp, vp, vp,
                                                                           vp, vp, vp]
+    lib.cb200_camera_plan_create_detect_receivers.argtypes = [vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, C.c_int, vp, vp, vp, vp, vp,
+                                                              vp, C.POINTER(C.c_void_p)]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -338,6 +340,42 @@ def detect_scan_extract_decode_chunks_receivers_dev(ctxs, pictures, receiver_of,
     _check(load_library().cb200_detect_scan_extract_decode_chunks_receivers_dev(
         hs, len(ctxs), C.cast(descs, C.c_void_p), len(pictures), flags, _hptr(cand), of.ctypes.data, tables[0][1] if tables else 0, ptrs,
         d_chunks, d_mask, d_status, d_mode, d_mode_masks))
+
+
+def _device_int32(t, n, what):
+    import torch
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != n:
+        raise Cb200Error(f"{what} is a contiguous int32 CUDA tensor of {n} values")
+    return t.data_ptr()
+
+
+def detect_receivers_camera_plan(ctxs, pictures, candidates, receiver_of, states, d_chunks, d_mask, d_status, d_mode, d_mode_masks=None,
+                                 flags=0, order="rgb"):
+    """detect_scan_extract_decode_chunks_receivers_dev captured once (cb200_camera_plan_create_detect_receivers): a CameraPlan over
+    the pictures (uint8 CUDA tensors) whose candidate masks and receivers are read at each launch from `candidates` (an int32 CUDA
+    tensor of n bit patterns, or None for every mode) and `receiver_of` (an int32 CUDA tensor of n values).  A slot whose receiver
+    lies outside [0, n_receivers) or whose candidates have no bit below len(ctxs) is empty: mode -1, mask 0, status EXTRACT_EMPTY.
+    states: one receiver_states tensor per context.  The outputs are device addresses, as for the direct call.  Write each batch's
+    pixels, candidates and map in stream order before its launch (on ctxs[0]'s stream); the plan keeps the tensors it binds alive
+    and belongs to every context of ctxs (closing any of them destroys it)"""
+    orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+    if len(orders) != len(pictures):
+        raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+    if len(states) != len(ctxs):
+        raise Cb200Error(f"{len(states)} state tables for {len(ctxs)} contexts")
+    of = _device_int32(receiver_of, len(pictures), "receiver_of")
+    cand = None if candidates is None else _device_int32(candidates, len(pictures), "candidates")
+    tables = [_states_ptr(s) for s in states]
+    if len({count for _, count in tables}) > 1:
+        raise Cb200Error("every state table holds the same receivers: " + ", ".join(str(count) for _, count in tables) + " entries")
+    hs = (C.c_void_p * max(len(ctxs), 1))(*[c._h.value for c in ctxs])
+    ptrs = (C.c_void_p * max(len(tables), 1))(*[p for p, _ in tables])
+    descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+    h = C.c_void_p()
+    _check(load_library().cb200_camera_plan_create_detect_receivers(
+        hs, len(ctxs), C.cast(descs, C.c_void_p), len(pictures), flags, cand, of, tables[0][1] if tables else 0, ptrs,
+        d_chunks, d_mask, d_status, d_mode, d_mode_masks, C.byref(h)))
+    return CameraPlan(ctxs[0], h, keep=(list(pictures), candidates, receiver_of, list(states)), ctxs=list(ctxs))
 
 
 def _hptr(a):
@@ -832,11 +870,12 @@ class Context:
 
 class CameraPlan:
     """a camera plan (cb200_camera_plan_*): launch() is one graph launch on the context's stream, or a child node of the capture
-    in progress on it (torch.cuda.graph); `graph` is the cudaGraph_t as an int.  The plan belongs to its context, which must outlive
-    it (closing the context destroys its plans)"""
+    in progress on it (torch.cuda.graph); `graph` is the cudaGraph_t as an int.  The plan belongs to its contexts (a detect receivers
+    plan: every one of its candidates), which must outlive it (closing any of them destroys the plan)"""
 
-    def __init__(self, ctx, handle, keep=()):
+    def __init__(self, ctx, handle, keep=(), ctxs=None):
         self.ctx, self._h = ctx, handle
+        self.ctxs = [ctx] if ctxs is None else ctxs
         self._keep = keep                  # the tensors a receivers plan binds
 
     def launch(self):
@@ -849,7 +888,8 @@ class CameraPlan:
         return g.value
 
     def close(self):
-        if self._h and self.ctx._h:
+        # a closed context has destroyed the plan already
+        if self._h and all(c._h for c in self.ctxs):
             self.ctx.lib.cb200_camera_plan_destroy(self._h)
         self._h = C.c_void_p()
 

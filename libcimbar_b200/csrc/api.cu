@@ -482,7 +482,8 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const u
             CK(flood_colour_launch(m, sw->lead->flood, d_rgb, n, sw->kept, c->d_cellvals, cc, st), "flood colour launch");
     } else {
         CK(flood_launch(m, c->flood, d_rgb, n, (flags & CB200_FLAG_NO_FALLBACK) != 0, exact_only, sharpen, d_sharp,
-                        c->d_cellvals, c->d_dirty, c->d_flags, d_trace, cc, st, sw ? sw->kept : nullptr), "flood launch");
+                        c->d_cellvals, c->d_dirty, c->d_flags, d_trace, cc, st, sw ? sw->kept : nullptr, sw ? sw->present : nullptr),
+           "flood launch");
     }
     mark(c);                                   // ev2: after K1x
     return CB200_OK;

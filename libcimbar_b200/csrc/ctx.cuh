@@ -25,8 +25,10 @@ void detect_destroy(DetectState* d);
 // the exact walk of a detect call (detect.cu), shared by the modes of one frame geometry: `lead` walks (flood_launch, the walk's
 // records kept in `kept`), every other context of the geometry takes its frame flags and colours that walk's positions in its own
 // palette and CCM (flood_colour_launch).  The walk reads only the geometry, the frames and their sharpen bytes, and K1's dirty
-// flag is a symbol decision, so each mode's cells equal what its own walk would give
-struct SharedWalk { cb200_ctx* lead; uint32_t* kept; };
+// flag is a symbol decision, so each mode's cells equal what its own walk would give.  present: NULL, or (a detect receivers plan,
+// whose geometries work on every slot) one device byte per frame, 0 for a slot no mode of the geometry decodes: the lead walks
+// only the others
+struct SharedWalk { cb200_ctx* lead; uint32_t* kept; const uint8_t* present; };
 void deskew_destroy(DeskewState* d);     // delete: its buffers free themselves
 void scan_destroy(ScanScratch* s);       // likewise
 void jpeg_destroy(JpegState* j);         // likewise
@@ -193,6 +195,32 @@ struct Receivers {
     Receivers(const int32_t* d_plan_map, cb200_receiver_state* states) : d_map(d_plan_map), d_states(states), empty_slots(true) {}
     size_t bytes() const { return map.size() * sizeof(int32_t); }
 };
+// a camera plan's own rules, checked after its batch's: n > 0, a non-null `out` (set to NULL) (plan.cu)
+int plan_rules(int n, cb200_camera_plan** out);
+// A detect receivers camera plan (plan.cu) is the detect receivers call's geometry loop (detect.cu) captured over n fixed slots.
+// DetectPlan: what its graph reads -- the plan's picture table, the caller's candidates (NULL: every mode) and map, read at each
+// launch, and one state table per mode; the lists the graph builds (detect_plan_words(n_modes, n) words: the modes' raw receivers,
+// maps and positions) and the geometries' present bytes (n_modes x n).  check_detect_plan: every argument check of
+// cb200_camera_plan_create_detect_receivers, before any CUDA call.  detect_plan_reserve: every buffer of the contexts the graph uses,
+// at b's size; frozen_only: only on the contexts with live plans, where it makes no CUDA call and refuses what would grow.
+// detect_plan_enqueue: the whole call on ctxs[0]'s stream, for the capture
+struct DetectPlan {
+    const PicDesc* d_table;
+    const uint32_t* d_cand;
+    const int32_t* d_of;
+    int receivers;
+    cb200_receiver_state* const* d_states;
+    int32_t* d_lists;
+    uint8_t* d_present;
+};
+size_t detect_plan_words(int n_modes, int n);
+int check_detect_plan(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags, const uint32_t* d_candidates,
+                      const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states, const uint8_t* d_chunks,
+                      const uint32_t* d_chunk_mask, const int32_t* d_extract_status, const int32_t* d_mode, cb200_camera_plan** out,
+                      CameraBatch& b);
+int detect_plan_reserve(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, uint32_t flags, bool frozen_only);
+int detect_plan_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                        int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks, const DetectPlan& dp);
 // the context is attached to a CCM chain (chain.cu)
 bool chain_attached(const cb200_ctx* c);
 }  // namespace cb200

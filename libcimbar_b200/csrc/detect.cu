@@ -16,6 +16,12 @@
 // under its candidate modes, each mode keeps one state table of receivers, and each geometry extracts, deskews and walks only the
 // pictures some of its modes decode (receivers_core.cuh: detect_lists).  A mode's other pictures of that sub-batch are empty slots,
 // as in a receivers plan: decoded, masked, reading and writing no state.  k_detect_select_at joins the results.
+//
+// A detect receivers plan (cb200_camera_plan_create_detect_receivers, plan.cu) captures the same geometry loop once over n fixed
+// slots.  Its candidates and map are read at each launch, so it has no sub-batches: every geometry works on all n slots, slot i is
+// picture i, and k_detect_plan_lists at the head of the graph builds from the two device arrays what detect_lists builds on the host
+// (receivers_core.cuh: plan_slot).  A slot that no mode of a geometry decodes is an empty slot of each of its modes, and the
+// geometry's walk skips it (SharedWalk::present), so a batch locked to one geometry walks that geometry only.
 #include "ctx.cuh"
 #include "receivers_core.cuh"
 
@@ -73,7 +79,8 @@ k_detect_select(const DetectArgs a, uint8_t* __restrict__ chunks, uint32_t* __re
 }
 
 // k_detect_select of a detect receivers call: mode k decoded picture i at position at[k * n + i] of its geometry's sub-batch, or not at
-// all (-1: its mask there counts as 0).  The status of a picture no mode took is its first candidate's
+// all (-1: its mask there counts as 0).  The status of a picture no mode took is its first candidate's; a detect receivers plan's
+// empty slot, which has no candidate, gets CB200_EXTRACT_EMPTY (and mode -1, mask 0, a zeroed record)
 __global__ void __launch_bounds__(256)
 k_detect_select_at(const DetectArgs a, const int32_t* __restrict__ at, int n, uint8_t* __restrict__ chunks, uint32_t* __restrict__ mask,
                    int32_t* __restrict__ status, int32_t* __restrict__ mode, uint32_t* __restrict__ mode_masks)
@@ -89,7 +96,7 @@ k_detect_select_at(const DetectArgs a, const int32_t* __restrict__ at, int n, ui
     if (threadIdx.x == 0) {
         mode[i] = sel;
         mask[i] = sel < 0 ? 0u : a.mask[sel][p_sel];
-        status[i] = sel < 0 ? a.status[first][p_first] : a.status[sel][p_sel];
+        status[i] = sel >= 0 ? a.status[sel][p_sel] : first >= 0 ? a.status[first][p_first] : CB200_EXTRACT_EMPTY;
         if (mode_masks)
             for (int k = 0; k < a.n_modes; ++k) {
                 const int p = at[(size_t)k * n + i];
@@ -102,27 +109,72 @@ k_detect_select_at(const DetectArgs a, const int32_t* __restrict__ at, int n, ui
     for (int b = threadIdx.x; b < a.slot; b += blockDim.x) dst[b] = b < have ? src[b] : 0;
 }
 
+// a detect receivers plan's lists at one launch, one thread per slot (receivers_core.cuh: plan_slot): every mode's raw receivers
+// (k_receivers_order then orders each), every geometry's present bytes and every mode's positions.  cand NULL: every mode
+struct PlanListArgs { int n_modes, n_geoms, receivers; int group[kDetectModes]; };
+__global__ void k_detect_plan_lists(const uint32_t* __restrict__ cand, const int32_t* __restrict__ receiver_of, int n, const PlanListArgs a,
+                                    int32_t* __restrict__ raw, uint8_t* __restrict__ present, int32_t* __restrict__ at)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    receivers::plan_slot(cand ? cand[i] : ~0u, receiver_of[i], a.receivers, a.n_modes, a.group, a.n_geoms, n, i, raw, present, at);
+}
+
+// a detect receivers plan's list words (DetectPlan::d_lists): n_modes x n raw receivers, n_modes x 2 n maps ([of | order]), then
+// n_modes x n positions
+size_t detect_plan_words(int n_modes, int n) { return 4 * (size_t)n_modes * (size_t)n; }
+static int32_t* plan_map(const DetectPlan& dp, int n_modes, int n, int k) { return dp.d_lists + (size_t)n_modes * n + 2 * (size_t)n * k; }
+static int32_t* plan_at(const DetectPlan& dp, int n_modes, int n) { return dp.d_lists + 3 * (size_t)n_modes * n; }
+
 static bool same_geometry(const Mode& a, const Mode& b)
 {
     return a.width == b.width && a.height == b.height && a.cells_x == b.cells_x && a.cells_y == b.cells_y && a.cell_offset == b.cell_offset &&
            a.corner == b.corner;
 }
 
+// the frame geometries of a set of contexts: group[k], and lead[g] = the first context of geometry g in priority order; returns
+// their count
+static int geometries(cb200_ctx* const* ctxs, int n_modes, int* group, int* lead)
+{
+    int ng = 0;
+    for (int k = 0; k < n_modes; ++k) {
+        int g = 0;
+        while (g < ng && !same_geometry(ctxs[lead[g]]->mode, ctxs[k]->mode)) ++g;
+        if (g == ng) lead[ng++] = k;
+        group[k] = g;
+    }
+    return ng;
+}
+
+// the side streams and events of ng geometries running at once
+static int detect_streams(DetectState* ds, int ng)
+{
+    if (!ds->fork) CK(cudaEventCreateWithFlags(&ds->fork, cudaEventDisableTiming), "cudaEventCreate detect fork");
+    for (int g = 0; g < ng; ++g) {
+        if (!ds->side[g]) CK(cudaStreamCreateWithFlags(&ds->side[g], cudaStreamNonBlocking), "cudaStreamCreate detect side stream");
+        if (!ds->join[g]) CK(cudaEventCreateWithFlags(&ds->join[g], cudaEventDisableTiming), "cudaEventCreate detect join");
+    }
+    return CB200_OK;
+}
+
 static std::string ctx_name(int k) { return "context " + std::to_string(k); }
 
-// the receivers checks of a detect receivers call, which need no context
+// the receivers checks of a detect receivers call, which need no context.  on_device (a plan): candidates and receiver_of are device
+// arrays that only a launch reads, so their pointers are checked instead of their entries
 static int check_detect_receivers(int n_modes, int n, const uint32_t* candidates, const int32_t* receiver_of, int n_receivers,
-                                  cb200_receiver_state* const* d_states)
+                                  cb200_receiver_state* const* d_states, bool on_device = false)
 {
-    for (int i = 0; candidates && i < n; ++i) {
+    if (on_device && reinterpret_cast<uintptr_t>(candidates) % 4) return fail(CB200_ERR_ARG, "d_candidates is not 4-byte aligned");
+    for (int i = 0; candidates && !on_device && i < n; ++i) {
         if (!candidates[i]) return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + " has no candidate mode (candidates = 0)");
         if (candidates[i] >> n_modes)
             return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + ": candidates = " + std::to_string(candidates[i]) + " has a bit at or above n_modes = " +
                                            std::to_string(n_modes));
     }
-    if (!receiver_of) return fail(CB200_ERR_ARG, "null receiver_of");
+    if (!receiver_of) return fail(CB200_ERR_ARG, on_device ? "null d_receiver_of" : "null receiver_of");
+    if (on_device && reinterpret_cast<uintptr_t>(receiver_of) % 4) return fail(CB200_ERR_ARG, "d_receiver_of is not 4-byte aligned");
     if (n_receivers < 1) return fail(CB200_ERR_ARG, "n_receivers < 1");
-    for (int i = 0; i < n; ++i)
+    for (int i = 0; !on_device && i < n; ++i)
         if (receiver_of[i] < 0 || receiver_of[i] >= n_receivers)
             return fail(CB200_ERR_ARG, "picture " + std::to_string(i) + ": receiver " + std::to_string(receiver_of[i]) + " outside [0, " +
                                        std::to_string(n_receivers) + ")");
@@ -143,8 +195,9 @@ static int check_detect_receivers(int n_modes, int n, const uint32_t* candidates
     return CB200_OK;
 }
 
-// the checks that read the contexts, after every other one
-static int check_detect_contexts(cb200_ctx* const* ctxs, int n_modes, int n)
+// the checks that read the contexts, after every other one.  A plan accepts contexts with live plans (their frozen buffers are
+// checked when it is made)
+static int check_detect_contexts(cb200_ctx* const* ctxs, int n_modes, int n, bool plan)
 {
     if (!ctxs) return fail(CB200_ERR_ARG, "null context list");
     for (int k = 0; k < n_modes; ++k)
@@ -160,7 +213,7 @@ static int check_detect_contexts(cb200_ctx* const* ctxs, int n_modes, int n)
                                            ": the candidates must share one device");
         if (c->stream != ctxs[0]->stream) return fail(CB200_ERR_ARG, ctx_name(k) + " is on another stream than context 0: the candidates must share one stream");
         if (chain_attached(c)) return fail(CB200_ERR_ARG, ctx_name(k) + " is linked to a CCM chain: chained contexts cannot be detect candidates");
-        if (!c->plans.empty()) return fail(CB200_ERR_ARG, ctx_name(k) + " has live camera plans: destroy them before a detect call");
+        if (!plan && !c->plans.empty()) return fail(CB200_ERR_ARG, ctx_name(k) + " has live camera plans: destroy them before a detect call");
         if (n > c->max_frames)
             return fail(CB200_ERR_ARG, "n = " + std::to_string(n) + " > max_frames = " + std::to_string(c->max_frames) + " of " + ctx_name(k));
     }
@@ -168,10 +221,10 @@ static int check_detect_contexts(cb200_ctx* const* ctxs, int n_modes, int n)
 }
 
 // every argument check, before any CUDA call: the ones that need no context first.  build: the call's batch builder; more: the
-// call's own checks that need no context (a detect receivers call's receivers)
+// call's own checks that need no context (a detect receivers call's receivers); plan: a plan's checks
 template <class Build, class More>
 static int check_detect(cb200_ctx* const* ctxs, int n_modes, uint32_t flags, Build&& build, const uint8_t* d_chunks, const uint32_t* d_chunk_mask,
-                        const int32_t* d_extract_status, const int32_t* d_mode, CameraBatch& b, More&& more)
+                        const int32_t* d_extract_status, const int32_t* d_mode, CameraBatch& b, More&& more, bool plan = false)
 {
     if (n_modes < 1 || n_modes > kDetectModes)
         return fail(CB200_ERR_ARG, "n_modes = " + std::to_string(n_modes) + ": between 1 and " + std::to_string(kDetectModes) + " candidate modes");
@@ -179,7 +232,7 @@ static int check_detect(cb200_ctx* const* ctxs, int n_modes, uint32_t flags, Bui
     if ((rc = build(b)) || (rc = check_spans(b))) return rc;
     if (!d_chunks || !d_chunk_mask || !d_extract_status || !d_mode) return fail(CB200_ERR_ARG, "null output");
     if ((rc = more())) return rc;
-    return check_detect_contexts(ctxs, n_modes, b.n());
+    return check_detect_contexts(ctxs, n_modes, b.n(), plan);
 }
 
 // a context's stream for the duration of one geometry's work, restored on every path out
@@ -195,21 +248,19 @@ struct DetectReceivers { const uint32_t* cand; const int32_t* of; int count; cb2
 // With dr (a detect receivers call), geometry g decodes only its sub-batch U_g (receivers_core.cuh: detect_lists), each of its modes
 // with its own receiver map over U_g and state table; a geometry or mode without pictures launches nothing.  The sub-batches' picture
 // tables (the scan table's entries, so their blurred offsets keep pointing into ctxs[0]'s scan), scan slots, maps and the selection's
-// positions travel behind the scan's picture table: one upload per call
+// positions travel behind the scan's picture table: one upload per call.
+// With dp (a detect receivers plan's capture), every geometry and mode works on all n slots with the plan's picture table, and the
+// lists come from k_detect_plan_lists at the head of the work, on the device
 static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
-                          int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks, const DetectReceivers* dr = nullptr)
+                          int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks, const DetectReceivers* dr = nullptr,
+                          const DetectPlan* dp = nullptr)
 {
     cb200_ctx* c0 = ctxs[0];
     const int n = b.n();
     int rc;
     // geometries: lead[g] = the first context of geometry g in priority order (with dr: the first that decodes pictures, or -1)
-    int group[kDetectModes], lead[kDetectModes], ng = 0;
-    for (int k = 0; k < n_modes; ++k) {
-        int g = 0;
-        while (g < ng && !same_geometry(ctxs[lead[g]]->mode, ctxs[k]->mode)) ++g;
-        if (g == ng) lead[ng++] = k;
-        group[k] = g;
-    }
+    int group[kDetectModes], lead[kDetectModes];
+    const int ng = geometries(ctxs, n_modes, group, lead);
     receivers::DetectLists lists;
     CameraBatch sub[kDetectModes];
     if (dr) {
@@ -236,21 +287,16 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
         const CameraBatch& bk = batch(group[k]);
         rc = camera_reserve_for(ctxs[k], bk.wh.data(), bk.n(), !dr && k == 0, lead[group[k]] == k); if (rc) return rc;
     }
-    CK(ds->status.ensure((size_t)n_modes * n), "cudaMalloc detect statuses");
+    // grown through grow(): a live detect plan's graph reads them
+    if ((rc = grow(c0, ds->status, (size_t)n_modes * n, "detect statuses"))) return rc;
     uint8_t* frames[kDetectModes];
     for (int g = 0; g < ng; ++g) {
         if (lead[g] < 0) continue;
         const cb200_ctx* L = ctxs[lead[g]];
-        CK(ds->kept[g].ensure((size_t)batch(g).n() * L->mode.num_cells), "cudaMalloc detect walk records");
+        if ((rc = grow(c0, ds->kept[g], (size_t)batch(g).n() * L->mode.num_cells, "detect walk records"))) return rc;
         rc = deskew_frames(ctxs[lead[g]], batch(g).n(), &frames[g]); if (rc) return rc;
     }
-    if (live > 1) {
-        if (!ds->fork) CK(cudaEventCreateWithFlags(&ds->fork, cudaEventDisableTiming), "cudaEventCreate detect fork");
-        for (int g = 0; g < ng; ++g) {
-            if (!ds->side[g]) CK(cudaStreamCreateWithFlags(&ds->side[g], cudaStreamNonBlocking), "cudaStreamCreate detect side stream");
-            if (!ds->join[g]) CK(cudaEventCreateWithFlags(&ds->join[g], cudaEventDisableTiming), "cudaEventCreate detect join");
-        }
-    }
+    if (live > 1 && (rc = detect_streams(ds, ng))) return rc;
     // dr's lists, in byte offsets from the tail's start: per geometry its picture table and scan slots, per mode its map, the positions
     std::vector<uint8_t> tail;
     size_t desc_at[kDetectModes] = {}, slots_at[kDetectModes] = {}, map_at[kDetectModes] = {}, pos_at = 0;
@@ -275,8 +321,19 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
     }
     const PicDesc* d_desc;
     const uint8_t* d_tail = nullptr;
-    rc = camera_scan(c0, b, nullptr, &d_desc, nullptr, dr ? &tail : nullptr, &d_tail); if (rc) return rc;
+    rc = camera_scan(c0, b, dp ? dp->d_table : nullptr, &d_desc, nullptr, dr ? &tail : nullptr, &d_tail); if (rc) return rc;
     cudaStream_t main = c0->stream;
+    if (dp) {                                // this launch's lists, then each mode's [of | order]
+        PlanListArgs la;
+        memset(&la, 0, sizeof(la));
+        la.n_modes = n_modes; la.n_geoms = ng; la.receivers = dp->receivers;
+        for (int k = 0; k < n_modes; ++k) la.group[k] = group[k];
+        k_detect_plan_lists<<<(n + 127) / 128, 128, 0, main>>>(dp->d_cand, dp->d_of, n, la, dp->d_lists, dp->d_present, plan_at(*dp, n_modes, n));
+        count_launch();
+        CK(cudaGetLastError(), "detect plan lists launch");
+        for (int k = 0; k < n_modes; ++k)
+            CK(receivers_order_launch(n, dp->d_lists + (size_t)k * n, dp->receivers, plan_map(*dp, n_modes, n, k), main), "receivers order launch");
+    }
     if (live > 1) {
         CK(cudaEventRecord(ds->fork, main), "record detect fork");
         for (int g = 0; g < ng; ++g) if (lead[g] >= 0) CK(cudaStreamWaitEvent(ds->side[g], ds->fork, 0), "wait detect fork");
@@ -284,13 +341,18 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
     // every geometry's modes in priority order, the lead first; every side stream is joined back even when one fails
     for (int g = 0; g < ng && !rc; ++g) {
         if (lead[g] < 0) continue;
-        const SharedWalk sw{ctxs[lead[g]], ds->kept[g].get()};
+        const SharedWalk sw{ctxs[lead[g]], ds->kept[g].get(), dp ? dp->d_present + (size_t)g * n : nullptr};
         const PicDesc* desc_g = dr ? reinterpret_cast<const PicDesc*>(d_tail + desc_at[g]) : d_desc;
         const int32_t* slots_g = dr ? reinterpret_cast<const int32_t*>(d_tail + slots_at[g]) : nullptr;
         for (int k = 0; k < n_modes && !rc; ++k) {
             if (group[k] != g || !decodes(k)) continue;
             cb200_ctx* c = ctxs[k];
             StreamSwap on(c, live > 1 ? ds->side[g] : main, &sw);
+            if (dp) {                        // a slot mode k does not decode is an empty slot of its map
+                Receivers r(plan_map(*dp, n_modes, n, k), dp->d_states[k]);
+                rc = camera_after_scan(c, c0, b, d_desc, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr, ds->status + (size_t)k * n, &r);
+                continue;
+            }
             if (!dr) {
                 rc = camera_after_scan(c, c0, b, d_desc, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr, ds->status + (size_t)k * n);
                 continue;
@@ -317,12 +379,50 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
         a.data[k] = c->d_data; a.data_bytes[k] = c->mode.data_bytes; a.mask[k] = c->d_mask; a.status[k] = ds->status + (size_t)k * n;
         if (a.data_bytes[k] > a.slot) a.slot = a.data_bytes[k];
     }
-    if (dr) k_detect_select_at<<<n, 256, 0, main>>>(a, reinterpret_cast<const int32_t*>(d_tail + pos_at), n, d_chunks, d_chunk_mask, d_extract_status,
-                                                    d_mode, d_mode_masks);
-    else k_detect_select<<<n, 256, 0, main>>>(a, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
+    if (dr || dp) {
+        const int32_t* at = dp ? plan_at(*dp, n_modes, n) : reinterpret_cast<const int32_t*>(d_tail + pos_at);
+        k_detect_select_at<<<n, 256, 0, main>>>(a, at, n, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
+    } else k_detect_select<<<n, 256, 0, main>>>(a, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
     count_launch();
     CK(cudaGetLastError(), "detect select launch");
     return CB200_OK;
+}
+
+int check_detect_plan(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags, const uint32_t* d_candidates,
+                      const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states, const uint8_t* d_chunks,
+                      const uint32_t* d_chunk_mask, const int32_t* d_extract_status, const int32_t* d_mode, cb200_camera_plan** out,
+                      CameraBatch& b)
+{
+    auto build = [&](CameraBatch& bb) { const int rc = picture_batch(pics, n, bb); return rc ? rc : plan_rules(n, out); };
+    auto more = [&] { return check_detect_receivers(n_modes, n, d_candidates, d_receiver_of, n_receivers, d_states, true); };
+    return check_detect(ctxs, n_modes, flags, build, d_chunks, d_chunk_mask, d_extract_status, d_mode, b, more, true);
+}
+
+int detect_plan_reserve(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, uint32_t flags, bool frozen_only)
+{
+    int group[kDetectModes], lead[kDetectModes];
+    const int ng = geometries(ctxs, n_modes, group, lead), n = b.n();
+    int rc;
+    for (int k = 0; k < n_modes; ++k) {      // what detect_enqueue reserves with every geometry live, and the decode's own buffers
+        cb200_ctx* c = ctxs[k];
+        if (frozen_only && c->plans.empty()) continue;
+        if ((rc = camera_reserve_for(c, b.wh.data(), n, k == 0, lead[group[k]] == k))) return rc;
+        if (!frozen_only && (rc = decode_reserve(c, flags, true))) return rc;
+    }
+    cb200_ctx* c0 = ctxs[0];
+    if (frozen_only && c0->plans.empty()) return CB200_OK;
+    if (!c0->detect) c0->detect = new DetectState();
+    DetectState* ds = c0->detect;
+    if ((rc = grow(c0, ds->status, (size_t)n_modes * n, "detect statuses"))) return rc;
+    for (int g = 0; g < ng; ++g)
+        if ((rc = grow(c0, ds->kept[g], (size_t)n * ctxs[lead[g]]->mode.num_cells, "detect walk records"))) return rc;
+    return frozen_only || ng < 2 ? CB200_OK : detect_streams(ds, ng);
+}
+
+int detect_plan_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                        int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks, const DetectPlan& dp)
+{
+    return detect_enqueue(ctxs, n_modes, b, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks, nullptr, &dp);
 }
 
 }  // namespace cb200

@@ -42,10 +42,12 @@ bool flood_workspace_fits(const FloodWorkspace& ws, int n_frames);
 // CB200_FRAME_INEXACT = needed but skipped (no_fallback).  d_sharpen_of: NULL = every frame is preprocessed as `sharpen` says;
 // else one byte per frame of the batch (device memory, nonzero = sharpen) and `sharpen` is ignored.
 // keep != NULL: the walk's per-cell records (x | y << 11 | sym << 22) of all n_frames listed frames stay there, in list order
-// (n_frames x num_cells words), instead of one chunk at a time in the workspace
+// (n_frames x num_cells words), instead of one chunk at a time in the workspace.  d_present != NULL: one device byte per frame, and
+// a frame whose byte is 0 is neither walked nor flagged (its K1 cells stand)
 cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb, int n_frames, bool no_fallback,
                          bool force_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
-                         uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st, uint32_t* keep = nullptr);
+                         uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st, uint32_t* keep = nullptr,
+                         const uint8_t* d_present = nullptr);
 // the colour pass of a walk that flood_launch ran on `walked` with `keep` = kept, for another mode of the same frame geometry: the
 // frames it listed get their colours (or, with cc.means, their mean colours) at the walk's positions and its symbols in d_cellvals
 cudaError_t flood_colour_launch(const Mode& m, const FloodWorkspace& walked, const uint8_t* d_rgb, int n_frames, const uint32_t* kept,

@@ -13,23 +13,36 @@
 // A receivers plan (cb200_camera_plan_create_receivers) is the receivers camera call captured so.  Its receiver map is the one
 // input the direct call builds on the host per batch: here k_receivers_order, captured at the head of the graph, builds it at each
 // launch from the caller's d_receiver_of into the plan's own d_map, and the rest of the graph reads it from there.
+//
+// A detect receivers plan (cb200_camera_plan_create_detect_receivers) is the detect receivers call captured so, over several
+// contexts: detect.cu's geometry loop on every context's buffers, with every context's stream swapped to the capture stream, and
+// the side streams' forks and joins becoming parallel branches of the graph.  Its candidates and map are read at each launch
+// (k_detect_plan_lists at the head of the graph builds every list into d_map and d_present).  It is registered in the plans of every
+// one of its contexts, so each of them freezes the buffers the graph uses, and destroying any of them destroys the plan.
 #include "ctx.cuh"
 
+#include <memory>
 #include <string>
 #include <vector>
 
 using namespace cb200;
 
 struct cb200_camera_plan {
-    cb200_ctx* ctx = nullptr;
+    cb200_ctx* ctx = nullptr;               // the context whose stream launches the plan (a detect plan: its first)
+    std::vector<cb200_ctx*> ctxs;           // every context whose buffers the graph uses: ctx, or a detect plan's candidates
     int n = 0;
     uint32_t flags = 0;
     DevBuf<uint8_t> d_table;                // n PicDesc, then the pictures grouped by blur radius
-    // a receivers plan: the caller's map and states, and the map the graph builds from it (n receivers, -1 = empty, then the order)
+    // a receivers plan: the caller's map and states, and the map the graph builds from it (n receivers, -1 = empty, then the order).
+    // A detect receivers plan: the caller's map and candidates, each mode's state table, and d_map holds the lists the graph builds
+    // (detect_plan_words), d_present the geometries' present bytes
     const int32_t* d_receiver_of = nullptr;
     int n_receivers = 0;
     cb200_receiver_state* d_states = nullptr;
     DevBuf<int32_t> d_map;
+    const uint32_t* d_candidates = nullptr;
+    std::vector<cb200_receiver_state*> d_mode_states;
+    DevBuf<uint8_t> d_present;
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     int kernels = 0;                        // kernel nodes of the graph (cb200_launch_count)
@@ -58,6 +71,14 @@ int check_frozen_camera(cb200_ctx* c, const int32_t* wh, int n) { return c->plan
 
 int check_frozen_scan(cb200_ctx* c, const int32_t* wh, int n) { return c->plans.empty() ? CB200_OK : scan_reserve(c, wh, n); }
 
+int plan_rules(int n, cb200_camera_plan** out)
+{
+    if (n == 0) return fail(CB200_ERR_ARG, "n = 0: a camera plan needs at least one picture");
+    if (!out) return fail(CB200_ERR_ARG, "null plan");
+    *out = nullptr;
+    return CB200_OK;
+}
+
 }  // namespace cb200
 
 namespace {
@@ -77,84 +98,71 @@ int count_kernel_nodes(cudaGraph_t g, int* kernels)
     return CB200_OK;
 }
 
-// camera_enqueue on the private stream `cap`, captured into p->graph.  The context's stream, timing and host CCM state are set aside
-// for the duration and restored: a capture runs nothing, so it changes nothing the host can observe
-int capture(cb200_camera_plan* p, cudaStream_t cap, const CameraBatch& b, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags,
-            int32_t* d_status)
+// enqueue(): the plan's work on the private stream `cap`, captured into p->graph.  Every context's stream, timing and host CCM state
+// are set aside for the duration and restored: a capture runs nothing, so it changes nothing the host can observe
+template <class Enqueue>
+int capture(cb200_camera_plan* p, cudaStream_t cap, Enqueue&& enqueue)
 {
-    cb200_ctx* c = p->ctx;
-    cudaEvent_t scratch_ev;                 // ccm_keep_last records c->ccm_ev: inside a capture that record joins the graph
-    CK(cudaEventCreateWithFlags(&scratch_ev, cudaEventDisableTiming), "cudaEventCreate");
-    const cudaStream_t stream = c->stream;
-    const bool timing = c->timing, pending = c->ccm_pending, pending_flag = c->ccm_pending_flag, active = c->ccm_active;
-    const int ccm_frames = c->ccm_frames, camera_n = camera_pictures(c);
+    struct Saved {
+        cudaStream_t stream; bool timing, pending, pending_flag, active; int ccm_frames, camera_n;
+        cudaEvent_t ccm_ev, scratch_ev;     // ccm_keep_last records c->ccm_ev: inside a capture that record joins the graph
+    };
+    std::vector<Saved> saved(p->ctxs.size());
+    for (size_t i = 0; i < saved.size(); ++i) {
+        const cudaError_t e = cudaEventCreateWithFlags(&saved[i].scratch_ev, cudaEventDisableTiming);
+        if (e != cudaSuccess) { while (i > 0) cudaEventDestroy(saved[--i].scratch_ev); return fail_cuda(e, "cudaEventCreate"); }
+    }
+    for (size_t i = 0; i < saved.size(); ++i) {
+        cb200_ctx* c = p->ctxs[i];
+        Saved& s = saved[i];
+        s.stream = c->stream; s.timing = c->timing; s.pending = c->ccm_pending; s.pending_flag = c->ccm_pending_flag; s.active = c->ccm_active;
+        s.ccm_frames = c->ccm_frames; s.camera_n = camera_pictures(c); s.ccm_ev = c->ccm_ev;
+        c->ccm_ev = s.scratch_ev;
+        c->stream = cap;
+        c->timing = false;
+        c->capturing = true;
+    }
     const unsigned long long launches = cb200_launch_count();
-    cudaEvent_t ccm_ev = c->ccm_ev;
-    c->ccm_ev = scratch_ev;
-    c->stream = cap;
-    c->timing = false;
-    c->capturing = true;
     int rc = CB200_OK;
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) rc = fail_cuda(e, "cudaStreamBeginCapture");
     if (!rc) {
-        const PicDesc* table = reinterpret_cast<const PicDesc*>(p->d_table.get());
-        if (!p->d_receiver_of) {
-            rc = camera_enqueue(c, b, p->flags, d_chunks, d_mask, d_frame_flags, d_status, table);
-        } else {
-            Receivers r(p->d_map.get(), p->d_states);
-            e = receivers_order_launch(p->n, p->d_receiver_of, p->n_receivers, p->d_map, cap);
-            rc = e != cudaSuccess ? fail_cuda(e, "receivers order launch")
-                                  : camera_enqueue(c, b, p->flags, d_chunks, d_mask, d_frame_flags, d_status, table, &r);
-        }
+        rc = enqueue();
         cudaGraph_t g = nullptr;
         e = cudaStreamEndCapture(cap, &g);
         if (!rc && e != cudaSuccess) rc = fail_cuda(e, "cudaStreamEndCapture");
         if (rc) { if (g) cudaGraphDestroy(g); } else p->graph = g;
     }
-    c->capturing = false;
-    c->timing = timing;
-    c->stream = stream;
-    c->ccm_ev = ccm_ev;
-    c->ccm_pending = pending; c->ccm_pending_flag = pending_flag; c->ccm_active = active;
-    c->ccm_frames = ccm_frames;
-    set_camera_pictures(c, camera_n);
-    cudaEventDestroy(scratch_ev);
+    for (size_t i = 0; i < saved.size(); ++i) {
+        cb200_ctx* c = p->ctxs[i];
+        const Saved& s = saved[i];
+        c->capturing = false;
+        c->timing = s.timing;
+        c->stream = s.stream;
+        c->ccm_ev = s.ccm_ev;
+        c->ccm_pending = s.pending; c->ccm_pending_flag = s.pending_flag; c->ccm_active = s.active;
+        c->ccm_frames = s.ccm_frames;
+        set_camera_pictures(c, s.camera_n);
+        cudaEventDestroy(s.scratch_ev);
+    }
     // the captured launches did not run: launch() counts them each time the graph does
     count_launch(-(int)(cb200_launch_count() - launches));
     return rc;
 }
 
-// a plan's own rules, checked after its batch's
-int plan_rules(int n, cb200_camera_plan** out)
+// a plan for the checked batch b (after every argument check), in p (its contexts, size, flags and bound pointers set; owned here):
+// the freeze check -- reserve(true), no CUDA call --, every buffer the graph uses grown -- reserve(false) --, the table uploaded, the
+// capture of enqueue(table), the graph instantiated, the plan registered with every one of its contexts
+template <class Reserve, class Enqueue>
+int make_plan(cb200_camera_plan* plan, const CameraBatch& b, Reserve&& reserve, Enqueue&& enqueue, cb200_camera_plan** out)
 {
-    if (n == 0) return fail(CB200_ERR_ARG, "n = 0: a camera plan needs at least one picture");
-    if (!out) return fail(CB200_ERR_ARG, "null plan");
-    *out = nullptr;
-    return CB200_OK;
-}
-
-// a plan for the checked batch b (after every argument check): the buffers grown, the table uploaded, the capture, the graph
-// instantiated.  recv: a receivers plan's bound map and states (its d_map is allocated here)
-struct PlanReceivers { const int32_t* d_receiver_of; int n_receivers; cb200_receiver_state* d_states; };
-
-int make_plan(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
-              int32_t* d_extract_status, const PlanReceivers* recv, cb200_camera_plan** out)
-{
-    const int n = b.n();
-    int rc = check_frozen_camera(c, b.wh.data(), n); if (rc) return rc;
+    std::unique_ptr<cb200_camera_plan> own(plan);
+    cb200_camera_plan* p = plan;
+    cb200_ctx* c = p->ctx;
+    int rc = reserve(true); if (rc) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
-    // every buffer the graph uses, at this batch's size (with plans already there, the freeze check above guarantees this grows nothing)
-    rc = camera_reserve(c, b.wh.data(), n); if (rc) return rc;
-    rc = decode_reserve(c, flags, recv != nullptr); if (rc) return rc;
-    cb200_camera_plan* p = new cb200_camera_plan();
-    p->ctx = c; p->n = n; p->flags = flags;
-    p->keeps_ccm = !recv && ((flags & CB200_FLAG_CC_SIMPLE) || ccm_fits(c->mode, flags));
-    if (recv) {
-        p->d_receiver_of = recv->d_receiver_of; p->n_receivers = recv->n_receivers; p->d_states = recv->d_states;
-        const cudaError_t e = p->d_map.ensure(2 * (size_t)n);
-        if (e != cudaSuccess) rc = fail_cuda(e, "cudaMalloc plan receiver map");
-    }
+    // with plans already there, the freeze check above guarantees this grows nothing
+    rc = reserve(false); if (rc) return rc;
     std::vector<uint8_t> table;
     cudaStream_t cap = nullptr;
     if (!rc) rc = pic_table(c, b, table);
@@ -165,22 +173,50 @@ int make_plan(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chu
         if (e == cudaSuccess) e = cudaStreamSynchronize(cap);
         if (e != cudaSuccess) rc = fail_cuda(e, "H2D plan picture table");
     }
-    if (!rc) rc = capture(p, cap, b, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    if (!rc) rc = capture(p, cap, [&] { return enqueue(reinterpret_cast<const PicDesc*>(p->d_table.get())); });
     if (cap) cudaStreamDestroy(cap);
     if (!rc) rc = count_kernel_nodes(p->graph, &p->kernels);
     if (!rc) { const cudaError_t e = cudaGraphInstantiate(&p->exec, p->graph, 0); if (e != cudaSuccess) rc = fail_cuda(e, "cudaGraphInstantiate"); }
     if (rc) {
         const std::string why = cb200_last_error();
         if (p->graph) cudaGraphDestroy(p->graph);
-        delete p;
         return fail(rc, why);
     }
+    own.release();
     // the graph starts from d_carry: unless a CCM is on its way there from the device, the host's goes there now (a receivers plan
     // reads no context CCM, but while plans exist d_carry mirrors the host's matrix for every plain one)
-    c->plans.push_back(p);
-    if (!c->ccm_pending && (rc = carry_from_host(c)) != CB200_OK) { cb200_camera_plan_destroy(p); return rc; }
+    for (cb200_ctx* x : p->ctxs) x->plans.push_back(p);
+    for (cb200_ctx* x : p->ctxs)
+        if (!x->ccm_pending && (rc = carry_from_host(x)) != CB200_OK) { cb200_camera_plan_destroy(p); return rc; }
     *out = p;
     return CB200_OK;
+}
+
+// a plain or receivers plan on context c (recv: the bound map and states; its d_map is allocated here)
+struct PlanReceivers { const int32_t* d_receiver_of; int n_receivers; cb200_receiver_state* d_states; };
+
+int make_camera_plan(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                     int32_t* d_extract_status, const PlanReceivers* recv, cb200_camera_plan** out)
+{
+    const int n = b.n();
+    cb200_camera_plan* p = new cb200_camera_plan();
+    p->ctx = c; p->ctxs.assign(1, c); p->n = n; p->flags = flags;
+    p->keeps_ccm = !recv && ((flags & CB200_FLAG_CC_SIMPLE) || ccm_fits(c->mode, flags));
+    if (recv) { p->d_receiver_of = recv->d_receiver_of; p->n_receivers = recv->n_receivers; p->d_states = recv->d_states; }
+    auto reserve = [&](bool frozen_only) {
+        if (frozen_only) return check_frozen_camera(c, b.wh.data(), n);
+        int rc = camera_reserve(c, b.wh.data(), n); if (rc) return rc;
+        if ((rc = decode_reserve(c, flags, recv != nullptr))) return rc;
+        if (recv) CK(p->d_map.ensure(2 * (size_t)n), "cudaMalloc plan receiver map");
+        return CB200_OK;
+    };
+    auto enqueue = [&](const PicDesc* table) {
+        if (!recv) return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, table);
+        Receivers r(p->d_map.get(), p->d_states);
+        CK(receivers_order_launch(n, p->d_receiver_of, p->n_receivers, p->d_map, c->stream), "receivers order launch");
+        return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, table, &r);
+    };
+    return make_plan(p, b, reserve, enqueue, out);
 }
 
 }  // namespace
@@ -196,7 +232,7 @@ int cb200_camera_plan_create(cb200_ctx* c, const int32_t* wh, int n, uint32_t fl
     int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
     if (check_host_ccm(c))
         return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
-    return make_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, out);
+    return make_camera_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, out);
 }
 
 int cb200_camera_plan_create_receivers(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, const int32_t* d_receiver_of,
@@ -212,7 +248,36 @@ int cb200_camera_plan_create_receivers(cb200_ctx* c, const cb200_picture* pics, 
     if (check_host_ccm(c))
         return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
     const PlanReceivers recv = {d_receiver_of, n_receivers, d_states};
-    return make_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
+    return make_camera_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
+}
+
+int cb200_camera_plan_create_detect_receivers(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags,
+                                              const uint32_t* d_candidates, const int32_t* d_receiver_of, int n_receivers,
+                                              cb200_receiver_state* const* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                              int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out)
+{
+    // the checks of cb200_detect_scan_extract_decode_chunks_receivers_dev (the pointers of the candidates and the map in place of
+    // their entries, which only a launch reads; live plans allowed), with the plan's own after the batch's
+    CameraBatch b;
+    int rc = check_detect_plan(ctxs, n_modes, pics, n, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks, d_chunk_mask,
+                               d_extract_status, d_mode, out, b);
+    if (rc) return rc;
+    cb200_camera_plan* p = new cb200_camera_plan();
+    p->ctx = ctxs[0]; p->ctxs.assign(ctxs, ctxs + n_modes); p->n = n; p->flags = flags;
+    p->d_receiver_of = d_receiver_of; p->n_receivers = n_receivers; p->d_candidates = d_candidates;
+    p->d_mode_states.assign(d_states, d_states + n_modes);
+    auto reserve = [&](bool frozen_only) {
+        int rc = detect_plan_reserve(ctxs, n_modes, b, flags, frozen_only);
+        if (rc || frozen_only) return rc;
+        CK(p->d_map.ensure(detect_plan_words(n_modes, n)), "cudaMalloc plan lists");
+        CK(p->d_present.ensure((size_t)n_modes * n), "cudaMalloc plan present slots");
+        return CB200_OK;
+    };
+    auto enqueue = [&](const PicDesc* table) {
+        const DetectPlan dp = {table, d_candidates, d_receiver_of, n_receivers, p->d_mode_states.data(), p->d_map.get(), p->d_present.get()};
+        return detect_plan_enqueue(ctxs, n_modes, b, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks, dp);
+    };
+    return make_plan(p, b, reserve, enqueue, out);
 }
 
 int cb200_camera_plan_launch(cb200_camera_plan* p)
@@ -233,9 +298,12 @@ int cb200_camera_plan_launch(cb200_camera_plan* p)
     }
     CK(cudaGraphLaunch(p->exec, c->stream), "cudaGraphLaunch");
     count_launch(p->kernels);
-    // the host state the direct call leaves behind (a receivers call reports every picture's matrix, CC_SIMPLE too)
-    set_camera_pictures(c, p->n);
-    if (p->d_receiver_of || !(p->flags & CB200_FLAG_CC_SIMPLE)) c->ccm_frames = p->n;
+    // the host state the direct call leaves behind (a receivers call reports every picture's matrix, CC_SIMPLE too; a detect plan's
+    // contexts each decoded all n slots)
+    for (cb200_ctx* x : p->ctxs) {
+        set_camera_pictures(x, p->n);
+        if (p->d_receiver_of || !(p->flags & CB200_FLAG_CC_SIMPLE)) x->ccm_frames = p->n;
+    }
     if (p->keeps_ccm) {
         CK(cudaEventRecord(c->ccm_ev, c->stream), "record ccm");
         c->ccm_pending = true;
@@ -262,8 +330,9 @@ int cb200_camera_plan_destroy(cb200_camera_plan* p)
     cudaDeviceSynchronize();
     if (p->exec) cudaGraphExecDestroy(p->exec);
     if (p->graph) cudaGraphDestroy(p->graph);
-    for (size_t i = 0; i < c->plans.size(); ++i)
-        if (c->plans[i] == p) { c->plans.erase(c->plans.begin() + (long)i); break; }
+    for (cb200_ctx* x : p->ctxs)             // a detect plan is registered with each of its contexts
+        for (size_t i = 0; i < x->plans.size(); ++i)
+            if (x->plans[i] == p) { x->plans.erase(x->plans.begin() + (long)i); break; }
     delete p;
     return CB200_OK;
 }

@@ -112,5 +112,31 @@ CB_HD int rank_part(const int32_t* of, int n, int receivers, uint64_t k, int j0,
     return below;
 }
 
+// The device side of a detect receivers call (a detect receivers camera plan, whose candidates and map are read at replay time:
+// k_detect_plan_lists in detect.cu).  There are no sub-batches: every geometry works on all n slots, and slot i is picture i.  Slot
+// i with candidates cand and receiver r is empty when r lies outside [0, receivers) or cand has no bit below n_modes (higher bits
+// are ignored); otherwise mode k decodes it when bit k is set.  plan_slot writes slot i's part of the lists:
+//   raw[k n + i]      mode k's receiver of the slot, -1 where k does not decode it (an empty slot of mode k's map);
+//   present[g n + i]  1 when some mode of geometry g decodes it, else 0: the geometry's walk skips the slot;
+//   at[k n + i]       i when k decodes it, else -1 (detect_lists' pos, with each geometry's sub-batch left in place).
+// So compacting raw[k], at[k] over the present slots of group[k] gives detect_lists on the non-empty slots alone
+CB_HD uint32_t plan_modes(uint32_t cand, int32_t r, int receivers, int n_modes)
+{
+    return empty_slot(r, receivers) ? 0u : cand & ((1u << n_modes) - 1u);
+}
+CB_HD void plan_slot(uint32_t cand, int32_t r, int receivers, int n_modes, const int* group, int n_geoms, int n, int i, int32_t* raw,
+                     uint8_t* present, int32_t* at)
+{
+    const uint32_t modes = plan_modes(cand, r, receivers, n_modes);
+    uint32_t geoms = 0;
+    for (int k = 0; k < n_modes; ++k) {
+        const bool in = (modes >> k & 1u) != 0;
+        raw[(size_t)k * n + i] = in ? r : -1;
+        at[(size_t)k * n + i] = in ? i : -1;
+        if (in) geoms |= 1u << group[k];
+    }
+    for (int g = 0; g < n_geoms; ++g) present[(size_t)g * n + i] = (uint8_t)(geoms >> g & 1u);
+}
+
 }  // namespace receivers
 }  // namespace cb200
