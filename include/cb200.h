@@ -383,6 +383,46 @@ int cb200_camera_plan_destroy(cb200_camera_plan* plan);
 int cb200_camera_plan_create_receivers(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags, const int32_t* d_receiver_of,
                                        int n_receivers, cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
                                        uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out);
+/* ---- receivers camera plans over device descriptors: any sizes, layouts and buffers per batch ------------------------------------
+
+   cb200_camera_plan_create_receivers with the picture descriptors in DEVICE memory too: d_pics is n descriptors of type
+   cb200_picture, 40 bytes each, 8-byte aligned, read when each launch runs, like d_receiver_of.  So every slot may hold a picture of another size, layout and
+   buffer at every launch (torchvision.io.decode_jpeg outputs where they lie, say); the caller writes the descriptors in stream order
+   before the launch (one n x 40-byte copy, or a kernel in the same capture).  bounds (HOST, read at create) is the range of pictures
+   the plan is sized for: short side in [min_short, max_short], long side at most max_long.  Everything else is as for
+   cb200_camera_plan_create_receivers.  At each launch:
+     EMPTY slot: its receiver lies outside [0, n_receivers), exactly as there.  Its descriptor is not read (unused slots need not be
+             filled); status CB200_EXTRACT_EMPTY, mask 0, no state read or written.
+     REFUSED slot: a non-empty slot whose descriptor a direct call would refuse (a null data pointer, an unknown layout, a negative
+             pitch, a row pitch below w x channels, overlapping planes, a span of 4 GB or more) or that lies outside the bounds.  Status
+             CB200_EXTRACT_REFUSED, and otherwise as an empty slot.  No memory behind a refused or empty descriptor is read: the plan
+             scans a small black picture of its own in that slot's place.
+     the others: every output and every state afterwards equal bit for bit what cb200_scan_extract_decode_chunks_receivers_dev gives
+             on those descriptors alone, in slot order (records, masks, frame flags, statuses, cb200_camera_transforms).
+   The graph is the same for every descriptor set: a kernel at its head checks the descriptors and builds the picture table, and the
+   blur reads its tile lists from there.  The scan's buffers are sized from the bounds: n x max_long x max_short blurred bytes.
+   CB200_ERR_ARG, before any CUDA call, naming the cause: the receiver arguments as for cb200_camera_plan_create_receivers; the flags;
+   n < 0; a null d_pics or one not 8-byte aligned; null bounds; min_short < 60; max_short > 4499 (the scan's 9-tap limit);
+   min_short > max_short; max_long < max_short; bounds whose blur tiles or scan rows would not fit 31 bits; then everything else
+   cb200_camera_plan_create_receivers refuses except the descriptors' contents. */
+typedef struct cb200_picture_bounds { int32_t min_short, max_short, max_long; } cb200_picture_bounds;
+#define CB200_EXTRACT_REFUSED (-4)    /* extract status of a plan slot whose descriptor the launch refused */
+int cb200_camera_plan_create_receivers_pictures_dev(cb200_ctx* ctx, const cb200_picture* d_pics, int n, const cb200_picture_bounds* bounds,
+                                                    uint32_t flags, const int32_t* d_receiver_of, int n_receivers,
+                                                    cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                                    uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out);
+/* cb200_camera_plan_create_detect_receivers (below) with its descriptors in DEVICE memory too, read at each launch within bounds, as
+   above.  A slot is EMPTY exactly as in that plan (receiver out of range, or no candidate bit below n_modes): its descriptor is not
+   read.  A non-empty slot whose descriptor is refused as above gets status CB200_EXTRACT_REFUSED and otherwise what an empty slot
+   gets: mode -1, mask 0, a zeroed record and mode-mask row, no state of any mode read or written.  The other slots equal bit for bit
+   what cb200_detect_scan_extract_decode_chunks_receivers_dev gives on those descriptors alone, in slot order: records, masks,
+   statuses, modes, mode masks and every mode's table.  CB200_ERR_ARG, before any CUDA call: n_modes, the flags, then d_pics and
+   bounds as above, then everything else cb200_camera_plan_create_detect_receivers refuses except the descriptors' contents. */
+int cb200_camera_plan_create_detect_receivers_pictures_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* d_pics, int n,
+                                                           const cb200_picture_bounds* bounds, uint32_t flags, const uint32_t* d_candidates,
+                                                           const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states,
+                                                           uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
+                                                           int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out);
 /* ---- auto mode: the sender's mode detected by decoding ----------------------------------------------------------------------
 
    The receiver's auto mode (the reference's web receiver tries 66, 68, 67 and 4 and keeps the first mode under which a frame gives

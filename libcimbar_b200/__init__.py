@@ -20,6 +20,7 @@ FLAG_SHARPEN_IF_NEEDED = 0x20     # camera entry points only: sharpen the pictur
 FRAME_FALLBACK = 0x1
 FRAME_INEXACT = 0x2
 EXTRACT_EMPTY = -3                # extract status of an empty slot of a receivers camera plan
+EXTRACT_REFUSED = -4              # extract status of a plan slot whose device descriptor the launch refused
 
 EXPORTS = [
     "cb200_last_error", "cb200_version", "cb200_create", "cb200_destroy", "cb200_get_info", "cb200_set_stream",
@@ -44,6 +45,7 @@ EXPORTS = [
     "cb200_detect_scan_extract_decode_chunks_dev", "cb200_scan_extract_decode_chunks_pictures_dev",
     "cb200_decode_chunks_receivers_dev", "cb200_scan_extract_decode_chunks_receivers_dev", "cb200_camera_plan_create_receivers",
     "cb200_detect_scan_extract_decode_chunks_receivers_dev", "cb200_camera_plan_create_detect_receivers",
+    "cb200_camera_plan_create_receivers_pictures_dev", "cb200_camera_plan_create_detect_receivers_pictures_dev",
 ]
 
 
@@ -185,6 +187,10 @@ def load_library():
                                                                           vp, vp, vp]
     lib.cb200_camera_plan_create_detect_receivers.argtypes = [vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, C.c_int, vp, vp, vp, vp, vp,
                                                               vp, C.POINTER(C.c_void_p)]
+    lib.cb200_camera_plan_create_receivers_pictures_dev.argtypes = [vp, vp, C.c_int, vp, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp,
+                                                                    C.POINTER(C.c_void_p)]
+    lib.cb200_camera_plan_create_detect_receivers_pictures_dev.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_uint32, vp, vp, C.c_int, vp, vp,
+                                                                           vp, vp, vp, vp, C.POINTER(C.c_void_p)]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -229,6 +235,18 @@ def picture(t, order="rgb"):
     if not t.is_cuda:
         raise Cb200Error("a picture must be in device memory (a CUDA tensor)")
     return Picture(t.data_ptr(), w, h, row, plane, lay)
+
+
+def picture_descriptors(tensors, order="rgb"):
+    """the cb200_picture descriptors of a list of uint8 CUDA tensors (see picture(); order: one string, or one per tensor) as an
+    (n, 40) uint8 host array: what a receivers_camera_plan_pictures_dev launch reads, to be copied to its device descriptors"""
+    orders = [order] * len(tensors) if isinstance(order, str) else list(order)
+    if len(orders) != len(tensors):
+        raise Cb200Error(f"{len(orders)} orders for {len(tensors)} pictures")
+    out = np.zeros((len(tensors), C.sizeof(Picture)), np.uint8)
+    for i, (t, o) in enumerate(zip(tensors, orders)):
+        out[i] = np.frombuffer(bytes(picture(t, o)), np.uint8)
+    return out
 
 
 def receiver_states(ccms, device=None):
@@ -376,6 +394,38 @@ def detect_receivers_camera_plan(ctxs, pictures, candidates, receiver_of, states
         hs, len(ctxs), C.cast(descs, C.c_void_p), len(pictures), flags, cand, of, tables[0][1] if tables else 0, ptrs,
         d_chunks, d_mask, d_status, d_mode, d_mode_masks, C.byref(h)))
     return CameraPlan(ctxs[0], h, keep=(list(pictures), candidates, receiver_of, list(states)), ctxs=list(ctxs))
+
+
+def _descriptor_tensor(d_pics):
+    import torch
+    if not isinstance(d_pics, torch.Tensor) or not d_pics.is_cuda or d_pics.dtype != torch.uint8 or not d_pics.is_contiguous() or \
+            d_pics.dim() != 2 or d_pics.shape[1] != C.sizeof(Picture):
+        raise Cb200Error(f"d_pics is a contiguous (n, {C.sizeof(Picture)}) uint8 CUDA tensor")
+    return d_pics.shape[0]
+
+
+def detect_receivers_camera_plan_pictures_dev(ctxs, d_pics, bounds, candidates, receiver_of, states, d_chunks, d_mask, d_status, d_mode,
+                                              d_mode_masks=None, flags=0):
+    """detect_receivers_camera_plan with the pictures' descriptors read from device memory at each launch too
+    (cb200_camera_plan_create_detect_receivers_pictures_dev): d_pics and bounds as for Context.receivers_camera_plan_pictures_dev.  A
+    slot whose descriptor the launch refuses gets mode -1, mask 0, a zeroed record and status EXTRACT_REFUSED; an empty slot (no
+    candidate, or a receiver out of range) EXTRACT_EMPTY, and its descriptor is not read"""
+    n = _descriptor_tensor(d_pics)
+    if len(states) != len(ctxs):
+        raise Cb200Error(f"{len(states)} state tables for {len(ctxs)} contexts")
+    of = _device_int32(receiver_of, n, "receiver_of")
+    cand = None if candidates is None else _device_int32(candidates, n, "candidates")
+    tables = [_states_ptr(s) for s in states]
+    if len({count for _, count in tables}) > 1:
+        raise Cb200Error("every state table holds the same receivers: " + ", ".join(str(count) for _, count in tables) + " entries")
+    hs = (C.c_void_p * max(len(ctxs), 1))(*[c._h.value for c in ctxs])
+    ptrs = (C.c_void_p * max(len(tables), 1))(*[p for p, _ in tables])
+    bd = (C.c_int32 * 3)(*[int(v) for v in bounds])
+    h = C.c_void_p()
+    _check(load_library().cb200_camera_plan_create_detect_receivers_pictures_dev(
+        hs, len(ctxs), d_pics.data_ptr(), n, C.cast(bd, C.c_void_p), flags, cand, of, tables[0][1] if tables else 0, ptrs,
+        d_chunks, d_mask, d_status, d_mode, d_mode_masks, C.byref(h)))
+    return CameraPlan(ctxs[0], h, keep=(d_pics, candidates, receiver_of, list(states)), ctxs=list(ctxs))
 
 
 def _hptr(a):
@@ -744,6 +794,27 @@ class Context:
         _check(self.lib.cb200_camera_plan_create_receivers(self._h, C.cast(descs, C.c_void_p), len(pictures), flags, receiver_of.data_ptr(),
                                                            count, ptr, chunks, mask, frame_flags, status, C.byref(h)))
         return CameraPlan(self, h, keep=(list(pictures), receiver_of, states))
+
+    def receivers_camera_plan_pictures_dev(self, d_pics, bounds, receiver_of, states, chunks, mask, status, frame_flags=None, flags=0):
+        """receivers_camera_plan with the pictures' descriptors read from device memory at each launch too
+        (cb200_camera_plan_create_receivers_pictures_dev): d_pics is a contiguous (n, 40) uint8 CUDA tensor of cb200_picture
+        descriptors (picture_descriptors() builds them on the host), so each launch's slots may hold pictures of any size, layout
+        and buffer within bounds = (min_short, max_short, max_long).  A slot whose descriptor the launch refuses (a rule a direct
+        call checks, or outside the bounds) gets mask 0 and status EXTRACT_REFUSED, an empty slot EXTRACT_EMPTY; neither reads
+        its pixels.  Write each batch's descriptors and map in stream order before its launch; the plan keeps the tensors it binds
+        alive (the pictures are the caller's to keep until the stream has passed each launch)"""
+        import torch
+        n = _descriptor_tensor(d_pics)
+        if not isinstance(receiver_of, torch.Tensor) or not receiver_of.is_cuda or receiver_of.dtype != torch.int32 or \
+                not receiver_of.is_contiguous() or receiver_of.numel() != n:
+            raise Cb200Error(f"receiver_of is a contiguous int32 CUDA tensor of {n} values")
+        bd = (C.c_int32 * 3)(*[int(v) for v in bounds])
+        ptr, count = _states_ptr(states)
+        h = C.c_void_p()
+        _check(self.lib.cb200_camera_plan_create_receivers_pictures_dev(self._h, d_pics.data_ptr(), n, C.cast(bd, C.c_void_p), flags,
+                                                                        receiver_of.data_ptr(), count, ptr, chunks, mask, frame_flags,
+                                                                        status, C.byref(h)))
+        return CameraPlan(self, h, keep=(d_pics, receiver_of, states))
 
     jpeg_info = staticmethod(jpeg_info)
 

@@ -4,6 +4,7 @@
 #include "cb200_common.cuh"
 #include "k1x_flood.cuh"
 #include "ccm.cuh"
+#include "pic_desc.cuh"
 
 #include <string>
 #include <vector>
@@ -65,28 +66,22 @@ int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t 
 // CB200_ERR_ARG for CB200_FLAG_SHARPEN together with CB200_FLAG_SHARPEN_IF_NEEDED, or CB200_FLAG_CC_SIMPLE with CB200_FLAG_CC_FIT
 // (scan.cu)
 int check_camera_flags(uint32_t flags);
-// one camera picture of a batch as the extractor kernels (scan.cu, deskew.cu) read it.  The host builds the table per call, for
-// uniform batches too: picture i of a packed batch starts at byte 3 * sum_{j<i} w_j h_j of the buffer (layout RGB, row pitch
-// 3 w), its blurred gray at sum_{j<i} w_j h_j
-struct PicDesc {
-    uint64_t src;        // device address of the picture's pixel (0, 0) (of its R plane when planar): layout_core.cuh reads it
-    uint64_t blur;       // byte offset of its blurred gray picture in the scan's buffer (k_scan_blur4 / k_scan_anchors)
-    int w, h;
-    int words;           // k_scan_blur4's word path: w % 4 == 0, the source's base and pitches and the blurred base 4-byte aligned
-    int tile0;           // first tile of the picture in the blur launch of its radius
-    uint64_t pitch;      // bytes from one row to the next
-    uint64_t plane;      // bytes from one plane to the next (CB200_LAYOUT_RGB_PLANAR)
-    int layout;          // CB200_LAYOUT_*
-};
+// PicDesc, one camera picture as the extractor kernels read it: pic_desc.cuh.
 // The pictures of one camera, corner or deskew call, whatever the caller passed in (scan.cu): one descriptor per picture, their
 // sizes n x (w, h) (what scan_reserve and check_frozen_* take), and `packed`: every picture is RGB with row pitch 3 w, so the
 // kernels run their packed (kLayouts = false) instantiations.  `host`: the pictures are still in host memory, stage_batch takes
-// them to the device.  One builder per kind of input applies that kind's per-picture rules, all before any CUDA call
+// them to the device.  One builder per kind of input applies that kind's per-picture rules, all before any CUDA call.
+// A plan over device descriptors (device_batch) has neither pics nor wh: d_pics holds dev_n descriptors the plan reads at each
+// launch, and `bounds` the sizes it is built for (what its buffers are sized from: the CameraBatch overloads of the reserve
+// functions below)
 struct CameraBatch {
     std::vector<cb200_picture> pics;
     std::vector<int32_t> wh;
     bool packed = true, host = false;
-    int n() const { return (int)(wh.size() / 2); }
+    const cb200_picture* d_pics = nullptr;
+    int dev_n = 0;
+    cb200_picture_bounds bounds = {};
+    int n() const { return d_pics ? dev_n : (int)(wh.size() / 2); }
     void pack(const uint8_t* d);       // the pictures of sizes wh back to back from d in packed RGB
 };
 // wh: n x (w, h) on the host.  CB200_ERR_ARG naming the picture if a size is outside what the scan restates (short side 60 ..
@@ -102,6 +97,20 @@ int packed_batch(const uint8_t* d, const int32_t* wh, int n, CameraBatch& b);
 int uniform_batch(const uint8_t* d, int w, int h, int n, CameraBatch& b);
 int host_batch(const uint8_t* const* pictures, const int32_t* wh, int n, CameraBatch& b);
 int picture_batch(const cb200_picture* pics, int n, CameraBatch& b);
+// n descriptors in device memory within bounds (cb200_camera_plan_create_receivers_pictures_dev): the pointer (null, 8-byte
+// alignment) and the bounds are checked, none of the descriptors is read
+int device_batch(const cb200_picture* d_pics, int n, const cb200_picture_bounds* bounds, CameraBatch& b);
+// The device table of a plan over device descriptors, which k_plan_pictures writes at each launch (scan.cu): n PicDesc; three lists of
+// n slots, the slots of blur radius group 0, 1, 2 in slot order; the groups' slot counts and tile counts (6 int); the effective
+// receiver map (n int32: the caller's, -1 for a refused slot); one refused byte per slot; the stand-in picture's row (zeros).
+// plan_pictures_launch enqueues k_plan_pictures on the context's stream; a detect plan passes its candidates (NULL: every mode)
+// and n_modes, and a slot without a candidate below n_modes is empty like one whose receiver is out of range
+struct PlanTable {
+    size_t order, groups, of, refused, standin, bytes;
+    explicit PlanTable(const CameraBatch& b);
+};
+int plan_pictures_launch(cb200_ctx* c, const CameraBatch& b, const int32_t* d_receiver_of, int receivers, uint8_t* d_table,
+                         const uint32_t* d_cand = nullptr, int n_modes = 1);
 // CB200_ERR_ARG naming the first picture that spans 4 GB or more: k_deskew's offsets inside a picture are 32-bit (scan.cu)
 int check_spans(const CameraBatch& b);
 // a host batch packed into the context's one staging buffer for host pictures, with one copy per run of adjacent pictures; the
@@ -142,6 +151,9 @@ int plan_frozen(const cb200_ctx* c, const char* buffer, size_t have, size_t need
 // frames and the exact walk's (scan.cu, deskew.cu, api.cu)
 int scan_reserve(cb200_ctx* c, const int32_t* wh, int n);
 int camera_reserve(cb200_ctx* c, const int32_t* wh, int n);
+// the same for a batch: its sizes, or a device batch's bounds
+int scan_reserve(cb200_ctx* c, const CameraBatch& b);
+int camera_reserve(cb200_ctx* c, const CameraBatch& b);
 int deskew_reserve(cb200_ctx* c, int n);
 int flood_reserve(cb200_ctx* c, int n);
 // the decode's buffers sized by max_frames, the CCM event and the slot map of these flags, and with `receivers` a receivers call's
@@ -152,6 +164,7 @@ int decode_reserve(cb200_ctx* c, uint32_t flags, bool receivers = false);
 int check_frozen_frames(cb200_ctx* c, int n);
 int check_frozen_deskew(cb200_ctx* c, int n);
 int check_frozen_camera(cb200_ctx* c, const int32_t* wh, int n);
+int check_frozen_camera(cb200_ctx* c, const CameraBatch& b);
 int check_frozen_scan(cb200_ctx* c, const int32_t* wh, int n);
 // the CCM a plan's graph starts from is d_carry: with plans, a matrix the host sets (cb200_set_ccm, cb200_fit_ccm, a new plan) is
 // copied there in stream order (api.cu)
@@ -186,11 +199,14 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
 // launch, where receiver -1 marks an empty slot (empty_slots: the kernels' variants that skip those)
 int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states,
                     bool on_device = false);
+// d_refused: NULL, or (a plan over device descriptors) one byte per slot, set where the launch refused the slot's descriptor: its
+// status becomes CB200_EXTRACT_REFUSED instead of CB200_EXTRACT_EMPTY
 struct Receivers {
     std::vector<int32_t> map;
     const int32_t* d_map = nullptr;
     cb200_receiver_state* d_states = nullptr;
     bool empty_slots = false;
+    const uint8_t* d_refused = nullptr;
     Receivers(const int32_t* receiver_of, int n, int n_receivers, cb200_receiver_state* states);
     Receivers(const int32_t* d_plan_map, cb200_receiver_state* states) : d_map(d_plan_map), d_states(states), empty_slots(true) {}
     size_t bytes() const { return map.size() * sizeof(int32_t); }
@@ -204,6 +220,7 @@ int plan_rules(int n, cb200_camera_plan** out);
 // cb200_camera_plan_create_detect_receivers, before any CUDA call.  detect_plan_reserve: every buffer of the contexts the graph uses,
 // at b's size; frozen_only: only on the contexts with live plans, where it makes no CUDA call and refuses what would grow.
 // detect_plan_enqueue: the whole call on ctxs[0]'s stream, for the capture
+// d_pics_table: a plan over device descriptors, its table for k_plan_pictures (PlanTable, = d_table), else NULL
 struct DetectPlan {
     const PicDesc* d_table;
     const uint32_t* d_cand;
@@ -212,9 +229,13 @@ struct DetectPlan {
     cb200_receiver_state* const* d_states;
     int32_t* d_lists;
     uint8_t* d_present;
+    uint8_t* d_pics_table;
 };
 size_t detect_plan_words(int n_modes, int n);
-int check_detect_plan(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags, const uint32_t* d_candidates,
+// bounds: NULL for cb200_camera_plan_create_detect_receivers (pics on the host), else the plan's bounds and pics in device memory
+// (device_batch's checks; a null bounds is refused there)
+int check_detect_plan(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, bool dev_pics, const cb200_picture_bounds* bounds,
+                      int n, uint32_t flags, const uint32_t* d_candidates,
                       const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states, const uint8_t* d_chunks,
                       const uint32_t* d_chunk_mask, const int32_t* d_extract_status, const int32_t* d_mode, cb200_camera_plan** out,
                       CameraBatch& b);

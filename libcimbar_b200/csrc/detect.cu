@@ -109,6 +109,14 @@ k_detect_select_at(const DetectArgs a, const int32_t* __restrict__ at, int n, ui
     for (int b = threadIdx.x; b < a.slot; b += blockDim.x) dst[b] = b < have ? src[b] : 0;
 }
 
+// a detect receivers plan over device descriptors: a slot whose descriptor the launch refused (k_plan_pictures) reports
+// CB200_EXTRACT_REFUSED; k_detect_select_at has given it what an empty slot gets otherwise
+__global__ void k_status_refused(const uint8_t* __restrict__ refused, int n, int32_t* __restrict__ status)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && refused[i]) status[i] = CB200_EXTRACT_REFUSED;
+}
+
 // a detect receivers plan's lists at one launch, one thread per slot (receivers_core.cuh: plan_slot): every mode's raw receivers
 // (k_receivers_order then orders each), every geometry's present bytes and every mode's positions.  cand NULL: every mode
 struct PlanListArgs { int n_modes, n_geoms, receivers; int group[kDetectModes]; };
@@ -285,7 +293,8 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
     for (int k = 0; k < n_modes; ++k) {
         if (!decodes(k)) continue;
         const CameraBatch& bk = batch(group[k]);
-        rc = camera_reserve_for(ctxs[k], bk.wh.data(), bk.n(), !dr && k == 0, lead[group[k]] == k); if (rc) return rc;
+        // (a device batch's scan buffers: camera_scan reserves them from the bounds)
+        rc = camera_reserve_for(ctxs[k], bk.wh.data(), bk.n(), !dr && k == 0 && !b.d_pics, lead[group[k]] == k); if (rc) return rc;
     }
     // grown through grow(): a live detect plan's graph reads them
     if ((rc = grow(c0, ds->status, (size_t)n_modes * n, "detect statuses"))) return rc;
@@ -319,6 +328,15 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
         for (int k = 0; k < n_modes; ++k) memcpy(tail.data() + map_at[k], lists.map[k].data(), sizeof(int32_t) * lists.map[k].size());
         memcpy(tail.data() + pos_at, lists.pos.data(), sizeof(int32_t) * lists.pos.size());
     }
+    // a plan over device descriptors: this launch's picture table first, and its map (refused slots emptied) in place of the caller's
+    const int32_t* d_of = dp ? dp->d_of : nullptr;
+    const uint8_t* d_refused = nullptr;
+    if (dp && dp->d_pics_table) {
+        rc = plan_pictures_launch(c0, b, dp->d_of, dp->receivers, dp->d_pics_table, dp->d_cand, n_modes); if (rc) return rc;
+        const PlanTable t(b);
+        d_of = reinterpret_cast<const int32_t*>(dp->d_pics_table + t.of);
+        d_refused = dp->d_pics_table + t.refused;
+    }
     const PicDesc* d_desc;
     const uint8_t* d_tail = nullptr;
     rc = camera_scan(c0, b, dp ? dp->d_table : nullptr, &d_desc, nullptr, dr ? &tail : nullptr, &d_tail); if (rc) return rc;
@@ -328,7 +346,7 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
         memset(&la, 0, sizeof(la));
         la.n_modes = n_modes; la.n_geoms = ng; la.receivers = dp->receivers;
         for (int k = 0; k < n_modes; ++k) la.group[k] = group[k];
-        k_detect_plan_lists<<<(n + 127) / 128, 128, 0, main>>>(dp->d_cand, dp->d_of, n, la, dp->d_lists, dp->d_present, plan_at(*dp, n_modes, n));
+        k_detect_plan_lists<<<(n + 127) / 128, 128, 0, main>>>(dp->d_cand, d_of, n, la, dp->d_lists, dp->d_present, plan_at(*dp, n_modes, n));
         count_launch();
         CK(cudaGetLastError(), "detect plan lists launch");
         for (int k = 0; k < n_modes; ++k)
@@ -385,15 +403,23 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
     } else k_detect_select<<<n, 256, 0, main>>>(a, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
     count_launch();
     CK(cudaGetLastError(), "detect select launch");
+    if (d_refused) {                         // k_detect_select_at made them empty slots: mode -1, mask 0, zeros
+        k_status_refused<<<(n + 127) / 128, 128, 0, main>>>(d_refused, n, d_extract_status);
+        count_launch();
+        CK(cudaGetLastError(), "refused status launch");
+    }
     return CB200_OK;
 }
 
-int check_detect_plan(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags, const uint32_t* d_candidates,
-                      const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states, const uint8_t* d_chunks,
-                      const uint32_t* d_chunk_mask, const int32_t* d_extract_status, const int32_t* d_mode, cb200_camera_plan** out,
-                      CameraBatch& b)
+int check_detect_plan(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, bool dev_pics, const cb200_picture_bounds* bounds,
+                      int n, uint32_t flags, const uint32_t* d_candidates, const int32_t* d_receiver_of, int n_receivers,
+                      cb200_receiver_state* const* d_states, const uint8_t* d_chunks, const uint32_t* d_chunk_mask,
+                      const int32_t* d_extract_status, const int32_t* d_mode, cb200_camera_plan** out, CameraBatch& b)
 {
-    auto build = [&](CameraBatch& bb) { const int rc = picture_batch(pics, n, bb); return rc ? rc : plan_rules(n, out); };
+    auto build = [&](CameraBatch& bb) {
+        const int rc = dev_pics ? device_batch(pics, n, bounds, bb) : picture_batch(pics, n, bb);
+        return rc ? rc : plan_rules(n, out);
+    };
     auto more = [&] { return check_detect_receivers(n_modes, n, d_candidates, d_receiver_of, n_receivers, d_states, true); };
     return check_detect(ctxs, n_modes, flags, build, d_chunks, d_chunk_mask, d_extract_status, d_mode, b, more, true);
 }
@@ -406,7 +432,8 @@ int detect_plan_reserve(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& 
     for (int k = 0; k < n_modes; ++k) {      // what detect_enqueue reserves with every geometry live, and the decode's own buffers
         cb200_ctx* c = ctxs[k];
         if (frozen_only && c->plans.empty()) continue;
-        if ((rc = camera_reserve_for(c, b.wh.data(), n, k == 0, lead[group[k]] == k))) return rc;
+        if ((rc = camera_reserve_for(c, b.wh.data(), n, k == 0 && !b.d_pics, lead[group[k]] == k))) return rc;
+        if (k == 0 && b.d_pics && (rc = scan_reserve(c, b))) return rc;      // sized from the bounds
         if (!frozen_only && (rc = decode_reserve(c, flags, true))) return rc;
     }
     cb200_ctx* c0 = ctxs[0];

@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include "../../include/cb200.h"
+#include "pic_desc.cuh"
 #include "scan_core.cuh"            // CB_HD
 
 namespace cb200 {
@@ -163,6 +164,64 @@ CB_HD void tap_pair(const uint8_t* p, uint64_t plane, int layout, const uint8_t*
     if (layout == CB200_LAYOUT_RGB_PLANAR) { planar_pair(p, plane, end, lo, hi); return; }
     load_bytes(p, end, (uint32_t)channels(layout) * 2u, lo, hi);
     pair_rgb(layout, lo, hi);
+}
+
+// The scan's Gaussian radius for a w x h picture (Scanner.h:93-103, :155-157): the kernel unit is the power of two above
+// 0.002 x the short side, plus one, at least 3 taps.  Short sides 60 .. 1499 give 3 taps, 1500 .. 2499 give 5, 2500 .. 4499 give 9
+CB_HD int blur_radius(int w, int h)
+{
+    unsigned v = (unsigned)((w < h ? w : h) * 0.002);
+    v--;
+    v |= v >> 1; v |= v >> 2; v |= v >> 4; v |= v >> 8; v |= v >> 16;
+    unsigned unit = v + 2;
+    if (unit < 3u) unit = 3u;
+    return (int)(unit / 2);
+}
+
+// The rule every camera call applies to a picture descriptor (scan.cu: picture_batch, check_picture_sizes and check_spans print
+// why, in that order): true when the calls refuse it -- a null data pointer, an unknown layout, a negative pitch, a short side below
+// 60 or a Gaussian beyond 9 taps (4500 pixels or more), a row pitch below w x channels, overlapping planes, a span of 4 GB or more.
+// With bounds (a plan that reads its descriptors from device memory) it also refuses a short side outside [min_short, max_short]
+// and a long side above max_long.  The pitch rules come before any product that could overflow: a row pitch of 4 GB or more is
+// refused whatever the rest says
+CB_HD bool picture_refused(const cb200_picture& p, const cb200_picture_bounds* bounds)
+{
+    if (!p.data || !known(p.layout) || p.row_pitch < 0 || p.plane_pitch < 0) return true;
+    const int s = p.w < p.h ? p.w : p.h, l = p.w < p.h ? p.h : p.w;
+    if (s < 60 || blur_radius(p.w, p.h) > 4) return true;
+    if (bounds && (s < bounds->min_short || s > bounds->max_short || l > bounds->max_long)) return true;
+    const int64_t lim = (int64_t)1 << 32, row = (int64_t)p.w * channels(p.layout);
+    const bool planar = p.layout == CB200_LAYOUT_RGB_PLANAR;
+    if (p.row_pitch < row || p.row_pitch >= lim || (planar && p.plane_pitch >= lim)) return true;
+    if (planar && p.plane_pitch < (int64_t)p.h * p.row_pitch) return true;
+    return (planar ? 2 * p.plane_pitch : 0) + (int64_t)(p.h - 1) * p.row_pitch + row >= lim;
+}
+
+constexpr int kBlurTileW = 128, kBlurTileH = 32;          // k_scan_blur4's tile
+
+CB_HD int64_t blur_tiles(int w, int h) { return (((int64_t)w + kBlurTileW - 1) / kBlurTileW) * (((int64_t)h + kBlurTileH - 1) / kBlurTileH); }
+// the blur radii 1, 2, 4 (3, 5, 9 taps) as the plan's radius groups 0, 1, 2
+CB_HD int radius_group(int R) { return R == 1 ? 0 : (R == 2 ? 1 : 2); }
+
+// Slot i of a plan over device descriptors (k_plan_pictures, scan.cu), everything but its tile0: the descriptor table entry, its blur
+// radius group and tile count.  An empty slot (its receiver out of range, or in a detect plan no candidate mode: the caller decides)
+// does not read its descriptor; it and a refused slot
+// get the plan's stand-in -- a black min_short x min_short RGB picture of pitch 0 at `standin`, which fails extraction.  The blurred
+// picture of slot i sits at i x slot_bytes (a multiple of 4) in the scan's buffer at blur_base; the word path is pic_table's rule
+struct PlanSlot { int group, tiles; bool refused; };
+CB_HD PlanSlot plan_slot(const cb200_picture* pics, bool empty, const cb200_picture_bounds& bounds, uint64_t standin, uint64_t blur_base,
+                         uint64_t slot_bytes, int i, PicDesc& d)
+{
+    cb200_picture p;
+    bool refused = false;
+    if (!empty) { p = pics[i]; refused = picture_refused(p, &bounds); }
+    if (empty || refused) p = cb200_picture{reinterpret_cast<const uint8_t*>(standin), bounds.min_short, bounds.min_short, 0, 0, CB200_LAYOUT_RGB};
+    const bool planar = p.layout == CB200_LAYOUT_RGB_PLANAR;
+    d.src = reinterpret_cast<uint64_t>(p.data); d.blur = (uint64_t)i * slot_bytes; d.w = p.w; d.h = p.h;
+    d.pitch = (uint64_t)p.row_pitch; d.plane = planar ? (uint64_t)p.plane_pitch : 0; d.layout = p.layout;
+    d.words = (p.w % 4 == 0) && (d.src % 4 == 0) && (d.pitch % 4 == 0) && (d.plane % 4 == 0) && ((blur_base + d.blur) % 4 == 0);
+    d.tile0 = 0;
+    return PlanSlot{radius_group(blur_radius(p.w, p.h)), (int)blur_tiles(p.w, p.h), refused && !empty};   // < 2^31: the bounds
 }
 
 }  // namespace layout

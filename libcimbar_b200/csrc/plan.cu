@@ -14,11 +14,17 @@
 // input the direct call builds on the host per batch: here k_receivers_order, captured at the head of the graph, builds it at each
 // launch from the caller's d_receiver_of into the plan's own d_map, and the rest of the graph reads it from there.
 //
+// A receivers plan over device descriptors (cb200_camera_plan_create_receivers_pictures_dev) reads the picture descriptors at each
+// launch too: k_plan_pictures (scan.cu), ahead of k_receivers_order, checks them and writes the picture table the host builds for the
+// other plans, and the plan's map with its refused slots emptied; the scan's buffers are sized from the plan's bounds.
+//
 // A detect receivers plan (cb200_camera_plan_create_detect_receivers) is the detect receivers call captured so, over several
 // contexts: detect.cu's geometry loop on every context's buffers, with every context's stream swapped to the capture stream, and
 // the side streams' forks and joins becoming parallel branches of the graph.  Its candidates and map are read at each launch
 // (k_detect_plan_lists at the head of the graph builds every list into d_map and d_present).  It is registered in the plans of every
-// one of its contexts, so each of them freezes the buffers the graph uses, and destroying any of them destroys the plan.
+// one of its contexts, so each of them freezes the buffers the graph uses, and destroying any of them destroys the plan.  Over device
+// descriptors (cb200_camera_plan_create_detect_receivers_pictures_dev), k_plan_pictures comes first and k_detect_plan_lists reads its
+// map, and k_status_refused marks the refused slots after the selection.
 #include "ctx.cuh"
 
 #include <memory>
@@ -68,6 +74,8 @@ int check_frozen_deskew(cb200_ctx* c, int n)
 }
 
 int check_frozen_camera(cb200_ctx* c, const int32_t* wh, int n) { return c->plans.empty() ? CB200_OK : camera_reserve(c, wh, n); }
+
+int check_frozen_camera(cb200_ctx* c, const CameraBatch& b) { return c->plans.empty() ? CB200_OK : camera_reserve(c, b); }
 
 int check_frozen_scan(cb200_ctx* c, const int32_t* wh, int n) { return c->plans.empty() ? CB200_OK : scan_reserve(c, wh, n); }
 
@@ -165,11 +173,13 @@ int make_plan(cb200_camera_plan* plan, const CameraBatch& b, Reserve&& reserve, 
     rc = reserve(false); if (rc) return rc;
     std::vector<uint8_t> table;
     cudaStream_t cap = nullptr;
-    if (!rc) rc = pic_table(c, b, table);
-    if (!rc) { const cudaError_t e = p->d_table.ensure(table.size()); if (e != cudaSuccess) rc = fail_cuda(e, "cudaMalloc plan picture table"); }
+    // a plan over device descriptors: its graph writes the table at each launch, and only the stand-in picture's row (zeros) is set here
+    if (!rc && !b.d_pics) rc = pic_table(c, b, table);
+    const size_t bytes = b.d_pics ? PlanTable(b).bytes : table.size();
+    if (!rc) { const cudaError_t e = p->d_table.ensure(bytes); if (e != cudaSuccess) rc = fail_cuda(e, "cudaMalloc plan picture table"); }
     if (!rc) { const cudaError_t e = cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking); if (e != cudaSuccess) rc = fail_cuda(e, "cudaStreamCreate"); }
     if (!rc) {   // the table goes up once, on the private stream, before anything can replay
-        cudaError_t e = cudaMemcpyAsync(p->d_table, table.data(), table.size(), cudaMemcpyHostToDevice, cap);
+        cudaError_t e = b.d_pics ? cudaMemsetAsync(p->d_table, 0, bytes, cap) : cudaMemcpyAsync(p->d_table, table.data(), bytes, cudaMemcpyHostToDevice, cap);
         if (e == cudaSuccess) e = cudaStreamSynchronize(cap);
         if (e != cudaSuccess) rc = fail_cuda(e, "H2D plan picture table");
     }
@@ -204,8 +214,8 @@ int make_camera_plan(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t
     p->keeps_ccm = !recv && ((flags & CB200_FLAG_CC_SIMPLE) || ccm_fits(c->mode, flags));
     if (recv) { p->d_receiver_of = recv->d_receiver_of; p->n_receivers = recv->n_receivers; p->d_states = recv->d_states; }
     auto reserve = [&](bool frozen_only) {
-        if (frozen_only) return check_frozen_camera(c, b.wh.data(), n);
-        int rc = camera_reserve(c, b.wh.data(), n); if (rc) return rc;
+        if (frozen_only) return check_frozen_camera(c, b);
+        int rc = camera_reserve(c, b); if (rc) return rc;
         if ((rc = decode_reserve(c, flags, recv != nullptr))) return rc;
         if (recv) CK(p->d_map.ensure(2 * (size_t)n), "cudaMalloc plan receiver map");
         return CB200_OK;
@@ -213,11 +223,44 @@ int make_camera_plan(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t
     auto enqueue = [&](const PicDesc* table) {
         if (!recv) return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, table);
         Receivers r(p->d_map.get(), p->d_states);
-        CK(receivers_order_launch(n, p->d_receiver_of, p->n_receivers, p->d_map, c->stream), "receivers order launch");
+        const int32_t* of = p->d_receiver_of;
+        if (b.d_pics) {   // device descriptors: k_plan_pictures first, and the order from its map, in which refused slots are empty
+            int rc = plan_pictures_launch(c, b, p->d_receiver_of, p->n_receivers, p->d_table); if (rc) return rc;
+            const PlanTable t(b);
+            of = reinterpret_cast<const int32_t*>(p->d_table + t.of);
+            r.d_refused = p->d_table + t.refused;
+        }
+        CK(receivers_order_launch(n, of, p->n_receivers, p->d_map, c->stream), "receivers order launch");
         return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, table, &r);
     };
     return make_plan(p, b, reserve, enqueue, out);
 }
+
+// a detect receivers plan for the checked batch b (descriptors on the host, or in device memory within bounds)
+int make_detect_plan(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, uint32_t flags, const uint32_t* d_candidates,
+                     const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states, uint8_t* d_chunks,
+                     uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out)
+{
+    const int n = b.n();
+    cb200_camera_plan* p = new cb200_camera_plan();
+    p->ctx = ctxs[0]; p->ctxs.assign(ctxs, ctxs + n_modes); p->n = n; p->flags = flags;
+    p->d_receiver_of = d_receiver_of; p->n_receivers = n_receivers; p->d_candidates = d_candidates;
+    p->d_mode_states.assign(d_states, d_states + n_modes);
+    auto reserve = [&](bool frozen_only) {
+        int rc = detect_plan_reserve(ctxs, n_modes, b, flags, frozen_only);
+        if (rc || frozen_only) return rc;
+        CK(p->d_map.ensure(detect_plan_words(n_modes, n)), "cudaMalloc plan lists");
+        CK(p->d_present.ensure((size_t)n_modes * n), "cudaMalloc plan present slots");
+        return CB200_OK;
+    };
+    auto enqueue = [&](const PicDesc* table) {
+        const DetectPlan dp = {table, d_candidates, d_receiver_of, n_receivers, p->d_mode_states.data(), p->d_map.get(), p->d_present.get(),
+                               b.d_pics ? p->d_table.get() : nullptr};
+        return detect_plan_enqueue(ctxs, n_modes, b, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks, dp);
+    };
+    return make_plan(p, b, reserve, enqueue, out);
+}
+
 
 }  // namespace
 
@@ -251,6 +294,23 @@ int cb200_camera_plan_create_receivers(cb200_ctx* c, const cb200_picture* pics, 
     return make_camera_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
 }
 
+int cb200_camera_plan_create_receivers_pictures_dev(cb200_ctx* c, const cb200_picture* d_pics, int n, const cb200_picture_bounds* bounds,
+                                                    uint32_t flags, const int32_t* d_receiver_of, int n_receivers,
+                                                    cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                                    uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out)
+{
+    // cb200_camera_plan_create_receivers' checks, with the descriptors' pointer and bounds in place of their contents (which each
+    // launch checks on the device)
+    int rc = check_receivers(c, d_receiver_of, n, n_receivers, d_states, true); if (rc) return rc;
+    auto build = [&](CameraBatch& b) { const int rc = device_batch(d_pics, n, bounds, b); return rc ? rc : plan_rules(n, out); };
+    CameraBatch b;
+    rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
+    if (check_host_ccm(c))
+        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
+    const PlanReceivers recv = {d_receiver_of, n_receivers, d_states};
+    return make_camera_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
+}
+
 int cb200_camera_plan_create_detect_receivers(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags,
                                               const uint32_t* d_candidates, const int32_t* d_receiver_of, int n_receivers,
                                               cb200_receiver_state* const* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
@@ -259,26 +319,28 @@ int cb200_camera_plan_create_detect_receivers(cb200_ctx* const* ctxs, int n_mode
     // the checks of cb200_detect_scan_extract_decode_chunks_receivers_dev (the pointers of the candidates and the map in place of
     // their entries, which only a launch reads; live plans allowed), with the plan's own after the batch's
     CameraBatch b;
-    int rc = check_detect_plan(ctxs, n_modes, pics, n, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks, d_chunk_mask,
-                               d_extract_status, d_mode, out, b);
+    int rc = check_detect_plan(ctxs, n_modes, pics, false, nullptr, n, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks,
+                               d_chunk_mask, d_extract_status, d_mode, out, b);
     if (rc) return rc;
-    cb200_camera_plan* p = new cb200_camera_plan();
-    p->ctx = ctxs[0]; p->ctxs.assign(ctxs, ctxs + n_modes); p->n = n; p->flags = flags;
-    p->d_receiver_of = d_receiver_of; p->n_receivers = n_receivers; p->d_candidates = d_candidates;
-    p->d_mode_states.assign(d_states, d_states + n_modes);
-    auto reserve = [&](bool frozen_only) {
-        int rc = detect_plan_reserve(ctxs, n_modes, b, flags, frozen_only);
-        if (rc || frozen_only) return rc;
-        CK(p->d_map.ensure(detect_plan_words(n_modes, n)), "cudaMalloc plan lists");
-        CK(p->d_present.ensure((size_t)n_modes * n), "cudaMalloc plan present slots");
-        return CB200_OK;
-    };
-    auto enqueue = [&](const PicDesc* table) {
-        const DetectPlan dp = {table, d_candidates, d_receiver_of, n_receivers, p->d_mode_states.data(), p->d_map.get(), p->d_present.get()};
-        return detect_plan_enqueue(ctxs, n_modes, b, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks, dp);
-    };
-    return make_plan(p, b, reserve, enqueue, out);
+    return make_detect_plan(ctxs, n_modes, b, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks, d_chunk_mask,
+                            d_extract_status, d_mode, d_mode_masks, out);
 }
+
+int cb200_camera_plan_create_detect_receivers_pictures_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* d_pics, int n,
+                                                           const cb200_picture_bounds* bounds, uint32_t flags, const uint32_t* d_candidates,
+                                                           const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states,
+                                                           uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
+                                                           int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out)
+{
+    // cb200_camera_plan_create_detect_receivers' checks, with the descriptors' pointer and bounds in place of their contents
+    CameraBatch b;
+    int rc = check_detect_plan(ctxs, n_modes, d_pics, true, bounds, n, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks,
+                               d_chunk_mask, d_extract_status, d_mode, out, b);
+    if (rc) return rc;
+    return make_detect_plan(ctxs, n_modes, b, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks, d_chunk_mask,
+                            d_extract_status, d_mode, d_mode_masks, out);
+}
+
 
 int cb200_camera_plan_launch(cb200_camera_plan* p)
 {

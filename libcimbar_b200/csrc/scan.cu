@@ -22,7 +22,9 @@
 #include "scan_core.cuh"
 #include "extract_core.cuh"
 #include "layout_core.cuh"
+#include "receivers_core.cuh"
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -87,17 +89,18 @@ template <int R> struct BlurKW {     // the 2R+1 coefficients as bytes of up to 
 // A CTA finds its picture by division when all listed pictures have one size (uniform_tiles tiles each), else by binary search.
 // kLayouts: the pictures' layouts and pitches come from the table; without it every picture is packed RGB (row pitch 3 w), the
 // code the packed batches have always run (fewer registers)
+// The tile body, shared by k_scan_blur4 (tile t = its block) and k_scan_blur4_list (a grid-stride loop over the listed tiles).  Every
+// shared array a tile writes is read only before its last barrier, so the next tile of the same CTA may start at once
+static_assert(kBlurTW == layout::kBlurTileW && kBlurTH == layout::kBlurTileH, "the plan's tile counts are the blur's");
 template <int R, bool kLayouts>
-__global__ void __launch_bounds__(kBlurThreads)
-k_scan_blur4(uint8_t* __restrict__ out, const PicDesc* __restrict__ desc, const int* __restrict__ order, int npics, int uniform_tiles,
-             unsigned* __restrict__ hist)
+__device__ __forceinline__ void blur_tile(uint8_t* __restrict__ out, const PicDesc* __restrict__ desc, const int* __restrict__ order, int npics,
+                                          int uniform_tiles, unsigned* __restrict__ hist, const int t)
 {
     constexpr int GH = kBlurTH + 2 * R, GP = kBlurTW + 8, NW = (2 * R + 1 + 3) / 4;      // gray pitch: interior at byte 4
     __shared__ __align__(16) uint8_t g[GH][GP];
     __shared__ __align__(16) uint16_t hs[GH][kBlurTW];
     __shared__ unsigned lh[256];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int t = (int)blockIdx.x;
     int k;
     if (uniform_tiles) {
         k = t / uniform_tiles;
@@ -185,6 +188,36 @@ k_scan_blur4(uint8_t* __restrict__ out, const PicDesc* __restrict__ desc, const 
     if (lh[tid]) atomicAdd(&hist[(size_t)pic * 256 + tid], lh[tid]);
 }
 
+template <int R, bool kLayouts>
+__global__ void __launch_bounds__(kBlurThreads)
+k_scan_blur4(uint8_t* __restrict__ out, const PicDesc* __restrict__ desc, const int* __restrict__ order, int npics, int uniform_tiles,
+             unsigned* __restrict__ hist)
+{
+    blur_tile<R, kLayouts>(out, desc, order, npics, uniform_tiles, hist, (int)blockIdx.x);
+}
+
+// k_scan_blur4 over a plan's device table (k_plan_pictures): radius group `group` lists counts[group] pictures in order, with
+// counts[3 + group] tiles between them, both written at this launch -- persistent CTAs walk the tiles, none idle while tiles remain
+template <int R>
+__global__ void __launch_bounds__(kBlurThreads)
+k_scan_blur4_list(uint8_t* __restrict__ out, const PicDesc* __restrict__ desc, const int* __restrict__ order, const int* __restrict__ counts,
+                  int group, unsigned* __restrict__ hist)
+{
+    const int npics = counts[group], tiles = counts[3 + group];
+    for (int t = (int)blockIdx.x; t < tiles; t += (int)gridDim.x) blur_tile<R, true>(out, desc, order, npics, 0, hist, t);
+}
+
+// k_scan_blur4_list's grid: as many CTAs as the GPU holds at once (more would wait for a whole CTA's share of the tiles), at most one
+// per tile of the largest batch
+template <int R>
+static int blur_list_grid(const cb200_ctx* c, int64_t most, unsigned* grid)
+{
+    int per_sm = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_scan_blur4_list<R>, kBlurThreads, 0), "blur occupancy");
+    *grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(most, (int64_t)per_sm * c->sm_count));
+    return CB200_OK;
+}
+
 // ---------------------------------------------------------------------------------------------- Otsu
 // cv::threshold(THRESH_OTSU) -> getThreshVal_Otsu_8u (modules/imgproc/src/thresh.cpp), double precision, operation for operation
 __global__ void k_scan_otsu(const unsigned* __restrict__ hist, const PicDesc* __restrict__ desc, int n, int* __restrict__ thr)
@@ -247,15 +280,7 @@ static ScanScratch* sstate(cb200_ctx* c)
     return c->scan;
 }
 
-static int scan_blur_radius(int w, int h)               // Scanner.h:93-103, :155-157
-{
-    unsigned v = (unsigned)((w < h ? w : h) * 0.002);
-    v--;
-    v |= v >> 1; v |= v >> 2; v |= v >> 4; v |= v >> 8; v |= v >> 16;
-    unsigned unit = v + 2;
-    if (unit < 3u) unit = 3u;
-    return (int)(unit / 2);
-}
+static int scan_blur_radius(int w, int h) { return layout::blur_radius(w, h); }
 
 int check_picture_sizes(const int32_t* wh, int n)
 {
@@ -361,10 +386,33 @@ int picture_batch(const cb200_picture* pics, int n, CameraBatch& b)
     return CB200_OK;
 }
 
+int device_batch(const cb200_picture* d_pics, int n, const cb200_picture_bounds* bounds, CameraBatch& b)
+{
+    if (n < 0) return fail(CB200_ERR_ARG, "n < 0");
+    if (!d_pics) return fail(CB200_ERR_ARG, "null d_pics");
+    if (reinterpret_cast<uintptr_t>(d_pics) % 8) return fail(CB200_ERR_ARG, "d_pics is not 8-byte aligned");
+    if (!bounds) return fail(CB200_ERR_ARG, "null bounds");
+    const cb200_picture_bounds bd = *bounds;
+    const std::string is = " (bounds " + std::to_string(bd.min_short) + ", " + std::to_string(bd.max_short) + ", " + std::to_string(bd.max_long) + ")";
+    if (bd.min_short < 60) return fail(CB200_ERR_ARG, "min_short < 60: the scan's row step would be 0" + is);
+    if (bd.max_short > 4499) return fail(CB200_ERR_ARG, "max_short > 4499: a short side of 4500 or more needs a Gaussian beyond 9 taps" + is);
+    if (bd.min_short > bd.max_short) return fail(CB200_ERR_ARG, "min_short > max_short" + is);
+    if (bd.max_long < bd.max_short) return fail(CB200_ERR_ARG, "max_long < max_short" + is);
+    // the largest picture in either orientation: its blur tiles over n slots, and the scan rows of the smallest short side
+    const int64_t tiles = std::max(layout::blur_tiles(bd.max_long, bd.max_short), layout::blur_tiles(bd.max_short, bd.max_long));
+    if (tiles * n > 0x7FFFFFFFll) return fail(CB200_ERR_ARG, "n x the blur tiles of a max_long x max_short picture exceed 2^31 - 1" + is);
+    const int64_t skip = bd.min_short / 60, rows = 2 * ((bd.max_long + skip - 1) / skip) + 4;
+    if (rows > 0x7FFFFFFFll) return fail(CB200_ERR_ARG, "the scan rows of a max_long picture exceed 2^31 - 1" + is);
+    b.pics.clear(); b.wh.clear();
+    b.d_pics = d_pics; b.dev_n = n; b.bounds = bd;
+    b.packed = false; b.host = false;
+    return CB200_OK;
+}
+
 int check_spans(const CameraBatch& b)
 {
     const int64_t lim = (int64_t)1 << 32;
-    for (int i = 0; i < b.n(); ++i) {
+    for (int i = 0; i < (int)b.pics.size(); ++i) {      // (a device batch: none on the host, each launch checks its own)
         const cb200_picture& p = b.pics[(size_t)i];
         const bool planar = p.layout == CB200_LAYOUT_RGB_PLANAR;
         if (p.row_pitch >= lim || (planar && p.plane_pitch >= lim) ||
@@ -402,16 +450,13 @@ static int scan_rows(int w, int h)
     return 2 * ((h + skip - 1) / skip) + 4;
 }
 
-int scan_reserve(cb200_ctx* c, const int32_t* wh, int n)
+// a device batch: each slot's blurred picture at a fixed offset, slot x this many bytes (a multiple of 4)
+static size_t plan_slot_bytes(const cb200_picture_bounds& bd) { return ((size_t)bd.max_long * (size_t)bd.max_short + 3) & ~(size_t)3; }
+
+// the scan's buffers for n pictures of npx pixels in all, whose scans take at most rows_cap rows
+static int scan_reserve_for(cb200_ctx* c, int n, size_t npx, int rows_cap)
 {
     ScanScratch* s = sstate(c);
-    size_t npx = 0;
-    int rows_cap = 0;
-    for (int i = 0; i < n; ++i) {
-        npx += (size_t)wh[2 * i] * (size_t)wh[2 * i + 1];
-        const int rc = scan_rows(wh[2 * i], wh[2 * i + 1]);
-        if (rc > rows_cap) rows_cap = rc;
-    }
     int rc;
     if ((rc = grow(c, s->d_blur, npx, "blurred pictures")) || (rc = grow(c, s->d_hist, 256 * (size_t)n, "histograms")) ||
         (rc = grow(c, s->d_thr, (size_t)n, "thresholds")) || (rc = grow(c, s->d_anchors, 4 * (size_t)n, "anchors")) ||
@@ -426,6 +471,27 @@ int scan_reserve(cb200_ctx* c, const int32_t* wh, int n)
         return rc;
     s->ws_pics = (int)np; s->ws_rows_cap = (int)rows;
     return CB200_OK;
+}
+
+int scan_reserve(cb200_ctx* c, const int32_t* wh, int n)
+{
+    size_t npx = 0;
+    int rows_cap = 0;
+    for (int i = 0; i < n; ++i) {
+        npx += (size_t)wh[2 * i] * (size_t)wh[2 * i + 1];
+        const int rc = scan_rows(wh[2 * i], wh[2 * i + 1]);
+        if (rc > rows_cap) rows_cap = rc;
+    }
+    return scan_reserve_for(c, n, npx, rows_cap);
+}
+
+// a device batch: every accepted picture's scan takes at most the rows of a min_short x max_long one (device_batch checked that
+// they fit an int)
+int scan_reserve(cb200_ctx* c, const CameraBatch& b)
+{
+    if (!b.d_pics) return scan_reserve(c, b.wh.data(), b.n());
+    const cb200_picture_bounds& bd = b.bounds;
+    return scan_reserve_for(c, b.n(), (size_t)b.n() * plan_slot_bytes(bd), scan_rows(bd.min_short, bd.max_long));
 }
 
 // the launch geometry of the blur: per radius its pictures, their first entry in the order list, their tiles, one size or not
@@ -473,6 +539,94 @@ static int pic_table(const ScanScratch* s, const CameraBatch& b, uint8_t* table,
     return CB200_OK;
 }
 
+PlanTable::PlanTable(const CameraBatch& b)
+{
+    const size_t n = (size_t)b.n();
+    order = sizeof(PicDesc) * n;
+    groups = order + sizeof(int) * 3 * n;
+    of = groups + sizeof(int) * 6;
+    refused = of + sizeof(int32_t) * n;
+    standin = (refused + n + 15) & ~(size_t)15;
+    bytes = standin + 3 * (size_t)b.bounds.min_short + 16;
+}
+
+// A plan's picture table from the descriptors and the map of this launch (layout::plan_slot per slot; in a detect plan, the
+// candidates too: a slot with no candidate mode below n_modes is empty, receivers::plan_modes), in one CTA whatever n: chunks
+// of kPlanThreads slots, each numbered by a block scan of six sums (per radius group: slots, tiles) on top of the chunks before it.
+// So each group's list is in slot order and its tiles are numbered consecutively in that order, as pic_table numbers them
+constexpr int kPlanThreads = 1024;
+__global__ void __launch_bounds__(kPlanThreads)
+k_plan_pictures(int n, const cb200_picture* __restrict__ pics, const int32_t* __restrict__ receiver_of, int receivers,
+                const uint32_t* __restrict__ cand, int n_modes, cb200_picture_bounds bounds, uint64_t standin, uint64_t blur_base, uint64_t slot_bytes, PicDesc* __restrict__ desc, int* __restrict__ order,
+                int* __restrict__ counts, int32_t* __restrict__ of, uint8_t* __restrict__ refused)
+{
+    __shared__ int wsum[kPlanThreads / 32][6];
+    __shared__ int carry[6];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid < 6) carry[tid] = 0;
+    __syncthreads();
+    for (int base = 0; base < n; base += kPlanThreads) {
+        const int i = base + tid;
+        layout::PlanSlot ps = {-1, 0, false};
+        PicDesc d;
+        int32_t r = -1;
+        if (i < n) {
+            r = receiver_of[i];
+            const bool empty = receivers::plan_modes(cand ? cand[i] : ~0u, r, receivers, n_modes) == 0;
+            ps = layout::plan_slot(pics, empty, bounds, standin, blur_base, slot_bytes, i, d);
+        }
+        int v[6];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { v[k] = ps.group == k; v[3 + k] = ps.group == k ? ps.tiles : 0; }
+#pragma unroll
+        for (int k = 0; k < 6; ++k)
+            for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(~0u, v[k], o); if (lane >= o) v[k] += u; }
+        if (lane == 31)
+            for (int k = 0; k < 6; ++k) wsum[warp][k] = v[k];
+        __syncthreads();
+        if (warp == 0)
+            for (int k = 0; k < 6; ++k) {
+                int x = wsum[lane][k];
+                for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(~0u, x, o); if (lane >= o) x += u; }
+                wsum[lane][k] = x;
+            }
+        __syncthreads();
+        if (i < n) {
+            int at = 0, tile0 = 0;
+#pragma unroll
+            for (int k = 0; k < 3; ++k)
+                if (ps.group == k) {
+                    at = carry[k] + (warp ? wsum[warp - 1][k] : 0) + v[k] - 1;
+                    tile0 = carry[3 + k] + (warp ? wsum[warp - 1][3 + k] : 0) + v[3 + k] - ps.tiles;
+                }
+            d.tile0 = tile0;
+            desc[i] = d;
+            order[(size_t)ps.group * n + at] = i;
+            of[i] = ps.refused ? -1 : r;
+            refused[i] = ps.refused;
+        }
+        __syncthreads();
+        if (tid < 6) carry[tid] += wsum[kPlanThreads / 32 - 1][tid];
+        __syncthreads();
+    }
+    if (tid < 6) counts[tid] = carry[tid];
+}
+
+int plan_pictures_launch(cb200_ctx* c, const CameraBatch& b, const int32_t* d_receiver_of, int receivers, uint8_t* d_table,
+                         const uint32_t* d_cand, int n_modes)
+{
+    const PlanTable t(b);
+    const ScanScratch* s = sstate(c);
+    k_plan_pictures<<<1, kPlanThreads, 0, c->stream>>>(b.n(), b.d_pics, d_receiver_of, receivers, d_cand, n_modes, b.bounds, reinterpret_cast<uint64_t>(d_table + t.standin),
+                                                      reinterpret_cast<uint64_t>(s->d_blur.get()), plan_slot_bytes(b.bounds),
+                                                      reinterpret_cast<PicDesc*>(d_table), reinterpret_cast<int*>(d_table + t.order),
+                                                      reinterpret_cast<int*>(d_table + t.groups), reinterpret_cast<int32_t*>(d_table + t.of),
+                                                      d_table + t.refused);
+    count_launch();
+    CK(cudaGetLastError(), "plan pictures launch");
+    return CB200_OK;
+}
+
 int camera_pictures(cb200_ctx* c) { return sstate(c)->camera_n; }
 void set_camera_pictures(cb200_ctx* c, int n) { sstate(c)->camera_n = n; }
 
@@ -493,11 +647,13 @@ int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, cons
     ScanScratch* s = sstate(c);
     cudaStream_t st = c->stream;
     const int n = b.n();
-    int err = scan_reserve(c, b.wh.data(), n); if (err) return err;
+    int err = scan_reserve(c, b); if (err) return err;
     const size_t table_bytes = (sizeof(PicDesc) + sizeof(int)) * (size_t)n;
     BlurGroups g;
     const PicDesc* d_desc = d_table;
-    if (d_table) {
+    if (b.d_pics) {
+        // a plan over device descriptors: k_plan_pictures writes d_table at each launch, the host knows no sizes
+    } else if (d_table) {
         std::vector<uint8_t> table(table_bytes);
         err = pic_table(s, b, table.data(), g); if (err) return err;
     } else {
@@ -526,7 +682,31 @@ int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, cons
     // cb200_set_timing: one event set per scan -- [blur + histogram (all radii), Otsu, anchors] through cb200_get_timing
     begin_timed_call(c);
     mark(c);
-    for (int R = 1; R <= 4; ++R) {
+    if (b.d_pics) {
+        // one launch per radius group the bounds reach (short sides min_short .. max_short), persistent CTAs over the listed tiles
+        const PlanTable t(b);
+        const uint8_t* tb = reinterpret_cast<const uint8_t*>(d_table);
+        const int* d_ord = reinterpret_cast<const int*>(tb + t.order);
+        const int* d_counts = reinterpret_cast<const int*>(tb + t.groups);
+        const cb200_picture_bounds& bd = b.bounds;
+        const int64_t most = (int64_t)n * std::max(layout::blur_tiles(bd.max_long, bd.max_short), layout::blur_tiles(bd.max_short, bd.max_long));
+        const int g0 = layout::radius_group(layout::blur_radius(bd.min_short, bd.min_short));
+        const int g1 = layout::radius_group(layout::blur_radius(bd.max_short, bd.max_short));
+        for (int gi = g0; gi <= g1; ++gi) {
+            const int* ord = d_ord + (size_t)gi * n;
+            unsigned grid = 0;
+            switch (gi) {
+            case 0: if ((err = blur_list_grid<1>(c, most, &grid))) return err;
+                    k_scan_blur4_list<1><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, d_counts, gi, s->d_hist); break;
+            case 1: if ((err = blur_list_grid<2>(c, most, &grid))) return err;
+                    k_scan_blur4_list<2><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, d_counts, gi, s->d_hist); break;
+            default: if ((err = blur_list_grid<4>(c, most, &grid))) return err;
+                     k_scan_blur4_list<4><<<grid, kBlurThreads, 0, st>>>(s->d_blur, d_desc, ord, d_counts, gi, s->d_hist); break;
+            }
+            count_launch();
+        }
+    }
+    for (int R = 1; R <= 4 && !b.d_pics; ++R) {
         if (!count[R]) continue;
         const int uniform = same[R] ? (int)(tiles[R] / count[R]) : 0;
         const unsigned grid = (unsigned)tiles[R];
@@ -606,12 +786,25 @@ __global__ void k_mask_failed(const int32_t* __restrict__ status, int n, uint32_
 
 // k_mask_failed in a receivers plan: an empty slot (receiver -1 in the plan's map, of) yields no chunks either, and its status,
 // which k_extract wrote before, becomes CB200_EXTRACT_EMPTY
-__global__ void k_mask_failed_empty(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of)
+__device__ __forceinline__ void mask_failed_empty(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of,
+                                                  const uint8_t* __restrict__ refused)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    if (of[i] < 0) status[i] = CB200_EXTRACT_EMPTY;
+    if (of[i] < 0) status[i] = refused && refused[i] ? CB200_EXTRACT_REFUSED : CB200_EXTRACT_EMPTY;
     if (status[i] <= 0) mask[i] = 0;
+}
+
+__global__ void k_mask_failed_empty(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of)
+{
+    mask_failed_empty(status, n, mask, of, nullptr);
+}
+
+// the same in a plan over device descriptors: a slot whose descriptor the launch refused (k_plan_pictures) gets CB200_EXTRACT_REFUSED
+__global__ void k_mask_failed_refused(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of,
+                                      const uint8_t* __restrict__ refused)
+{
+    mask_failed_empty(status, n, mask, of, refused);
 }
 
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks)
@@ -626,6 +819,13 @@ int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool 
 }
 
 int camera_reserve(cb200_ctx* c, const int32_t* wh, int n) { return camera_reserve_for(c, wh, n, true, true); }
+
+int camera_reserve(cb200_ctx* c, const CameraBatch& b)
+{
+    if (!b.d_pics) return camera_reserve(c, b.wh.data(), b.n());
+    const int rc = camera_reserve_for(c, nullptr, b.n(), false, true);
+    return rc ? rc : scan_reserve(c, b);
+}
 
 int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
                       bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status, Receivers* recv,
@@ -646,7 +846,9 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     if (deskew) { rc = deskew_launch(c, b, s->d_minv, d_desc, frames); if (rc) return rc; }
     rc = decode_chunks(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, d_chunks, d_mask, d_frame_flags, d_sharp, true, recv);
     if (rc) return rc;
-    if (recv && recv->empty_slots) k_mask_failed_empty<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv->d_map);
+    if (recv && recv->d_refused)
+        k_mask_failed_refused<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv->d_map, recv->d_refused);
+    else if (recv && recv->empty_slots) k_mask_failed_empty<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv->d_map);
     else k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
     count_launch();
     CK(cudaGetLastError(), "mask launch");
@@ -659,7 +861,7 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
 int camera_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags,
                    int32_t* d_status, const PicDesc* d_table, Receivers* recv)
 {
-    int rc = camera_reserve(c, b.wh.data(), b.n()); if (rc) return rc;
+    int rc = camera_reserve(c, b); if (rc) return rc;
     uint8_t* frames;
     rc = deskew_frames(c, b.n(), &frames); if (rc) return rc;
     const PicDesc* d_desc;
