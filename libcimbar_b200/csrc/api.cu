@@ -521,9 +521,9 @@ int receivers_ccm(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, con
     if (flags & CB200_FLAG_CC_SIMPLE) {
         CK(ccm_simple_launch(c->mode, d_rgb, n, c->d_ccm, c->stream), "ccm launch");
         CK(cudaMemsetAsync(c->d_ccm_active, 1, (size_t)n, c->stream), "set ccm flags");
-        CK(receivers_keep_launch(n, d_of, d_of + n, c->d_ccm, r.d_states, c->stream, r.empty_slots), "receivers keep launch");
+        CK(receivers_keep_launch(n, d_of, d_of + n, c->d_ccm, r.d_states, c->stream), "receivers keep launch");
     } else {
-        CK(receivers_gather_launch(n, d_of, r.d_states, c->d_ccm, c->d_ccm_active, c->stream, r.empty_slots), "receivers gather launch");
+        CK(receivers_gather_launch(n, d_of, r.d_states, c->d_ccm, c->d_ccm_active, c->stream), "receivers gather launch");
     }
     memset(&cc, 0, sizeof(cc));
     cc.per_frame = c->d_ccm; cc.active = 1;
@@ -854,7 +854,7 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
         // across ranks: this stripe's fits out, the CCM entering the stripe in (from the lower ranks' fits of the same step)
         if (chained) { rc = chain_publish_link(c, n, c->d_fit, c->d_fit_valid, initial, &initial); if (rc) return rc; }
         if (recv) CK(ccm_carry_receivers_launch(n, recv->d_map, recv->d_map + n, c->d_fit, c->d_fit_valid, recv->d_states, c->d_ccm,
-                                                c->d_ccm_active, c->stream, recv->empty_slots), "ccm carry");
+                                                c->d_ccm_active, c->stream), "ccm carry");
         else CK(ccm_carry_launch(n, c->d_fit, c->d_fit_valid, initial, c->d_ccm, c->d_ccm_active, c->stream), "ccm carry");
         CK(ccm_apply_launch(m, c->d_means, n, c->d_ccm, c->d_ccm_active, c->d_cellvals, c->stream), "ccm apply");
         c->ccm_frames = n;

@@ -371,13 +371,11 @@ k_ccm_carry(int n_frames, const float* __restrict__ fit, const uint8_t* __restri
 // k_ccm_carry for a batch of several receivers: the same two-level max scan, over the receiver-major order and with the segment
 // starts scanned alongside (receivers_core.cuh), so each picture takes its own receiver's last fit or entry state.  used and
 // used_active are written in batch order; each receiver's last picture writes its exit state, after every entry state is read.
-// kEmpty (a receivers plan's map): slots of receiver -1 are empty, the last run of the order; they read and write no state and
-// decode without a CCM
-template <bool kEmpty>
-__device__ __forceinline__ void ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order,
-                                                    const float* __restrict__ fit, const uint8_t* __restrict__ valid,
-                                                    cb200_receiver_state* __restrict__ states, float* __restrict__ used,
-                                                    uint8_t* __restrict__ used_active)
+// Slots of receiver -1 are empty, the last run of the order; they read and write no state and decode without a CCM
+__global__ void __launch_bounds__(1024)
+k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ fit,
+                      const uint8_t* __restrict__ valid, cb200_receiver_state* __restrict__ states, float* __restrict__ used,
+                      uint8_t* __restrict__ used_active)
 {
     __shared__ int seg_fit[1024], seg_start[1024];
     const int t = threadIdx.x;
@@ -395,7 +393,7 @@ __device__ __forceinline__ void ccm_carry_receivers(int n_frames, const int32_t*
     c = t > 0 ? receivers::Carry{seg_fit[t - 1], seg_start[t - 1]} : receivers::Carry{-1, 0};
     for (int j = j0; j < j1; ++j) {
         const int f = order[j], g = receivers::step(of, order, valid, j, c);
-        if (kEmpty && of[f] < 0) {
+        if (of[f] < 0) {
             for (int i = 0; i < 9; ++i) used[(size_t)f * 9 + i] = 0.0f;
             used_active[f] = 0;
             continue;
@@ -408,39 +406,22 @@ __device__ __forceinline__ void ccm_carry_receivers(int n_frames, const int32_t*
     for (int j = j0; j < j1; ++j) {
         if (!receivers::closes(of, order, n_frames, j)) continue;
         const int f = order[j];
-        if (kEmpty && of[f] < 0) continue;
+        if (of[f] < 0) continue;
         cb200_receiver_state& x = states[of[f]];
         for (int i = 0; i < 9; ++i) x.ccm[i] = used[(size_t)f * 9 + i];
         x.active = used_active[f];
     }
 }
 
-__global__ void __launch_bounds__(1024)
-k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ fit,
-                      const uint8_t* __restrict__ valid, cb200_receiver_state* __restrict__ states, float* __restrict__ used,
-                      uint8_t* __restrict__ used_active)
-{
-    ccm_carry_receivers<false>(n_frames, of, order, fit, valid, states, used, used_active);
-}
-
-__global__ void __launch_bounds__(1024)
-k_ccm_carry_receivers_empty(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ fit,
-                            const uint8_t* __restrict__ valid, cb200_receiver_state* __restrict__ states, float* __restrict__ used,
-                            uint8_t* __restrict__ used_active)
-{
-    ccm_carry_receivers<true>(n_frames, of, order, fit, valid, states, used, used_active);
-}
-
 // without a CC flag every picture decodes with its receiver's matrix.  An inactive receiver's pictures get the identity: the colour
 // decision on integer means through the identity is exactly the decision without a CCM (see k_ccm_apply), so one K1 instantiation
-// serves the whole batch.  kEmpty: an empty slot (receiver -1) gets the identity too
-template <bool kEmpty>
-__device__ __forceinline__ void receivers_gather(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
-                                                 float* __restrict__ ccm, uint8_t* __restrict__ active)
+// serves the whole batch.  An empty slot (receiver -1) gets the identity too
+__global__ void k_receivers_gather(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
+                                   float* __restrict__ ccm, uint8_t* __restrict__ active)
 {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_frames) return;
-    if (kEmpty && of[f] < 0) {
+    if (of[f] < 0) {
         for (int i = 0; i < 9; ++i) ccm[(size_t)f * 9 + i] = i % 4 == 0 ? 1.0f : 0.0f;
         active[f] = 0;
         return;
@@ -451,42 +432,17 @@ __device__ __forceinline__ void receivers_gather(int n_frames, const int32_t* __
     active[f] = a ? 1 : 0;
 }
 
-__global__ void k_receivers_gather(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
-                                   float* __restrict__ ccm, uint8_t* __restrict__ active)
-{
-    receivers_gather<false>(n_frames, of, states, ccm, active);
-}
-
-__global__ void k_receivers_gather_empty(int n_frames, const int32_t* __restrict__ of, const cb200_receiver_state* __restrict__ states,
-                                         float* __restrict__ ccm, uint8_t* __restrict__ active)
-{
-    receivers_gather<true>(n_frames, of, states, ccm, active);
-}
-
-// CC_SIMPLE: each receiver keeps the matrix of its last picture (kEmpty: the run of empty slots keeps nothing)
-template <bool kEmpty>
-__device__ __forceinline__ void receivers_keep(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order,
-                                               const float* __restrict__ ccm, cb200_receiver_state* __restrict__ states)
+// CC_SIMPLE: each receiver keeps the matrix of its last picture (the run of empty slots keeps nothing)
+__global__ void k_receivers_keep(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ ccm,
+                                 cb200_receiver_state* __restrict__ states)
 {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n_frames || !receivers::closes(of, order, n_frames, j)) return;
     const int f = order[j];
-    if (kEmpty && of[f] < 0) return;
+    if (of[f] < 0) return;
     cb200_receiver_state& x = states[of[f]];
     for (int i = 0; i < 9; ++i) x.ccm[i] = ccm[(size_t)f * 9 + i];
     x.active = 1;
-}
-
-__global__ void k_receivers_keep(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ ccm,
-                                 cb200_receiver_state* __restrict__ states)
-{
-    receivers_keep<false>(n_frames, of, order, ccm, states);
-}
-
-__global__ void k_receivers_keep_empty(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order,
-                                       const float* __restrict__ ccm, cb200_receiver_state* __restrict__ states)
-{
-    receivers_keep<true>(n_frames, of, order, ccm, states);
 }
 
 // a receivers plan's map from the receiver indices the caller wrote for this launch (receivers_core.cuh): of[i] = slot i's
@@ -572,27 +528,21 @@ cudaError_t ccm_apply_launch(const Mode& m, const uint32_t* d_means, int n_frame
     return cudaGetLastError();
 }
 cudaError_t ccm_carry_receivers_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_fit, const uint8_t* d_valid,
-                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st, bool empty_slots)
+                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st)
 {
-    if (empty_slots) k_ccm_carry_receivers_empty<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active);
-    else k_ccm_carry_receivers<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active);
-    count_launch();
+    k_ccm_carry_receivers<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active); count_launch();
     return cudaGetLastError();
 }
 cudaError_t receivers_gather_launch(int n_frames, const int32_t* d_of, const cb200_receiver_state* d_states, float* d_ccm, uint8_t* d_active,
-                                    cudaStream_t st, bool empty_slots)
+                                    cudaStream_t st)
 {
-    if (empty_slots) k_receivers_gather_empty<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_states, d_ccm, d_active);
-    else k_receivers_gather<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_states, d_ccm, d_active);
-    count_launch();
+    k_receivers_gather<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_states, d_ccm, d_active); count_launch();
     return cudaGetLastError();
 }
 cudaError_t receivers_keep_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_ccm, cb200_receiver_state* d_states,
-                                  cudaStream_t st, bool empty_slots)
+                                  cudaStream_t st)
 {
-    if (empty_slots) k_receivers_keep_empty<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_order, d_ccm, d_states);
-    else k_receivers_keep<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_order, d_ccm, d_states);
-    count_launch();
+    k_receivers_keep<<<(n_frames + 127) / 128, 128, 0, st>>>(n_frames, d_of, d_order, d_ccm, d_states); count_launch();
     return cudaGetLastError();
 }
 cudaError_t receivers_order_launch(int n, const int32_t* d_receiver_of, int receivers, int32_t* d_map, cudaStream_t st)

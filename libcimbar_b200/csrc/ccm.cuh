@@ -86,15 +86,14 @@ cudaError_t ccm_apply_launch(const Mode& m, const uint32_t* d_means, int n_frame
 // d_order = the stable receiver-major order, d_states = the receivers' states.  ccm_carry_receivers_launch: the CC_FIT carry of each
 // receiver over its own pictures, from its entry state, its exit state written back by its last picture.  receivers_gather_launch:
 // each picture's receiver matrix into d_ccm / d_active.  receivers_keep_launch: the matrix d_ccm holds for each receiver's last
-// picture into its state, active.  empty_slots (a receivers plan's map, built by receivers_order_launch): d_of may hold -1, an
-// empty slot, which reads and writes no state and decodes without a CCM
+// picture into its state, active.  Receiver -1 in d_of (a receivers plan's map, built by receivers_order_launch, or a mode's map
+// in a detect receivers call) is an empty slot, which reads and writes no state and decodes without a CCM
 cudaError_t ccm_carry_receivers_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_fit, const uint8_t* d_valid,
-                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st,
-                                       bool empty_slots = false);
+                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st);
 cudaError_t receivers_gather_launch(int n_frames, const int32_t* d_of, const cb200_receiver_state* d_states, float* d_ccm, uint8_t* d_active,
-                                    cudaStream_t st, bool empty_slots = false);
+                                    cudaStream_t st);
 cudaError_t receivers_keep_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_ccm, cb200_receiver_state* d_states,
-                                  cudaStream_t st, bool empty_slots = false);
+                                  cudaStream_t st);
 // a receivers plan's map of n slots into d_map (2 n int32): each slot's receiver from d_receiver_of, -1 where it lies outside
 // [0, receivers), then the receiver-major order with the empty slots last (receivers_core.cuh).  One kernel
 cudaError_t receivers_order_launch(int n, const int32_t* d_receiver_of, int receivers, int32_t* d_map, cudaStream_t st);

@@ -195,8 +195,9 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
 // Receivers(...) then builds `map` on the host: the n receiver indices, then the receiver-major order (receivers_core.cuh); d_map is
 // its device copy once uploaded (the camera calls: behind the picture table; the frame call: in cb200_ctx::d_recv).
 // A receivers camera plan reads its map on the device: check_receivers with on_device checks the pointer (null, 4-byte alignment)
-// instead of the indices, and Receivers(d_map, states) has no host map -- d_map is the plan's, built by k_receivers_order at each
-// launch, where receiver -1 marks an empty slot (empty_slots: the kernels' variants that skip those)
+// instead of the indices.  Receivers(d_map, states) has no host map: d_map is a device map already, the plan's (built by
+// k_receivers_order at each launch) or a detect call's mode's.  In every map receiver -1 marks an empty slot, which reads and
+// writes no state, gets mask 0 and status CB200_EXTRACT_EMPTY
 int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states,
                     bool on_device = false);
 // d_refused: NULL, or (a plan over device descriptors) one byte per slot, set where the launch refused the slot's descriptor: its
@@ -205,10 +206,9 @@ struct Receivers {
     std::vector<int32_t> map;
     const int32_t* d_map = nullptr;
     cb200_receiver_state* d_states = nullptr;
-    bool empty_slots = false;
     const uint8_t* d_refused = nullptr;
     Receivers(const int32_t* receiver_of, int n, int n_receivers, cb200_receiver_state* states);
-    Receivers(const int32_t* d_plan_map, cb200_receiver_state* states) : d_map(d_plan_map), d_states(states), empty_slots(true) {}
+    Receivers(const int32_t* d_map_, cb200_receiver_state* states) : d_map(d_map_), d_states(states) {}
     size_t bytes() const { return map.size() * sizeof(int32_t); }
 };
 // a camera plan's own rules, checked after its batch's: n > 0, a non-null `out` (set to NULL) (plan.cu)

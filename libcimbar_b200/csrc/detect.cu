@@ -15,7 +15,8 @@
 // cb200_detect_scan_extract_decode_chunks_receivers_dev adds receivers (a decode service's sessions): picture i is decoded only
 // under its candidate modes, each mode keeps one state table of receivers, and each geometry extracts, deskews and walks only the
 // pictures some of its modes decode (receivers_core.cuh: detect_lists).  A mode's other pictures of that sub-batch are empty slots,
-// as in a receivers plan: decoded, masked, reading and writing no state.  k_detect_select_at joins the results.
+// as in a receivers plan: decoded, masked, reading and writing no state.  k_detect_select joins the results at each picture's
+// position in the sub-batches.
 //
 // A detect receivers plan (cb200_camera_plan_create_detect_receivers, plan.cu) captures the same geometry loop once over n fixed
 // slots.  Its candidates and map are read at each launch, so it has no sub-batches: every geometry works on all n slots, slot i is
@@ -56,39 +57,20 @@ struct DetectArgs {
     const int32_t* status[kDetectModes];
 };
 
-// one CTA per picture: the first mode with a chunk, its record, mask and status
+// one CTA per picture: the first mode with a chunk, its record, mask and status.  at: NULL (mode k decoded picture i at position i),
+// or (a detect receivers call or plan) mode k decoded picture i at position at[k * n + i] of its geometry's sub-batch, or not at all
+// (-1: its mask there counts as 0).  The status of a picture no mode took is its first candidate's; a detect receivers plan's empty
+// slot, which has no candidate, gets CB200_EXTRACT_EMPTY (and mode -1, mask 0, a zeroed record).  refused: NULL, or (a plan over
+// device descriptors) one byte per slot, set where the launch refused the slot's descriptor: that slot, empty otherwise, reports
+// CB200_EXTRACT_REFUSED
 __global__ void __launch_bounds__(256)
-k_detect_select(const DetectArgs a, uint8_t* __restrict__ chunks, uint32_t* __restrict__ mask, int32_t* __restrict__ status,
-                int32_t* __restrict__ mode, uint32_t* __restrict__ mode_masks)
-{
-    const int i = blockIdx.x;
-    int sel = -1;
-    for (int k = 0; k < a.n_modes; ++k)
-        if (sel < 0 && a.mask[k][i] != 0) sel = k;
-    if (threadIdx.x == 0) {
-        mode[i] = sel;
-        mask[i] = sel < 0 ? 0u : a.mask[sel][i];
-        status[i] = a.status[sel < 0 ? 0 : sel][i];
-        if (mode_masks)
-            for (int k = 0; k < a.n_modes; ++k) mode_masks[(size_t)i * a.n_modes + k] = a.mask[k][i];
-    }
-    const int have = sel < 0 ? 0 : a.data_bytes[sel];
-    const uint8_t* src = sel < 0 ? nullptr : a.data[sel] + (size_t)i * have;
-    uint8_t* dst = chunks + (size_t)i * a.slot;
-    for (int b = threadIdx.x; b < a.slot; b += blockDim.x) dst[b] = b < have ? src[b] : 0;
-}
-
-// k_detect_select of a detect receivers call: mode k decoded picture i at position at[k * n + i] of its geometry's sub-batch, or not at
-// all (-1: its mask there counts as 0).  The status of a picture no mode took is its first candidate's; a detect receivers plan's
-// empty slot, which has no candidate, gets CB200_EXTRACT_EMPTY (and mode -1, mask 0, a zeroed record)
-__global__ void __launch_bounds__(256)
-k_detect_select_at(const DetectArgs a, const int32_t* __restrict__ at, int n, uint8_t* __restrict__ chunks, uint32_t* __restrict__ mask,
-                   int32_t* __restrict__ status, int32_t* __restrict__ mode, uint32_t* __restrict__ mode_masks)
+k_detect_select(const DetectArgs a, const int32_t* __restrict__ at, const uint8_t* __restrict__ refused, int n, uint8_t* __restrict__ chunks,
+                uint32_t* __restrict__ mask, int32_t* __restrict__ status, int32_t* __restrict__ mode, uint32_t* __restrict__ mode_masks)
 {
     const int i = blockIdx.x;
     int sel = -1, first = -1, p_sel = 0, p_first = 0;
     for (int k = 0; k < a.n_modes; ++k) {
-        const int p = at[(size_t)k * n + i];
+        const int p = at ? at[(size_t)k * n + i] : i;
         if (p < 0) continue;
         if (first < 0) { first = k; p_first = p; }
         if (sel < 0 && a.mask[k][p] != 0) { sel = k; p_sel = p; }
@@ -96,10 +78,10 @@ k_detect_select_at(const DetectArgs a, const int32_t* __restrict__ at, int n, ui
     if (threadIdx.x == 0) {
         mode[i] = sel;
         mask[i] = sel < 0 ? 0u : a.mask[sel][p_sel];
-        status[i] = sel >= 0 ? a.status[sel][p_sel] : first >= 0 ? a.status[first][p_first] : CB200_EXTRACT_EMPTY;
+        status[i] = refused && refused[i] ? CB200_EXTRACT_REFUSED : sel >= 0 ? a.status[sel][p_sel] : first >= 0 ? a.status[first][p_first] : CB200_EXTRACT_EMPTY;
         if (mode_masks)
             for (int k = 0; k < a.n_modes; ++k) {
-                const int p = at[(size_t)k * n + i];
+                const int p = at ? at[(size_t)k * n + i] : i;
                 mode_masks[(size_t)i * a.n_modes + k] = p < 0 ? 0u : a.mask[k][p];
             }
     }
@@ -107,14 +89,6 @@ k_detect_select_at(const DetectArgs a, const int32_t* __restrict__ at, int n, ui
     const uint8_t* src = sel < 0 ? nullptr : a.data[sel] + (size_t)p_sel * have;
     uint8_t* dst = chunks + (size_t)i * a.slot;
     for (int b = threadIdx.x; b < a.slot; b += blockDim.x) dst[b] = b < have ? src[b] : 0;
-}
-
-// a detect receivers plan over device descriptors: a slot whose descriptor the launch refused (k_plan_pictures) reports
-// CB200_EXTRACT_REFUSED; k_detect_select_at has given it what an empty slot gets otherwise
-__global__ void k_status_refused(const uint8_t* __restrict__ refused, int n, int32_t* __restrict__ status)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && refused[i]) status[i] = CB200_EXTRACT_REFUSED;
 }
 
 // a detect receivers plan's lists at one launch, one thread per slot (receivers_core.cuh: plan_slot): every mode's raw receivers
@@ -366,19 +340,11 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
             if (group[k] != g || !decodes(k)) continue;
             cb200_ctx* c = ctxs[k];
             StreamSwap on(c, live > 1 ? ds->side[g] : main, &sw);
-            if (dp) {                        // a slot mode k does not decode is an empty slot of its map
-                Receivers r(plan_map(*dp, n_modes, n, k), dp->d_states[k]);
-                rc = camera_after_scan(c, c0, b, d_desc, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr, ds->status + (size_t)k * n, &r);
-                continue;
-            }
-            if (!dr) {
-                rc = camera_after_scan(c, c0, b, d_desc, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr, ds->status + (size_t)k * n);
-                continue;
-            }
-            Receivers r(reinterpret_cast<const int32_t*>(d_tail + map_at[k]), dr->d_states[k]);
-            r.empty_slots = lists.count[k] < batch(g).n();       // without empty slots, the direct receivers call's kernels
+            // a plan or a receivers call decodes under mode k's map, in which a slot the mode does not decode is empty
+            const int32_t* map_k = dp ? plan_map(*dp, n_modes, n, k) : dr ? reinterpret_cast<const int32_t*>(d_tail + map_at[k]) : nullptr;
+            Receivers r(map_k, dp ? dp->d_states[k] : dr ? dr->d_states[k] : nullptr);
             rc = camera_after_scan(c, c0, batch(g), desc_g, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr, ds->status + (size_t)k * n,
-                                   &r, slots_g);
+                                   map_k ? &r : nullptr, slots_g);
         }
     }
     if (live > 1) {
@@ -397,17 +363,10 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
         a.data[k] = c->d_data; a.data_bytes[k] = c->mode.data_bytes; a.mask[k] = c->d_mask; a.status[k] = ds->status + (size_t)k * n;
         if (a.data_bytes[k] > a.slot) a.slot = a.data_bytes[k];
     }
-    if (dr || dp) {
-        const int32_t* at = dp ? plan_at(*dp, n_modes, n) : reinterpret_cast<const int32_t*>(d_tail + pos_at);
-        k_detect_select_at<<<n, 256, 0, main>>>(a, at, n, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
-    } else k_detect_select<<<n, 256, 0, main>>>(a, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
+    const int32_t* at = dp ? plan_at(*dp, n_modes, n) : dr ? reinterpret_cast<const int32_t*>(d_tail + pos_at) : nullptr;
+    k_detect_select<<<n, 256, 0, main>>>(a, at, d_refused, n, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
     count_launch();
     CK(cudaGetLastError(), "detect select launch");
-    if (d_refused) {                         // k_detect_select_at made them empty slots: mode -1, mask 0, zeros
-        k_status_refused<<<(n + 127) / 128, 128, 0, main>>>(d_refused, n, d_extract_status);
-        count_launch();
-        CK(cudaGetLastError(), "refused status launch");
-    }
     return CB200_OK;
 }
 

@@ -24,7 +24,7 @@
 // (k_detect_plan_lists at the head of the graph builds every list into d_map and d_present).  It is registered in the plans of every
 // one of its contexts, so each of them freezes the buffers the graph uses, and destroying any of them destroys the plan.  Over device
 // descriptors (cb200_camera_plan_create_detect_receivers_pictures_dev), k_plan_pictures comes first and k_detect_plan_lists reads its
-// map, and k_status_refused marks the refused slots after the selection.
+// map, and the selection gives the refused slots their status.
 #include "ctx.cuh"
 
 #include <memory>
@@ -202,12 +202,19 @@ int make_plan(cb200_camera_plan* plan, const CameraBatch& b, Reserve&& reserve, 
     return CB200_OK;
 }
 
-// a plain or receivers plan on context c (recv: the bound map and states; its d_map is allocated here)
+// a plain or receivers plan on context c (recv: the bound map and states; its d_map is allocated here) over the batch `build`
+// makes: the direct camera call's checks, with the plan's own after the batch's and after the CCM chain's, then the plan
 struct PlanReceivers { const int32_t* d_receiver_of; int n_receivers; cb200_receiver_state* d_states; };
 
-int make_camera_plan(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+template <class Build>
+int make_camera_plan(cb200_ctx* c, Build&& build, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
                      int32_t* d_extract_status, const PlanReceivers* recv, cb200_camera_plan** out)
 {
+    auto plan_build = [&](CameraBatch& b) { const int rc = build(b); return rc ? rc : plan_rules(b.n(), out); };
+    CameraBatch b;
+    int rc = check_camera_call(c, flags, plan_build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
+    if (check_host_ccm(c))
+        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
     const int n = b.n();
     cb200_camera_plan* p = new cb200_camera_plan();
     p->ctx = c; p->ctxs.assign(1, c); p->n = n; p->flags = flags;
@@ -269,13 +276,9 @@ extern "C" {
 int cb200_camera_plan_create(cb200_ctx* c, const int32_t* wh, int n, uint32_t flags, const uint8_t* d_pictures, uint8_t* d_chunks,
                              uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out)
 {
-    // the checks of cb200_scan_extract_decode_chunks_ragged_dev, with the plan's own after the batch's and after the CCM chain's
-    auto build = [&](CameraBatch& b) { const int rc = packed_batch(d_pictures, wh, n, b); return rc ? rc : plan_rules(n, out); };
-    CameraBatch b;
-    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
-    if (check_host_ccm(c))
-        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
-    return make_camera_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, out);
+    // the checks of cb200_scan_extract_decode_chunks_ragged_dev, then the plan's own
+    auto build = [&](CameraBatch& b) { return packed_batch(d_pictures, wh, n, b); };
+    return make_camera_plan(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, out);
 }
 
 int cb200_camera_plan_create_receivers(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, const int32_t* d_receiver_of,
@@ -285,13 +288,9 @@ int cb200_camera_plan_create_receivers(cb200_ctx* c, const cb200_picture* pics, 
     // the checks of cb200_scan_extract_decode_chunks_receivers_dev (the map's pointer in place of its indices, which only a launch
     // reads), then the plan's own as cb200_camera_plan_create makes them
     int rc = check_receivers(c, d_receiver_of, n, n_receivers, d_states, true); if (rc) return rc;
-    auto build = [&](CameraBatch& b) { const int rc = picture_batch(pics, n, b); return rc ? rc : plan_rules(n, out); };
-    CameraBatch b;
-    rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
-    if (check_host_ccm(c))
-        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
+    auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
     const PlanReceivers recv = {d_receiver_of, n_receivers, d_states};
-    return make_camera_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
+    return make_camera_plan(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
 }
 
 int cb200_camera_plan_create_receivers_pictures_dev(cb200_ctx* c, const cb200_picture* d_pics, int n, const cb200_picture_bounds* bounds,
@@ -302,13 +301,9 @@ int cb200_camera_plan_create_receivers_pictures_dev(cb200_ctx* c, const cb200_pi
     // cb200_camera_plan_create_receivers' checks, with the descriptors' pointer and bounds in place of their contents (which each
     // launch checks on the device)
     int rc = check_receivers(c, d_receiver_of, n, n_receivers, d_states, true); if (rc) return rc;
-    auto build = [&](CameraBatch& b) { const int rc = device_batch(d_pics, n, bounds, b); return rc ? rc : plan_rules(n, out); };
-    CameraBatch b;
-    rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output"); if (rc) return rc;
-    if (check_host_ccm(c))
-        return fail(CB200_ERR_ARG, "the context is linked to a CCM chain, whose step the host sets per call: no camera plan");
+    auto build = [&](CameraBatch& b) { return device_batch(d_pics, n, bounds, b); };
     const PlanReceivers recv = {d_receiver_of, n_receivers, d_states};
-    return make_camera_plan(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
+    return make_camera_plan(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
 }
 
 int cb200_camera_plan_create_detect_receivers(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags,

@@ -777,34 +777,16 @@ __global__ void k_extract(const int4* __restrict__ anchors, const int* __restric
     if (sharpen) sharpen[i] = st == 2;             // CB200_FLAG_SHARPEN_IF_NEEDED: the CLI sharpens exactly the NEEDS_SHARPEN pictures
 }
 
-// a picture that failed extraction yields no chunks
-__global__ void k_mask_failed(const int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && status[i] <= 0) mask[i] = 0;
-}
-
-// k_mask_failed in a receivers plan: an empty slot (receiver -1 in the plan's map, of) yields no chunks either, and its status,
-// which k_extract wrote before, becomes CB200_EXTRACT_EMPTY
-__device__ __forceinline__ void mask_failed_empty(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of,
-                                                  const uint8_t* __restrict__ refused)
+// a picture that failed extraction yields no chunks.  of: NULL, or the receivers map, where an empty slot (receiver -1) yields no
+// chunks either and its status, which k_extract wrote before, becomes CB200_EXTRACT_EMPTY -- CB200_EXTRACT_REFUSED where refused
+// (NULL, or a plan over device descriptors: k_plan_pictures refused the slot's descriptor) is set
+__global__ void k_mask_failed(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of,
+                              const uint8_t* __restrict__ refused)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    if (of[i] < 0) status[i] = refused && refused[i] ? CB200_EXTRACT_REFUSED : CB200_EXTRACT_EMPTY;
+    if (of && of[i] < 0) status[i] = refused && refused[i] ? CB200_EXTRACT_REFUSED : CB200_EXTRACT_EMPTY;
     if (status[i] <= 0) mask[i] = 0;
-}
-
-__global__ void k_mask_failed_empty(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of)
-{
-    mask_failed_empty(status, n, mask, of, nullptr);
-}
-
-// the same in a plan over device descriptors: a slot whose descriptor the launch refused (k_plan_pictures) gets CB200_EXTRACT_REFUSED
-__global__ void k_mask_failed_refused(int32_t* __restrict__ status, int n, uint32_t* __restrict__ mask, const int32_t* __restrict__ of,
-                                      const uint8_t* __restrict__ refused)
-{
-    mask_failed_empty(status, n, mask, of, refused);
 }
 
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks)
@@ -846,10 +828,7 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     if (deskew) { rc = deskew_launch(c, b, s->d_minv, d_desc, frames); if (rc) return rc; }
     rc = decode_chunks(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, d_chunks, d_mask, d_frame_flags, d_sharp, true, recv);
     if (rc) return rc;
-    if (recv && recv->d_refused)
-        k_mask_failed_refused<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv->d_map, recv->d_refused);
-    else if (recv && recv->empty_slots) k_mask_failed_empty<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv->d_map);
-    else k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask);
+    k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv ? recv->d_map : nullptr, recv ? recv->d_refused : nullptr);
     count_launch();
     CK(cudaGetLastError(), "mask launch");
     return CB200_OK;
