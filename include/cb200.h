@@ -411,6 +411,40 @@ int cb200_camera_plan_create_receivers_pictures_dev(cb200_ctx* ctx, const cb200_
                                                     uint32_t flags, const int32_t* d_receiver_of, int n_receivers,
                                                     cb200_receiver_state* d_states, uint8_t* d_chunks, uint32_t* d_chunk_mask,
                                                     uint8_t* d_frame_flags, int32_t* d_extract_status, cb200_camera_plan** out);
+/* ---- per-receiver decode flags: each receiver's sharpen policy and colour correction from a device table -----------------------
+
+   A decode service whose sessions differ in their settings (the web receiver sharpens every picture with CC_FIT, the CLI guesses
+   sharpening, CB200_FLAG_SHARPEN_IF_NEEDED, with any colour correction) decodes them in one batch with a receiver flags table:
+   d_receiver_flags, n_receivers uint32 words in DEVICE memory, 4-byte aligned, read in stream order by the direct call and when each
+   launch runs by the plan (it is bound at create, so a session changes its settings between launches by writing its own word).
+   Word r holds receiver r's per-receiver bits: at most one of CB200_FLAG_SHARPEN / CB200_FLAG_SHARPEN_IF_NEEDED and at most one of
+   CB200_FLAG_CC_SIMPLE / CB200_FLAG_CC_FIT.  The call's own flags keep every other bit (CB200_FLAG_NO_INTERLEAVE, NO_FALLBACK) and
+   may hold none of those four.
+     valid word: receiver r's pictures get, bit for bit, what the mirrored call gives on r's pictures alone, in batch order, with
+             flags | d_receiver_flags[r]: records, masks, frame flags, extract statuses, cb200_camera_transforms,
+             cb200_get_frame_ccms, and d_states[r] afterwards.
+     invalid word (any other bit, or both bits of one pair): r's pictures get status CB200_EXTRACT_REFUSED, mask 0 and a zeroed
+             record; d_states[r] is neither read nor written.
+   Everything else is as for the mirrored function: empty slots in the plan, receivers without a picture, the context's CCM.  Every
+   picture takes the fitted-CCM route (mean colours, then the colour decision per picture with its receiver's matrix), so a uniform
+   table costs about one CC_FIT call.
+   CB200_ERR_ARG, before any CUDA call, naming the cause: a null d_receiver_flags or one not 4-byte aligned; a per-receiver bit in
+   flags; then everything the mirrored function refuses, in its order.
+   cb200_scan_extract_decode_chunks_receivers_flags_dev mirrors cb200_scan_extract_decode_chunks_receivers_dev;
+   cb200_camera_plan_create_receivers_pictures_flags_dev mirrors cb200_camera_plan_create_receivers_pictures_dev;
+   cb200_detect_scan_extract_decode_chunks_receivers_flags_dev mirrors cb200_detect_scan_extract_decode_chunks_receivers_dev, and
+   cb200_camera_plan_create_detect_receivers_pictures_flags_dev mirrors cb200_camera_plan_create_detect_receivers_pictures_dev (below):
+   one table serves every candidate mode, and for a valid word the contract also covers modes, mode masks and every mode's table.  A
+   refused receiver's pictures also get mode -1 and a zeroed mode-mask row, and no mode's table is read or written for it. */
+int cb200_scan_extract_decode_chunks_receivers_flags_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags,
+                                                         const int32_t* receiver_of, int n_receivers, cb200_receiver_state* d_states,
+                                                         const uint32_t* d_receiver_flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                                         uint8_t* d_frame_flags, int32_t* d_extract_status);
+int cb200_camera_plan_create_receivers_pictures_flags_dev(cb200_ctx* ctx, const cb200_picture* d_pics, int n, const cb200_picture_bounds* bounds,
+                                                          uint32_t flags, const int32_t* d_receiver_of, int n_receivers,
+                                                          cb200_receiver_state* d_states, const uint32_t* d_receiver_flags, uint8_t* d_chunks,
+                                                          uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status,
+                                                          cb200_camera_plan** out);
 /* cb200_camera_plan_create_detect_receivers (below) with its descriptors in DEVICE memory too, read at each launch within bounds, as
    above.  A slot is EMPTY exactly as in that plan (receiver out of range, or no candidate bit below n_modes): its descriptor is not
    read.  A non-empty slot whose descriptor is refused as above gets status CB200_EXTRACT_REFUSED and otherwise what an empty slot
@@ -423,6 +457,19 @@ int cb200_camera_plan_create_detect_receivers_pictures_dev(cb200_ctx* const* ctx
                                                            const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states,
                                                            uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
                                                            int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out);
+/* the receiver flags forms of the detect receivers call and its plan over device descriptors (see "per-receiver decode flags" above):
+   d_receiver_flags follows d_states */
+int cb200_detect_scan_extract_decode_chunks_receivers_flags_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n,
+                                                                uint32_t flags, const uint32_t* candidates, const int32_t* receiver_of,
+                                                                int n_receivers, cb200_receiver_state* const* d_states,
+                                                                const uint32_t* d_receiver_flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                                                int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks);
+int cb200_camera_plan_create_detect_receivers_pictures_flags_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* d_pics, int n,
+                                                                 const cb200_picture_bounds* bounds, uint32_t flags, const uint32_t* d_candidates,
+                                                                 const int32_t* d_receiver_of, int n_receivers,
+                                                                 cb200_receiver_state* const* d_states, const uint32_t* d_receiver_flags,
+                                                                 uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
+                                                                 int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out);
 /* ---- auto mode: the sender's mode detected by decoding ----------------------------------------------------------------------
 
    The receiver's auto mode (the reference's web receiver tries 66, 68, 67 and 4 and keeps the first mode under which a frame gives

@@ -46,6 +46,8 @@ EXPORTS = [
     "cb200_decode_chunks_receivers_dev", "cb200_scan_extract_decode_chunks_receivers_dev", "cb200_camera_plan_create_receivers",
     "cb200_detect_scan_extract_decode_chunks_receivers_dev", "cb200_camera_plan_create_detect_receivers",
     "cb200_camera_plan_create_receivers_pictures_dev", "cb200_camera_plan_create_detect_receivers_pictures_dev",
+    "cb200_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_receivers_pictures_flags_dev",
+    "cb200_detect_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_detect_receivers_pictures_flags_dev",
 ]
 
 
@@ -191,6 +193,13 @@ def load_library():
                                                                     C.POINTER(C.c_void_p)]
     lib.cb200_camera_plan_create_detect_receivers_pictures_dev.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_uint32, vp, vp, C.c_int, vp, vp,
                                                                            vp, vp, vp, vp, C.POINTER(C.c_void_p)]
+    lib.cb200_scan_extract_decode_chunks_receivers_flags_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp, vp]
+    lib.cb200_camera_plan_create_receivers_pictures_flags_dev.argtypes = [vp, vp, C.c_int, vp, C.c_uint32, vp, C.c_int, vp, vp, vp, vp,
+                                                                          vp, vp, C.POINTER(C.c_void_p)]
+    lib.cb200_detect_scan_extract_decode_chunks_receivers_flags_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, C.c_int, vp,
+                                                                                vp, vp, vp, vp, vp, vp]
+    lib.cb200_camera_plan_create_detect_receivers_pictures_flags_dev.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_uint32, vp, vp, C.c_int,
+                                                                                 vp, vp, vp, vp, vp, vp, vp, C.POINTER(C.c_void_p)]
     lib.cb200_selfcheck.argtypes = [C.c_int]
     lib.cb200_mode_info.argtypes = [C.c_int, C.POINTER(Info)]
     lib.cb200_interleave_indices.argtypes = [C.c_int, u16p]
@@ -283,6 +292,15 @@ def _states_ptr(states):
     return states.data_ptr(), states.numel() * states.element_size() // 40
 
 
+def _flags_table(receiver_flags, count):
+    """the device address of a receiver flags table: a contiguous uint32 / int32 CUDA tensor of one word per receiver"""
+    import torch
+    if not isinstance(receiver_flags, torch.Tensor) or not receiver_flags.is_cuda or not receiver_flags.is_contiguous() or \
+            receiver_flags.dtype not in (torch.int32, torch.uint32) or receiver_flags.numel() != count:
+        raise Cb200Error(f"receiver_flags is a contiguous uint32 or int32 CUDA tensor of {count} words, one per receiver")
+    return receiver_flags.data_ptr()
+
+
 def launch_count():
     """kernels launched by libcb200 in this process so far"""
     return int(load_library().cb200_launch_count())
@@ -331,13 +349,15 @@ def detect_scan_extract_decode_chunks_dev(ctxs, d_pictures, wh, d_chunks, d_mask
 
 
 def detect_scan_extract_decode_chunks_receivers_dev(ctxs, pictures, receiver_of, states, d_chunks, d_mask, d_status, d_mode, candidates=None,
-                                                    d_mode_masks=None, flags=0, order="rgb"):
+                                                    d_mode_masks=None, flags=0, order="rgb", receiver_flags=None):
     """The auto mode for pictures of many receivers, enqueue-only (cb200_detect_scan_extract_decode_chunks_receivers_dev): picture i
     (a uint8 CUDA tensor, as for Context.scan_extract_decode_chunks_receivers_dev) belongs to receiver receiver_of[i] and is decoded
     under ctxs[k] when bit k of candidates[i] is set (candidates: n bitmasks, or None for every mode).  states: one receiver_states
     tensor per context, each receiver's state under that mode.  For every k, the pictures with bit k get what
     Context.scan_extract_decode_chunks_receivers_dev on ctxs[k] gives on those pictures alone with states[k]; the outputs select among
-    them as detect_scan_extract_decode_chunks_dev does (d_mode: the index into ctxs, or -1)"""
+    them as detect_scan_extract_decode_chunks_dev does (d_mode: the index into ctxs, or -1).  receiver_flags: None, or a receiver
+    flags table as for Context.scan_extract_decode_chunks_receivers_dev, one word per receiver for every mode
+    (cb200_detect_scan_extract_decode_chunks_receivers_flags_dev)"""
     orders = [order] * len(pictures) if isinstance(order, str) else list(order)
     if len(orders) != len(pictures):
         raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
@@ -355,9 +375,15 @@ def detect_scan_extract_decode_chunks_receivers_dev(ctxs, pictures, receiver_of,
     hs = (C.c_void_p * max(len(ctxs), 1))(*[c._h.value for c in ctxs])
     ptrs = (C.c_void_p * max(len(tables), 1))(*[p for p, _ in tables])
     descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
-    _check(load_library().cb200_detect_scan_extract_decode_chunks_receivers_dev(
-        hs, len(ctxs), C.cast(descs, C.c_void_p), len(pictures), flags, _hptr(cand), of.ctypes.data, tables[0][1] if tables else 0, ptrs,
-        d_chunks, d_mask, d_status, d_mode, d_mode_masks))
+    count = tables[0][1] if tables else 0
+    if receiver_flags is None:
+        _check(load_library().cb200_detect_scan_extract_decode_chunks_receivers_dev(
+            hs, len(ctxs), C.cast(descs, C.c_void_p), len(pictures), flags, _hptr(cand), of.ctypes.data, count, ptrs,
+            d_chunks, d_mask, d_status, d_mode, d_mode_masks))
+        return
+    _check(load_library().cb200_detect_scan_extract_decode_chunks_receivers_flags_dev(
+        hs, len(ctxs), C.cast(descs, C.c_void_p), len(pictures), flags, _hptr(cand), of.ctypes.data, count, ptrs,
+        _flags_table(receiver_flags, count), d_chunks, d_mask, d_status, d_mode, d_mode_masks))
 
 
 def _device_int32(t, n, what):
@@ -405,11 +431,12 @@ def _descriptor_tensor(d_pics):
 
 
 def detect_receivers_camera_plan_pictures_dev(ctxs, d_pics, bounds, candidates, receiver_of, states, d_chunks, d_mask, d_status, d_mode,
-                                              d_mode_masks=None, flags=0):
+                                              d_mode_masks=None, flags=0, receiver_flags=None):
     """detect_receivers_camera_plan with the pictures' descriptors read from device memory at each launch too
     (cb200_camera_plan_create_detect_receivers_pictures_dev): d_pics and bounds as for Context.receivers_camera_plan_pictures_dev.  A
     slot whose descriptor the launch refuses gets mode -1, mask 0, a zeroed record and status EXTRACT_REFUSED; an empty slot (no
-    candidate, or a receiver out of range) EXTRACT_EMPTY, and its descriptor is not read"""
+    candidate, or a receiver out of range) EXTRACT_EMPTY, and its descriptor is not read.  receiver_flags: None, or a receiver flags
+    table bound here and read at each launch (cb200_camera_plan_create_detect_receivers_pictures_flags_dev)"""
     n = _descriptor_tensor(d_pics)
     if len(states) != len(ctxs):
         raise Cb200Error(f"{len(states)} state tables for {len(ctxs)} contexts")
@@ -422,10 +449,16 @@ def detect_receivers_camera_plan_pictures_dev(ctxs, d_pics, bounds, candidates, 
     ptrs = (C.c_void_p * max(len(tables), 1))(*[p for p, _ in tables])
     bd = (C.c_int32 * 3)(*[int(v) for v in bounds])
     h = C.c_void_p()
-    _check(load_library().cb200_camera_plan_create_detect_receivers_pictures_dev(
-        hs, len(ctxs), d_pics.data_ptr(), n, C.cast(bd, C.c_void_p), flags, cand, of, tables[0][1] if tables else 0, ptrs,
+    count = tables[0][1] if tables else 0
+    if receiver_flags is None:
+        _check(load_library().cb200_camera_plan_create_detect_receivers_pictures_dev(
+            hs, len(ctxs), d_pics.data_ptr(), n, C.cast(bd, C.c_void_p), flags, cand, of, count, ptrs,
+            d_chunks, d_mask, d_status, d_mode, d_mode_masks, C.byref(h)))
+        return CameraPlan(ctxs[0], h, keep=(d_pics, candidates, receiver_of, list(states)), ctxs=list(ctxs))
+    _check(load_library().cb200_camera_plan_create_detect_receivers_pictures_flags_dev(
+        hs, len(ctxs), d_pics.data_ptr(), n, C.cast(bd, C.c_void_p), flags, cand, of, count, ptrs, _flags_table(receiver_flags, count),
         d_chunks, d_mask, d_status, d_mode, d_mode_masks, C.byref(h)))
-    return CameraPlan(ctxs[0], h, keep=(d_pics, candidates, receiver_of, list(states)), ctxs=list(ctxs))
+    return CameraPlan(ctxs[0], h, keep=(d_pics, candidates, receiver_of, list(states), receiver_flags), ctxs=list(ctxs))
 
 
 def _hptr(a):
@@ -752,17 +785,25 @@ class Context:
         _check(self.lib.cb200_decode_chunks_receivers_dev(self._h, d_rgb, n, flags, of.ctypes.data, count, ptr, d_chunks, d_mask, d_flags))
 
     def scan_extract_decode_chunks_receivers_dev(self, pictures, receiver_of, states, d_chunks, d_mask, d_status, d_flags=None, flags=0,
-                                                 order="rgb"):
+                                                 order="rgb", receiver_flags=None):
         """scan_extract_decode_chunks_pictures_dev for pictures of several receivers: picture i belongs to receiver receiver_of[i]
-        (host), each receiver decodes with its own state in `states` (receiver_states) and leaves its new one there.  Enqueue-only"""
+        (host), each receiver decodes with its own state in `states` (receiver_states) and leaves its new one there.  Enqueue-only.
+        receiver_flags: None, or a receiver flags table (cb200_scan_extract_decode_chunks_receivers_flags_dev): a contiguous uint32 or
+        int32 CUDA tensor with one word per receiver, that receiver's SHARPEN / SHARPEN_IF_NEEDED and CC_SIMPLE / CC_FIT bits, read
+        in stream order; `flags` then holds none of those bits.  A receiver with an invalid word gets status EXTRACT_REFUSED"""
         orders = [order] * len(pictures) if isinstance(order, str) else list(order)
         if len(orders) != len(pictures):
             raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
         of = _receiver_map(receiver_of, len(pictures))
         ptr, count = _states_ptr(states)
         descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
-        _check(self.lib.cb200_scan_extract_decode_chunks_receivers_dev(self._h, C.cast(descs, C.c_void_p), len(pictures), flags, of.ctypes.data,
-                                                                       count, ptr, d_chunks, d_mask, d_flags, d_status))
+        if receiver_flags is None:
+            _check(self.lib.cb200_scan_extract_decode_chunks_receivers_dev(self._h, C.cast(descs, C.c_void_p), len(pictures), flags,
+                                                                           of.ctypes.data, count, ptr, d_chunks, d_mask, d_flags, d_status))
+            return
+        _check(self.lib.cb200_scan_extract_decode_chunks_receivers_flags_dev(self._h, C.cast(descs, C.c_void_p), len(pictures), flags,
+                                                                             of.ctypes.data, count, ptr, _flags_table(receiver_flags, count),
+                                                                             d_chunks, d_mask, d_flags, d_status))
 
     def camera_plan(self, wh, flags, pictures, chunks, mask, frame_flags, status):
         """scan_extract_decode_chunks_dev for pictures of sizes wh (n x (w, h), host) with these flags, captured once in a CUDA graph
@@ -795,14 +836,17 @@ class Context:
                                                            count, ptr, chunks, mask, frame_flags, status, C.byref(h)))
         return CameraPlan(self, h, keep=(list(pictures), receiver_of, states))
 
-    def receivers_camera_plan_pictures_dev(self, d_pics, bounds, receiver_of, states, chunks, mask, status, frame_flags=None, flags=0):
+    def receivers_camera_plan_pictures_dev(self, d_pics, bounds, receiver_of, states, chunks, mask, status, frame_flags=None, flags=0,
+                                           receiver_flags=None):
         """receivers_camera_plan with the pictures' descriptors read from device memory at each launch too
         (cb200_camera_plan_create_receivers_pictures_dev): d_pics is a contiguous (n, 40) uint8 CUDA tensor of cb200_picture
         descriptors (picture_descriptors() builds them on the host), so each launch's slots may hold pictures of any size, layout
         and buffer within bounds = (min_short, max_short, max_long).  A slot whose descriptor the launch refuses (a rule a direct
         call checks, or outside the bounds) gets mask 0 and status EXTRACT_REFUSED, an empty slot EXTRACT_EMPTY; neither reads
         its pixels.  Write each batch's descriptors and map in stream order before its launch; the plan keeps the tensors it binds
-        alive (the pictures are the caller's to keep until the stream has passed each launch)"""
+        alive (the pictures are the caller's to keep until the stream has passed each launch).  receiver_flags: None, or a receiver
+        flags table as for scan_extract_decode_chunks_receivers_dev, bound here and read at each launch
+        (cb200_camera_plan_create_receivers_pictures_flags_dev)"""
         import torch
         n = _descriptor_tensor(d_pics)
         if not isinstance(receiver_of, torch.Tensor) or not receiver_of.is_cuda or receiver_of.dtype != torch.int32 or \
@@ -811,10 +855,16 @@ class Context:
         bd = (C.c_int32 * 3)(*[int(v) for v in bounds])
         ptr, count = _states_ptr(states)
         h = C.c_void_p()
-        _check(self.lib.cb200_camera_plan_create_receivers_pictures_dev(self._h, d_pics.data_ptr(), n, C.cast(bd, C.c_void_p), flags,
-                                                                        receiver_of.data_ptr(), count, ptr, chunks, mask, frame_flags,
-                                                                        status, C.byref(h)))
-        return CameraPlan(self, h, keep=(d_pics, receiver_of, states))
+        if receiver_flags is None:
+            _check(self.lib.cb200_camera_plan_create_receivers_pictures_dev(self._h, d_pics.data_ptr(), n, C.cast(bd, C.c_void_p), flags,
+                                                                            receiver_of.data_ptr(), count, ptr, chunks, mask, frame_flags,
+                                                                            status, C.byref(h)))
+            return CameraPlan(self, h, keep=(d_pics, receiver_of, states))
+        _check(self.lib.cb200_camera_plan_create_receivers_pictures_flags_dev(self._h, d_pics.data_ptr(), n, C.cast(bd, C.c_void_p), flags,
+                                                                              receiver_of.data_ptr(), count, ptr,
+                                                                              _flags_table(receiver_flags, count), chunks, mask,
+                                                                              frame_flags, status, C.byref(h)))
+        return CameraPlan(self, h, keep=(d_pics, receiver_of, states, receiver_flags))
 
     jpeg_info = staticmethod(jpeg_info)
 

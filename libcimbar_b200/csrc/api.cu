@@ -801,7 +801,10 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
 {
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
-    const bool fit = ccm_fits(m, flags), chained = chain_linked(c, flags);
+    // a receiver flags table: every frame takes the fitted-CCM route, whatever its receiver's CC bit, and the mode fits the frames of
+    // CC_FIT receivers (k_ccm_fit and k_ccm_simple read the table, k_ccm_carry_receivers takes each CC_SIMPLE frame's matrix as a fit)
+    const uint32_t* words = recv ? recv->d_words : nullptr;
+    const bool fit = ccm_fits(m, words ? CB200_FLAG_CC_FIT : flags), chained = chain_linked(c, flags);
     // the CCM going into frame 0 is only known on the device -- always so for a camera plan, whose graph replays later.  A receivers
     // call reads no context CCM, so a receivers plan takes the direct receivers call's route
     bool carried = enqueue_only && !(flags & CB200_FLAG_CC_SIMPLE) && c->capturing && !recv;
@@ -810,7 +813,7 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
         if (q == cudaErrorNotReady) carried = true;
         else if (q != cudaSuccess) return fail_cuda(q, "query ccm");
     }
-    const bool fitted = fit || carried || chained;                 // the fitted-CCM route
+    const bool fitted = fit || carried || chained || words;        // the fitted-CCM route
     unsigned parts = fitted ? kCcm | (n > 0 ? kFitted : 0u) : (recv || (flags & CB200_FLAG_CC_SIMPLE)) ? kCcm : 0u;
     if (recv) parts |= kReceivers;
     if (d_sel_bytes) parts |= kSchedule;
@@ -847,14 +850,16 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
         mark(c);                               // ev3
         if (fit) {
             CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream, 0, m.nblocks_sym), "rs launch (symbols)");
-            CK(ccm_fit_launch(m, d_rgb, d_chunks, c->d_ok, idx, n, c->d_fit, c->d_fit_valid, c->stream), "ccm fit");
+            CK(ccm_fit_launch(m, d_rgb, d_chunks, c->d_ok, idx, n, c->d_fit, c->d_fit_valid, c->stream, nullptr, words, words ? recv->d_map : nullptr),
+               "ccm fit");
         } else {
             CK(cudaMemsetAsync(c->d_fit_valid, 0, (size_t)n, c->stream), "memset fit flags");
         }
+        if (words) CK(ccm_simple_launch(m, d_rgb, n, c->d_fit, c->stream, words, recv->d_map, c->d_fit_valid), "ccm launch");
         // across ranks: this stripe's fits out, the CCM entering the stripe in (from the lower ranks' fits of the same step)
         if (chained) { rc = chain_publish_link(c, n, c->d_fit, c->d_fit_valid, initial, &initial); if (rc) return rc; }
         if (recv) CK(ccm_carry_receivers_launch(n, recv->d_map, recv->d_map + n, c->d_fit, c->d_fit_valid, recv->d_states, c->d_ccm,
-                                                c->d_ccm_active, c->stream), "ccm carry");
+                                                c->d_ccm_active, c->stream, words, fit), "ccm carry");
         else CK(ccm_carry_launch(n, c->d_fit, c->d_fit_valid, initial, c->d_ccm, c->d_ccm_active, c->stream), "ccm carry");
         CK(ccm_apply_launch(m, c->d_means, n, c->d_ccm, c->d_ccm_active, c->d_cellvals, c->stream), "ccm apply");
         c->ccm_frames = n;

@@ -28,11 +28,17 @@ __device__ __forceinline__ bool matx33_inv_rn(const float* a, float* b)
 }
 
 // one thread per frame: calculateWhite (dark layout: anchors top-left, bottom-left, top-right; 4x4 means; floor 1) and
-// get_adaptation_matrix<von_kries>(white, (255,255,255)) = T.inv() * diag((T*desired) / (T*white)) * T
-__global__ void k_ccm_simple(const Mode m, const uint8_t* __restrict__ rgb, int n_frames, float* __restrict__ ccm)
+// get_adaptation_matrix<von_kries>(white, (255,255,255)) = T.inv() * diag((T*desired) / (T*white)) * T.  words: NULL, or a receiver
+// flags table with the batch's map `of`: only the frames of CC_SIMPLE receivers get their matrix, and their `valid` byte is set
+__global__ void k_ccm_simple(const Mode m, const uint8_t* __restrict__ rgb, int n_frames, float* __restrict__ ccm,
+                             const uint32_t* __restrict__ words, const int32_t* __restrict__ of, uint8_t* __restrict__ valid)
 {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_frames) return;
+    if (words) {
+        if (of[f] < 0 || !(words[of[f]] & receivers::kWordCcSimple)) return;
+        valid[f] = 1;
+    }
     const int W = m.width, H = m.height;
     const uint8_t* frame = rgb + (size_t)f * W * H * 3;
     const int tl = 30 - 2, right = W - 30 - 2, bottom = H - 30 - 2;       // Config::anchor_size() == 30, padding 0
@@ -60,9 +66,10 @@ __global__ void k_ccm_simple(const Mode m, const uint8_t* __restrict__ rgb, int 
     for (int i = 0; i < 9; ++i) ccm[(size_t)f * 9 + i] = out[i];
 }
 
-cudaError_t ccm_simple_launch(const Mode& m, const uint8_t* d_rgb, int n_frames, float* d_ccm, cudaStream_t st)
+cudaError_t ccm_simple_launch(const Mode& m, const uint8_t* d_rgb, int n_frames, float* d_ccm, cudaStream_t st, const uint32_t* d_words,
+                              const int32_t* d_of, uint8_t* d_valid)
 {
-    k_ccm_simple<<<(n_frames + 63) / 64, 64, 0, st>>>(m, d_rgb, n_frames, d_ccm); count_launch();
+    k_ccm_simple<<<(n_frames + 63) / 64, 64, 0, st>>>(m, d_rgb, n_frames, d_ccm, d_words, d_of, d_valid); count_launch();
     return cudaGetLastError();
 }
 
@@ -221,10 +228,12 @@ struct FitSmem {
     int has;
 };
 
-// one warp per frame
+// one warp per frame.  words: NULL, or a receiver flags table with the batch's map `of`: only the frames of CC_FIT receivers are
+// fitted, every other one gets valid 0
 __global__ void __launch_bounds__(128)
 k_ccm_fit(const Mode m, const uint8_t* __restrict__ rgb, const uint8_t* __restrict__ data, const uint8_t* __restrict__ ok,
-          const uint16_t* __restrict__ idx, int n_frames, float* __restrict__ fit, uint8_t* __restrict__ valid, const GivenHeader given)
+          const uint16_t* __restrict__ idx, int n_frames, float* __restrict__ fit, uint8_t* __restrict__ valid, const GivenHeader given,
+          const uint32_t* __restrict__ words, const int32_t* __restrict__ of)
 {
     __shared__ FitSmem sm[4];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -266,6 +275,7 @@ k_ccm_fit(const Mode m, const uint8_t* __restrict__ rgb, const uint8_t* __restri
         s.radioactive = radioactive;
         s.has = (hdr[0] | hdr[1] | hdr[2] | hdr[3]) != 0;
     }
+    if (lane == 0 && words && (of[f] < 0 || !(words[of[f]] & receivers::kWordCcFit))) s.has = 0;
     __syncwarp();
     if (!s.has || m.color_bits == 0) { if (lane == 0) valid[f] = 0; return; }
 
@@ -371,11 +381,15 @@ k_ccm_carry(int n_frames, const float* __restrict__ fit, const uint8_t* __restri
 // k_ccm_carry for a batch of several receivers: the same two-level max scan, over the receiver-major order and with the segment
 // starts scanned alongside (receivers_core.cuh), so each picture takes its own receiver's last fit or entry state.  used and
 // used_active are written in batch order; each receiver's last picture writes its exit state, after every entry state is read.
-// Slots of receiver -1 are empty, the last run of the order; they read and write no state and decode without a CCM
+// Slots of receiver -1 are empty; they read and write no state and decode without a CCM.  They are the last run of the order, except
+// that a receiver flags table's refused receivers (emptied by k_extract after the order was built) leave runs of -1 in its middle:
+// the segments compare neighbours, so every run stays its own.  words: NULL, or
+// a receiver flags table (valid then marks the fits and the CC_SIMPLE matrices alike): the pictures of a receiver whose word passes
+// its CCM through (receivers::word_passes, with `fits` the mode's) take k_receivers_gather's matrix and write no state
 __global__ void __launch_bounds__(1024)
 k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ fit,
                       const uint8_t* __restrict__ valid, cb200_receiver_state* __restrict__ states, float* __restrict__ used,
-                      uint8_t* __restrict__ used_active)
+                      uint8_t* __restrict__ used_active, const uint32_t* __restrict__ words, bool fits)
 {
     __shared__ int seg_fit[1024], seg_start[1024];
     const int t = threadIdx.x;
@@ -399,6 +413,11 @@ k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_
             continue;
         }
         const cb200_receiver_state& e = states[of[f]];
+        if (words && receivers::word_passes(words[of[f]], fits)) {
+            for (int i = 0; i < 9; ++i) used[(size_t)f * 9 + i] = e.active ? e.ccm[i] : (i % 4 == 0 ? 1.0f : 0.0f);
+            used_active[f] = e.active ? 1 : 0;
+            continue;
+        }
         for (int i = 0; i < 9; ++i) used[(size_t)f * 9 + i] = g >= 0 ? fit[(size_t)g * 9 + i] : e.ccm[i];
         used_active[f] = (g >= 0 || e.active != 0) ? 1 : 0;
     }
@@ -406,7 +425,7 @@ k_ccm_carry_receivers(int n_frames, const int32_t* __restrict__ of, const int32_
     for (int j = j0; j < j1; ++j) {
         if (!receivers::closes(of, order, n_frames, j)) continue;
         const int f = order[j];
-        if (of[f] < 0) continue;
+        if (of[f] < 0 || (words && receivers::word_passes(words[of[f]], fits))) continue;
         cb200_receiver_state& x = states[of[f]];
         for (int i = 0; i < 9; ++i) x.ccm[i] = used[(size_t)f * 9 + i];
         x.active = used_active[f];
@@ -432,7 +451,7 @@ __global__ void k_receivers_gather(int n_frames, const int32_t* __restrict__ of,
     active[f] = a ? 1 : 0;
 }
 
-// CC_SIMPLE: each receiver keeps the matrix of its last picture (the run of empty slots keeps nothing)
+// CC_SIMPLE: each receiver keeps the matrix of its last picture (a run of empty slots keeps nothing)
 __global__ void k_receivers_keep(int n_frames, const int32_t* __restrict__ of, const int32_t* __restrict__ order, const float* __restrict__ ccm,
                                  cb200_receiver_state* __restrict__ states)
 {
@@ -506,12 +525,13 @@ k_ccm_apply(const Mode m, const uint32_t* __restrict__ means, int n_frames, cons
 }  // namespace
 
 cudaError_t ccm_fit_launch(const Mode& m, const uint8_t* d_rgb, const uint8_t* d_data, const uint8_t* d_ok, const uint16_t* d_idx,
-                           int n_frames, float* d_fit, uint8_t* d_valid, cudaStream_t st, const GivenHeader* given)
+                           int n_frames, float* d_fit, uint8_t* d_valid, cudaStream_t st, const GivenHeader* given, const uint32_t* d_words,
+                           const int32_t* d_of)
 {
     GivenHeader g;
     memset(&g, 0, sizeof(g));
     if (given) g = *given;
-    k_ccm_fit<<<(n_frames + 3) / 4, 128, 0, st>>>(m, d_rgb, d_data, d_ok, d_idx, n_frames, d_fit, d_valid, g); count_launch();
+    k_ccm_fit<<<(n_frames + 3) / 4, 128, 0, st>>>(m, d_rgb, d_data, d_ok, d_idx, n_frames, d_fit, d_valid, g, d_words, d_of); count_launch();
     return cudaGetLastError();
 }
 cudaError_t ccm_carry_launch(int n_frames, const float* d_fit, const uint8_t* d_valid, const CcmArg& initial, float* d_used,
@@ -528,9 +548,11 @@ cudaError_t ccm_apply_launch(const Mode& m, const uint32_t* d_means, int n_frame
     return cudaGetLastError();
 }
 cudaError_t ccm_carry_receivers_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_fit, const uint8_t* d_valid,
-                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st)
+                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st,
+                                       const uint32_t* d_words, bool fits)
 {
-    k_ccm_carry_receivers<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active); count_launch();
+    k_ccm_carry_receivers<<<1, 1024, 0, st>>>(n_frames, d_of, d_order, d_fit, d_valid, d_states, d_used, d_used_active, d_words, fits);
+    count_launch();
     return cudaGetLastError();
 }
 cudaError_t receivers_gather_launch(int n_frames, const int32_t* d_of, const cb200_receiver_state* d_states, float* d_ccm, uint8_t* d_active,

@@ -69,15 +69,20 @@ __device__ __forceinline__ uint32_t best_color_ccm(const float* ccm, const Mode&
     return best;
 }
 
-cudaError_t ccm_simple_launch(const Mode& m, const uint8_t* d_rgb, int n_frames, float* d_ccm, cudaStream_t st);
+// d_words: NULL, or a receiver flags table with the batch's map d_of (receivers_core.cuh): only the frames of CC_SIMPLE receivers get
+// their matrix, and their d_valid byte is set (the receivers carry then takes it as the receiver's new matrix)
+cudaError_t ccm_simple_launch(const Mode& m, const uint8_t* d_rgb, int n_frames, float* d_ccm, cudaStream_t st, const uint32_t* d_words = nullptr,
+                              const int32_t* d_of = nullptr, uint8_t* d_valid = nullptr);
 // color_correction == 2, after the symbol stream's RS pass: per frame the header the aligned_stream callbacks leave behind,
 // the colours it predicts, the fit (fit[f], valid[f]); then the carry (a frame without a fit keeps its predecessor's CCM,
 // frame 0 the context's) into used[f] / used_active[f]; then the colour decision of every cell from the stored means
 // given != nullptr (single frame): the header is not derived from the RS output but handed in by the caller
-// (CimbReader::init_ccm on a host that ran CimbReader::update_metadata itself); d_data / d_ok are then unused
+// (CimbReader::init_ccm on a host that ran CimbReader::update_metadata itself); d_data / d_ok are then unused.
+// d_words: NULL, or a receiver flags table with the batch's map d_of: only the frames of CC_FIT receivers are fitted
 struct GivenHeader { uint8_t hdr[6]; uint8_t use; uint8_t pad; uint32_t radioactive; };
 cudaError_t ccm_fit_launch(const Mode& m, const uint8_t* d_rgb, const uint8_t* d_data, const uint8_t* d_ok, const uint16_t* d_idx,
-                           int n_frames, float* d_fit, uint8_t* d_valid, cudaStream_t st, const GivenHeader* given = nullptr);
+                           int n_frames, float* d_fit, uint8_t* d_valid, cudaStream_t st, const GivenHeader* given = nullptr,
+                           const uint32_t* d_words = nullptr, const int32_t* d_of = nullptr);
 cudaError_t ccm_carry_launch(int n_frames, const float* d_fit, const uint8_t* d_valid, const CcmArg& initial, float* d_used,
                              uint8_t* d_used_active, cudaStream_t st);
 cudaError_t ccm_apply_launch(const Mode& m, const uint32_t* d_means, int n_frames, const float* d_used, const uint8_t* d_used_active,
@@ -88,8 +93,11 @@ cudaError_t ccm_apply_launch(const Mode& m, const uint32_t* d_means, int n_frame
 // each picture's receiver matrix into d_ccm / d_active.  receivers_keep_launch: the matrix d_ccm holds for each receiver's last
 // picture into its state, active.  Receiver -1 in d_of (a receivers plan's map, built by receivers_order_launch, or a mode's map
 // in a detect receivers call) is an empty slot, which reads and writes no state and decodes without a CCM
+// d_words: NULL, or a receiver flags table (valid marks fits and CC_SIMPLE matrices alike; fits: the mode fits CC_FIT frames): a
+// receiver whose word passes its CCM through gets k_receivers_gather's matrices and keeps its state
 cudaError_t ccm_carry_receivers_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_fit, const uint8_t* d_valid,
-                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st);
+                                       cb200_receiver_state* d_states, float* d_used, uint8_t* d_used_active, cudaStream_t st,
+                                       const uint32_t* d_words = nullptr, bool fits = false);
 cudaError_t receivers_gather_launch(int n_frames, const int32_t* d_of, const cb200_receiver_state* d_states, float* d_ccm, uint8_t* d_active,
                                     cudaStream_t st);
 cudaError_t receivers_keep_launch(int n_frames, const int32_t* d_of, const int32_t* d_order, const float* d_ccm, cb200_receiver_state* d_states,

@@ -66,6 +66,8 @@ int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t 
 // CB200_ERR_ARG for CB200_FLAG_SHARPEN together with CB200_FLAG_SHARPEN_IF_NEEDED, or CB200_FLAG_CC_SIMPLE with CB200_FLAG_CC_FIT
 // (scan.cu)
 int check_camera_flags(uint32_t flags);
+// CB200_ERR_ARG for a receiver flags table that is null or not 4-byte aligned, or call flags with a per-receiver bit (scan.cu)
+int check_receiver_flags(const uint32_t* d_receiver_flags, uint32_t flags);
 // PicDesc, one camera picture as the extractor kernels read it: pic_desc.cuh.
 // The pictures of one camera, corner or deskew call, whatever the caller passed in (scan.cu): one descriptor per picture, their
 // sizes n x (w, h) (what scan_reserve and check_frozen_* take), and `packed`: every picture is RGB with row pitch 3 w, so the
@@ -201,13 +203,31 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
 int check_receivers(const cb200_ctx* c, const int32_t* receiver_of, int n, int n_receivers, const cb200_receiver_state* d_states,
                     bool on_device = false);
 // d_refused: NULL, or (a plan over device descriptors) one byte per slot, set where the launch refused the slot's descriptor: its
-// status becomes CB200_EXTRACT_REFUSED instead of CB200_EXTRACT_EMPTY
+// status becomes CB200_EXTRACT_REFUSED instead of CB200_EXTRACT_EMPTY.
+// d_words: NULL, or a receiver flags table (the _receivers_flags_dev calls; receivers_core.cuh, word_refused): k_extract empties the
+// map entry of every slot whose receiver's word is invalid and sets its refused byte, and writes every slot's sharpen byte from its
+// receiver's word; every frame takes the fitted-CCM route, with the CCM kind of its receiver's word (decode_chunks).  The direct call's
+// refused bytes travel zeroed behind its map (refused_bytes), so d_refused is always set with d_words.  A refused receiver's slots
+// become runs of receiver -1 that may sit in the middle of the order; the carry and the masks compare neighbours and read no state
+// for them
 struct Receivers {
     std::vector<int32_t> map;
     const int32_t* d_map = nullptr;
     cb200_receiver_state* d_states = nullptr;
     const uint8_t* d_refused = nullptr;
+    const uint32_t* d_words = nullptr;
+    // with d_words: the table's size, and each scanned picture's receiver (NULL: d_map's, the map of a call without sub-batches; a
+    // detect call's caller map, whose pictures each mode's sub-batch or empty slots leave out)
+    int receivers = 0;
+    const int32_t* d_pic_of = nullptr;
     Receivers(const int32_t* receiver_of, int n, int n_receivers, cb200_receiver_state* states);
+    // a direct call with a flags table: n zero bytes behind the map, d_refused once the map is on the device
+    void refused_bytes(int n) { map.resize(2 * (size_t)n + ((size_t)n + 3) / 4, 0); }
+    void map_on_device(const int32_t* d, int n)
+    {
+        d_map = d;
+        if (d_words) d_refused = reinterpret_cast<const uint8_t*>(d + 2 * (size_t)n);
+    }
     Receivers(const int32_t* d_map_, cb200_receiver_state* states) : d_map(d_map_), d_states(states) {}
     size_t bytes() const { return map.size() * sizeof(int32_t); }
 };
@@ -230,6 +250,7 @@ struct DetectPlan {
     int32_t* d_lists;
     uint8_t* d_present;
     uint8_t* d_pics_table;
+    const uint32_t* d_words;         // a receiver flags table (plans over device descriptors only), else NULL
 };
 size_t detect_plan_words(int n_modes, int n);
 // bounds: NULL for cb200_camera_plan_create_detect_receivers (pics on the host), else the plan's bounds and pics in device memory

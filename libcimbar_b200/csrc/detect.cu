@@ -225,7 +225,9 @@ struct StreamSwap {
 };
 
 // a detect receivers call's receivers: the candidate modes and the receiver map of every picture (host), one state table per mode
-struct DetectReceivers { const uint32_t* cand; const int32_t* of; int count; cb200_receiver_state* const* d_states; };
+// (and a receiver flags table, else NULL: every mode reads it, each scanned picture's receiver travels with the lists, and every mode
+// has refused bytes of its own over its geometry's sub-batch)
+struct DetectReceivers { const uint32_t* cand; const int32_t* of; int count; cb200_receiver_state* const* d_states; const uint32_t* words; };
 
 // With dr (a detect receivers call), geometry g decodes only its sub-batch U_g (receivers_core.cuh: detect_lists), each of its modes
 // with its own receiver map over U_g and state table; a geometry or mode without pictures launches nothing.  The sub-batches' picture
@@ -282,7 +284,7 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
     if (live > 1 && (rc = detect_streams(ds, ng))) return rc;
     // dr's lists, in byte offsets from the tail's start: per geometry its picture table and scan slots, per mode its map, the positions
     std::vector<uint8_t> tail;
-    size_t desc_at[kDetectModes] = {}, slots_at[kDetectModes] = {}, map_at[kDetectModes] = {}, pos_at = 0;
+    size_t desc_at[kDetectModes] = {}, slots_at[kDetectModes] = {}, map_at[kDetectModes] = {}, pos_at = 0, of_at = 0, refused_at = 0;
     if (dr) {
         static_assert(sizeof(PicDesc) % 8 == 0, "the sub-batch tables follow each other 8-byte aligned");
         std::vector<uint8_t> table;
@@ -293,7 +295,8 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
         for (int g = 0; g < ng; ++g) { slots_at[g] = at; at += sizeof(int32_t) * lists.slots[g].size(); }
         for (int k = 0; k < n_modes; ++k) { map_at[k] = at; at += sizeof(int32_t) * lists.map[k].size(); }
         pos_at = at; at += sizeof(int32_t) * lists.pos.size();
-        tail.resize(at);
+        if (dr->words) { of_at = at; at += sizeof(int32_t) * (size_t)n; refused_at = at; at += (size_t)n_modes * n; }
+        tail.assign(at, 0);
         for (int g = 0; g < ng; ++g) {
             PicDesc* d = reinterpret_cast<PicDesc*>(tail.data() + desc_at[g]);
             for (size_t j = 0; j < lists.slots[g].size(); ++j) d[j] = desc[lists.slots[g][j]];
@@ -301,6 +304,7 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
         }
         for (int k = 0; k < n_modes; ++k) memcpy(tail.data() + map_at[k], lists.map[k].data(), sizeof(int32_t) * lists.map[k].size());
         memcpy(tail.data() + pos_at, lists.pos.data(), sizeof(int32_t) * lists.pos.size());
+        if (dr->words) memcpy(tail.data() + of_at, dr->of, sizeof(int32_t) * (size_t)n);
     }
     // a plan over device descriptors: this launch's picture table first, and its map (refused slots emptied) in place of the caller's
     const int32_t* d_of = dp ? dp->d_of : nullptr;
@@ -343,6 +347,13 @@ static int detect_enqueue(cb200_ctx* const* ctxs, int n_modes, const CameraBatch
             // a plan or a receivers call decodes under mode k's map, in which a slot the mode does not decode is empty
             const int32_t* map_k = dp ? plan_map(*dp, n_modes, n, k) : dr ? reinterpret_cast<const int32_t*>(d_tail + map_at[k]) : nullptr;
             Receivers r(map_k, dp ? dp->d_states[k] : dr ? dr->d_states[k] : nullptr);
+            if (dp && dp->d_words) {           // the launch's map, refused descriptors emptied; refused bytes shared by the modes
+                r.d_words = dp->d_words; r.receivers = dp->receivers; r.d_pic_of = d_of;
+                r.d_refused = d_refused;
+            } else if (dr && dr->words) {
+                r.d_words = dr->words; r.receivers = dr->count; r.d_pic_of = reinterpret_cast<const int32_t*>(d_tail + of_at);
+                r.d_refused = d_tail + refused_at + (size_t)k * n;
+            }
             rc = camera_after_scan(c, c0, batch(g), desc_g, flags, frames[g], k == lead[g], c->d_data, c->d_mask, nullptr, ds->status + (size_t)k * n,
                                    map_k ? &r : nullptr, slots_g);
         }
@@ -428,11 +439,10 @@ extern "C" int cb200_detect_scan_extract_decode_chunks_dev(cb200_ctx* const* ctx
     return detect_enqueue(ctxs, n_modes, b, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
 }
 
-extern "C" int cb200_detect_scan_extract_decode_chunks_receivers_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n,
-                                                                     uint32_t flags, const uint32_t* candidates, const int32_t* receiver_of,
-                                                                     int n_receivers, cb200_receiver_state* const* d_states, uint8_t* d_chunks,
-                                                                     uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode,
-                                                                     uint32_t* d_mode_masks)
+static int detect_receivers_call(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n, uint32_t flags,
+                                 const uint32_t* candidates, const int32_t* receiver_of, int n_receivers, cb200_receiver_state* const* d_states,
+                                 const uint32_t* words, uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode,
+                                 uint32_t* d_mode_masks)
 {
     CameraBatch b;
     auto build = [&](CameraBatch& bb) { return picture_batch(pics, n, bb); };
@@ -442,6 +452,28 @@ extern "C" int cb200_detect_scan_extract_decode_chunks_receivers_dev(cb200_ctx* 
     CK(cudaSetDevice(ctxs[0]->device), "cudaSetDevice");
     std::vector<uint32_t> all;
     if (!candidates) all.assign((size_t)n, (1u << n_modes) - 1);
-    const DetectReceivers dr = {candidates ? candidates : all.data(), receiver_of, n_receivers, d_states};
+    const DetectReceivers dr = {candidates ? candidates : all.data(), receiver_of, n_receivers, d_states, words};
     return detect_enqueue(ctxs, n_modes, b, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks, &dr);
+}
+
+extern "C" int cb200_detect_scan_extract_decode_chunks_receivers_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics, int n,
+                                                                     uint32_t flags, const uint32_t* candidates, const int32_t* receiver_of,
+                                                                     int n_receivers, cb200_receiver_state* const* d_states, uint8_t* d_chunks,
+                                                                     uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode,
+                                                                     uint32_t* d_mode_masks)
+{
+    return detect_receivers_call(ctxs, n_modes, pics, n, flags, candidates, receiver_of, n_receivers, d_states, nullptr, d_chunks, d_chunk_mask,
+                                 d_extract_status, d_mode, d_mode_masks);
+}
+
+extern "C" int cb200_detect_scan_extract_decode_chunks_receivers_flags_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* pics,
+                                                                           int n, uint32_t flags, const uint32_t* candidates,
+                                                                           const int32_t* receiver_of, int n_receivers,
+                                                                           cb200_receiver_state* const* d_states, const uint32_t* d_receiver_flags,
+                                                                           uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
+                                                                           int32_t* d_mode, uint32_t* d_mode_masks)
+{
+    const int rc = check_receiver_flags(d_receiver_flags, flags); if (rc) return rc;
+    return detect_receivers_call(ctxs, n_modes, pics, n, flags, candidates, receiver_of, n_receivers, d_states, d_receiver_flags, d_chunks,
+                                 d_chunk_mask, d_extract_status, d_mode, d_mode_masks);
 }

@@ -204,7 +204,7 @@ int make_plan(cb200_camera_plan* plan, const CameraBatch& b, Reserve&& reserve, 
 
 // a plain or receivers plan on context c (recv: the bound map and states; its d_map is allocated here) over the batch `build`
 // makes: the direct camera call's checks, with the plan's own after the batch's and after the CCM chain's, then the plan
-struct PlanReceivers { const int32_t* d_receiver_of; int n_receivers; cb200_receiver_state* d_states; };
+struct PlanReceivers { const int32_t* d_receiver_of; int n_receivers; cb200_receiver_state* d_states; const uint32_t* d_words; };
 
 template <class Build>
 int make_camera_plan(cb200_ctx* c, Build&& build, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
@@ -230,6 +230,8 @@ int make_camera_plan(cb200_ctx* c, Build&& build, uint32_t flags, uint8_t* d_chu
     auto enqueue = [&](const PicDesc* table) {
         if (!recv) return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, table);
         Receivers r(p->d_map.get(), p->d_states);
+        r.d_words = recv->d_words;
+        r.receivers = p->n_receivers;
         const int32_t* of = p->d_receiver_of;
         if (b.d_pics) {   // device descriptors: k_plan_pictures first, and the order from its map, in which refused slots are empty
             int rc = plan_pictures_launch(c, b, p->d_receiver_of, p->n_receivers, p->d_table); if (rc) return rc;
@@ -246,7 +248,8 @@ int make_camera_plan(cb200_ctx* c, Build&& build, uint32_t flags, uint8_t* d_chu
 // a detect receivers plan for the checked batch b (descriptors on the host, or in device memory within bounds)
 int make_detect_plan(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, uint32_t flags, const uint32_t* d_candidates,
                      const int32_t* d_receiver_of, int n_receivers, cb200_receiver_state* const* d_states, uint8_t* d_chunks,
-                     uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out)
+                     uint32_t* d_chunk_mask, int32_t* d_extract_status, int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out,
+                     const uint32_t* d_words = nullptr)
 {
     const int n = b.n();
     cb200_camera_plan* p = new cb200_camera_plan();
@@ -262,7 +265,7 @@ int make_detect_plan(cb200_ctx* const* ctxs, int n_modes, const CameraBatch& b, 
     };
     auto enqueue = [&](const PicDesc* table) {
         const DetectPlan dp = {table, d_candidates, d_receiver_of, n_receivers, p->d_mode_states.data(), p->d_map.get(), p->d_present.get(),
-                               b.d_pics ? p->d_table.get() : nullptr};
+                               b.d_pics ? p->d_table.get() : nullptr, d_words};
         return detect_plan_enqueue(ctxs, n_modes, b, flags, d_chunks, d_chunk_mask, d_extract_status, d_mode, d_mode_masks, dp);
     };
     return make_plan(p, b, reserve, enqueue, out);
@@ -289,7 +292,7 @@ int cb200_camera_plan_create_receivers(cb200_ctx* c, const cb200_picture* pics, 
     // reads), then the plan's own as cb200_camera_plan_create makes them
     int rc = check_receivers(c, d_receiver_of, n, n_receivers, d_states, true); if (rc) return rc;
     auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
-    const PlanReceivers recv = {d_receiver_of, n_receivers, d_states};
+    const PlanReceivers recv = {d_receiver_of, n_receivers, d_states, nullptr};
     return make_camera_plan(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
 }
 
@@ -302,7 +305,21 @@ int cb200_camera_plan_create_receivers_pictures_dev(cb200_ctx* c, const cb200_pi
     // launch checks on the device)
     int rc = check_receivers(c, d_receiver_of, n, n_receivers, d_states, true); if (rc) return rc;
     auto build = [&](CameraBatch& b) { return device_batch(d_pics, n, bounds, b); };
-    const PlanReceivers recv = {d_receiver_of, n_receivers, d_states};
+    const PlanReceivers recv = {d_receiver_of, n_receivers, d_states, nullptr};
+    return make_camera_plan(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
+}
+
+int cb200_camera_plan_create_receivers_pictures_flags_dev(cb200_ctx* c, const cb200_picture* d_pics, int n, const cb200_picture_bounds* bounds,
+                                                          uint32_t flags, const int32_t* d_receiver_of, int n_receivers,
+                                                          cb200_receiver_state* d_states, const uint32_t* d_receiver_flags, uint8_t* d_chunks,
+                                                          uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status,
+                                                          cb200_camera_plan** out)
+{
+    // the table's own checks, then cb200_camera_plan_create_receivers_pictures_dev's
+    int rc = check_receiver_flags(d_receiver_flags, flags); if (rc) return rc;
+    if ((rc = check_receivers(c, d_receiver_of, n, n_receivers, d_states, true))) return rc;
+    auto build = [&](CameraBatch& b) { return device_batch(d_pics, n, bounds, b); };
+    const PlanReceivers recv = {d_receiver_of, n_receivers, d_states, d_receiver_flags};
     return make_camera_plan(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &recv, out);
 }
 
@@ -334,6 +351,24 @@ int cb200_camera_plan_create_detect_receivers_pictures_dev(cb200_ctx* const* ctx
     if (rc) return rc;
     return make_detect_plan(ctxs, n_modes, b, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks, d_chunk_mask,
                             d_extract_status, d_mode, d_mode_masks, out);
+}
+
+
+int cb200_camera_plan_create_detect_receivers_pictures_flags_dev(cb200_ctx* const* ctxs, int n_modes, const cb200_picture* d_pics, int n,
+                                                                 const cb200_picture_bounds* bounds, uint32_t flags, const uint32_t* d_candidates,
+                                                                 const int32_t* d_receiver_of, int n_receivers,
+                                                                 cb200_receiver_state* const* d_states, const uint32_t* d_receiver_flags,
+                                                                 uint8_t* d_chunks, uint32_t* d_chunk_mask, int32_t* d_extract_status,
+                                                                 int32_t* d_mode, uint32_t* d_mode_masks, cb200_camera_plan** out)
+{
+    // the table's own checks, then cb200_camera_plan_create_detect_receivers_pictures_dev's
+    int rc = check_receiver_flags(d_receiver_flags, flags); if (rc) return rc;
+    CameraBatch b;
+    rc = check_detect_plan(ctxs, n_modes, d_pics, true, bounds, n, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks,
+                           d_chunk_mask, d_extract_status, d_mode, out, b);
+    if (rc) return rc;
+    return make_detect_plan(ctxs, n_modes, b, flags, d_candidates, d_receiver_of, n_receivers, d_states, d_chunks, d_chunk_mask,
+                            d_extract_status, d_mode, d_mode_masks, out, d_receiver_flags);
 }
 
 

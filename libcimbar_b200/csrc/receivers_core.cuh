@@ -47,7 +47,8 @@ CB_HD int step(const int32_t* of, const int32_t* order, const uint8_t* valid, in
 }
 
 // the host side: the stable receiver-major order of n pictures of receivers [0, receivers), every of[i] in range or -1 for an empty
-// slot (a detect receivers call's, below), which goes after every other
+// slot (a detect receivers call's, below), which goes after every other.  (A receiver flags table's refused receivers are emptied
+// on the device after the order is built: their runs of -1 stay where their receivers were)
 inline void make_order(const int32_t* of, int n, int receivers, int32_t* order)
 {
     std::vector<int32_t> first((size_t)receivers + 2, 0);
@@ -137,6 +138,23 @@ CB_HD void plan_slot(uint32_t cand, int32_t r, int receivers, int n_modes, const
     }
     for (int g = 0; g < n_geoms; ++g) present[(size_t)g * n + i] = (uint8_t)(geoms >> g & 1u);
 }
+
+// A receiver flags table (cb200_scan_extract_decode_chunks_receivers_flags_dev and its plan): one word per receiver with that
+// receiver's own sharpen policy and colour correction, read on the device.  A word is valid when it holds no bit but these four, and
+// at most one of each pair (as check_camera_flags requires of a call's flags); a receiver with an invalid word is refused.  Bits
+// 0x2 SHARPEN, 0x20 SHARPEN_IF_NEEDED, 0x4 CC_SIMPLE, 0x8 CC_FIT (include/cb200.h)
+constexpr uint32_t kWordSharpen = 0x2u, kWordSharpenIfNeeded = 0x20u, kWordCcSimple = 0x4u, kWordCcFit = 0x8u;
+constexpr uint32_t kWordBits = kWordSharpen | kWordSharpenIfNeeded | kWordCcSimple | kWordCcFit;
+CB_HD bool word_refused(uint32_t w)
+{
+    return (w & ~kWordBits) != 0 || (w & (kWordSharpen | kWordSharpenIfNeeded)) == (kWordSharpen | kWordSharpenIfNeeded) ||
+           (w & (kWordCcSimple | kWordCcFit)) == (kWordCcSimple | kWordCcFit);
+}
+// a valid word's sharpen decision for a picture whose extract status is st (2: NEEDS_SHARPEN), as the call with those flags makes it
+CB_HD bool word_sharpens(uint32_t w, int st) { return (w & kWordSharpen) != 0 || ((w & kWordSharpenIfNeeded) != 0 && st == 2); }
+// a valid word whose receiver's CCM passes through the call unchanged (no CC bit, or CC_FIT in a mode that never fits: `fits` false),
+// as the call with those flags leaves it; its pictures decode with the receiver's matrix, the identity when it is inactive
+CB_HD bool word_passes(uint32_t w, bool fits) { return !(w & kWordCcSimple) && !((w & kWordCcFit) && fits); }
 
 }  // namespace receivers
 }  // namespace cb200

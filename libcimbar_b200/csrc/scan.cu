@@ -668,7 +668,7 @@ int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, cons
         if (tail) memcpy(h_table + tail_at, tail->data(), tail->size());
         err = c->upload.send(st, slot, s->d_table, bytes); if (err) return err;
         d_desc = reinterpret_cast<const PicDesc*>(s->d_table.get());
-        if (recv) recv->d_map = reinterpret_cast<const int32_t*>(s->d_table + table_bytes);
+        if (recv) recv->map_on_device(reinterpret_cast<const int32_t*>(s->d_table + table_bytes), n);
         if (tail) *d_tail = s->d_table + tail_at;
     }
     if (d_desc_out) *d_desc_out = d_desc;
@@ -763,10 +763,15 @@ static int scan_results(cb200_ctx* c, int n, int32_t* anchors, int32_t* count, u
 }
 
 // Extractor::extract (Extractor.h:30-46) of every picture of a scan, on the device: one thread per picture.  slots: NULL, or picture
-// i of a sub-batch is the scan's picture slots[i] (a detect receivers call's geometry)
+// i of a sub-batch is the scan's picture slots[i] (a detect receivers call's geometry).  words: NULL, or a receiver flags table
+// (Receivers::d_words) with the batch's map `of` and refused bytes: a slot whose receiver's word is invalid leaves the map (receiver
+// -1) as refused, and every other slot's sharpen byte follows its receiver's word (an empty slot is not sharpened).  The receiver is
+// the picture's (pic_of, indexed as the scan's pictures and checked against [0, receivers)), so every mode of a detect call's geometry
+// takes the same sharpen bytes, whichever of them decodes the picture
+struct ExtractWords { const uint32_t* words; const int32_t* pic_of; int receivers; int32_t* of; uint8_t* refused; };
 __global__ void k_extract(const int4* __restrict__ anchors, const int* __restrict__ count, const int* __restrict__ scan_status, int n,
                           int width, int height, int32_t* __restrict__ status, double* __restrict__ minv, double* __restrict__ fwd,
-                          uint8_t* __restrict__ sharpen, const int32_t* __restrict__ slots)
+                          uint8_t* __restrict__ sharpen, const int32_t* __restrict__ slots, const ExtractWords xw)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -774,7 +779,16 @@ __global__ void k_extract(const int4* __restrict__ anchors, const int* __restric
     const int st = extract::extract_picture(reinterpret_cast<const Anchor*>(anchors + 4 * (size_t)s), count[s], (scan_status[s] & kScanOverflow) != 0,
                                             width, height, fwd + 9 * (size_t)i, minv + 9 * (size_t)i);
     status[i] = st;
-    if (sharpen) sharpen[i] = st == 2;             // CB200_FLAG_SHARPEN_IF_NEEDED: the CLI sharpens exactly the NEEDS_SHARPEN pictures
+    if (xw.words) {
+        const int32_t r = xw.pic_of[s];
+        const bool in = (uint32_t)r < (uint32_t)xw.receivers;          // !receivers::empty_slot(r, xw.receivers)
+        const uint32_t w = in ? xw.words[r] : 0u;
+        const bool bad = in && receivers::word_refused(w);
+        if (bad) { xw.of[i] = -1; xw.refused[i] = 1; }
+        sharpen[i] = in && !bad && receivers::word_sharpens(w, st);
+    } else if (sharpen) {
+        sharpen[i] = st == 2;                      // CB200_FLAG_SHARPEN_IF_NEEDED: the CLI sharpens exactly the NEEDS_SHARPEN pictures
+    }
 }
 
 // a picture that failed extraction yields no chunks.  of: NULL, or the receivers map, where an empty slot (receiver -1) yields no
@@ -787,6 +801,14 @@ __global__ void k_mask_failed(int32_t* __restrict__ status, int n, uint32_t* __r
     if (i >= n) return;
     if (of && of[i] < 0) status[i] = refused && refused[i] ? CB200_EXTRACT_REFUSED : CB200_EXTRACT_EMPTY;
     if (status[i] <= 0) mask[i] = 0;
+}
+
+// a receivers call with a flags table: the record (record_bytes) of every refused picture zeroed, one CTA per picture
+__global__ void k_zero_refused(const int32_t* __restrict__ status, uint8_t* __restrict__ records, int record_bytes)
+{
+    if (status[blockIdx.x] != CB200_EXTRACT_REFUSED) return;
+    uint8_t* r = records + (size_t)blockIdx.x * record_bytes;
+    for (int k = threadIdx.x; k < record_bytes; k += blockDim.x) r[k] = 0;
 }
 
 int camera_reserve_for(cb200_ctx* c, const int32_t* wh, int n, bool scans, bool walks)
@@ -817,10 +839,16 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     const int n = b.n();
     ScanScratch* s = sstate(c);
     const ScanScratch* s0 = scanned->scan;
-    const bool if_needed = (flags & CB200_FLAG_SHARPEN_IF_NEEDED) != 0;
+    // a flags table's slots are refused and their sharpen bytes written by k_extract, which may rewrite the map in place (the map is
+    // this call's upload, or the plan's own)
+    const uint32_t* words = recv ? recv->d_words : nullptr;
+    const bool if_needed = (flags & CB200_FLAG_SHARPEN_IF_NEEDED) != 0 || words;
     uint8_t* d_sharp = if_needed ? c->d_sel + 4 * (size_t)n : nullptr;
+    ExtractWords xw = {};
+    if (words) xw = {words, recv->d_pic_of ? recv->d_pic_of : recv->d_map, recv->receivers, const_cast<int32_t*>(recv->d_map),
+                     const_cast<uint8_t*>(recv->d_refused)};
     k_extract<<<(n + 127) / 128, 128, 0, c->stream>>>(s0->d_anchors, s0->d_count, s0->d_status, n, m.width, m.height, d_status, s->d_minv, s->d_fwd, d_sharp,
-                                                      d_slots);
+                                                      d_slots, xw);
     count_launch();
     CK(cudaGetLastError(), "extract launch");
     s->camera_n = n;
@@ -831,6 +859,11 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv ? recv->d_map : nullptr, recv ? recv->d_refused : nullptr);
     count_launch();
     CK(cudaGetLastError(), "mask launch");
+    if (words) {
+        k_zero_refused<<<n, 256, 0, c->stream>>>(d_status, d_chunks, m.data_bytes);
+        count_launch();
+        CK(cudaGetLastError(), "zero refused launch");
+    }
     return CB200_OK;
 }
 
@@ -846,6 +879,16 @@ int camera_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* 
     const PicDesc* d_desc;
     rc = camera_scan(c, b, d_table, &d_desc, recv); if (rc) return rc;
     return camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_mask, d_frame_flags, d_status, recv);
+}
+
+int check_receiver_flags(const uint32_t* d_receiver_flags, uint32_t flags)
+{
+    if (!d_receiver_flags) return fail(CB200_ERR_ARG, "null d_receiver_flags");
+    if (reinterpret_cast<uintptr_t>(d_receiver_flags) % 4) return fail(CB200_ERR_ARG, "d_receiver_flags is not 4-byte aligned");
+    if (flags & receivers::kWordBits)
+        return fail(CB200_ERR_ARG, "flags hold a per-receiver bit (SHARPEN, SHARPEN_IF_NEEDED, CC_SIMPLE, CC_FIT): those come from "
+                                   "d_receiver_flags");
+    return CB200_OK;
 }
 
 int check_camera_flags(uint32_t flags)
@@ -876,8 +919,8 @@ static int scan_extract_decode(cb200_ctx* c, Build&& build, uint32_t flags, uint
     return fetch_fountain(c, n, s->d_ext_status, chunks_out, chunk_count, chunk_mask, frame_flags, extract_status);
 }
 
-// the receiver arguments of cb200_scan_extract_decode_chunks_receivers_dev
-struct ReceiverArgs { const int32_t* of; int n, count; cb200_receiver_state* d_states; };
+// the receiver arguments of cb200_scan_extract_decode_chunks_receivers_dev (and the flags table of its _flags_ form, else NULL)
+struct ReceiverArgs { const int32_t* of; int n, count; cb200_receiver_state* d_states; const uint32_t* d_words; };
 
 // the enqueue-only camera entry points on device pictures.  A receivers call (ra) checks its receivers first; it is never chained,
 // so with no pictures it does nothing
@@ -893,6 +936,7 @@ static int scan_extract_decode_dev(cb200_ctx* c, Build&& build, uint32_t flags, 
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     if (!ra) return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
     Receivers r(ra->of, b.n(), ra->count, ra->d_states);
+    if ((r.d_words = ra->d_words)) { r.refused_bytes(b.n()); r.receivers = ra->count; }
     return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, &r);
 }
 
@@ -1017,7 +1061,18 @@ int cb200_scan_extract_decode_chunks_receivers_dev(cb200_ctx* c, const cb200_pic
                                                    uint8_t* d_frame_flags, int32_t* d_extract_status)
 {
     auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
-    const ReceiverArgs ra = {receiver_of, n, n_receivers, d_states};
+    const ReceiverArgs ra = {receiver_of, n, n_receivers, d_states, nullptr};
+    return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &ra);
+}
+
+int cb200_scan_extract_decode_chunks_receivers_flags_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags,
+                                                         const int32_t* receiver_of, int n_receivers, cb200_receiver_state* d_states,
+                                                         const uint32_t* d_receiver_flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                                         uint8_t* d_frame_flags, int32_t* d_extract_status)
+{
+    int rc = check_receiver_flags(d_receiver_flags, flags); if (rc) return rc;
+    auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
+    const ReceiverArgs ra = {receiver_of, n, n_receivers, d_states, d_receiver_flags};
     return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &ra);
 }
 
