@@ -577,10 +577,11 @@ int cb200_camera_plan_create_detect_receivers(cb200_ctx* const* ctxs, int n_mode
    three channels are equal) or three YCbCr components (JFIF, no APP marker, or Adobe APP14 with transform 1), luma sampling 1x1,
    2x1, 1x2 or 2x2 with chroma 1x1 (4:4:4, 4:2:2, 4:4:0, 4:2:0), any restart interval, EXIF orientation 1-8, and output sizes the
    camera path accepts (short side 60 .. 4499).  Anything else -- arithmetic coding, 12-bit, lossless, hierarchical, CMYK, Adobe
-   transform 0 / 2, other sampling layouts such as 4:1:1, a progressive script that leaves the first coefficients incomplete,
-   truncated headers, bytes that are not a JPEG file -- fails the whole call with CB200_ERR_ARG before any CUDA call, and
-   cb200_last_error names the picture and the reason.  Entropy-coded data that turn out corrupt or truncated are found on the
-   device: that picture gets status -2 (and is written black); the other pictures are unaffected. */
+   transform 0 / 2, other sampling layouts such as 4:1:1, truncated headers, bytes that are not a JPEG file -- fails the whole call
+   with CB200_ERR_ARG before any CUDA call, and cb200_last_error names the picture and the reason.  Entropy-coded data that turn
+   out corrupt or truncated are found on the device: that picture gets status -2 (and is written black); the other pictures are
+   unaffected.  After a file's first scan, whatever would be refused (a marker that cannot follow a scan, a malformed marker
+   segment, a progressive script that leaves the first coefficients incomplete) is taken for corrupt data too: status -2. */
 
 /* the output size of one file (after the EXIF orientation), or CB200_ERR_ARG with the refusal reason.  Host only: no context,
    no CUDA call */

@@ -7,13 +7,17 @@
 //   jdhuff.c  jpeg_make_d_derived_tbl (canonical codes, 9-bit look-ahead), decode_mcu (sequential), HUFF_EXTEND
 //   jdphuff.c decode_mcu_DC_first / _AC_first / _DC_refine / _AC_refine (EOBRUN, correction bits), start_pass_phuff_decoder's checks
 //   jidctint.c jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2) with the post-IDCT range limit
-//   jdsample.c h2v1_fancy_upsample, h1v2_fancy_upsample, h2v2_fancy_upsample (edge samples replicated, as jdmainct.c's context rows)
+//   jdsample.c h2v1_fancy_upsample, h1v2_fancy_upsample, h2v2_fancy_upsample (edge samples replicated, as jdmainct.c's context rows);
+//              h2v1_upsample / h2v2_upsample (plain replication) where jinit_upsampler picks them: a component downsampled
+//              horizontally whose downsampled_width is 2 or less (pictures up to 4 pixels wide in 4:2:2 and 4:2:0)
 //   jdcolor.c  build_ycc_rgb_table + ycc_rgb_convert (SCALEBITS 16), gray_rgb_convert
 //   OpenCV     JpegDecoder's first APP1 -> ExifReader orientation -> ApplyExifOrientation (flip / transpose)
 // Supported: SOF0/1/2, 8-bit, one component or three YCbCr components, luma 1x1 / 2x1 / 1x2 / 2x2 with chroma 1x1, any restart
 // interval.  Everything else is refused by parse() with a reason.  Corrupt entropy-coded data (a code that is not in the table, a
 // run past the band, a segment that ends early or carries whole unused bytes) is detected, not repaired: the segment's decode
-// reports it and the picture is reported, never decoded approximately.
+// reports it and the picture is reported, never decoded approximately.  After the first scan, whatever parse() would refuse (a
+// marker that cannot follow a scan, a malformed marker segment, bytes that are not a marker, a scan script cut short) is such
+// data too: a lost FF 00 stuffing byte or a flipped bit makes a false marker of any kind.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -453,89 +457,110 @@ JD_HD bool decode_refine(const uint8_t* u, uint32_t ulen, const Pic& P, const Sc
 
 // ---- IDCT, upsampling, colour ---------------------------------------------------------------------------------------------
 
-JD_HD uint8_t idct_limit(int v)          // the post-IDCT range limit (v centred on 0)
+JD_HD uint8_t idct_limit(int64_t v)      // the post-IDCT range limit (v centred on 0)
 {
     v += 128;
     return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v);
 }
 
-// jpeg_idct_islow: the 64 coefficients of one block (natural order) with their quantisation table -> 8 x 8 samples at out (stride)
-JD_HD void idct_islow(const int16_t* in, const uint16_t* q, uint8_t* out, size_t stride)
+JD_HD int wrap32(int64_t v) { return (int)(uint32_t)(uint64_t)v; }   // (int) of a JLONG, as jidctint.c stores its workspace
+
+JD_HD void note_wide(int* wide, int64_t v, int64_t lo, int64_t hi) { if (wide && (v < lo || v > hi)) *wide = 1; }
+
+// jpeg_idct_islow: the 64 coefficients of one block (natural order) with their quantisation table -> 8 x 8 samples at out (stride).
+// The arithmetic is jidctint.c's: 64-bit intermediates (JLONG on LP64), an int workspace, so no input overflows.  Where libjpeg-
+// turbo's own IDCTs disagree -- a dequantised coefficient or a workspace value beyond 16 bits (its SIMD IDCT's pmullw / packssdw),
+// an output beyond [-512, 511] before the range limit (its C IDCT's `& RANGE_MASK` wraps) -- this one clamps, and *wide (when
+// given) is set to 1.  No encoder writes such blocks; damaged or hand-made coefficients can
+JD_HD void idct_islow(const int16_t* in, const uint16_t* q, uint8_t* out, size_t stride, int* wide = nullptr)
 {
     constexpr int CB = 13, P1 = 2;
-    constexpr int F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633, F1501 = 12299,
-                  F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
+    constexpr int64_t F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633, F1501 = 12299,
+                      F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
     int ws[64];
     for (int c = 0; c < 8; ++c) {
         const int16_t* ip = in + c;
         const uint16_t* qp = q + c;
         int* wp = ws + c;
+        int64_t dq[8];                                        // DEQUANTIZE: 16 x 16-bit products (MULTIPLIER short)
+        for (int r = 0; r < 8; ++r) {
+            dq[r] = (int64_t)((int)ip[8 * r] * (int)(int16_t)qp[8 * r]);
+            note_wide(wide, dq[r], -32768, 32767);
+        }
         if (!ip[8] && !ip[16] && !ip[24] && !ip[32] && !ip[40] && !ip[48] && !ip[56]) {
-            const int dc = (int)ip[0] * (int)(int16_t)qp[0] * (1 << P1);
-            for (int r = 0; r < 8; ++r) wp[8 * r] = dc;
+            const int64_t dc = dq[0] * (1 << P1);
+            note_wide(wide, dc, -32768, 32767);
+            for (int r = 0; r < 8; ++r) wp[8 * r] = wrap32(dc);
             continue;
         }
-        int z2 = (int)ip[16] * (int)(int16_t)qp[16], z3 = (int)ip[48] * (int)(int16_t)qp[48];
-        int z1 = (z2 + z3) * F0541;
-        int tmp2 = z1 + z3 * -F1847, tmp3 = z1 + z2 * F0765;
-        z2 = (int)ip[0] * (int)(int16_t)qp[0];
-        z3 = (int)ip[32] * (int)(int16_t)qp[32];
-        int tmp0 = (int)((unsigned)(z2 + z3) << CB), tmp1 = (int)((unsigned)(z2 - z3) << CB);
-        const int tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
-        tmp0 = (int)ip[56] * (int)(int16_t)qp[56];
-        tmp1 = (int)ip[40] * (int)(int16_t)qp[40];
-        tmp2 = (int)ip[24] * (int)(int16_t)qp[24];
-        tmp3 = (int)ip[8] * (int)(int16_t)qp[8];
+        int64_t z2 = dq[2], z3 = dq[6];
+        int64_t z1 = (z2 + z3) * F0541;
+        int64_t tmp2 = z1 + z3 * -F1847, tmp3 = z1 + z2 * F0765;
+        z2 = dq[0];
+        z3 = dq[4];
+        int64_t tmp0 = (z2 + z3) * (1 << CB), tmp1 = (z2 - z3) * (1 << CB);
+        const int64_t tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
+        tmp0 = dq[7]; tmp1 = dq[5]; tmp2 = dq[3]; tmp3 = dq[1];
         z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2;
-        int z4 = tmp1 + tmp3;
-        const int z5 = (z3 + z4) * F1175;
+        int64_t z4 = tmp1 + tmp3;
+        const int64_t z5 = (z3 + z4) * F1175;
         tmp0 *= F0298; tmp1 *= F2053; tmp2 *= F3072; tmp3 *= F1501;
         z1 *= -F0899; z2 *= -F2562; z3 *= -F1961; z4 *= -F0390;
         z3 += z5; z4 += z5;
         tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
-        constexpr int S = CB - P1, R = 1 << (S - 1);
-        wp[0] = (tmp10 + tmp3 + R) >> S;  wp[56] = (tmp10 - tmp3 + R) >> S;
-        wp[8] = (tmp11 + tmp2 + R) >> S;  wp[48] = (tmp11 - tmp2 + R) >> S;
-        wp[16] = (tmp12 + tmp1 + R) >> S; wp[40] = (tmp12 - tmp1 + R) >> S;
-        wp[24] = (tmp13 + tmp0 + R) >> S; wp[32] = (tmp13 - tmp0 + R) >> S;
+        constexpr int S = CB - P1;
+        constexpr int64_t R = (int64_t)1 << (S - 1);
+        const int64_t v[8] = {tmp10 + tmp3, tmp11 + tmp2, tmp12 + tmp1, tmp13 + tmp0, tmp13 - tmp0, tmp12 - tmp1, tmp11 - tmp2, tmp10 - tmp3};
+        for (int r = 0; r < 8; ++r) {
+            const int64_t d = (v[r] + R) >> S;
+            note_wide(wide, d, -32768, 32767);
+            wp[8 * r] = wrap32(d);
+        }
     }
     for (int r = 0; r < 8; ++r) {
         const int* wp = ws + 8 * r;
         uint8_t* op = out + (size_t)r * stride;
         if (!wp[1] && !wp[2] && !wp[3] && !wp[4] && !wp[5] && !wp[6] && !wp[7]) {
-            const uint8_t v = idct_limit((wp[0] + (1 << (P1 + 2))) >> (P1 + 3));
+            const int64_t d = ((int64_t)wp[0] + (1 << (P1 + 2))) >> (P1 + 3);
+            note_wide(wide, d, -512, 511);
+            const uint8_t v = idct_limit(d);
             for (int c = 0; c < 8; ++c) op[c] = v;
             continue;
         }
-        int z2 = wp[2], z3 = wp[6];
-        int z1 = (z2 + z3) * F0541;
-        int tmp2 = z1 + z3 * -F1847, tmp3 = z1 + z2 * F0765;
-        int tmp0 = (int)((unsigned)(wp[0] + wp[4]) << CB), tmp1 = (int)((unsigned)(wp[0] - wp[4]) << CB);
-        const int tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
+        int64_t z2 = wp[2], z3 = wp[6];
+        int64_t z1 = (z2 + z3) * F0541;
+        int64_t tmp2 = z1 + z3 * -F1847, tmp3 = z1 + z2 * F0765;
+        int64_t tmp0 = ((int64_t)wp[0] + wp[4]) * (1 << CB), tmp1 = ((int64_t)wp[0] - wp[4]) * (1 << CB);
+        const int64_t tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
         tmp0 = wp[7]; tmp1 = wp[5]; tmp2 = wp[3]; tmp3 = wp[1];
         z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2;
-        int z4 = tmp1 + tmp3;
-        const int z5 = (z3 + z4) * F1175;
+        int64_t z4 = tmp1 + tmp3;
+        const int64_t z5 = (z3 + z4) * F1175;
         tmp0 *= F0298; tmp1 *= F2053; tmp2 *= F3072; tmp3 *= F1501;
         z1 *= -F0899; z2 *= -F2562; z3 *= -F1961; z4 *= -F0390;
         z3 += z5; z4 += z5;
         tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
-        constexpr int S = CB + P1 + 3, R = 1 << (S - 1);
-        op[0] = idct_limit((tmp10 + tmp3 + R) >> S); op[7] = idct_limit((tmp10 - tmp3 + R) >> S);
-        op[1] = idct_limit((tmp11 + tmp2 + R) >> S); op[6] = idct_limit((tmp11 - tmp2 + R) >> S);
-        op[2] = idct_limit((tmp12 + tmp1 + R) >> S); op[5] = idct_limit((tmp12 - tmp1 + R) >> S);
-        op[3] = idct_limit((tmp13 + tmp0 + R) >> S); op[4] = idct_limit((tmp13 - tmp0 + R) >> S);
+        constexpr int S = CB + P1 + 3;
+        constexpr int64_t R = (int64_t)1 << (S - 1);
+        const int64_t v[8] = {tmp10 + tmp3, tmp11 + tmp2, tmp12 + tmp1, tmp13 + tmp0, tmp13 - tmp0, tmp12 - tmp1, tmp11 - tmp2, tmp10 - tmp3};
+        for (int c = 0; c < 8; ++c) {
+            const int64_t d = (v[c] + R) >> S;
+            note_wide(wide, d, -512, 511);
+            op[c] = idct_limit(d);
+        }
     }
 }
 
-// one full-resolution sample (x, y) of component C, upsampled as jdsample.c's fancy upsamplers do
+// one full-resolution sample (x, y) of component C, upsampled as jdsample.c's jinit_upsampler chooses: a component downsampled
+// horizontally (h2v1, h2v2) is filtered only when its downsampled_width is above 2, else replicated (h2v1_upsample /
+// h2v2_upsample, which do not filter vertically either); h1v2 is always filtered
 JD_HD int sample(const uint8_t* planes, const Pic& P, const Comp& C, int x, int y)
 {
     const uint8_t* p = planes + C.plane;
     const size_t st = (size_t)C.bw * 8;
     const int hr = P.hmax / C.h, vr = P.vmax / C.v;
     const int cx = x / hr, cy = y / vr;
-    if (hr == 1 && vr == 1) return p[(size_t)cy * st + cx];
+    if ((hr == 1 && vr == 1) || (hr == 2 && C.dw <= 2)) return p[(size_t)cy * st + cx];
     if (vr == 1) {                       // h2v1
         const int n = (x & 1) ? (cx + 1 < C.dw ? cx + 1 : cx) : (cx > 0 ? cx - 1 : 0);
         return (3 * p[(size_t)cy * st + cx] + p[(size_t)cy * st + n] + ((x & 1) ? 2 : 1)) >> 2;
@@ -648,7 +673,8 @@ inline int exif_orientation(const uint8_t* d, size_t len)
 }
 
 // the markers of one file: "" and P filled, or the reason the file is refused.  Entropy-coded data are only split at their
-// restart markers here; a file that ends inside them or before its last scan is accepted with P.pic.bad = 1
+// restart markers here; a file that ends inside them or before its last scan, or whose markers after its first scan would be
+// refused, is accepted with P.pic.bad = 1
 inline std::string parse(const uint8_t* f, size_t n, Parsed& P)
 {
     P = Parsed();
@@ -666,222 +692,229 @@ inline std::string parse(const uint8_t* f, size_t n, Parsed& P)
     int coef_bits[3][64];
     for (auto& cb : coef_bits) for (int& v : cb) v = -1;
     bool progressive = false, in_scan = false;
-    while (!eoi) {
-        // the next marker: FF (fill FFs) code
-        if (pos >= n || f[pos] != 0xFF) {
-            if (!P.scans.empty() && pos >= n) { pic.bad = 1; break; }    // ends after a scan's data without EOI
-            return P.scans.empty() ? "truncated or malformed JPEG header" : "malformed JPEG marker after a scan";
-        }
-        while (pos < n && f[pos] == 0xFF) ++pos;
-        if (pos >= n) { if (P.scans.empty()) return "truncated JPEG header"; pic.bad = 1; break; }
-        const unsigned m = f[pos++];
-        if (m == 0xD9) { eoi = true; break; }
-        if (m == 0xD8 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) {
-            if (m >= 0xD0 && m <= 0xD7 && !P.scans.empty()) { pic.bad = 1; continue; }   // a restart marker out of place
-            return "unexpected marker in the JPEG header";
-        }
-        if (pos + 2 > n) { if (P.scans.empty()) return "truncated JPEG header"; pic.bad = 1; break; }
-        const size_t len = be16(f + pos);
-        if (len < 2 || pos + len > n) { if (P.scans.empty()) return "truncated JPEG header"; pic.bad = 1; break; }
-        const uint8_t* d = f + pos + 2;
-        const size_t dl = len - 2;
-        pos += len;
-        if (m == 0xC0 || m == 0xC1 || m == 0xC2) {
-            if (frame) return "more than one frame header";
-            frame = true;
-            progressive = m == 0xC2;
-            if (dl < 6) return "truncated frame header";
-            if (d[0] != 8) return std::to_string(d[0]) + "-bit samples (only 8-bit JPEG is supported)";
-            pic.h = (int)be16(d + 1); pic.w = (int)be16(d + 3); pic.ncomp = d[5];
-            if (pic.h == 0) return "a frame header with height 0 (DNL) is not supported";
-            if (pic.w == 0) return "a frame header with width 0";
-            if (pic.ncomp == 4) return "4 components (CMYK / YCCK) are not supported";
-            if (pic.ncomp != 1 && pic.ncomp != 3) return std::to_string(pic.ncomp) + " components (only grey or YCbCr are supported)";
-            if (dl < 6 + 3 * (size_t)pic.ncomp) return "truncated frame header";
-            for (int c = 0; c < pic.ncomp; ++c) {
-                cid[c] = d[6 + 3 * c];
-                pic.comp[c].h = d[7 + 3 * c] >> 4; pic.comp[c].v = d[7 + 3 * c] & 15;
-                cq[c] = d[8 + 3 * c];
-                if (pic.comp[c].h < 1 || pic.comp[c].h > 4 || pic.comp[c].v < 1 || pic.comp[c].v > 4 || cq[c] > 3)
-                    return "a frame header with bad sampling factors or table numbers";
-            }
-            if (pic.ncomp == 3) {
-                const Comp* c = pic.comp;
-                if (c[1].h != 1 || c[1].v != 1 || c[2].h != 1 || c[2].v != 1 || c[0].h > 2 || c[0].v > 2)
-                    return "sampling " + std::to_string(c[0].h) + "x" + std::to_string(c[0].v) + ", " + std::to_string(c[1].h) + "x" +
-                           std::to_string(c[1].v) + ", " + std::to_string(c[2].h) + "x" + std::to_string(c[2].v) +
-                           " (only 4:4:4, 4:2:2, 4:4:0 and 4:2:0 are supported)";
-                pic.hmax = c[0].h; pic.vmax = c[0].v;
-            } else {
-                pic.hmax = pic.comp[0].h; pic.vmax = pic.comp[0].v;
-            }
-            const int mcux = (pic.w + 8 * pic.hmax - 1) / (8 * pic.hmax), mcuy = (pic.h + 8 * pic.vmax - 1) / (8 * pic.vmax);
-            for (int c = 0; c < pic.ncomp; ++c) {
-                Comp& C = pic.comp[c];
-                if (pic.ncomp == 1) { C.h = C.v = 1; pic.hmax = pic.vmax = 1; }   // one component: one block per MCU
-                const int mx = pic.ncomp == 1 ? (pic.w + 7) / 8 : mcux, my = pic.ncomp == 1 ? (pic.h + 7) / 8 : mcuy;
-                C.bw = mx * C.h; C.bh = my * C.v;
-                C.wib = (pic.w * C.h + 8 * pic.hmax - 1) / (8 * pic.hmax);
-                C.hib = (pic.h * C.v + 8 * pic.vmax - 1) / (8 * pic.vmax);
-                C.dw = (pic.w * C.h + pic.hmax - 1) / pic.hmax;
-                C.dh = (pic.h * C.v + pic.vmax - 1) / pic.vmax;
-            }
-        } else if (m == 0xC3 || (m >= 0xC5 && m <= 0xC7)) {
-            return "lossless or hierarchical JPEG (SOF" + std::to_string(m - 0xC0) + ") is not supported";
-        } else if ((m >= 0xC9 && m <= 0xCB) || (m >= 0xCD && m <= 0xCF) || m == 0xCC) {
-            return "arithmetic-coded JPEG is not supported";
-        } else if (m == 0xC8 || (m >= 0xF0 && m <= 0xFD) || m == 0xDE || m == 0xDF) {
-            return "unsupported JPEG extension marker";
-        } else if (m == 0xC4) {
-            size_t o = 0;
-            while (o < dl) {
-                if (o + 17 > dl) return "truncated Huffman table";
-                const int tc = d[o] >> 4, th = d[o] & 15;
-                if (tc > 1 || th > 3) return "bad Huffman table number";
-                int cnt = 0;
-                for (int l = 0; l < 16; ++l) cnt += d[o + 1 + l];
-                if (cnt > 256 || o + 17 + (size_t)cnt > dl) return "bad Huffman table";
-                Huff t;
-                const std::string why = derive(d + o + 1, d + o + 17, cnt, tc == 0, t);
-                if (!why.empty()) return why;
-                (tc == 0 ? dc_tab : ac_tab)[th] = (int)P.huffs.size();
-                P.huffs.push_back(t);
-                o += 17 + (size_t)cnt;
-            }
-        } else if (m == 0xDB) {
-            size_t o = 0;
-            while (o < dl) {
-                const int pq = d[o] >> 4, tq = d[o] & 15;
-                if (pq > 1 || tq > 3 || o + 1 + 64 * (size_t)(pq + 1) > dl) return "bad quantisation table";
-                for (int k = 0; k < 64; ++k)
-                    qtab[tq][zigzag(k)] = (uint16_t)(pq ? be16(d + o + 1 + 2 * k) : d[o + 1 + k]);
-                qdef[tq] = true;
-                o += 1 + 64 * (size_t)(pq + 1);
-            }
-        } else if (m == 0xDD) {
-            if (dl < 2) return "truncated restart interval";
-            restart = (int)be16(d);
-        } else if (m == 0xDC) {
-            return "a DNL marker is not supported";
-        } else if (m == 0xE0) {
-            if (dl >= 5 && !memcmp(d, "JFIF", 5)) jfif = true;
-        } else if (m == 0xE1) {
-            if (!exif_seen && P.scans.empty()) { exif_seen = true; pic.orient = exif_orientation(d, dl); }
-        } else if (m == 0xEE) {
-            if (dl >= 12 && !memcmp(d, "Adobe", 5)) { adobe = true; adobe_transform = d[11]; }
-        } else if (m == 0xDA) {
-            if (!frame) return "a scan before the frame header";
-            if (dl < 1) return "truncated scan header";
-            Scan sc;
-            memset(&sc, 0, sizeof(sc));
-            sc.ncomp = d[0];
-            if (sc.ncomp < 1 || sc.ncomp > pic.ncomp || dl < 4 + 2 * (size_t)sc.ncomp) return "bad scan header";
-            const uint8_t* e = d + 1 + 2 * sc.ncomp;
-            sc.ss = e[0]; sc.se = e[1];
-            const int ah = e[2] >> 4;
-            sc.al = e[2] & 15;
-            int comps[4];
-            for (int j = 0; j < sc.ncomp; ++j) {
-                int c = -1;
-                for (int k = 0; k < pic.ncomp; ++k) if (cid[k] == d[1 + 2 * j]) c = k;
-                if (c < 0) return "a scan names a component the frame does not have";
-                comps[j] = c;
-                const int td = d[2 + 2 * j] >> 4, ta = d[2 + 2 * j] & 15;
-                if (td > 3 || ta > 3) return "bad Huffman table number in a scan";
-                const bool need_dc = !progressive || (sc.ss == 0 && ah == 0), need_ac = !progressive || sc.ss > 0;
-                if ((need_dc && dc_tab[td] < 0) || (need_ac && ac_tab[ta] < 0)) return "a scan uses an undefined Huffman table";
-                sc.dc[j] = (uint32_t)(dc_tab[td] < 0 ? 0 : dc_tab[td]);
-                sc.ac[j] = (uint32_t)(ac_tab[ta] < 0 ? 0 : ac_tab[ta]);
-                if (!latched[c]) {
-                    if (!qdef[cq[c]]) return "a component's quantisation table is not defined";
-                    P.quant.resize(64 * (size_t)pic.ncomp);
-                    memcpy(&P.quant[64 * (size_t)c], qtab[cq[c]], sizeof(qtab[0]));
-                    latched[c] = true;
+    // Once a scan has been read, whatever the marker walk would refuse is taken for corrupt data: a lost FF 00 stuffing byte or a
+    // flipped bit turns entropy-coded bytes into a false marker of any kind (or into bytes that are not a marker), with any length
+    // and contents.  So after the first scan a refusal marks the picture (status -2) instead of failing the whole call
+    const auto markers = [&]() -> std::string {
+        while (!eoi) {
+            // the next marker: FF (fill FFs) code
+            if (pos >= n || f[pos] != 0xFF) return "truncated or malformed JPEG header";
+            while (pos < n && f[pos] == 0xFF) ++pos;
+            if (pos >= n) return "truncated JPEG header";
+            const unsigned m = f[pos++];
+            if (m == 0xD9) { eoi = true; break; }
+            const bool between_scans = m == 0xC4 || m == 0xDA || m == 0xDB || m == 0xDD || (m >= 0xE0 && m <= 0xEF) || m == 0xFE;
+            if (!P.scans.empty() && !between_scans) return "a marker that cannot follow a scan";
+            if (m == 0xD8 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) return "unexpected marker in the JPEG header";
+            if (pos + 2 > n) return "truncated JPEG header";
+            const size_t len = be16(f + pos);
+            if (len < 2 || pos + len > n) return "truncated JPEG header";
+            const uint8_t* d = f + pos + 2;
+            const size_t dl = len - 2;
+            pos += len;
+            if (m == 0xC0 || m == 0xC1 || m == 0xC2) {
+                if (frame) return "more than one frame header";
+                frame = true;
+                progressive = m == 0xC2;
+                if (dl < 6) return "truncated frame header";
+                if (d[0] != 8) return std::to_string(d[0]) + "-bit samples (only 8-bit JPEG is supported)";
+                pic.h = (int)be16(d + 1); pic.w = (int)be16(d + 3); pic.ncomp = d[5];
+                if (pic.h == 0) return "a frame header with height 0 (DNL) is not supported";
+                if (pic.w == 0) return "a frame header with width 0";
+                if (pic.ncomp == 4) return "4 components (CMYK / YCCK) are not supported";
+                if (pic.ncomp != 1 && pic.ncomp != 3) return std::to_string(pic.ncomp) + " components (only grey or YCbCr are supported)";
+                if (dl < 6 + 3 * (size_t)pic.ncomp) return "truncated frame header";
+                for (int c = 0; c < pic.ncomp; ++c) {
+                    cid[c] = d[6 + 3 * c];
+                    pic.comp[c].h = d[7 + 3 * c] >> 4; pic.comp[c].v = d[7 + 3 * c] & 15;
+                    cq[c] = d[8 + 3 * c];
+                    if (pic.comp[c].h < 1 || pic.comp[c].h > 4 || pic.comp[c].v < 1 || pic.comp[c].v > 4 || cq[c] > 3)
+                        return "a frame header with bad sampling factors or table numbers";
                 }
-            }
-            if (progressive) {
-                bool bad = sc.ss == 0 ? sc.se != 0 : (sc.ss > sc.se || sc.se > 63 || sc.ncomp != 1);
-                if (ah != 0 && sc.al != ah - 1) bad = true;
-                if (sc.al > 13) bad = true;
-                if (bad) return "an invalid progressive scan";
+                if (pic.ncomp == 3) {
+                    const Comp* c = pic.comp;
+                    if (c[1].h != 1 || c[1].v != 1 || c[2].h != 1 || c[2].v != 1 || c[0].h > 2 || c[0].v > 2)
+                        return "sampling " + std::to_string(c[0].h) + "x" + std::to_string(c[0].v) + ", " + std::to_string(c[1].h) + "x" +
+                               std::to_string(c[1].v) + ", " + std::to_string(c[2].h) + "x" + std::to_string(c[2].v) +
+                               " (only 4:4:4, 4:2:2, 4:4:0 and 4:2:0 are supported)";
+                    pic.hmax = c[0].h; pic.vmax = c[0].v;
+                } else {
+                    pic.hmax = pic.comp[0].h; pic.vmax = pic.comp[0].v;
+                }
+                const int mcux = (pic.w + 8 * pic.hmax - 1) / (8 * pic.hmax), mcuy = (pic.h + 8 * pic.vmax - 1) / (8 * pic.vmax);
+                for (int c = 0; c < pic.ncomp; ++c) {
+                    Comp& C = pic.comp[c];
+                    if (pic.ncomp == 1) { C.h = C.v = 1; pic.hmax = pic.vmax = 1; }   // one component: one block per MCU
+                    const int mx = pic.ncomp == 1 ? (pic.w + 7) / 8 : mcux, my = pic.ncomp == 1 ? (pic.h + 7) / 8 : mcuy;
+                    C.bw = mx * C.h; C.bh = my * C.v;
+                    C.wib = (pic.w * C.h + 8 * pic.hmax - 1) / (8 * pic.hmax);
+                    C.hib = (pic.h * C.v + 8 * pic.vmax - 1) / (8 * pic.vmax);
+                    C.dw = (pic.w * C.h + pic.hmax - 1) / pic.hmax;
+                    C.dh = (pic.h * C.v + pic.vmax - 1) / pic.vmax;
+                }
+            } else if (m == 0xC3 || (m >= 0xC5 && m <= 0xC7)) {
+                return "lossless or hierarchical JPEG (SOF" + std::to_string(m - 0xC0) + ") is not supported";
+            } else if ((m >= 0xC9 && m <= 0xCB) || (m >= 0xCD && m <= 0xCF) || m == 0xCC) {
+                return "arithmetic-coded JPEG is not supported";
+            } else if (m == 0xC8 || (m >= 0xF0 && m <= 0xFD) || m == 0xDE || m == 0xDF) {
+                return "unsupported JPEG extension marker";
+            } else if (m == 0xC4) {
+                size_t o = 0;
+                while (o < dl) {
+                    if (o + 17 > dl) return "truncated Huffman table";
+                    const int tc = d[o] >> 4, th = d[o] & 15;
+                    if (tc > 1 || th > 3) return "bad Huffman table number";
+                    int cnt = 0;
+                    for (int l = 0; l < 16; ++l) cnt += d[o + 1 + l];
+                    if (cnt > 256 || o + 17 + (size_t)cnt > dl) return "bad Huffman table";
+                    Huff t;
+                    const std::string why = derive(d + o + 1, d + o + 17, cnt, tc == 0, t);
+                    if (!why.empty()) return why;
+                    (tc == 0 ? dc_tab : ac_tab)[th] = (int)P.huffs.size();
+                    P.huffs.push_back(t);
+                    o += 17 + (size_t)cnt;
+                }
+            } else if (m == 0xDB) {
+                size_t o = 0;
+                while (o < dl) {
+                    const int pq = d[o] >> 4, tq = d[o] & 15;
+                    if (pq > 1 || tq > 3 || o + 1 + 64 * (size_t)(pq + 1) > dl) return "bad quantisation table";
+                    for (int k = 0; k < 64; ++k)
+                        qtab[tq][zigzag(k)] = (uint16_t)(pq ? be16(d + o + 1 + 2 * k) : d[o + 1 + k]);
+                    qdef[tq] = true;
+                    o += 1 + 64 * (size_t)(pq + 1);
+                }
+            } else if (m == 0xDD) {
+                if (dl < 2) return "truncated restart interval";
+                restart = (int)be16(d);
+            } else if (m == 0xDC) {
+                return "a DNL marker is not supported";
+            } else if (m == 0xE0) {
+                if (dl >= 5 && !memcmp(d, "JFIF", 5)) jfif = true;
+            } else if (m == 0xE1) {
+                if (!exif_seen && P.scans.empty()) { exif_seen = true; pic.orient = exif_orientation(d, dl); }
+            } else if (m == 0xEE) {
+                if (dl >= 12 && !memcmp(d, "Adobe", 5)) { adobe = true; adobe_transform = d[11]; }
+            } else if (m == 0xDA) {
+                if (!frame) return "a scan before the frame header";
+                if (dl < 1) return "truncated scan header";
+                Scan sc;
+                memset(&sc, 0, sizeof(sc));
+                sc.ncomp = d[0];
+                if (sc.ncomp < 1 || sc.ncomp > pic.ncomp || dl < 4 + 2 * (size_t)sc.ncomp) return "bad scan header";
+                const uint8_t* e = d + 1 + 2 * sc.ncomp;
+                sc.ss = e[0]; sc.se = e[1];
+                const int ah = e[2] >> 4;
+                sc.al = e[2] & 15;
+                int comps[4];
                 for (int j = 0; j < sc.ncomp; ++j) {
-                    int* cb = coef_bits[comps[j]];
-                    if (sc.ss > 0 && cb[0] < 0) return "an AC scan before the component's DC scan";
-                    for (int k = sc.ss; k <= sc.se; ++k) {
-                        if (ah != (cb[k] < 0 ? 0 : cb[k])) return "an inconsistent progression sequence";
-                        cb[k] = sc.al;
+                    int c = -1;
+                    for (int k = 0; k < pic.ncomp; ++k) if (cid[k] == d[1 + 2 * j]) c = k;
+                    if (c < 0) return "a scan names a component the frame does not have";
+                    comps[j] = c;
+                    const int td = d[2 + 2 * j] >> 4, ta = d[2 + 2 * j] & 15;
+                    if (td > 3 || ta > 3) return "bad Huffman table number in a scan";
+                    const bool need_dc = !progressive || (sc.ss == 0 && ah == 0), need_ac = !progressive || sc.ss > 0;
+                    if ((need_dc && dc_tab[td] < 0) || (need_ac && ac_tab[ta] < 0)) return "a scan uses an undefined Huffman table";
+                    sc.dc[j] = (uint32_t)(dc_tab[td] < 0 ? 0 : dc_tab[td]);
+                    sc.ac[j] = (uint32_t)(ac_tab[ta] < 0 ? 0 : ac_tab[ta]);
+                    if (!latched[c]) {
+                        if (!qdef[cq[c]]) return "a component's quantisation table is not defined";
+                        P.quant.resize(64 * (size_t)pic.ncomp);
+                        memcpy(&P.quant[64 * (size_t)c], qtab[cq[c]], sizeof(qtab[0]));
+                        latched[c] = true;
                     }
                 }
-                sc.kind = sc.ss == 0 ? (ah ? kDcRefine : kDcFirst) : (ah ? kAcRefine : kAcFirst);
-            } else {
-                sc.kind = kSequential;
-                for (int j = 0; j < sc.ncomp; ++j) for (int k = 0; k < 64; ++k) coef_bits[comps[j]][k] = 0;
-            }
-            // the MCU
-            int mcus;
-            if (sc.ncomp == 1) {
-                const Comp& C = pic.comp[comps[0]];
-                sc.blocks = 1; sc.bcomp[0] = (uint8_t)comps[0]; sc.mcux = C.wib;
-                mcus = C.wib * C.hib;
-            } else {
-                sc.mcux = (pic.w + 8 * pic.hmax - 1) / (8 * pic.hmax);
-                mcus = sc.mcux * ((pic.h + 8 * pic.vmax - 1) / (8 * pic.vmax));
-                for (int j = 0; j < sc.ncomp; ++j) {
-                    const Comp& C = pic.comp[comps[j]];
-                    for (int yy = 0; yy < C.v; ++yy)
-                        for (int xx = 0; xx < C.h; ++xx) {
-                            if (sc.blocks >= kMaxBlocks) return "too many blocks in an MCU";
-                            sc.bcomp[sc.blocks] = (uint8_t)comps[j]; sc.bslot[sc.blocks] = (uint8_t)j;
-                            sc.bdx[sc.blocks] = (uint8_t)xx; sc.bdy[sc.blocks] = (uint8_t)yy; ++sc.blocks;
+                if (progressive) {
+                    bool bad = sc.ss == 0 ? sc.se != 0 : (sc.ss > sc.se || sc.se > 63 || sc.ncomp != 1);
+                    if (ah != 0 && sc.al != ah - 1) bad = true;
+                    if (sc.al > 13) bad = true;
+                    if (bad) return "an invalid progressive scan";
+                    for (int j = 0; j < sc.ncomp; ++j) {
+                        int* cb = coef_bits[comps[j]];
+                        if (sc.ss > 0 && cb[0] < 0) return "an AC scan before the component's DC scan";
+                        for (int k = sc.ss; k <= sc.se; ++k) {
+                            if (ah != (cb[k] < 0 ? 0 : cb[k])) return "an inconsistent progression sequence";
+                            cb[k] = sc.al;
                         }
-                }
-            }
-            const uint32_t si = (uint32_t)P.scans.size();
-            P.scans.push_back(sc);
-            // the entropy-coded data: split at RSTn, up to the next other marker
-            const int nseg = restart ? (mcus + restart - 1) / restart : 1;
-            int found = 0;
-            size_t begin = pos;
-            in_scan = true;
-            while (in_scan) {
-                const uint8_t* ff = pos < n ? (const uint8_t*)memchr(f + pos, 0xFF, n - pos) : nullptr;
-                size_t i = ff ? (size_t)(ff - f) : n;
-                size_t j = i + 1;
-                while (j < n && f[j] == 0xFF) ++j;             // fill bytes before a marker
-                if (i >= n || j >= n) {                        // the file ends inside the scan's data
-                    if (found < nseg) {
-                        Seg s = {si, (uint32_t)(found * restart), (uint32_t)(restart ? (mcus - found * restart < restart ? mcus - found * restart : restart) : mcus), 0, begin, i < n ? i : n};
-                        P.segs.push_back(s);
-                        ++found;
                     }
-                    pic.bad = 1; pos = n; in_scan = false; eoi = true;
-                    break;
-                }
-                const unsigned mk = f[j];
-                if (mk == 0x00) {                              // stuffed FF 00 (after fill bytes: not restated)
-                    if (j != i + 1) pic.bad = 1;
-                    pos = j + 1;
-                    continue;
-                }
-                if (found < nseg) {
-                    const uint32_t m0 = (uint32_t)(found * restart);
-                    Seg s = {si, m0, (uint32_t)(restart ? (mcus - (int)m0 < restart ? mcus - (int)m0 : restart) : mcus), 0, begin, i};
-                    P.segs.push_back(s);
+                    sc.kind = sc.ss == 0 ? (ah ? kDcRefine : kDcFirst) : (ah ? kAcRefine : kAcFirst);
                 } else {
-                    pic.bad = 1;                               // more intervals than MCUs
+                    sc.kind = kSequential;
+                    for (int j = 0; j < sc.ncomp; ++j) for (int k = 0; k < 64; ++k) coef_bits[comps[j]][k] = 0;
                 }
-                ++found;
-                if (mk >= 0xD0 && mk <= 0xD7) {
-                    if ((int)(mk - 0xD0) != ((found - 1) & 7) || !restart) pic.bad = 1;
-                    pos = begin = j + 1;
+                // the MCU
+                int mcus;
+                if (sc.ncomp == 1) {
+                    const Comp& C = pic.comp[comps[0]];
+                    sc.blocks = 1; sc.bcomp[0] = (uint8_t)comps[0]; sc.mcux = C.wib;
+                    mcus = C.wib * C.hib;
                 } else {
-                    pos = j - 1;                               // the marker's FF
-                    in_scan = false;
+                    sc.mcux = (pic.w + 8 * pic.hmax - 1) / (8 * pic.hmax);
+                    mcus = sc.mcux * ((pic.h + 8 * pic.vmax - 1) / (8 * pic.vmax));
+                    for (int j = 0; j < sc.ncomp; ++j) {
+                        const Comp& C = pic.comp[comps[j]];
+                        for (int yy = 0; yy < C.v; ++yy)
+                            for (int xx = 0; xx < C.h; ++xx) {
+                                if (sc.blocks >= kMaxBlocks) return "too many blocks in an MCU";
+                                sc.bcomp[sc.blocks] = (uint8_t)comps[j]; sc.bslot[sc.blocks] = (uint8_t)j;
+                                sc.bdx[sc.blocks] = (uint8_t)xx; sc.bdy[sc.blocks] = (uint8_t)yy; ++sc.blocks;
+                            }
+                    }
                 }
+                const uint32_t si = (uint32_t)P.scans.size();
+                P.scans.push_back(sc);
+                // the entropy-coded data: split at RSTn, up to the next other marker
+                const int nseg = restart ? (mcus + restart - 1) / restart : 1;
+                int found = 0;
+                size_t begin = pos;
+                in_scan = true;
+                while (in_scan) {
+                    const uint8_t* ff = pos < n ? (const uint8_t*)memchr(f + pos, 0xFF, n - pos) : nullptr;
+                    size_t i = ff ? (size_t)(ff - f) : n;
+                    size_t j = i + 1;
+                    while (j < n && f[j] == 0xFF) ++j;             // fill bytes before a marker
+                    if (i >= n || j >= n) {                        // the file ends inside the scan's data
+                        if (found < nseg) {
+                            Seg s = {si, (uint32_t)(found * restart), (uint32_t)(restart ? (mcus - found * restart < restart ? mcus - found * restart : restart) : mcus), 0, begin, i < n ? i : n};
+                            P.segs.push_back(s);
+                            ++found;
+                        }
+                        pic.bad = 1; pos = n; in_scan = false; eoi = true;
+                        break;
+                    }
+                    const unsigned mk = f[j];
+                    if (mk == 0x00) {                              // stuffed FF 00 (after fill bytes: not restated)
+                        if (j != i + 1) pic.bad = 1;
+                        pos = j + 1;
+                        continue;
+                    }
+                    if (found < nseg) {
+                        const uint32_t m0 = (uint32_t)(found * restart);
+                        Seg s = {si, m0, (uint32_t)(restart ? (mcus - (int)m0 < restart ? mcus - (int)m0 : restart) : mcus), 0, begin, i};
+                        P.segs.push_back(s);
+                    } else {
+                        pic.bad = 1;                               // more intervals than MCUs
+                    }
+                    ++found;
+                    if (mk >= 0xD0 && mk <= 0xD7) {
+                        if ((int)(mk - 0xD0) != ((found - 1) & 7) || !restart) pic.bad = 1;
+                        pos = begin = j + 1;
+                    } else {
+                        pos = j - 1;                               // the marker's FF
+                        in_scan = false;
+                    }
+                }
+                if (found < nseg) pic.bad = 1;
             }
-            if (found < nseg) pic.bad = 1;
+            // other APPn, COM: skipped
         }
-        // other APPn, COM: skipped
+        return "";
+    };
+    const std::string why = markers();
+    if (!why.empty()) {
+        if (P.scans.empty()) return why;
+        pic.bad = 1;
     }
     if (!frame) return "no frame header";
     if (P.scans.empty()) return "no scan";
@@ -896,12 +929,11 @@ inline std::string parse(const uint8_t* f, size_t n, Parsed& P)
     }
     for (int c = 0; c < pic.ncomp; ++c) {
         if (!latched[c]) { pic.bad = 1; P.quant.resize(64 * (size_t)pic.ncomp); }   // a component without its scan: data missing
-        // libjpeg smooths blocks whose first coefficients are not at full precision when the output starts; a complete file has them all
+        // libjpeg smooths blocks whose first coefficients are not at full precision when the output starts, which is not restated.
+        // A complete file has them all; a script cut short (a truncated file, or a false EOI: a lost FF 00 before a D9 byte) is
+        // corrupt data
         for (int k = 0; k < 10; ++k)
-            if (coef_bits[c][k] != 0) {
-                if (!eoi || pic.bad) { pic.bad = 1; break; }
-                return "a progressive scan script that leaves coefficients incomplete (libjpeg would smooth its blocks)";
-            }
+            if (coef_bits[c][k] != 0) { pic.bad = 1; break; }
     }
     pic.ow = pic.orient >= 5 ? pic.h : pic.w;
     pic.oh = pic.orient >= 5 ? pic.w : pic.h;

@@ -18,9 +18,11 @@ int jc_info(const uint8_t* file, uint64_t size, int* wh, char* why, int why_cap)
     return 0;
 }
 
-// the RGB8 picture into rgb (cap bytes): 0, -2 for corrupt data, 1 refused (why), 2 too small a buffer
-int jc_decode(const uint8_t* file, uint64_t size, uint8_t* rgb, uint64_t cap, int* wh, char* why, int why_cap)
+// the RGB8 picture into rgb (cap bytes): 0, -2 for corrupt data, 1 refused (why), 2 too small a buffer.  *wide: the blocks whose
+// IDCT leaves the range where libjpeg-turbo's C and SIMD IDCTs agree (idct_islow), where cv2's bytes depend on its build
+int jc_decode_wide(const uint8_t* file, uint64_t size, uint8_t* rgb, uint64_t cap, int* wh, char* why, int why_cap, int* wide)
 {
+    *wide = 0;
     std::vector<Parsed> ps(1);
     const std::string r = parse(file, size, ps[0]);
     if (!r.empty()) { snprintf(why, (size_t)why_cap, "%s", r.c_str()); return 1; }
@@ -73,13 +75,22 @@ int jc_decode(const uint8_t* file, uint64_t size, uint8_t* rgb, uint64_t cap, in
     for (int c = 0; c < P.ncomp; ++c) {
         const Comp& C = P.comp[c];
         for (int by = 0; by < C.bh; ++by)
-            for (int bx = 0; bx < C.bw; ++bx)
+            for (int bx = 0; bx < C.bw; ++bx) {
+                int w = 0;
                 idct_islow(coef.data() + C.coef + ((size_t)by * C.bw + bx) * 64, quant + C.quant,
-                           planes.data() + C.plane + (size_t)by * 8 * C.bw * 8 + (size_t)bx * 8, (size_t)C.bw * 8);
+                           planes.data() + C.plane + (size_t)by * 8 * C.bw * 8 + (size_t)bx * 8, (size_t)C.bw * 8, &w);
+                *wide += w;
+            }
     }
     for (int y = 0; y < P.oh; ++y)
         for (int x = 0; x < P.ow; ++x) pixel_rgb(planes.data(), P, x, y, rgb + P.out + 3 * ((size_t)y * P.ow + x));
     return 0;
+}
+
+int jc_decode(const uint8_t* file, uint64_t size, uint8_t* rgb, uint64_t cap, int* wh, char* why, int why_cap)
+{
+    int wide;
+    return jc_decode_wide(file, size, rgb, cap, wh, why, why_cap, &wide);
 }
 
 }  // extern "C"
