@@ -297,6 +297,27 @@ typedef struct cb200_picture {
    and the flags and outputs cb200_scan_extract_decode_chunks_ragged_dev refuses. */
 int cb200_scan_extract_decode_chunks_pictures_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags, uint8_t* d_chunks,
                                                   uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+/* ---- several pictures of one frame ----------------------------------------------------------------------------------------------
+
+   cb200_scan_extract_decode_chunks_pictures_dev plus one decode per group of pictures of the same frame, so that a frame no single
+   picture decodes may still decode from several.  group_of (HOST, n entries, read before the call returns) puts picture i in group
+   group_of[i] of m, or in none (-1).  Picture i takes part in its group iff its extract status is 1 or 2.  Per cell the group's frame
+   takes the value bits (symbol | colour << symbol_bits) that (1) most participating pictures hold, then (2) whose smallest walk
+   distance (the best Hamming distance of the cell's symbol, cb200_cell_trace.distance) is smallest, then (3) of the earliest picture
+   in batch order -- each picture's final cell bytes, after colour correction.  That frame then takes the ordinary de-interleave
+   (CB200_FLAG_NO_INTERLEAVE honoured), Reed-Solomon and chunk rule, with no colour correction of its own.
+   Per picture: records, masks, frame flags, extract statuses, cb200_camera_transforms, the sharpen selection and the CCM carry
+   (the context's CCM afterwards, cb200_get_frame_ccms) are, bit for bit, those of cb200_scan_extract_decode_chunks_pictures_dev on
+   the same arguments.  Per group: d_group_chunks / d_group_mask are m slots in cb200_decode_chunks_dev's fixed-slot layout, and
+   d_group_used[g] the number of pictures that took part; a group without one gets a zeroed record, mask 0 and 0.  With m = 0 the
+   call is the pictures call.  Enqueue-only, with that call's waits: the group table travels in its one upload.  A group holds at
+   most 16 pictures.  CB200_ERR_ARG, before any CUDA call: everything the pictures call refuses; then m < 0 or m > max_frames,
+   CB200_FLAG_NO_FALLBACK with m > 0 (the vote needs every picture's walk), a null group_of with m > 0, an entry outside [-1, m) or
+   a 17th picture of one group (naming the picture), null group outputs with m > 0. */
+int cb200_scan_extract_decode_chunks_combined_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, const int32_t* group_of, int m,
+                                                  uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                                                  int32_t* d_extract_status, uint8_t* d_group_chunks, uint32_t* d_group_mask,
+                                                  int32_t* d_group_used);
 /* ---- receivers: pictures of many decoders in one batch ------------------------------------------------------------------------
 
    A batch of the calls above is one decoder: under CC_FIT a picture without a usable header takes the matrix of the picture before

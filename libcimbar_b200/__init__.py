@@ -48,6 +48,7 @@ EXPORTS = [
     "cb200_camera_plan_create_receivers_pictures_dev", "cb200_camera_plan_create_detect_receivers_pictures_dev",
     "cb200_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_receivers_pictures_flags_dev",
     "cb200_detect_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_detect_receivers_pictures_flags_dev",
+    "cb200_scan_extract_decode_chunks_combined_dev",
 ]
 
 
@@ -182,6 +183,7 @@ def load_library():
     lib.cb200_camera_plan_destroy.argtypes = [vp]
     lib.cb200_detect_scan_extract_decode_chunks_dev.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_pictures_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
+    lib.cb200_scan_extract_decode_chunks_combined_dev.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp, vp, vp]
     lib.cb200_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp]
     lib.cb200_camera_plan_create_receivers.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp, vp]
@@ -776,6 +778,23 @@ class Context:
         descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
         _check(self.lib.cb200_scan_extract_decode_chunks_pictures_dev(self._h, C.cast(descs, C.c_void_p), len(pictures), flags, d_chunks,
                                                                       d_mask, d_flags, d_status))
+
+    def scan_extract_decode_chunks_combined_dev(self, pictures, group_of, m, d_chunks, d_mask, d_status, d_group_chunks, d_group_mask,
+                                                d_group_used, d_flags=None, flags=0, order="rgb"):
+        """scan_extract_decode_chunks_pictures_dev plus one decode per group of pictures of the same frame
+        (cb200_scan_extract_decode_chunks_combined_dev): picture i belongs to group group_of[i] of m (host; -1 = none), and each
+        group's frame takes, per cell, the vote of its pictures that extracted (status 1 or 2).  d_group_chunks / d_group_mask /
+        d_group_used (int32: the pictures that took part) are m slots in device memory.  Enqueue-only"""
+        orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+        if len(orders) != len(pictures):
+            raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+        of = None if group_of is None else np.ascontiguousarray(group_of, dtype=np.int32).reshape(-1)
+        if of is not None and len(of) != len(pictures):
+            raise Cb200Error(f"{len(of)} group_of entries for {len(pictures)} pictures")
+        descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+        _check(self.lib.cb200_scan_extract_decode_chunks_combined_dev(
+            self._h, C.cast(descs, C.c_void_p), len(pictures), None if of is None else of.ctypes.data, m, flags, d_chunks, d_mask, d_flags,
+            d_status, d_group_chunks, d_group_mask, d_group_used))
 
     def decode_chunks_receivers_dev(self, d_rgb, n, receiver_of, states, d_chunks, d_mask, d_flags=None, flags=0):
         """decode_chunks_dev for frames of several receivers: frame i belongs to receiver receiver_of[i] (host), each receiver decodes

@@ -418,9 +418,10 @@ int upload_selection(cb200_ctx* c, const uint8_t* sel, int n, const int nl[2], c
 // must not carry CB200_FLAG_SHARPEN then).  A selection of one kind only takes the list-less path of that kind.
 // d_sel_bytes (instead of sel): the selection is n bytes at c->d_sel + 4 n on the device; the lists are built there and K1 takes
 // their lengths from the device (both kinds are launched, one may be empty).  given: the CCM of the colour decisions, instead of
-// the one the flags and the context give
+// the one the flags and the context give.  d_trace alone: every frame goes through the exact walk, K1 does not run (the cell calls);
+// with walk_all: K1 runs and flags the frames as without a trace, and the walk also takes every frame for its trace (the combined call)
 int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sel, CellTrace* d_trace = nullptr,
-              uint32_t* d_means = nullptr, const uint8_t* d_sel_bytes = nullptr, const CcmArg* given = nullptr)
+              uint32_t* d_means = nullptr, const uint8_t* d_sel_bytes = nullptr, const CcmArg* given = nullptr, bool walk_all = false)
 {
     const Mode& m = c->mode;
     cudaStream_t st = c->stream;
@@ -438,7 +439,7 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const u
         int rc = ccm_arg(c, cc); if (rc) return rc;
     }
     bool sharpen = (flags & CB200_FLAG_SHARPEN) != 0;
-    const bool exact_only = d_trace != nullptr;   // a cell trace needs the walk itself
+    const bool exact_only = d_trace != nullptr && !walk_all;   // a cell trace needs the walk itself
     // nl[k] frames of kind k (0 = plain, 1 = sharpened), listed in d_list[k] (NULL: all n frames of the batch)
     int nl[2] = {sharpen ? 0 : n, sharpen ? n : 0};
     const uint32_t* d_list[2] = {nullptr, nullptr};
@@ -481,7 +482,7 @@ int run_cells(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const u
         if (!(flags & CB200_FLAG_NO_FALLBACK))
             CK(flood_colour_launch(m, sw->lead->flood, d_rgb, n, sw->kept, c->d_cellvals, cc, st), "flood colour launch");
     } else {
-        CK(flood_launch(m, c->flood, d_rgb, n, (flags & CB200_FLAG_NO_FALLBACK) != 0, exact_only, sharpen, d_sharp,
+        CK(flood_launch(m, c->flood, d_rgb, n, (flags & CB200_FLAG_NO_FALLBACK) != 0, exact_only, walk_all, sharpen, d_sharp,
                         c->d_cellvals, c->d_dirty, c->d_flags, d_trace, cc, st, sw ? sw->kept : nullptr, sw ? sw->present : nullptr),
            "flood launch");
     }
@@ -797,7 +798,8 @@ int cb200_rs_correct_dev(cb200_ctx* c, const uint8_t* d_raw, int n, uint8_t* d_d
 }  // extern "C"
 
 int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
-                         uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes, bool enqueue_only, Receivers* recv)
+                         uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes, bool enqueue_only, Receivers* recv,
+                         CellTrace* d_trace)
 {
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     const Mode& m = c->mode;
@@ -839,14 +841,17 @@ int cb200::decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t fla
     if (!fitted) {
         CcmArg own;
         if (recv) { rc = receivers_ccm(c, d_rgb, n, flags, *recv, own); if (rc) return rc; c->ccm_frames = n; }
-        rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen, nullptr, nullptr, d_sel_bytes, recv ? &own : nullptr); if (rc) return rc;
+        rc = run_cells(c, d_rgb, n, flags & ~CB200_FLAG_CC_FIT, sharpen, d_trace, nullptr, d_sel_bytes, recv ? &own : nullptr, d_trace != nullptr);
+        if (rc) return rc;
         mark(c);                               // ev3: (no separate pack kernel on this path: the RS kernel gathers from the cell bytes)
         CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch");
     } else {
         // color_correction == 2: symbols (+ mean colours) -> RS of the symbol stream -> header -> CCM fit -> colours -> RS of
         // the colour stream (Decoder.h:83-117)
         if (!recv) { rc = entry_ccm(c, carried, initial); if (rc) return rc; }
-        rc = run_cells(c, d_rgb, n, flags & ~(CB200_FLAG_CC_FIT | CB200_FLAG_CC_SIMPLE), sharpen, nullptr, c->d_means, d_sel_bytes); if (rc) return rc;
+        rc = run_cells(c, d_rgb, n, flags & ~(CB200_FLAG_CC_FIT | CB200_FLAG_CC_SIMPLE), sharpen, d_trace, c->d_means, d_sel_bytes, nullptr,
+                       d_trace != nullptr);
+        if (rc) return rc;
         mark(c);                               // ev3
         if (fit) {
             CK(k2_rs_fused_launch(m, c->d_cellvals, idx, n, d_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream, 0, m.nblocks_sym), "rs launch (symbols)");

@@ -56,10 +56,12 @@ int file_status(cb200_ctx* c, const int* d_bad, int n, int32_t* d_status, uint32
 // enqueue_only: a CCM still on its way from an earlier batch is not waited for but read from c->d_carry on the device (k_ccm_carry:
 // a batch without a fit then takes the fitted-CCM route with no fits, deciding every colour as K1 would with that matrix)
 // recv: a _receivers_dev call's receivers (the CCM of each picture is its receiver's; the context's CCM is neither read nor changed)
+// d_trace: n x num_cells records, where the exact walk, which then takes every frame, writes each cell's trace (the combined call;
+// under CC_FIT in the first pass).  K1 and the frame flags are as without it, and so are the cells
 struct Receivers;
 int decode_chunks(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* d_chunks,
                   uint32_t* d_chunk_mask, uint8_t* d_frame_flags, const uint8_t* d_sel_bytes = nullptr, bool enqueue_only = false,
-                  Receivers* recv = nullptr);
+                  Receivers* recv = nullptr, CellTrace* d_trace = nullptr);
 // decode_chunks into the context's buffers, then fetch_fountain (api.cu)
 int decode_fountain_to_host(cb200_ctx* c, const uint8_t* d_rgb, int n, uint32_t flags, const uint8_t* sharpen, uint8_t* chunks_out,
                             uint32_t* chunk_count, uint32_t* chunk_mask, uint8_t* frame_flags);
@@ -191,7 +193,7 @@ int camera_scan(cb200_ctx* c, const CameraBatch& b, const PicDesc* d_table, cons
                 const std::vector<uint8_t>* tail = nullptr, const uint8_t** d_tail = nullptr);
 int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
                       bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status,
-                      Receivers* recv = nullptr, const int32_t* d_slots = nullptr);
+                      Receivers* recv = nullptr, const int32_t* d_slots = nullptr, CellTrace* d_trace = nullptr);
 // the receivers of a _receivers_dev call (include/cb200.h).  check_receivers: CB200_ERR_ARG, before any CUDA call, for a null
 // receiver map, null or misaligned states, n_receivers < 1, a receiver index out of range, a context linked to a CCM chain (api.cu).
 // Receivers(...) then builds `map` on the host: the n receiver indices, then the receiver-major order (receivers_core.cuh); d_map is
@@ -322,6 +324,10 @@ struct cb200_ctx {
     cb200::DevBuf<uint8_t> d_fit_valid;     // max_frames
     cb200::DevBuf<uint8_t> d_ccm_active;    // max_frames: the frame is decoded with d_ccm[f]
     cb200::DevBuf<int32_t> d_recv;          // a receivers frame call's map (Receivers::map): max_frames x 2
+    // a combined camera call (cb200_scan_extract_decode_chunks_combined_dev): the groups' voted cell bytes (m x num_cells) and the
+    // walk's cell traces of the pictures (n x num_cells), both grown through grow()
+    cb200::DevBuf<uint8_t> d_combined;
+    cb200::DevBuf<cb200::CellTrace> d_traces;
     int ccm_frames = 0;              // frames of the last call that took the fitted-CCM route (cb200_get_frame_ccms)
     cudaEvent_t ccm_ev = nullptr;    // recorded after the D2H copies of the last batch's CCM (ccm_resolve waits on it)
     cb200::GatherState* gather = nullptr;   // multi-GPU chunk-record window (gather.cu)
@@ -352,18 +358,29 @@ namespace cb200 {
 inline void begin_timed_call(cb200_ctx* c) { if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; } }
 inline void mark(cb200_ctx* c) { if (c->timing && c->ev_count[c->cur] < 8) cudaEventRecord(c->ev[c->cur][c->ev_count[c->cur]++], c->stream); }
 
+// the groups of a combined camera call (cb200_scan_extract_decode_chunks_combined_dev): the host group_of (n entries), the number of
+// groups m and whether its three group outputs are all non-null.  check_groups: CB200_ERR_ARG for CB200_FLAG_NO_FALLBACK with m > 0,
+// m < 0, a null group_of with m > 0, an entry outside [-1, m) or a group of more than combine::kMaxGroup pictures (naming the
+// picture), null group outputs with m > 0; no CUDA call, no context needed (scan.cu)
+struct CameraGroups { const int32_t* of; int m; bool outputs; };
+int check_groups(uint32_t flags, const CameraGroups& g, int n);
+
 // the checks every camera and corner call shares, in this order and before any CUDA call: the flags; the batch, from the call's
-// builder `build` (which may add the call's own checks that come before the context), and the 4 GB span rule of the deskew; the
-// context; `missing` (the message for a null output, or nullptr); n against max_frames; the CCM chain.  The frozen buffers the
-// call would grow are checked by the caller (check_frozen_*), which knows which ones it uses
+// builder `build` (which may add the call's own checks that come before the context), and the 4 GB span rule of the deskew; a
+// combined call's groups (check_groups); the context; `missing` (the message for a null output, or nullptr); n, and a combined
+// call's m, against max_frames; the CCM chain.  The frozen buffers the call would grow are checked by the caller (check_frozen_*),
+// which knows which ones it uses
 template <class Build>
-int check_camera_call(cb200_ctx* c, uint32_t flags, Build&& build, CameraBatch& b, const char* missing)
+int check_camera_call(cb200_ctx* c, uint32_t flags, Build&& build, CameraBatch& b, const char* missing, const CameraGroups* groups = nullptr)
 {
     int rc = check_camera_flags(flags); if (rc) return rc;
     if ((rc = build(b)) || (rc = check_spans(b))) return rc;
+    if (groups && (rc = check_groups(flags, *groups, b.n()))) return rc;
     if (!c) return fail(CB200_ERR_ARG, "null context");
     if (missing) return fail(CB200_ERR_ARG, missing);
     if (b.n() > c->max_frames) return fail(CB200_ERR_ARG, "n = " + std::to_string(b.n()) + " > max_frames = " + std::to_string(c->max_frames));
+    if (groups && groups->m > c->max_frames)
+        return fail(CB200_ERR_ARG, "m = " + std::to_string(groups->m) + " > max_frames = " + std::to_string(c->max_frames));
     return check_chain_call(c, flags);
 }
 }  // namespace cb200

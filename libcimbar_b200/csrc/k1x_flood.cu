@@ -42,9 +42,10 @@ __constant__ uint4 cx_tiles_slot[16];            // (L_lo, L_hi, symbol, 0) at t
 
 // ---------------------------------------------------------------------------------------------- work list
 // order-preserving compaction of the frames that need the exact walk; also writes the per-frame flags.  present: NULL, or one byte
-// per frame, 0 for a frame nobody reads (a detect receivers plan's slot that no mode of the geometry decodes): never listed
+// per frame, 0 for a frame nobody reads (a detect receivers plan's slot that no mode of the geometry decodes): never listed.
+// list_all: every frame is listed (walked for its cell trace) while the flags stay as K1's dirty bits decide
 __global__ void __launch_bounds__(1024)
-k_flood_list(const uint32_t* __restrict__ dirty, int n_frames, int no_fallback, int force_all, uint8_t* __restrict__ frame_flags,
+k_flood_list(const uint32_t* __restrict__ dirty, int n_frames, int no_fallback, int force_all, int list_all, uint8_t* __restrict__ frame_flags,
              uint32_t* __restrict__ list, uint32_t* __restrict__ counters, int n_counters, const uint8_t* __restrict__ present)
 {
     __shared__ uint32_t warp_off[32];
@@ -55,8 +56,9 @@ k_flood_list(const uint32_t* __restrict__ dirty, int n_frames, int no_fallback, 
     __syncthreads();
     for (int start = 0; start < n_frames; start += 1024) {
         const int f = start + tid;
-        const bool need = f < n_frames && (force_all || (dirty[f] & kFrameDirtyK1)) && (!present || present[f]);
-        const bool take = need && !no_fallback;
+        const bool in = f < n_frames && (!present || present[f]);
+        const bool need = in && (force_all || (dirty[f] & kFrameDirtyK1));
+        const bool take = (need || (in && list_all)) && !no_fallback;
         if (f < n_frames) frame_flags[f] = need ? (no_fallback ? 0x2 : 0x1) : 0;   // CB200_FRAME_INEXACT / CB200_FRAME_FALLBACK
         const uint32_t b = __ballot_sync(0xffffffffu, take);
         const uint32_t prefix = __popc(b & ((1u << lane) - 1u));
@@ -982,14 +984,14 @@ cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int n_fram
 }
 
 cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb, int n_frames, bool no_fallback,
-                         bool force_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
+                         bool force_all, bool list_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
                          uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st, uint32_t* keep, const uint8_t* d_present)
 {
     if (n_frames <= 0) return cudaSuccess;
     cudaError_t e = flood_workspace_ensure(m, ws, n_frames);
     if (e != cudaSuccess) return e;
     const int nchunks = (n_frames + ws.entry_cap - 1) / ws.entry_cap;
-    k_flood_list<<<1, 1024, 0, st>>>(d_dirty, n_frames, no_fallback ? 1 : 0, force_all ? 1 : 0, d_flags, ws.list, ws.counters, 1 + nchunks,
+    k_flood_list<<<1, 1024, 0, st>>>(d_dirty, n_frames, no_fallback ? 1 : 0, force_all ? 1 : 0, list_all ? 1 : 0, d_flags, ws.list, ws.counters, 1 + nchunks,
                                      d_present); count_launch();
     if (no_fallback) return cudaGetLastError();
     for (int c = 0; c < nchunks; ++c) {

@@ -39,13 +39,14 @@ cudaError_t flood_workspace_create(const Mode& m, int sm_count, const uint16_t* 
 cudaError_t flood_workspace_ensure(const Mode& m, FloodWorkspace& ws, int n_frames);
 bool flood_workspace_fits(const FloodWorkspace& ws, int n_frames);
 // writes d_flags[f] for every frame: 0 = K1 result stands, CB200_FRAME_FALLBACK = re-decoded here,
-// CB200_FRAME_INEXACT = needed but skipped (no_fallback).  d_sharpen_of: NULL = every frame is preprocessed as `sharpen` says;
+// CB200_FRAME_INEXACT = needed but skipped (no_fallback).  list_all: every frame is walked (for d_trace), the flags stay as the
+// dirty bits decide -- a frame K1 did not flag gets the cells K1 gave it (DESIGN.md §3, "Exactness").  d_sharpen_of: NULL = every frame is preprocessed as `sharpen` says;
 // else one byte per frame of the batch (device memory, nonzero = sharpen) and `sharpen` is ignored.
 // keep != NULL: the walk's per-cell records (x | y << 11 | sym << 22) of all n_frames listed frames stay there, in list order
 // (n_frames x num_cells words), instead of one chunk at a time in the workspace.  d_present != NULL: one device byte per frame, and
 // a frame whose byte is 0 is neither walked nor flagged (its K1 cells stand)
 cudaError_t flood_launch(const Mode& m, FloodWorkspace& ws, const uint8_t* d_rgb, int n_frames, bool no_fallback,
-                         bool force_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
+                         bool force_all, bool list_all, bool sharpen, const uint8_t* d_sharpen_of, uint8_t* d_cellvals, const uint32_t* d_dirty,
                          uint8_t* d_flags, CellTrace* d_trace, const CcmArg& cc, cudaStream_t st, uint32_t* keep = nullptr,
                          const uint8_t* d_present = nullptr);
 // the colour pass of a walk that flood_launch ran on `walked` with `keep` = kept, for another mode of the same frame geometry: the

@@ -23,6 +23,8 @@
 #include "extract_core.cuh"
 #include "layout_core.cuh"
 #include "receivers_core.cuh"
+#include "combine_core.cuh"
+#include "k2_rs.cuh"
 
 #include <algorithm>
 #include <string>
@@ -833,7 +835,7 @@ int camera_reserve(cb200_ctx* c, const CameraBatch& b)
 
 int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch& b, const PicDesc* d_desc, uint32_t flags, uint8_t* frames,
                       bool deskew, uint8_t* d_chunks, uint32_t* d_mask, uint8_t* d_frame_flags, int32_t* d_status, Receivers* recv,
-                      const int32_t* d_slots)
+                      const int32_t* d_slots, CellTrace* d_trace)
 {
     const Mode& m = c->mode;
     const int n = b.n();
@@ -854,7 +856,8 @@ int camera_after_scan(cb200_ctx* c, const cb200_ctx* scanned, const CameraBatch&
     s->camera_n = n;
     int rc;
     if (deskew) { rc = deskew_launch(c, b, s->d_minv, d_desc, frames); if (rc) return rc; }
-    rc = decode_chunks(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, d_chunks, d_mask, d_frame_flags, d_sharp, true, recv);
+    rc = decode_chunks(c, frames, n, flags & ~CB200_FLAG_SHARPEN_IF_NEEDED, nullptr, d_chunks, d_mask, d_frame_flags, d_sharp, true, recv,
+                       d_trace);
     if (rc) return rc;
     k_mask_failed<<<(n + 127) / 128, 128, 0, c->stream>>>(d_status, n, d_mask, recv ? recv->d_map : nullptr, recv ? recv->d_refused : nullptr);
     count_launch();
@@ -938,6 +941,108 @@ static int scan_extract_decode_dev(cb200_ctx* c, Build&& build, uint32_t flags, 
     Receivers r(ra->of, b.n(), ra->count, ra->d_states);
     if ((r.d_words = ra->d_words)) { r.refused_bytes(b.n()); r.receivers = ra->count; }
     return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, &r);
+}
+
+// ---- the combined call (cb200_scan_extract_decode_chunks_combined_dev): per-cell vote over groups of pictures of one frame
+int check_groups(uint32_t flags, const CameraGroups& g, int n)
+{
+    if (g.m > 0 && (flags & CB200_FLAG_NO_FALLBACK))
+        return fail(CB200_ERR_ARG, "CB200_FLAG_NO_FALLBACK with m > 0: the vote needs every picture's walk");
+    if (g.m < 0) return fail(CB200_ERR_ARG, "m = " + std::to_string(g.m) + " < 0");
+    if (!g.of) return g.m > 0 ? fail(CB200_ERR_ARG, "null group_of with m > 0") : CB200_OK;
+    int at = 0;
+    switch (combine::group_error(g.of, n, g.m, &at)) {
+    case 1: return fail(CB200_ERR_ARG, "picture " + std::to_string(at) + ": group " + std::to_string(g.of[at]) + " outside [-1, " +
+                                       std::to_string(g.m) + ")");
+    case 2: return fail(CB200_ERR_ARG, "picture " + std::to_string(at) + ": group " + std::to_string(g.of[at]) + " has more than " +
+                                       std::to_string(combine::kMaxGroup) + " pictures");
+    default: break;
+    }
+    if (g.m > 0 && !g.outputs) return fail(CB200_ERR_ARG, "null group output");
+    return CB200_OK;
+}
+
+// the combined call's own buffers: the groups' cells and the pictures' traces.  With live plans grow() makes no CUDA call and refuses
+// what would grow, so the call runs this before any CUDA call then
+static int combine_reserve(cb200_ctx* c, int n, int m)
+{
+    const size_t cells = (size_t)c->mode.num_cells;
+    int rc;
+    if ((rc = grow(c, c->d_combined, (size_t)m * cells, "combined cells")) || (rc = grow(c, c->d_traces, (size_t)n * cells, "cell traces")))
+        return rc;
+    return CB200_OK;
+}
+
+// combine::vote per (group, cell), one thread each, over the CSR group table (offsets[0 .. m], members): the participating pictures'
+// value bits from their final cell bytes and their walk distances from the trace, into the groups' contiguous cell frames; the cell-0
+// thread of a group writes its participant count
+__global__ void k_combine(int m, int cells, const int32_t* __restrict__ offsets, const int32_t* __restrict__ members,
+                          const int32_t* __restrict__ status, const uint8_t* __restrict__ cellvals, const CellTrace* __restrict__ trace,
+                          uint8_t* __restrict__ out, int32_t* __restrict__ used)
+{
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)m * cells) return;
+    const int g = (int)(t / cells), cell = (int)(t - (long long)g * cells);
+    uint8_t v[combine::kMaxGroup], d[combine::kMaxGroup];
+    int k = 0;
+    for (int j = offsets[g], end = offsets[g + 1]; j < end; ++j) {
+        const int p = members[j];
+        if (!combine::takes_part(status[p])) continue;
+        const size_t at = (size_t)p * cells + cell;
+        v[k] = cellvals[at] & combine::kValueBits;
+        d[k] = trace[at].distance;
+        ++k;
+    }
+    out[t] = k ? combine::vote(v, d, k) : 0;
+    if (cell == 0) used[g] = k;
+}
+
+// every group of a call without pictures: zeroed records, mask 0, no pictures
+static int combine_empty(cb200_ctx* c, int m, uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    CK(cudaMemsetAsync(d_group_chunks, 0, (size_t)m * c->mode.data_bytes, c->stream), "memset group records");
+    CK(cudaMemsetAsync(d_group_mask, 0, sizeof(uint32_t) * (size_t)m, c->stream), "memset group masks");
+    CK(cudaMemsetAsync(d_group_used, 0, sizeof(int32_t) * (size_t)m, c->stream), "memset group counts");
+    return CB200_OK;
+}
+
+// camera_enqueue with the group table behind the picture table (one upload) and the walk's traces kept, then the vote and the
+// groups' decode: the route of a call without colour correction (k2_rs_fused_launch: the frame-pair kernel where it applies), the
+// chunk masks, and mask 0 for a group without pictures (k_mask_failed on the counts).  Four launches more than the pictures call
+static int combine_enqueue(cb200_ctx* c, const CameraBatch& b, const int32_t* group_of, int m, uint32_t flags, uint8_t* d_chunks,
+                           uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, uint8_t* d_group_chunks,
+                           uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    const Mode& md = c->mode;
+    const int n = b.n();
+    int rc;
+    if ((rc = combine_reserve(c, n, m)) || (rc = camera_reserve(c, b))) return rc;
+    uint8_t* frames;
+    if ((rc = deskew_frames(c, n, &frames))) return rc;
+    std::vector<int32_t> table((size_t)m + 1 + (size_t)n);
+    combine::group_table(group_of, n, m, table.data(), table.data() + m + 1);
+    table.resize((size_t)m + 1 + (size_t)table[(size_t)m]);
+    std::vector<uint8_t> tail(table.size() * sizeof(int32_t));
+    memcpy(tail.data(), table.data(), tail.size());
+    const PicDesc* d_desc;
+    const uint8_t* d_tail;
+    if ((rc = camera_scan(c, b, nullptr, &d_desc, nullptr, &tail, &d_tail))) return rc;
+    rc = camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, nullptr,
+                           c->d_traces);
+    if (rc) return rc;
+    const int32_t* d_offsets = reinterpret_cast<const int32_t*>(d_tail);
+    const long long threads = (long long)m * md.num_cells;
+    k_combine<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(m, md.num_cells, d_offsets, d_offsets + m + 1, d_extract_status,
+                                                                       c->d_cellvals, c->d_traces, c->d_combined, d_group_used);
+    count_launch();
+    CK(cudaGetLastError(), "combine launch");
+    const uint16_t* idx = (flags & CB200_FLAG_NO_INTERLEAVE) ? c->d_idx_ident.get() : c->d_idx.get();
+    CK(k2_rs_fused_launch(md, c->d_combined, idx, m, d_group_chunks, c->d_ok, c->d_rho, c->sm_count, c->stream), "rs launch (groups)");
+    CK(k2_mask_launch(md, c->d_ok, m, d_group_mask, c->stream), "mask launch (groups)");
+    k_mask_failed<<<(m + 127) / 128, 128, 0, c->stream>>>(d_group_used, m, d_group_mask, nullptr, nullptr);
+    count_launch();
+    CK(cudaGetLastError(), "group mask launch");
+    return CB200_OK;
 }
 
 // the scan entry points: the batch, the context and the count output checked, the batch staged and scanned, the results copied out
@@ -1054,6 +1159,28 @@ int cb200_scan_extract_decode_chunks_pictures_dev(cb200_ctx* c, const cb200_pict
 {
     auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
     return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+}
+
+int cb200_scan_extract_decode_chunks_combined_dev(cb200_ctx* c, const cb200_picture* pics, int n, const int32_t* group_of, int m, uint32_t flags,
+                                                  uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status,
+                                                  uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    CameraBatch b;
+    auto build = [&](CameraBatch& bb) { return picture_batch(pics, n, bb); };
+    const CameraGroups groups = {group_of, m, d_group_chunks && d_group_mask && d_group_used};
+    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output", &groups);
+    if (rc) return rc;
+    const int nb = b.n();
+    if (nb == 0) {
+        if ((rc = empty_stripe(c, flags, true)) || m == 0) return rc;
+        CK(cudaSetDevice(c->device), "cudaSetDevice");
+        return combine_empty(c, m, d_group_chunks, d_group_mask, d_group_used);
+    }
+    if ((rc = check_frozen_camera(c, b.wh.data(), nb)) || (m > 0 && !c->plans.empty() && (rc = combine_reserve(c, nb, m)))) return rc;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    if (m == 0) return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    return combine_enqueue(c, b, group_of, m, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, d_group_chunks, d_group_mask,
+                           d_group_used);
 }
 
 int cb200_scan_extract_decode_chunks_receivers_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, const int32_t* receiver_of,
