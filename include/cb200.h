@@ -318,6 +318,22 @@ int cb200_scan_extract_decode_chunks_combined_dev(cb200_ctx* ctx, const cb200_pi
                                                   uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
                                                   int32_t* d_extract_status, uint8_t* d_group_chunks, uint32_t* d_group_mask,
                                                   int32_t* d_group_used);
+/* cb200_scan_extract_decode_chunks_combined_dev with groups the device finds from the pictures' own cells, for a caller that does not
+   know which pictures show one frame (a camera loop, files in any order).  match(i, j): pictures i and j both have extract status 1
+   or 2, and at least half of the cells have equal symbol bits (value & ((1 << symbol_bits) - 1) of the final cell bytes; the colour
+   bits do not count, a colour cast changes them).  In batch order, a picture with status 1 or 2 joins the group of the earliest
+   earlier leader it matches whose group has fewer than 16 pictures, else it becomes a leader.  A group is a leader with at least one
+   other picture, numbered in its leader's batch order.  d_group_of (device, n entries) gets each picture's group or -1 (alone, or
+   status other than 1 or 2), d_group_count (device, one int) the number of groups.  d_group_chunks / d_group_mask / d_group_used are
+   n / 2 slots (the most groups n pictures form): slots [0, count) are bit for bit those of the combined call given that group_of and
+   m = count; the other slots get a zeroed record, mask 0 and 0.  n = 0 or 1 gives count 0.  Per picture, everything is that of
+   cb200_scan_extract_decode_chunks_pictures_dev.  Enqueue-only, with that call's waits: the groups never reach the host.
+   CB200_ERR_ARG, before any CUDA call: everything the pictures call refuses; then CB200_FLAG_NO_FALLBACK (the vote needs every
+   picture's walk) and a null group output, whatever n is. */
+int cb200_scan_extract_decode_chunks_grouped_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags, uint8_t* d_chunks,
+                                                 uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status,
+                                                 int32_t* d_group_of, int32_t* d_group_count, uint8_t* d_group_chunks,
+                                                 uint32_t* d_group_mask, int32_t* d_group_used);
 /* ---- receivers: pictures of many decoders in one batch ------------------------------------------------------------------------
 
    A batch of the calls above is one decoder: under CC_FIT a picture without a usable header takes the matrix of the picture before

@@ -48,7 +48,7 @@ EXPORTS = [
     "cb200_camera_plan_create_receivers_pictures_dev", "cb200_camera_plan_create_detect_receivers_pictures_dev",
     "cb200_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_receivers_pictures_flags_dev",
     "cb200_detect_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_detect_receivers_pictures_flags_dev",
-    "cb200_scan_extract_decode_chunks_combined_dev",
+    "cb200_scan_extract_decode_chunks_combined_dev", "cb200_scan_extract_decode_chunks_grouped_dev",
 ]
 
 
@@ -184,6 +184,7 @@ def load_library():
     lib.cb200_detect_scan_extract_decode_chunks_dev.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_pictures_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_combined_dev.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp, vp, vp]
+    lib.cb200_scan_extract_decode_chunks_grouped_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.cb200_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp]
     lib.cb200_camera_plan_create_receivers.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp, vp]
@@ -795,6 +796,20 @@ class Context:
         _check(self.lib.cb200_scan_extract_decode_chunks_combined_dev(
             self._h, C.cast(descs, C.c_void_p), len(pictures), None if of is None else of.ctypes.data, m, flags, d_chunks, d_mask, d_flags,
             d_status, d_group_chunks, d_group_mask, d_group_used))
+
+    def scan_extract_decode_chunks_grouped_dev(self, pictures, d_chunks, d_mask, d_status, d_group_of, d_group_count, d_group_chunks,
+                                               d_group_mask, d_group_used, d_flags=None, flags=0, order="rgb"):
+        """scan_extract_decode_chunks_combined_dev with the groups found on the device (cb200_scan_extract_decode_chunks_grouped_dev):
+        pictures whose cells agree on at least half of the symbols form groups of up to 16, each led by its earliest picture.
+        d_group_of (int32, one per picture: its group or -1) and d_group_count (one int32) are device outputs, and d_group_chunks /
+        d_group_mask / d_group_used are len(pictures) // 2 slots in device memory; slots past the count are zeroed.  Enqueue-only"""
+        orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+        if len(orders) != len(pictures):
+            raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+        descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+        _check(self.lib.cb200_scan_extract_decode_chunks_grouped_dev(
+            self._h, C.cast(descs, C.c_void_p), len(pictures), flags, d_chunks, d_mask, d_flags, d_status, d_group_of, d_group_count,
+            d_group_chunks, d_group_mask, d_group_used))
 
     def decode_chunks_receivers_dev(self, d_rgb, n, receiver_of, states, d_chunks, d_mask, d_flags=None, flags=0):
         """decode_chunks_dev for frames of several receivers: frame i belongs to receiver receiver_of[i] (host), each receiver decodes

@@ -79,5 +79,88 @@ inline void group_table(const int32_t* group_of, int n, int m, int32_t* offsets,
     for (int i = 0; i < n; ++i) if (group_of[i] >= 0) members[next[(size_t)group_of[i]]++] = i;
 }
 
+// ---- finding the groups (cb200_scan_extract_decode_chunks_grouped_dev): pictures of one frame agree on their cells' symbol bits.
+// The colour bits do not take part: a colour cast changes them on a third of the cells of the same frame.
+//   match(i, j): both pictures take part (takes_part) and 2 * agree(i, j) >= cells, where agree counts the cells whose symbol bits
+//                (value & ((1 << symbol_bits) - 1), from the final cell bytes) are equal.
+//   assignment, in batch order: a picture that takes part joins the group of the earliest earlier leader it matches whose group has
+//                fewer than kMaxGroup pictures; with none it becomes a leader.  A group is a leader with at least one other picture;
+//                groups are numbered in their leaders' batch order, and every other picture gets group -1.
+// k_pair_match (scan.cu) packs the symbol bits eight cells to a word (pack_symbols) and counts differing ones (differing_symbols);
+// k_assign_groups applies the assignment over its match rows with the same word helpers (open_matches, join) as assign_groups here.
+
+// the number of cells of a and b (cells bytes each) whose symbol bits are equal
+CB_HD int agree(const uint8_t* a, const uint8_t* b, int cells, int symbol_bits)
+{
+    const int mask = (1 << symbol_bits) - 1;
+    int same = 0;
+    for (int k = 0; k < cells; ++k) same += ((a[k] ^ b[k]) & mask) == 0;
+    return same;
+}
+
+CB_HD bool match(int agreeing, int cells) { return 2 * agreeing >= cells; }
+
+// the symbol bits (symbol_bits <= 4) of eight cell bytes (little-endian in v) as eight nibbles, cell k at bits 4k
+CB_HD uint32_t pack_symbols(uint64_t v, int symbol_bits)
+{
+    v &= 0x0101010101010101ull * (uint64_t)((1u << symbol_bits) - 1);
+    v = (v | (v >> 4)) & 0x00FF00FF00FF00FFull;
+    v = (v | (v >> 8)) & 0x0000FFFF0000FFFFull;
+    return (uint32_t)(v | (v >> 16));
+}
+
+// the number of nibbles in which two packed words differ
+CB_HD int differing_symbols(uint32_t a, uint32_t b)
+{
+    uint32_t x = a ^ b;
+    x |= x >> 2;
+    x |= x >> 1;
+#if defined(__CUDA_ARCH__)
+    return __popc(x & 0x11111111u);
+#else
+    return __builtin_popcount(x & 0x11111111u);
+#endif
+}
+
+// match rows: row i holds bit j (word j / 32, bit j % 32) set iff match(i, j), for j < i; bits from i on are not read.  open: one bit
+// per picture, set while it is a leader whose group has fewer than kMaxGroup pictures.  open_matches: word w of row i's candidates
+CB_HD uint32_t open_matches(const uint32_t* row, const uint32_t* open, int i, int w)
+{
+    if (w > i >> 5) return 0;
+    const uint32_t below = w < i >> 5 ? ~0u : (1u << (i & 31)) - 1u;
+    return row[w] & open[w] & below;
+}
+
+// picture i joins leader j (j == i: i leads a new group); size[] counts each leader's pictures
+CB_HD void join(int i, int j, int32_t* size, uint32_t* open)
+{
+    if (j == i) { size[i] = 1; open[i >> 5] |= 1u << (i & 31); return; }
+    if (++size[j] == kMaxGroup) open[j >> 5] &= ~(1u << (j & 31));
+}
+
+// the assignment of the rule over n pictures' match rows (`words` words each) and extract statuses: group_of[0 .. n), returns the
+// number of groups.  (k_assign_groups searches a row's words in parallel, a warp's lanes over 32 words at a time)
+inline int assign_groups(const uint32_t* rows, size_t words, const int32_t* status, int n, int32_t* group_of)
+{
+    std::vector<uint32_t> open(words ? words : 1, 0u);
+    std::vector<int32_t> size((size_t)n, 0), lead((size_t)n, -1);
+    for (int i = 0; i < n; ++i) {
+        if (!takes_part(status[i])) continue;
+        int j = i;
+        for (int w = 0; w <= i >> 5 && j == i; ++w) {
+            const uint32_t x = open_matches(rows + (size_t)i * words, open.data(), i, w);
+            if (x) j = 32 * w + __builtin_ctz(x);
+        }
+        join(i, j, size.data(), open.data());
+        lead[(size_t)i] = j;
+    }
+    std::vector<int32_t> number((size_t)n, -1);
+    int groups = 0;
+    for (int i = 0; i < n; ++i)
+        if (lead[(size_t)i] == i && size[(size_t)i] >= 2) number[(size_t)i] = groups++;
+    for (int i = 0; i < n; ++i) group_of[i] = lead[(size_t)i] < 0 ? -1 : number[(size_t)lead[(size_t)i]];
+    return groups;
+}
+
 }  // namespace combine
 }  // namespace cb200

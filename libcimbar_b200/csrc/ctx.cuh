@@ -328,6 +328,10 @@ struct cb200_ctx {
     // walk's cell traces of the pictures (n x num_cells), both grown through grow()
     cb200::DevBuf<uint8_t> d_combined;
     cb200::DevBuf<cb200::CellTrace> d_traces;
+    // a grouped camera call (cb200_scan_extract_decode_chunks_grouped_dev): the pictures' match rows (n x ceil(n / 32) words) and the
+    // group table (n / 2 + 1 offsets, n members) followed by the assignment's scratch (2 n), both grown through grow()
+    cb200::DevBuf<uint32_t> d_pairs;
+    cb200::DevBuf<int32_t> d_groups;
     int ccm_frames = 0;              // frames of the last call that took the fitted-CCM route (cb200_get_frame_ccms)
     cudaEvent_t ccm_ev = nullptr;    // recorded after the D2H copies of the last batch's CCM (ccm_resolve waits on it)
     cb200::GatherState* gather = nullptr;   // multi-GPU chunk-record window (gather.cu)
@@ -358,11 +362,17 @@ namespace cb200 {
 inline void begin_timed_call(cb200_ctx* c) { if (c->timing) { c->cur = (int)(c->calls % cb200_ctx::kEvSets); c->calls++; c->ev_count[c->cur] = 0; } }
 inline void mark(cb200_ctx* c) { if (c->timing && c->ev_count[c->cur] < 8) cudaEventRecord(c->ev[c->cur][c->ev_count[c->cur]++], c->stream); }
 
+// the groups of a grouped camera call's n >= 2 pictures, enqueued: the match rows into c->d_pairs, then d_group_of, d_group_count and
+// the group table of n / 2 slots in c->d_groups (offsets, members), from the final cell bytes and the extract statuses (group.cu)
+int find_groups(cb200_ctx* c, int n, const int32_t* d_status, int32_t* d_group_of, int32_t* d_group_count);
+
 // the groups of a combined camera call (cb200_scan_extract_decode_chunks_combined_dev): the host group_of (n entries), the number of
 // groups m and whether its three group outputs are all non-null.  check_groups: CB200_ERR_ARG for CB200_FLAG_NO_FALLBACK with m > 0,
 // m < 0, a null group_of with m > 0, an entry outside [-1, m) or a group of more than combine::kMaxGroup pictures (naming the
-// picture), null group outputs with m > 0; no CUDA call, no context needed (scan.cu)
-struct CameraGroups { const int32_t* of; int m; bool outputs; };
+// picture), null group outputs with m > 0; no CUDA call, no context needed (scan.cu).  found: the grouped call
+// (cb200_scan_extract_decode_chunks_grouped_dev), whose groups the device finds: CB200_ERR_ARG for CB200_FLAG_NO_FALLBACK and for
+// null group outputs (its five), whatever n is
+struct CameraGroups { const int32_t* of; int m; bool outputs; bool found = false; };
 int check_groups(uint32_t flags, const CameraGroups& g, int n);
 
 // the checks every camera and corner call shares, in this order and before any CUDA call: the flags; the batch, from the call's

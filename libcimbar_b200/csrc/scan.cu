@@ -946,6 +946,10 @@ static int scan_extract_decode_dev(cb200_ctx* c, Build&& build, uint32_t flags, 
 // ---- the combined call (cb200_scan_extract_decode_chunks_combined_dev): per-cell vote over groups of pictures of one frame
 int check_groups(uint32_t flags, const CameraGroups& g, int n)
 {
+    if (g.found) {
+        if (flags & CB200_FLAG_NO_FALLBACK) return fail(CB200_ERR_ARG, "CB200_FLAG_NO_FALLBACK: the vote needs every picture's walk");
+        return g.outputs ? CB200_OK : fail(CB200_ERR_ARG, "null group output");
+    }
     if (g.m > 0 && (flags & CB200_FLAG_NO_FALLBACK))
         return fail(CB200_ERR_ARG, "CB200_FLAG_NO_FALLBACK with m > 0: the vote needs every picture's walk");
     if (g.m < 0) return fail(CB200_ERR_ARG, "m = " + std::to_string(g.m) + " < 0");
@@ -962,13 +966,17 @@ int check_groups(uint32_t flags, const CameraGroups& g, int n)
     return CB200_OK;
 }
 
-// the combined call's own buffers: the groups' cells and the pictures' traces.  With live plans grow() makes no CUDA call and refuses
-// what would grow, so the call runs this before any CUDA call then
-static int combine_reserve(cb200_ctx* c, int n, int m)
+// the combined and grouped calls' own buffers: the groups' cells and the pictures' traces, and with `pairs` (the grouped call) the
+// match rows and the group table with the assignment's scratch.  With live plans grow() makes no CUDA call and refuses what would
+// grow, so the calls run this before any CUDA call then
+static int combine_reserve(cb200_ctx* c, int n, int m, bool pairs)
 {
     const size_t cells = (size_t)c->mode.num_cells;
     int rc;
     if ((rc = grow(c, c->d_combined, (size_t)m * cells, "combined cells")) || (rc = grow(c, c->d_traces, (size_t)n * cells, "cell traces")))
+        return rc;
+    if (pairs && ((rc = grow(c, c->d_pairs, (size_t)n * (((size_t)n + 31) / 32), "match rows")) ||
+                  (rc = grow(c, c->d_groups, (size_t)m + 1 + 3 * (size_t)n, "group table"))))
         return rc;
     return CB200_OK;
 }
@@ -1006,33 +1014,30 @@ static int combine_empty(cb200_ctx* c, int m, uint8_t* d_group_chunks, uint32_t*
     return CB200_OK;
 }
 
-// camera_enqueue with the group table behind the picture table (one upload) and the walk's traces kept, then the vote and the
-// groups' decode: the route of a call without colour correction (k2_rs_fused_launch: the frame-pair kernel where it applies), the
-// chunk masks, and mask 0 for a group without pictures (k_mask_failed on the counts).  Four launches more than the pictures call
-static int combine_enqueue(cb200_ctx* c, const CameraBatch& b, const int32_t* group_of, int m, uint32_t flags, uint8_t* d_chunks,
-                           uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, uint8_t* d_group_chunks,
-                           uint32_t* d_group_mask, int32_t* d_group_used)
+// camera_enqueue with the walk's traces kept and `tail` (or nothing) behind the picture table, at *d_tail on the device
+static int combine_pictures(cb200_ctx* c, const CameraBatch& b, int m, bool pairs, const std::vector<uint8_t>* tail, const uint8_t** d_tail,
+                            uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
 {
-    const Mode& md = c->mode;
     const int n = b.n();
     int rc;
-    if ((rc = combine_reserve(c, n, m)) || (rc = camera_reserve(c, b))) return rc;
+    if ((rc = combine_reserve(c, n, m, pairs)) || (rc = camera_reserve(c, b))) return rc;
     uint8_t* frames;
     if ((rc = deskew_frames(c, n, &frames))) return rc;
-    std::vector<int32_t> table((size_t)m + 1 + (size_t)n);
-    combine::group_table(group_of, n, m, table.data(), table.data() + m + 1);
-    table.resize((size_t)m + 1 + (size_t)table[(size_t)m]);
-    std::vector<uint8_t> tail(table.size() * sizeof(int32_t));
-    memcpy(tail.data(), table.data(), tail.size());
     const PicDesc* d_desc;
-    const uint8_t* d_tail;
-    if ((rc = camera_scan(c, b, nullptr, &d_desc, nullptr, &tail, &d_tail))) return rc;
-    rc = camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, nullptr,
-                           c->d_traces);
-    if (rc) return rc;
-    const int32_t* d_offsets = reinterpret_cast<const int32_t*>(d_tail);
+    if ((rc = camera_scan(c, b, nullptr, &d_desc, nullptr, tail, d_tail))) return rc;
+    return camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, nullptr,
+                             c->d_traces);
+}
+
+// the vote and the decode of the m groups of the table at d_table (offsets[0 .. m], then the members): the route of a call without
+// colour correction (k2_rs_fused_launch: the frame-pair kernel where it applies), the chunk masks, and mask 0 for a group without
+// pictures (k_mask_failed on the counts).  Four launches
+static int combine_groups(cb200_ctx* c, int m, const int32_t* d_table, uint32_t flags, const int32_t* d_extract_status, uint8_t* d_group_chunks,
+                          uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    const Mode& md = c->mode;
     const long long threads = (long long)m * md.num_cells;
-    k_combine<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(m, md.num_cells, d_offsets, d_offsets + m + 1, d_extract_status,
+    k_combine<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(m, md.num_cells, d_table, d_table + m + 1, d_extract_status,
                                                                        c->d_cellvals, c->d_traces, c->d_combined, d_group_used);
     count_launch();
     CK(cudaGetLastError(), "combine launch");
@@ -1043,6 +1048,39 @@ static int combine_enqueue(cb200_ctx* c, const CameraBatch& b, const int32_t* gr
     count_launch();
     CK(cudaGetLastError(), "group mask launch");
     return CB200_OK;
+}
+
+// the combined call with groups: the group table travels behind the picture table (one upload).  Four launches more than the
+// pictures call
+static int combine_enqueue(cb200_ctx* c, const CameraBatch& b, const int32_t* group_of, int m, uint32_t flags, uint8_t* d_chunks,
+                           uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, uint8_t* d_group_chunks,
+                           uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    const int n = b.n();
+    std::vector<int32_t> table((size_t)m + 1 + (size_t)n);
+    combine::group_table(group_of, n, m, table.data(), table.data() + m + 1);
+    table.resize((size_t)m + 1 + (size_t)table[(size_t)m]);
+    std::vector<uint8_t> tail(table.size() * sizeof(int32_t));
+    memcpy(tail.data(), table.data(), tail.size());
+    const uint8_t* d_tail;
+    int rc = combine_pictures(c, b, m, false, &tail, &d_tail, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    if (rc) return rc;
+    return combine_groups(c, m, reinterpret_cast<const int32_t*>(d_tail), flags, d_extract_status, d_group_chunks, d_group_mask, d_group_used);
+}
+
+// ---- the grouped call (cb200_scan_extract_decode_chunks_grouped_dev): the groups found on the device from the pictures' cells
+// the grouped call after the argument checks, n >= 2: the pictures call with traces, find_groups (group.cu) into d_group_of,
+// d_group_count and the table in c->d_groups (n / 2 slots), then combine_groups over the slots.  Six launches more than the pictures
+// call, and no wait of its own
+static int grouped_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                           int32_t* d_extract_status, int32_t* d_group_of, int32_t* d_group_count, uint8_t* d_group_chunks,
+                           uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    const int n = b.n(), slots = n / 2;
+    int rc = combine_pictures(c, b, slots, true, nullptr, nullptr, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    if (rc) return rc;
+    if ((rc = find_groups(c, n, d_extract_status, d_group_of, d_group_count))) return rc;
+    return combine_groups(c, slots, c->d_groups, flags, d_extract_status, d_group_chunks, d_group_mask, d_group_used);
 }
 
 // the scan entry points: the batch, the context and the count output checked, the batch staged and scanned, the results copied out
@@ -1176,11 +1214,40 @@ int cb200_scan_extract_decode_chunks_combined_dev(cb200_ctx* c, const cb200_pict
         CK(cudaSetDevice(c->device), "cudaSetDevice");
         return combine_empty(c, m, d_group_chunks, d_group_mask, d_group_used);
     }
-    if ((rc = check_frozen_camera(c, b.wh.data(), nb)) || (m > 0 && !c->plans.empty() && (rc = combine_reserve(c, nb, m)))) return rc;
+    if ((rc = check_frozen_camera(c, b.wh.data(), nb)) || (m > 0 && !c->plans.empty() && (rc = combine_reserve(c, nb, m, false)))) return rc;
     CK(cudaSetDevice(c->device), "cudaSetDevice");
     if (m == 0) return camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
     return combine_enqueue(c, b, group_of, m, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, d_group_chunks, d_group_mask,
                            d_group_used);
+}
+
+int cb200_scan_extract_decode_chunks_grouped_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, uint8_t* d_chunks,
+                                                 uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, int32_t* d_group_of,
+                                                 int32_t* d_group_count, uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    CameraBatch b;
+    auto build = [&](CameraBatch& bb) { return picture_batch(pics, n, bb); };
+    const CameraGroups groups = {nullptr, 0, d_group_of && d_group_count && d_group_chunks && d_group_mask && d_group_used, true};
+    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output", &groups);
+    if (rc) return rc;
+    const int nb = b.n();
+    if (nb == 0) {
+        rc = empty_stripe(c, flags, true);
+    } else {
+        if ((rc = check_frozen_camera(c, b.wh.data(), nb)) || (nb >= 2 && !c->plans.empty() && (rc = combine_reserve(c, nb, nb / 2, true))))
+            return rc;
+        CK(cudaSetDevice(c->device), "cudaSetDevice");
+        if (nb >= 2)
+            return grouped_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, d_group_of, d_group_count,
+                                   d_group_chunks, d_group_mask, d_group_used);
+        rc = camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
+    }
+    if (rc) return rc;
+    // fewer than two pictures form no group
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    CK(cudaMemsetAsync(d_group_of, 0xFF, sizeof(int32_t) * (size_t)nb, c->stream), "memset group_of");
+    CK(cudaMemsetAsync(d_group_count, 0, sizeof(int32_t), c->stream), "memset group count");
+    return CB200_OK;
 }
 
 int cb200_scan_extract_decode_chunks_receivers_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, const int32_t* receiver_of,
