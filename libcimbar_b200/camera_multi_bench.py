@@ -28,7 +28,7 @@ def main():
     import torch.distributed as dist
     import libcimbar_b200 as cb
     from libcimbar_b200.dist import CameraExchange, stripe
-    from libcimbar_b200.ragged_bench import card, load_pictures
+    from libcimbar_b200.bench_support import card, load_pictures
     dist.init_process_group("gloo")
     rank, world = dist.get_rank(), dist.get_world_size()
     dev_index = int(os.environ.get("LOCAL_RANK", rank)) % torch.cuda.device_count()

@@ -17,7 +17,7 @@ import json
 
 import numpy as np
 
-from libcimbar_b200.ragged_bench import card, load_pictures
+from libcimbar_b200.bench_support import card, load_pictures
 
 
 def main():

@@ -19,7 +19,7 @@ import time
 
 import numpy as np
 
-from libcimbar_b200.ragged_bench import card, load_pictures
+from libcimbar_b200.bench_support import card, load_pictures
 
 
 def idle_ms(torch, fn):

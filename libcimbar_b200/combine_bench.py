@@ -13,20 +13,14 @@ Without a CUDA device it fails."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 
+from libcimbar_b200.bench_support import card
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True,
-                       check=True).stdout.strip()
-    name, power = [x.strip() for x in q.split(",")]
-    return name, power
 
 
 def main():

@@ -21,7 +21,7 @@ import time
 
 import numpy as np
 
-from libcimbar_b200.ragged_bench import ROOT, card, load_pictures
+from libcimbar_b200.bench_support import ROOT, card, load_pictures
 
 CANDIDATES = [66, 68, 67, 4]
 

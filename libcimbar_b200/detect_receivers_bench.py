@@ -22,21 +22,7 @@ import time
 
 import numpy as np
 
-from libcimbar_b200.ragged_bench import card, load_pictures
-from libcimbar_b200.receivers_bench import photographs
-
-MODES = [66, 68, 67, 4]
-
-
-def candidates(mix, D):
-    """per receiver: its candidate bits"""
-    auto = (1 << len(MODES)) - 1
-    locked = [1 << MODES.index(68 if r % 2 == 0 else 4) for r in range(D)]
-    if mix == "auto":
-        return [auto] * D
-    if mix == "locked":
-        return locked
-    return [auto if r % 10 == 0 else locked[r] for r in range(D)]
+from libcimbar_b200.bench_support import MODES, candidates, card, load_pictures, photographs
 
 
 def main():

@@ -19,7 +19,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
 
-from libcimbar_b200.combine_bench import card  # noqa: E402
+from libcimbar_b200.bench_support import card  # noqa: E402
 
 
 def bench(cb, torch, frames, per, iters, warmup):

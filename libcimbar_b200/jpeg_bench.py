@@ -19,7 +19,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
-from libcimbar_b200.ragged_bench import GLOB, ROOT, card
+from libcimbar_b200.bench_support import GLOB, ROOT, card, timed
 
 
 def load_files():
@@ -34,21 +34,6 @@ def load_files():
             ok, buf = cv2.imencode(".jpg", cv2.cvtColor(big, cv2.COLOR_RGB2BGR), [cv2.IMWRITE_JPEG_PROGRESSIVE, 1])
             out.append(buf.tobytes())
     return out
-
-
-def timed(fn, rounds, stream):
-    """best and all of `rounds` runs of fn, CUDA events on the context's stream around it (host work inside the call included)"""
-    import torch
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    ms = []
-    for _ in range(rounds):
-        torch.cuda.synchronize()
-        e0.record(stream)
-        fn()
-        e1.record(stream)
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return min(ms), ms
 
 
 def main():

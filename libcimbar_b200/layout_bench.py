@@ -20,7 +20,7 @@ import json
 
 import numpy as np
 
-from .ragged_bench import card, load_pictures
+from libcimbar_b200.bench_support import card, load_pictures
 
 LAYOUTS = ["bgr", "rgba", "bgra", "planar"]
 

@@ -19,7 +19,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
-from libcimbar_b200.ragged_bench import ROOT, card
+from libcimbar_b200.bench_support import ROOT, card, timed
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 FRAMES = {68: ["b__tr_0.png", "b__tr_1.png", "b__tr_2.png", "b__tr_3.png"], 4: ["6bit__4color_ecc30_fountain_0.png"]}
@@ -32,21 +32,6 @@ def load_files():
         ok, buf = cv2.imencode(".png", cv2.imread(f, cv2.IMREAD_COLOR))
         out.append(buf.tobytes())
     return out
-
-
-def timed(fn, rounds, stream):
-    """best and all of `rounds` runs of fn, CUDA events on the context's stream around it (host work inside the call included)"""
-    import torch
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    ms = []
-    for _ in range(rounds):
-        torch.cuda.synchronize()
-        e0.record(stream)
-        fn()
-        e1.record(stream)
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return min(ms), ms
 
 
 def rgb_of(data):

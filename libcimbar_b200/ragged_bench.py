@@ -15,33 +15,10 @@ Prints one JSON line: pictures/s and ms per step of each, the scan / decode kern
 name and power limit, and whether (a) and (b) returned the same chunks."""
 import argparse
 import json
-import os
-import subprocess
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-GLOB = ["4_30_802", "4_30_f0_177_ccm", "4_30_f0_627", "4_30_f0_627_extract", None, "4_30_f1_360", "4_30_f2_246", "4_30_f2_734"]
-
-
-def load_pictures():
-    import cv2
-
-    def load(name):
-        img = cv2.imread(os.path.join(ROOT, "tests", "golden", "6bit__%s.jpg" % name), cv2.IMREAD_COLOR)
-        return np.ascontiguousarray(cv2.cvtColor(img, cv2.COLOR_BGR2RGB))
-    return [load(n) if n else cv2.resize(load("4_30_f1_360"), None, fx=2.8, fy=2.8) for n in GLOB]
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                           text=True, timeout=30).stdout.strip()
-        name, power = [s.strip() for s in q.split(",")]
-        return name, power
-    except Exception as e:          # the numbers are reported without it, never estimated
-        return "unknown (%s)" % e, "unknown"
+from libcimbar_b200.bench_support import card, load_pictures
 
 
 def main():

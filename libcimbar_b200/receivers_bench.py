@@ -20,30 +20,11 @@ its call is reported for every shape.  Under mode B the 4C pictures of the pool 
 but yield no chunks; the mode-B photographs decode."""
 import argparse
 import json
-import os
 import time
 
 import numpy as np
 
-from libcimbar_b200.ragged_bench import ROOT, card, load_pictures
-
-
-def photographs():
-    import cv2
-    out = []
-    for name in ("b__ex2434.jpg", "b__ex380.jpg"):
-        img = cv2.imread(os.path.join(ROOT, "tests", "golden", name), cv2.IMREAD_COLOR)
-        out.append(np.ascontiguousarray(cv2.cvtColor(img, cv2.COLOR_BGR2RGB)))
-    return out
-
-
-def entry_states(D):
-    """distinct active matrices: a mild cast that differs per receiver"""
-    out = []
-    for r in range(D):
-        g = 1.0 + 0.002 * (r % 50)
-        out.append(np.diag([g, 1.0, 2.0 - g]).astype(np.float32))
-    return out
+from libcimbar_b200.bench_support import card, entry_states, load_pictures, photographs
 
 
 def main():

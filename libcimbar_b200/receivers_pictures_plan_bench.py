@@ -22,9 +22,7 @@ import time
 
 import numpy as np
 
-from libcimbar_b200.detect_receivers_bench import MODES, candidates
-from libcimbar_b200.ragged_bench import card, load_pictures
-from libcimbar_b200.receivers_bench import entry_states, photographs
+from libcimbar_b200.bench_support import MODES, candidates, card, entry_states, load_pictures, photographs
 
 
 def main():

@@ -18,8 +18,7 @@ import time
 
 import numpy as np
 
-from libcimbar_b200.ragged_bench import card, load_pictures
-from libcimbar_b200.receivers_bench import entry_states, photographs
+from libcimbar_b200.bench_support import card, entry_states, load_pictures, photographs
 
 
 def main():

@@ -15,7 +15,8 @@ import numpy as np
 import libcimbar_b200 as cb
 
 
-def card():
+def device_card():
+    """the card as NVML gives it: name, enforced power limit in W as a number, maximum SM clock"""
     import torch
     out = {"name": torch.cuda.get_device_name(), "power_limit_w": None}
     try:
@@ -90,7 +91,7 @@ def main():
 
     out = {"metric": "decoded cimbar frames/sec with a per-frame sharpen choice (mode %d)" % args.mode, "unit": "frames/s",
            "frames_per_step": B, "steps_per_round": K, "rounds": 2, "warmup": W,
-           "pattern": "seeded permutation: %d of %d frames sharpened" % (int(sel.sum()), B), "card": card()}
+           "pattern": "seeded permutation: %d of %d frames sharpened" % (int(sel.sum()), B), "card": device_card()}
     for name, a in acc.items():
         ms = sum(a["ms"]) / len(a["ms"])
         out[name] = {"value": B / (ms * 1e-3), "ms_per_step": ms, "ms_per_step_rounds": a["ms"],

@@ -17,11 +17,11 @@ CAST_CAMERA = (0.4, 0.7, 1.0)
 
 
 def crafted(gains):
-    """the fountain frames of test_gpu_rs_crafted.cc_pool (mode B) rendered under a colour cast: frames 0, 1, 3, 4 fit their own
+    """the fountain frames of crafted_rs.cc_pool (mode B) rendered under a colour cast: frames 0, 1, 3, 4 fit their own
     matrix (frame 1 only after RS correction, frame 3 from its second chunk); frame 2 has no header, so it decodes its colours with
     whatever CCM it is handed, and under these casts its colour blocks and colour-stream chunks come out differently with the
     matrix of a fitted frame than without one"""
-    from test_gpu_rs_crafted import ORA, cc_pool, raw_to_cells
+    from crafted_rs import ORA, cc_pool, raw_to_cells
     g, _, raw, _ = cc_pool(68)
     out = []
     for r in raw:

@@ -9,8 +9,8 @@ import pytest
 
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
-from test_abi_jpeg_args import PHOTO
-from test_abi_png_args import BASE as PNG
+from cpu_support import PHOTO
+from png_corpus import BASE as PNG
 
 
 @pytest.fixture(scope="module", autouse=True)

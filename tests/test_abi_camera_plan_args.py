@@ -10,7 +10,7 @@ import pytest
 
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
-from test_abi_ragged_args import GOOD, batch, err, lib
+from cpu_support import GOOD, batch, err, lib
 
 
 @pytest.fixture(scope="module", autouse=True)

@@ -13,7 +13,7 @@ import pytest
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
 from libcimbar_b200.dist import stripe
-from test_abi_ragged_args import err, lib
+from cpu_support import err, lib
 
 
 @pytest.fixture(scope="module", autouse=True)

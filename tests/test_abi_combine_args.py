@@ -10,7 +10,7 @@ import pytest
 
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
-from test_abi_layout_args import good, with_
+from cpu_support import good, with_
 
 
 @pytest.fixture(scope="module", autouse=True)

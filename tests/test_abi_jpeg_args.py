@@ -10,7 +10,7 @@ import pytest
 
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
-from jpeg_matrix import golden_files
+from cpu_support import PHOTO
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -31,7 +31,6 @@ def encode(img, **kw):
     return buf.tobytes()
 
 
-PHOTO = dict(golden_files())["6bit__4_30_f0_627.jpg"]
 IMG = np.random.default_rng(5).integers(0, 256, (120, 160, 3), dtype=np.uint8)
 
 

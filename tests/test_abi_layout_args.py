@@ -9,6 +9,7 @@ import pytest
 
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
+from cpu_support import err, good, with_
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -20,18 +21,7 @@ def lib():
     return cb.load_library()
 
 
-def err(rc, text):
-    msg = lib().cb200_last_error()
-    assert rc == -1 and text in msg, msg
-
-
 CH = {cb.LAYOUT_RGB: 3, cb.LAYOUT_BGR: 3, cb.LAYOUT_RGBA: 4, cb.LAYOUT_BGRA: 4, cb.LAYOUT_RGB_PLANAR: 1}
-
-
-def good():
-    """descriptors of four well-formed pictures (stand-in addresses: never dereferenced before the checks)"""
-    return [cb.Picture(0x10000, 1280, 960, 3 * 1280, 0, cb.LAYOUT_BGR), cb.Picture(0x20001, 955, 637, 4 * 955 + 9, 0, cb.LAYOUT_RGBA),
-            cb.Picture(0x30003, 960, 1280, 1024, 1024 * 1300, cb.LAYOUT_RGB_PLANAR), cb.Picture(0x40000, 640, 480, 4 * 640, 0, cb.LAYOUT_BGRA)]
 
 
 def call(pics, n=None, flags=0, null_array=False):
@@ -41,13 +31,6 @@ def call(pics, n=None, flags=0, null_array=False):
     return lib().cb200_scan_extract_decode_chunks_pictures_dev(None, None if null_array else C.cast(arr, C.c_void_p),
                                                                len(pics) if n is None else n, flags, out.ctypes.data,
                                                                out.ctypes.data, None, st.ctypes.data)
-
-
-def with_(i, **kw):
-    pics = good()
-    for k, v in kw.items():
-        setattr(pics[i], k, v)
-    return pics
 
 
 def test_good_arguments_reach_the_context_check():

@@ -9,37 +9,12 @@ import pytest
 
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
+from cpu_support import GOOD, batch, err, lib
 
 
 @pytest.fixture(scope="module", autouse=True)
 def built():
     cbbuild.build()
-
-
-LIB = None
-
-
-def lib():
-    global LIB
-    if LIB is None:
-        LIB = cb.load_library()
-    return LIB
-
-
-def err(rc, text):
-    msg = lib().cb200_last_error()
-    assert rc == -1 and text in msg, msg
-
-
-def batch(shapes):
-    """host pictures of the given (h, w), their pointer array and wh"""
-    pics = [np.zeros((h, w, 3), np.uint8) for h, w in shapes]
-    ptrs = (C.c_void_p * len(pics))(*[p.ctypes.data for p in pics])
-    wh = np.array([(w, h) for h, w in shapes], np.int32).reshape(-1, 2)
-    return pics, ptrs, wh
-
-
-GOOD = [(960, 1280), (1280, 960), (637, 955)]
 
 
 def calls(ptrs, wh, n, flags=0):

@@ -3,20 +3,16 @@ for the host (tests/cpp/combine_core_host.cpp) and checked against a literal num
 (1) the value most participating pictures hold, (2) among values tied on count the one with the smallest walk distance among its
 pictures, (3) the value of the earliest picture.  The group table is a stable counting sort of group_of into CSR offsets."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from host_harness import build_harness
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("combine_core") / "combine_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(ROOT, "tests", "cpp", "combine_core_host.cpp")])
-    L = C.CDLL(so)
+    L = build_harness(tmp_path_factory, "combine_core_host")
     L.cc_vote.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     L.cc_takes_part.argtypes = [C.c_int32]
     L.cc_group_error.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int)]

@@ -6,17 +6,9 @@ import pytest
 
 import libcimbar_b200 as cb
 from oracle_lib import Oracle, load_sample
+from cpu_support import camera_view
 
 ORA = Oracle()
-
-
-def camera_view(frame, quad, size):
-    """a synthetic camera image: the 1024x1024 frame seen in perspective inside a larger picture (made with cv2)"""
-    import cv2
-    h, w = frame.shape[:2]
-    src = np.float32([[0, 0], [w, 0], [0, h], [w, h]])
-    M = cv2.getPerspectiveTransform(src, np.float32(quad))
-    return cv2.warpPerspective(frame, M, size, flags=cv2.INTER_LINEAR)
 
 
 def test_perspective_transform_matches_cv2_bit_for_bit():

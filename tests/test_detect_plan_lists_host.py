@@ -13,6 +13,7 @@ import subprocess
 
 import numpy as np
 import pytest
+from cpu_support import run
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INT_MIN, INT_MAX = -2 ** 31, 2 ** 31 - 1
@@ -41,7 +42,6 @@ def plan_lists(exe, cand, of, receivers, group):
 
 def direct_lists(exe, cand, of, receivers, group):
     """detect_lists over these (non-empty) pictures: (U_g per geometry, counts, maps, positions)"""
-    from test_detect_receivers_core_host import run
     return run(exe, cand, of, receivers, group)
 
 

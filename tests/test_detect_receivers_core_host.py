@@ -10,6 +10,7 @@ import subprocess
 
 import numpy as np
 import pytest
+from cpu_support import run
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -19,22 +20,6 @@ def exe(tmp_path_factory):
     path = str(tmp_path_factory.mktemp("detect_lists") / "detect_lists_host")
     subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", path, os.path.join(ROOT, "tests", "cpp", "detect_lists_host.cpp")])
     return path
-
-
-def run(exe, cand, of, receivers, group):
-    n, k = len(cand), len(group)
-    data = np.concatenate([np.array([n, receivers, k], np.int32), np.asarray(group, np.int32), np.asarray(cand, np.uint32).view(np.int32),
-                           np.asarray(of, np.int32)]).tobytes()
-    out = np.frombuffer(subprocess.run([exe], input=data, stdout=subprocess.PIPE, check=True).stdout, np.int32)
-    at = 0
-    slots, counts, maps = [], [], []
-    for _ in range(k):
-        m = int(out[at]); slots.append(out[at + 1:at + 1 + m]); at += 1 + m
-    for _ in range(k):
-        counts.append(int(out[at])); m = int(out[at + 1]); maps.append(out[at + 2:at + 2 + m]); at += 2 + m
-    pos = out[at:].reshape(k, n)
-    assert at + k * n == len(out)
-    return slots, counts, maps, pos
 
 
 def model_order(of, receivers):

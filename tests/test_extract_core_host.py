@@ -3,8 +3,6 @@ cb200_perspective_transform and the deskew use on the host) compiled for the hos
 oracle's Corners, the transform against cb200_perspective_transform and cv2.getPerspectiveTransform, the inverse against cv2.invert --
 bit for bit.  The GPU test (tests/test_gpu_camera_dev.py) compares the device's transforms with the same references."""
 import ctypes as C
-import os
-import subprocess
 
 import cv2
 import numpy as np
@@ -14,8 +12,8 @@ import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
 from ragged_samples import GLOB, sample
 from scan_oracle_lib import ScanOracle
+from host_harness import build_harness
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = ScanOracle()
 MODES = [(1024, 1024), (1024, 720), (736, 637)]
 AN = 30
@@ -24,10 +22,7 @@ AN = 30
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
     cbbuild.build()
-    so = str(tmp_path_factory.mktemp("extract_core") / "extract_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so,
-                           os.path.join(ROOT, "tests", "cpp", "extract_core_host.cpp")])
-    lib = C.CDLL(so)
+    lib = build_harness(tmp_path_factory, "extract_core_host", "-ffp-contract=off")
     vp = C.c_void_p
     lib.ec_extract.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     lib.ec_transform.argtypes = [vp, vp, vp]

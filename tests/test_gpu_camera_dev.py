@@ -8,24 +8,14 @@ import cv2
 import numpy as np
 import pytest
 
-from oracle_lib import load_sample
 from ragged_samples import GLOB, sample
 from scan_oracle_lib import ScanOracle
-from test_gpu_sharpen_select import ORA, dense
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import ORA, batch_b, cli_loop, dense, packed, pad, same_ccm
 
 pytestmark = pytest.mark.gpu
 
 SO = ScanOracle()
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
-
-
-def pad(rgb, top, bottom, left, right):
-    return cv2.copyMakeBorder(rgb, top, bottom, left, right, cv2.BORDER_CONSTANT, value=(0, 0, 0))
 
 
 def batch_4c():
@@ -36,55 +26,6 @@ def batch_4c():
     pics.append(pad(sample("6bit/4_30_f1_360.jpg"), 90, 70, 200, 140))
     pics.append(sample("6bit/4_30_f2_734.jpg"))
     return pics
-
-
-def batch_b():
-    """the two mode-B photographs, a zero-padded and an upscaled variant of each, and a noise picture"""
-    a, b = load_sample("b/ex2434.jpg"), load_sample("b/ex380.jpg")
-    noise = np.random.default_rng(53).integers(0, 256, (800, 1000, 3), dtype=np.uint8)
-    return [a, pad(b, 200, 160, 240, 300), noise, cv2.resize(a, None, fx=1.3, fy=1.3), b, pad(a, 60, 40, 80, 20),
-            cv2.resize(b, None, fx=1.6, fy=1.6)]
-
-
-_loops = {}
-
-
-def cli_loop(mode_val, name, pics, cc, sharpen):
-    """the reference CLI's loop: sharpen = 'no' / 'all' / 'needed' (--preprocess 0 / 1 / -1); FAILURE pictures are skipped.  Returns
-    per picture (status, corners, (good, dense chunks, mask)) and the decoder's CCM at the end"""
-    key = (mode_val, name, cc, sharpen)
-    if key in _loops:
-        return _loops[key]
-    m = ORA.mode(mode_val)
-    an, W, H = 30, m.image_size_x, m.image_size_y
-    dst = np.array([[an, an], [W - an, an], [an, H - an], [W - an, H - an]], np.float32)
-    out = []
-    ORA.set_ccm(None)
-    try:
-        for rgb in pics:
-            anchors, _ = SO.scan(rgb)
-            if anchors is None or len(anchors) < 4:
-                out.append((0, None, None))
-                continue
-            xy = SO.corners(anchors)
-            status = 1 if SO.is_granular_scale(xy, W, H) else 2
-            frame = cv2.warpPerspective(rgb, cv2.getPerspectiveTransform(np.array(xy, np.float32).reshape(4, 2), dst), (W, H),
-                                        flags=cv2.INTER_LINEAR)
-            sh = {"no": False, "all": True, "needed": status == 2}[sharpen]
-            good, chunks, mask = ORA.decode_fountain(m, frame, sharpen=sh, color_correction=cc)
-            out.append((status, xy, (good, chunks.copy(), mask)))
-        ccm = ORA.get_ccm()
-    finally:
-        ORA.set_ccm(None)
-    _loops[key] = (out, ccm)
-    return _loops[key]
-
-
-def packed(pics):
-    import torch
-    d = torch.cat([torch.from_numpy(np.ascontiguousarray(p).reshape(-1)) for p in pics]).cuda()
-    wh = np.array([(p.shape[1], p.shape[0]) for p in pics], np.int32).reshape(-1, 2)
-    return d, wh
 
 
 class Outputs:
@@ -129,10 +70,6 @@ def check_against_loop(m, got, want, what):
         cnt, rows = dense(m, chunks[i], int(mask[i]))
         assert mask[i] == wmask and cnt * m.chunk_size == good, (what, i)
         assert np.array_equal(rows, wchunks[:cnt]), (what, i)
-
-
-def same_ccm(a, b):
-    return (a is None) == (b is None) and (a is None or np.array_equal(a, b))
 
 
 FLAGS = [("no", 0, 0), ("all", "SHARPEN", 0), ("needed", "SHARPEN_IF_NEEDED", 0), ("needed", "SHARPEN_IF_NEEDED", "CC_SIMPLE"),

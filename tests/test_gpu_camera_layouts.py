@@ -9,14 +9,9 @@ import pytest
 
 from oracle_lib import load_sample
 from ragged_samples import GLOB, sample
+from gpu_support import cb  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def odd_crop(rgb):

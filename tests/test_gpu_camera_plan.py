@@ -15,16 +15,12 @@ import pytest
 
 from oracle_lib import load_sample
 from ragged_samples import GLOB, sample
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import pad, same_ccm
 
 pytestmark = pytest.mark.gpu
 
 K = 6
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def radius(w, h):
@@ -33,10 +29,6 @@ def radius(w, h):
     for s in (1, 2, 4, 8, 16):
         v |= v >> s
     return max((v + 2) & 0xFFFFFFFF, 3) // 2
-
-
-def pad(rgb, top, bottom, left, right):
-    return cv2.copyMakeBorder(rgb, top, bottom, left, right, cv2.BORDER_CONSTANT, value=(0, 0, 0))
 
 
 def ragged_4c():
@@ -115,10 +107,6 @@ class Out:
 
     def host(self):
         return [tuple(t.cpu().numpy() for t in s) for s in self.saved]
-
-
-def same_ccm(a, b):
-    return (a is None) == (b is None) and (a is None or np.array_equal(a, b))
 
 
 def direct_sequence(cb, mode_val, batches, flags_seq, between=None):

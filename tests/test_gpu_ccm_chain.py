@@ -17,12 +17,7 @@ ROOT = os.path.dirname(HERE)
 sys.path.insert(0, HERE)
 
 import chain_batches as CB  # noqa: E402
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
+from gpu_support import cb  # noqa: F401  (fixtures)
 
 
 def _gpus():

@@ -12,17 +12,12 @@ import pytest
 
 from combine_fixtures import ORA, capture, clean_picture, fitted_cells, group_expectation, picture_cells
 from ragged_samples import sample
+from gpu_support import cb  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
 MODES = [68, 67, 66, 4, 8]
 FLAGS = ["none", "SHARPEN_IF_NEEDED", "CC_SIMPLE", "CC_FIT"]
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def flag_bits(cb, name):

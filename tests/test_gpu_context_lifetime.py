@@ -5,16 +5,11 @@ import numpy as np
 import pytest
 
 from ragged_samples import GLOB, sample
-from test_deskew import camera_view
-from test_gpu_sharpen_select import POOL, check_dense, dense, oracle, pool
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import POOL, check_dense, dense, frame_pool, oracle
+from cpu_support import camera_view
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def test_dev_entry_points_only_enqueue(cb):
@@ -23,7 +18,7 @@ def test_dev_entry_points_only_enqueue(cb):
     import cv2
     import torch
     n = 4
-    m, frames = pool(68)
+    m, frames = frame_pool(68)
     idx = np.arange(n) % POOL
     sel = np.array([1, 0, 0, 1], np.uint8)
     quads = [[[210, 130], [1480, 190], [160, 1350], [1530, 1290]], [[40, 60], [1500, 20], [80, 1360], [1540, 1430]]] * 2
@@ -98,7 +93,7 @@ def test_destroy_returns_every_buffer(cb):
     """five contexts, each driven through every lazily grown buffer, then destroyed: the process's device memory (NVML, per
     process -- other jobs share the card) ends where it started"""
     n = 6
-    m, frames = pool(68)
+    m, frames = frame_pool(68)
     batch = frames[np.arange(n) % POOL]
     sel = np.arange(n) % 2 == 1
     pictures = [sample(s) for s in GLOB[:n]]

@@ -6,127 +6,15 @@ modes, with the scan done once and one exact walk per frame geometry.
   - for every flag combination of the camera tests and several candidate sets, each context ends exactly where a direct call on
     it would: masks, records, statuses, transforms and the CCM carried over two calls;
   - the walk runs once per geometry (one for 68 / 4 / 8, three for 66 / 68 / 67 / 4), and the geometries' walks overlap."""
-import cv2
 import numpy as np
 import pytest
 
 from oracle_lib import load_sample
 from ragged_samples import GLOB, sample
-from test_gpu_camera_dev import batch_b, cli_loop, packed
-from test_gpu_sharpen_select import ORA, dense
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import Detect, FLAGS, ORA, RECV, cli_loop, contexts, dense, detect, exact_pictures, mixed_pictures, packed, rendered
 
 pytestmark = pytest.mark.gpu
-
-RECV = [66, 68, 67, 4]                                  # the reference receiver's candidates, in its order
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
-
-
-def pad(rgb, top, bottom, left, right):
-    return cv2.copyMakeBorder(rgb, top, bottom, left, right, cv2.BORDER_CONSTANT, value=(0, 0, 0))
-
-
-def mixed_pictures():
-    """the mode-B photographs (padded and upscaled variants among them) interleaved with the 4C sample photographs, and a noise
-    picture; returns the pictures and their kind ('b', '4c', 'noise')"""
-    b = [p for i, p in enumerate(batch_b()) if i != 2]            # batch_b's third picture is its noise picture
-    c = [sample(s) for s in GLOB]
-    noise = np.random.default_rng(61).integers(0, 256, (900, 1100, 3), dtype=np.uint8)
-    pics, kinds = [], []
-    for i in range(max(len(b), len(c))):
-        if i < len(b):
-            pics.append(b[i]); kinds.append("b")
-        if i < len(c):
-            pics.append(c[i]); kinds.append("4c")
-        if i == 2:
-            pics.append(noise); kinds.append("noise")
-    return pics, kinds
-
-
-def with_anchors(frame):
-    """a rendered frame of any geometry as a camera picture: the four anchor squares of a real encoder frame pasted into its corners
-    (as chain_batches.with_anchors does for 1024 x 1024; they lie outside every cell of the 8x8 modes)"""
-    tr, c = load_sample("b/tr_0.png"), 62
-    f = frame.copy()
-    H, W = f.shape[:2]
-    for ys, ts in ((slice(0, c), slice(0, c)), (slice(H - c, H), slice(1024 - c, 1024))):
-        for xs, us in ((slice(0, c), slice(0, c)), (slice(W - c, W), slice(1024 - c, 1024))):
-            f[ys, xs] = tr[ts, us]
-    return f
-
-
-_rendered = {}
-
-
-def rendered(cb, mode_val):
-    """two camera pictures of a random-payload frame of this mode: zero-padded, and upscaled with a perspective tilt"""
-    if mode_val in _rendered:
-        return _rendered[mode_val]
-    import torch
-    ctx = cb.Context(mode_val, max_frames=1)
-    info = ctx.info
-    payload = torch.from_numpy(np.random.default_rng(900 + mode_val).integers(0, 256, info.data_bytes, dtype=np.uint8)).cuda()
-    cells = torch.zeros(info.total_cells, dtype=torch.uint8, device="cuda")
-    ctx.encode_cells_dev(payload.data_ptr(), 1, cells.data_ptr())
-    ctx.sync()
-    ctx.close()
-    frame = with_anchors(ORA.render_frame(ORA.mode(mode_val), cells.cpu().numpy()))
-    H, W = frame.shape[:2]
-    big = pad(frame, 90, 110, 120, 80)
-    src = np.float32([[0, 0], [W, 0], [0, H], [W, H]])
-    dst = np.float32([[40, 30], [1.3 * W + 20, 10], [10, 1.3 * H + 30], [1.3 * W + 50, 1.3 * H + 60]])
-    tilt = cv2.warpPerspective(frame, cv2.getPerspectiveTransform(src, dst), (int(1.3 * W) + 100, int(1.3 * H) + 100), flags=cv2.INTER_LINEAR)
-    _rendered[mode_val] = [big, tilt]
-    return _rendered[mode_val]
-
-
-_streams = []
-
-
-def contexts(cb, modes, n):
-    """candidate contexts of these modes, all on one stream (the detect call runs on the stream its contexts share)"""
-    import torch
-    _streams.append(torch.cuda.Stream())
-    ctxs = [cb.Context(m, max_frames=n) for m in modes]
-    for c in ctxs:
-        c.set_stream(_streams[-1].cuda_stream)
-    return ctxs
-
-
-class Detect:
-    """device outputs of one detect call over n pictures with these contexts"""
-
-    def __init__(self, ctxs, n):
-        import torch
-        self.n, self.k = n, len(ctxs)
-        self.slot = max(c.info.data_bytes for c in ctxs)
-        self.chunks = torch.full((n * self.slot,), 0xA5, dtype=torch.uint8, device="cuda")
-        self.mask = torch.full((n,), -7, dtype=torch.int32, device="cuda")
-        self.status = torch.full((n,), 7, dtype=torch.int32, device="cuda")
-        self.mode = torch.full((n,), 9, dtype=torch.int32, device="cuda")
-        self.mode_masks = torch.full((n * self.k,), -7, dtype=torch.int32, device="cuda")
-
-    def call(self, cb, ctxs, d, wh, flags):
-        cb.detect_scan_extract_decode_chunks_dev(ctxs, d.data_ptr(), wh, self.chunks.data_ptr(), self.mask.data_ptr(), self.status.data_ptr(),
-                                                 self.mode.data_ptr(), self.mode_masks.data_ptr(), flags=flags)
-
-    def host(self):
-        return (self.chunks.cpu().numpy().reshape(self.n, self.slot), self.mask.cpu().numpy().view(np.uint32), self.status.cpu().numpy(),
-                self.mode.cpu().numpy(), self.mode_masks.cpu().numpy().view(np.uint32).reshape(self.n, self.k))
-
-
-def detect(cb, ctxs, pics, flags):
-    import torch
-    d, wh = packed(pics)
-    out = Detect(ctxs, len(pics))
-    torch.cuda.synchronize()
-    out.call(cb, ctxs, d, wh, flags)
-    ctxs[0].sync()
-    return out.host()
 
 
 def direct(cb, ctx, pics, flags):
@@ -210,14 +98,7 @@ def test_rendered_frames_are_detected_as_their_mode(cb, mode_val):
 
 
 # ------------------------------------------------------------------------------------------------ exactness
-FLAGS = [("SHARPEN_IF_NEEDED", 0), (0, 0), ("SHARPEN", 0), ("SHARPEN_IF_NEEDED", "CC_SIMPLE"), ("SHARPEN_IF_NEEDED", "CC_FIT"),
-         ("SHARPEN", "CC_FIT")]
 SETS = [RECV, [4, 67, 68, 66], [68, 4, 8]]
-
-
-def exact_pictures(cb):
-    pics, _ = mixed_pictures()
-    return pics[:9] + rendered(cb, 66)[:1] + rendered(cb, 67)[1:] + pics[9:]
 
 
 @pytest.mark.parametrize("modes", SETS, ids=lambda s: "-".join(map(str, s)))

@@ -11,16 +11,10 @@ candidate bit k, in batch order) with mode k's table; then the detect call's sel
 import numpy as np
 import pytest
 
-from test_gpu_detect import FLAGS, RECV, contexts, exact_pictures
-from test_gpu_receivers import camera_call, layouts
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import FLAGS, Out, RECV, camera_call, close, contexts, detect, entry_states, exact_pictures, layouts, run
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 @pytest.fixture(scope="module")
@@ -29,50 +23,6 @@ def pool(cb):
     pics = exact_pictures(cb)
     ts, orders = layouts(pics)
     return ts, orders
-
-
-def entry_states(n_receivers, seed):
-    """distinct entry states: inactive, and colour casts of different strengths"""
-    rng = np.random.default_rng(seed)
-    out = []
-    for r in range(n_receivers):
-        if r % 4 == 0:
-            out.append(None)
-        else:
-            out.append(np.diag(rng.uniform(0.7, 1.3, 3)).astype(np.float32) + np.float32(0.01) * rng.standard_normal((3, 3)).astype(np.float32))
-    return out
-
-
-class Out:
-    """device outputs of one call over n pictures with these contexts"""
-
-    def __init__(self, ctxs, n):
-        import torch
-        self.n, self.k = n, len(ctxs)
-        self.slot = max(c.info.data_bytes for c in ctxs)
-        self.chunks = torch.full((n * self.slot,), 0xA5, dtype=torch.uint8, device="cuda")
-        self.mask = torch.full((n,), -7, dtype=torch.int32, device="cuda")
-        self.status = torch.full((n,), 7, dtype=torch.int32, device="cuda")
-        self.mode = torch.full((n,), 9, dtype=torch.int32, device="cuda")
-        self.mode_masks = torch.full((n * self.k,), -7, dtype=torch.int32, device="cuda")
-
-    def call(self, cb, ctxs, ts, orders, of, states, cand, flags):
-        cb.detect_scan_extract_decode_chunks_receivers_dev(ctxs, ts, of, states, self.chunks.data_ptr(), self.mask.data_ptr(), self.status.data_ptr(),
-                                                           self.mode.data_ptr(), candidates=cand, d_mode_masks=self.mode_masks.data_ptr(),
-                                                           flags=flags, order=orders)
-
-    def host(self):
-        return (self.chunks.cpu().numpy().reshape(self.n, self.slot), self.mask.cpu().numpy().view(np.uint32), self.status.cpu().numpy(),
-                self.mode.cpu().numpy(), self.mode_masks.cpu().numpy().view(np.uint32).reshape(self.n, self.k))
-
-
-def run(cb, ctxs, ts, orders, of, states, cand, flags):
-    import torch
-    out = Out(ctxs, len(ts))
-    torch.cuda.synchronize()
-    out.call(cb, ctxs, ts, orders, of, states, cand, flags)
-    ctxs[0].sync()
-    return out.host()
 
 
 def per_mode(cb, refs, ts, orders, of, tables, cand, flags):
@@ -113,12 +63,6 @@ def check_selected(ctxs, got, want):
 def same_tables(a, b):
     import torch
     return all(torch.equal(x, y) for x, y in zip(a, b))
-
-
-def close(*lists):
-    for cs in lists:
-        for c in cs:
-            c.close()
 
 
 # ------------------------------------------------------------------------------------------------ exactness
@@ -191,7 +135,6 @@ def test_one_mode_is_the_receivers_call(cb, pool, mode, flags):
 def test_null_candidates_and_one_receiver_is_the_detect_call(cb, pool, flags):
     """every picture under every mode for one receiver whose entry state is each context's CCM: the detect call's outputs, and each
     table ends at its context's CCM"""
-    from test_gpu_detect import detect
     flags = sum(getattr(cb, "FLAG_" + f) for f in flags.split("|"))
     ts, orders = pool
     pics = exact_pictures(cb)                                   # the pool's pictures, packed RGB for the detect call

@@ -17,17 +17,10 @@ pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
-from test_gpu_detect import FLAGS, RECV, exact_pictures  # noqa: E402
-from test_gpu_detect_receivers import entry_states, run  # noqa: E402
-from test_gpu_detect_receivers_plan import close, contexts, launches, nonempty  # noqa: E402
-from test_gpu_receivers_pictures_plan import KINDS, as_tensor, bounds_of, resized  # noqa: E402
-from test_gpu_receivers_plan import graph_kernel_nodes  # noqa: E402
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
+from gpu_support import cb  # noqa: E402,F401  (fixtures)
+from gpu_support import (  # noqa: E402
+    FLAGS, KINDS, RECV, as_tensor, bounds_of, close, entry_states, exact_pictures, graph_kernel_nodes, launches, nonempty, resized,
+    run, stream_contexts)
 
 
 @pytest.fixture(scope="module")
@@ -108,8 +101,8 @@ def test_mixed_sizes_and_candidates_every_launch_equal_the_direct_call(cb, pool,
     assert lo >= 160                                                       # premise: room for a picture below the bounds
     small = resized(pool[0], lo - 60)
     rng = np.random.default_rng(len(modes) * 100 + flags)
-    ctxs, stream = contexts(cb, modes, n)
-    refs, _ = contexts(cb, modes, n)
+    ctxs, stream = stream_contexts(cb, modes, n)
+    refs, _ = stream_contexts(cb, modes, n)
     try:
         entries = entry_states(R, flags + K)
         states = [cb.receiver_states(entries) for _ in modes]
@@ -147,7 +140,7 @@ def test_all_refused_then_all_empty_with_stale_descriptors(cb, pool):
     modes = RECV
     n, K, R = 6, len(modes), 4
     flags = cb.FLAG_SHARPEN_IF_NEEDED | cb.FLAG_CC_FIT
-    ctxs, stream = contexts(cb, modes, n)
+    ctxs, stream = stream_contexts(cb, modes, n)
     try:
         entries = entry_states(R, 5)
         states = [cb.receiver_states(entries) for _ in modes]
@@ -182,8 +175,8 @@ def test_inside_an_outer_graph_with_captured_copies(cb, pool):
     modes = [68, 4]
     n, K, R = 6, 2, 4
     flags = cb.FLAG_SHARPEN_IF_NEEDED | cb.FLAG_CC_FIT
-    ctxs, stream = contexts(cb, modes, n)
-    refs, _ = contexts(cb, modes, n)
+    ctxs, stream = stream_contexts(cb, modes, n)
+    refs, _ = stream_contexts(cb, modes, n)
     try:
         entries = entry_states(R, 3)
         states = [cb.receiver_states(entries) for _ in modes]
@@ -223,7 +216,7 @@ def test_freezing_and_null_candidates(cb, pool):
     import torch
     modes = [68, 4]
     n, R = 4, 3
-    ctxs, stream = contexts(cb, modes, 2 * n)
+    ctxs, stream = stream_contexts(cb, modes, 2 * n)
     try:
         states = [cb.receiver_states(entry_states(R, 1)) for _ in modes]
         bounds = bounds_of(pool)

@@ -23,34 +23,15 @@ pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
-from test_gpu_detect import FLAGS, RECV, exact_pictures  # noqa: E402
-from test_gpu_detect_receivers import entry_states, run  # noqa: E402
-from test_gpu_receivers import layouts  # noqa: E402
-from test_gpu_receivers_plan import graph_kernel_nodes  # noqa: E402
-
-INT_MIN, INT_MAX = -2 ** 31, 2 ** 31 - 1
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
+from gpu_support import cb  # noqa: E402,F401  (fixtures)
+from gpu_support import (  # noqa: E402
+    FLAGS, RECV, close, entry_states, exact_pictures, graph_kernel_nodes, launches, layouts, nonempty, run, stream_contexts)
 
 
 @pytest.fixture(scope="module")
 def pics(cb):
     """the detect receivers tests' pool: mode-B / 4C photographs, rendered 66 and 67 frames, a noise picture"""
     return exact_pictures(cb)
-
-
-def contexts(cb, modes, n):
-    """candidate contexts on one new stream: (contexts, stream)"""
-    import torch
-    stream = torch.cuda.Stream()
-    ctxs = [cb.Context(m, max_frames=n) for m in modes]
-    for c in ctxs:
-        c.set_stream(stream.cuda_stream)
-    return ctxs, stream
 
 
 def variant(pics, k):
@@ -96,10 +77,6 @@ class Slots:
                 self.mode_masks.cpu().numpy().view(np.uint32))
 
 
-def nonempty(cand, of, K, R):
-    return np.flatnonzero((np.asarray(of, np.int64) >= 0) & (np.asarray(of, np.int64) < R) & (np.asarray(cand, np.uint32) & np.uint32((1 << K) - 1) != 0))
-
-
 def check_launch(cb, got, refs, slots, ts, orders, cand, of, R, ref_states, flags):
     """got (a launch's records) against the direct call on refs over the non-empty slots alone; ref_states advance in place"""
     K = len(refs)
@@ -116,31 +93,6 @@ def check_launch(cb, got, refs, slots, ts, orders, cand, of, R, ref_states, flag
     return idx
 
 
-def launches(n, K, R, rng, modes):
-    """five launches' (candidates, map): all-auto, all locked to one mode, mixed sessions, empty slots of both kinds, random"""
-    auto = (1 << K) - 1
-    lock = 1 << (modes.index(68) if 68 in modes else 0)
-    of = [rng.integers(0, R - 1, n) for _ in range(5)]          # receiver R - 1 never has a picture
-    sess_lock = rng.integers(0, K, R)
-    sess_auto = rng.random(R) < 0.3
-    mixed = np.where(sess_auto[of[2]], auto, 1 << sess_lock[of[2]])
-    holes = rng.integers(1, auto + 1, n)
-    holes[::4] = 0                                              # no candidate
-    holes[1::6] = 1 << (K + 1 + np.arange(len(holes[1::6])) % (31 - K))    # only bits at or above n_modes
-    of3 = of[3].copy()
-    of3[2::5] = np.array([-1, R, INT_MIN, INT_MAX, R + 7])[np.arange(len(of3[2::5])) % 5]
-    rand_of = rng.integers(-2, R + 2, n)
-    rand_of[rand_of == R - 1] = R                               # out of range instead: receiver R - 1 still has no picture
-    rand_cand = rng.integers(0, 1 << (K + 2), n)
-    return [(np.full(n, auto), of[0]), (np.full(n, lock), of[1]), (mixed, of[2]), (holes, of3), (rand_cand, rand_of)]
-
-
-def close(*lists):
-    for cs in lists:
-        for c in cs:
-            c.close()
-
-
 # ------------------------------------------------------------------------------------------------ exactness
 SETS = {"one-mode": [68], "one-geometry": [68, 4], "three-geometries": RECV}
 
@@ -153,8 +105,8 @@ def test_each_launch_equals_the_direct_call_on_its_nonempty_slots(cb, pics, mode
     flags = (getattr(cb, "FLAG_" + sflag) if sflag else 0) | (getattr(cb, "FLAG_" + ccflag) if ccflag else 0)
     n, K, R = len(pics), len(modes), 6
     rng = np.random.default_rng(len(modes) * 100 + flags)
-    ctxs, stream = contexts(cb, modes, n)
-    refs, _ = contexts(cb, modes, n)
+    ctxs, stream = stream_contexts(cb, modes, n)
+    refs, _ = stream_contexts(cb, modes, n)
     try:
         entries = entry_states(R, flags + K)
         states = [cb.receiver_states(entries) for _ in modes]
@@ -189,8 +141,8 @@ def test_null_candidates_and_untouched_receivers(cb, pics):
     import torch
     n, K, R = len(pics), len(RECV), 6
     flags = cb.FLAG_SHARPEN_IF_NEEDED | cb.FLAG_CC_FIT
-    ctxs, _ = contexts(cb, RECV, n)
-    refs, _ = contexts(cb, RECV, n)
+    ctxs, _ = stream_contexts(cb, RECV, n)
+    refs, _ = stream_contexts(cb, RECV, n)
     try:
         states = [cb.receiver_states(entry_states(R, 40 + k)) for k in range(K)]
         for s in states:
@@ -234,7 +186,7 @@ def test_a_locked_batch_walks_one_geometry(cb, pics):
     import torch
     n, K, R = len(pics), len(RECV), 4
     flags = cb.FLAG_SHARPEN_IF_NEEDED | cb.FLAG_CC_FIT
-    ctxs, _ = contexts(cb, RECV, n)
+    ctxs, _ = stream_contexts(cb, RECV, n)
     try:
         states = [cb.receiver_states(entry_states(R, 50)) for _ in RECV]
         slots = Slots(ctxs, pics)
@@ -264,7 +216,7 @@ def test_launch_count_is_the_graphs_kernels_for_every_map(cb, pics, flags):
     import torch
     n, K, R = len(pics), len(RECV), 5
     rng = np.random.default_rng(9)
-    ctxs, _ = contexts(cb, RECV, n)
+    ctxs, _ = stream_contexts(cb, RECV, n)
     try:
         states = [cb.receiver_states(entry_states(R, 60)) for _ in RECV]
         slots = Slots(ctxs, pics)
@@ -290,8 +242,8 @@ def test_inside_an_outer_graph_with_captured_copies(cb, pics):
     n, K, R = len(pics), len(RECV), 5
     flags = cb.FLAG_SHARPEN_IF_NEEDED | cb.FLAG_CC_FIT
     rng = np.random.default_rng(77)
-    ctxs, stream = contexts(cb, RECV, n)
-    refs, _ = contexts(cb, RECV, n)
+    ctxs, stream = stream_contexts(cb, RECV, n)
+    refs, _ = stream_contexts(cb, RECV, n)
     try:
         states = [cb.receiver_states(entry_states(R, 70)) for _ in RECV]
         ref_states = [s.clone() for s in states]
@@ -327,8 +279,8 @@ def test_two_plans_double_buffered_and_launch_only_enqueues(cb, pics):
     n, K, R = len(pics), len(RECV), 5
     flags = cb.FLAG_SHARPEN_IF_NEEDED | cb.FLAG_CC_FIT
     rng = np.random.default_rng(5)
-    ctxs, stream = contexts(cb, RECV, n)
-    refs, _ = contexts(cb, RECV, n)
+    ctxs, stream = stream_contexts(cb, RECV, n)
+    refs, _ = stream_contexts(cb, RECV, n)
     try:
         states = [cb.receiver_states(entry_states(R, 80)) for _ in RECV]
         ref_states = [s.clone() for s in states]
@@ -373,7 +325,7 @@ def test_live_plan_freezes_every_context_and_closing_one_destroys_it(cb, pics):
     import torch
     n, R = len(pics), 3
     small = pics[:4]
-    ctxs, _ = contexts(cb, RECV, n)
+    ctxs, _ = stream_contexts(cb, RECV, n)
     try:
         states = [cb.receiver_states(entry_states(R, 90)) for _ in RECV]
         # every context's own camera buffers at n pictures: only the detect call's buffers are still small

@@ -19,12 +19,12 @@ def _frame_with_header(ora, info, header, seed):
 
 def test_refused_flags_leave_the_staged_frames_in_place():
     import libcimbar_b200 as cb
-    from test_gpu_parity import ORA, _tint
+    from gpu_support import ORA, tint
     ctx = cb.Context(68, max_frames=2)
     header = [0x00, 0x01, 0x86, 0xA0, 0x00, 0x05]
     frame = _frame_with_header(ORA, ctx.info, header, seed=61)
-    a = np.stack([_tint(frame[None], (0.8, 0.6, 1.0))[0]] * 2)
-    b = np.stack([_tint(frame[None], (1.0, 0.7, 0.55))[0]] * 2)
+    a = np.stack([tint(frame[None], (0.8, 0.6, 1.0))[0]] * 2)
+    b = np.stack([tint(frame[None], (1.0, 0.7, 0.55))[0]] * 2)
     ctx.decode_fountain(a)
     launches = cb.launch_count()
     both = cb.FLAG_CC_SIMPLE | cb.FLAG_CC_FIT

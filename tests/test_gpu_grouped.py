@@ -13,6 +13,7 @@ import pytest
 from combine_fixtures import clean_picture, fitted_cells, picture_cells
 from group_fixtures import capture_of, frame_captures, rule_groups, seeded_frame
 from ragged_samples import sample
+from gpu_support import cb  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
@@ -20,12 +21,6 @@ MODES = [68, 67, 66, 4, 8]
 FLAGS = ["none", "SHARPEN_IF_NEEDED", "CC_SIMPLE", "CC_FIT"]
 PHOTOS = ["6bit/4_30_f0_627.jpg", "6bit/4_30_f0_177_ccm.jpg", "6bit/4_30_f1_360.jpg", "6bit/4_30_f2_246.jpg", "6bit/4_30_f2_734.jpg",
           "6bit/4_30_802.jpg"]
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def flag_bits(cb, name):

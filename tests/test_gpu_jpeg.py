@@ -8,14 +8,10 @@ import numpy as np
 import pytest
 
 from jpeg_matrix import cv2_rgb, golden_files, matrix, photo_files
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import packed, same_ccm
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def decode_dev(cb, ctx, files):
@@ -69,13 +65,6 @@ class Outputs:
                 self.flags.cpu().numpy())
 
 
-def packed(pics):
-    import torch
-    d = torch.cat([torch.from_numpy(np.ascontiguousarray(p).reshape(-1)) for p in pics]).cuda()
-    wh = np.array([(p.shape[1], p.shape[0]) for p in pics], np.int32).reshape(-1, 2)
-    return d, wh
-
-
 def batches_of(mode_val):
     """three batches of golden photographs of the mode (each photograph once, the B ones twice)"""
     files = [d for _, d in photo_files("6bit" if mode_val == 4 else "b")]
@@ -102,10 +91,6 @@ def reference(cb, mode_val, batches, flags, pics_of=None):
     ccm = ref.get_ccm()
     ref.close()
     return out, ccm
-
-
-def same_ccm(a, b):
-    return (a is None) == (b is None) and (a is None or np.array_equal(a, b))
 
 
 @pytest.mark.parametrize("mode_val", [4, 68])

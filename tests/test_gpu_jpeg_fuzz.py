@@ -8,8 +8,7 @@ import pytest
 
 from jpeg_fuzz import corpus, mutations, orphaned_ff, restart_class, walk
 from jpeg_matrix import cv2_rgb
-from test_jpeg_core_host import core  # noqa: F401  (the host build as a fixture)
-from test_jpeg_fuzz_host import decode_wide
+from cpu_support import core, decode_wide  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 

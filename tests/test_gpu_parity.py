@@ -7,45 +7,15 @@ import hashlib
 import numpy as np
 import pytest
 
-from oracle_lib import Oracle, load_sample, manifest, _ptr
+from oracle_lib import load_sample, manifest, _ptr
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import ORA, synth_frames, tint
 
 pytestmark = pytest.mark.gpu
-
-ORA = Oracle()
 
 
 def sha(a):
     return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
-
-
-def synth_frames(mode_val, n, seed, error_rate=0.0, noise_tiles=False):
-    """payload -> RS-encoded cells -> frames, optionally replacing a fraction of cells with a different valid tile
-    (keeps the drift-0 pass exact) or with random 8x8 noise (SURVEY 8d config 3)."""
-    m = ORA.mode(mode_val)
-    rng = np.random.default_rng(seed)
-    nbytes = (ORA.capacity(m) // m.ecc_block_size) * (m.ecc_block_size - m.ecc_bytes)
-    payloads = rng.integers(0, 256, (n, nbytes), dtype=np.uint8)
-    frames = np.zeros((n, m.image_size_y, m.image_size_x, 3), dtype=np.uint8)
-    for f in range(n):
-        cells = ORA.payload_to_cells(m, payloads[f])
-        k = int(round(error_rate * m.total_cells))
-        bad = rng.choice(m.total_cells, k, replace=False) if k else np.zeros(0, dtype=np.int64)
-        if k and not noise_tiles:
-            nvals = 1 << (m.symbol_bits + m.color_bits)
-            cells[bad] = (cells[bad] + rng.integers(1, nvals, k, dtype=np.uint8)) % nvals
-        frames[f] = ORA.render_frame(m, cells)
-        if k and noise_tiles:
-            xs, ys = np.zeros(m.total_cells, np.int32), np.zeros(m.total_cells, np.int32)
-            ORA.lib.cbo_cell_positions(C.byref(m), 0, _ptr(xs, C.c_int), _ptr(ys, C.c_int))
-            for i in bad:
-                frames[f, ys[i]:ys[i] + 8, xs[i]:xs[i] + 8] = rng.integers(0, 256, (8, 8, 3), dtype=np.uint8)
-    return m, payloads, frames
 
 
 # ------------------------------------------------------------------------------------------------ goldens
@@ -228,7 +198,7 @@ def test_noise_tiles_and_rs_failures_match_oracle(cb, mode_val, rate):
         good, ochunks, omask = ORA.decode_fountain(m, frames[f])
         assert mask[f] == omask and count[f] * m.chunk_size == good
         assert np.array_equal(chunks[f][:count[f]], ochunks[:count[f]])
-    tinted = _tint(frames, (0.75, 1.0, 0.85))
+    tinted = tint(frames, (0.75, 1.0, 0.85))
     raw1, ff1 = ctx.decode_raw(tinted, flags=cb.FLAG_CC_SIMPLE)
     assert all(int(x) & cb.FRAME_FALLBACK for x in ff1)
     try:
@@ -582,12 +552,6 @@ def test_fountain_file_round_trip_with_frame_loss(cb):
 
 
 # ------------------------------------------------------------------------------------------------ colour correction (CCM)
-def _tint(frames, gains):
-    """a coloured cast: per-channel gain, the kind of error a CCM exists to undo"""
-    out = frames.astype(np.float32) * np.asarray(gains, np.float32)
-    return np.clip(np.rint(out), 0, 255).astype(np.uint8)
-
-
 @pytest.mark.parametrize("idx", [0, 2])
 def test_ccm_reference_goldens_on_gpu(cb, idx):
     # CimbReaderTest.cpp:181-214 / :239-272: with the printed CCM active the first six reads give colours 0,1,1,2,2,2;
@@ -620,7 +584,7 @@ def test_ccm_reference_goldens_on_gpu(cb, idx):
 def test_ccm_on_clean_frames_goes_through_k1(cb, mode_val):
     # tinted synthetic frames stay on the drift-0 kernel (K1's CCM variant); the matrix is an arbitrary strong one
     m, payloads, frames = synth_frames(mode_val, 3, seed=41)
-    frames = _tint(frames, (0.62, 0.95, 0.8))
+    frames = tint(frames, (0.62, 0.95, 0.8))
     mat = np.array([[1.61, 0.02, -0.11], [-0.07, 1.05, 0.03], [-0.2, -0.15, 1.45]], np.float32)
     ctx = cb.Context(mode_val, max_frames=3)
     ctx.set_ccm(mat)
@@ -644,8 +608,8 @@ def test_ccm_on_clean_frames_goes_through_k1(cb, mode_val):
 def test_simple_color_correction_matches_oracle(cb):
     # color_correction == 1 (simpleColorCorrection, CimbReader.cpp:55-93): per-frame von Kries matrix from the anchors
     m, payloads, frames = synth_frames(68, 4, seed=43)
-    frames[1] = _tint(frames[1:2], (0.7, 1.0, 0.9))[0]
-    frames[2] = _tint(frames[2:3], (1.0, 0.55, 0.8))[0]
+    frames[1] = tint(frames[1:2], (0.7, 1.0, 0.9))[0]
+    frames[2] = tint(frames[2:3], (1.0, 0.55, 0.8))[0]
     frames[3] = load_sample("b/ex380.jpg")                      # camera frame: exact walk + CCM
     ctx = cb.Context(68, max_frames=4)
     raw, ff = ctx.decode_raw(frames, flags=cb.FLAG_CC_SIMPLE)
@@ -687,7 +651,7 @@ def test_color_correction_2_fit_matches_oracle(cb):
     # first symbol chunks are destroyed (header comes from a later chunk), and a frame with no decodable chunk at all
     # (keeps the previous frame's CCM)
     m, payloads, synth = synth_frames(68, 3, seed=47)
-    synth[0] = _tint(synth[0:1], (0.8, 0.6, 1.0))[0]
+    synth[0] = tint(synth[0:1], (0.8, 0.6, 1.0))[0]
     rng = np.random.default_rng(9)
     xs, ys = np.zeros(m.total_cells, np.int32), np.zeros(m.total_cells, np.int32)
     ORA.lib.cbo_cell_positions(C.byref(m), 0, _ptr(xs, C.c_int), _ptr(ys, C.c_int))
@@ -725,7 +689,7 @@ def test_color_correction_2_fit_matches_oracle(cb):
 @pytest.mark.parametrize("mode_val", [8, 67])
 def test_color_correction_2_other_modes(cb, mode_val):
     m, payloads, frames = synth_frames(mode_val, 3, seed=53)
-    frames[1] = _tint(frames[1:2], (0.9, 0.7, 0.75))[0]
+    frames[1] = tint(frames[1:2], (0.9, 0.7, 0.75))[0]
     want = _oracle_fountain_batch(m, frames, 2)
     ctx = cb.Context(mode_val, max_frames=3)
     chunks, counts, masks, ff = ctx.decode_fountain(frames, flags=cb.FLAG_CC_FIT)

@@ -14,15 +14,11 @@ import pytest
 import png_matrix as pm
 from jpeg_matrix import photo_files
 from oracle_lib import manifest
-from test_abi_png_args import ACCEPTED, CORRUPT
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import packed, same_ccm
+from png_corpus import ACCEPTED, CORRUPT
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def decode_dev(cb, ctx, files):
@@ -102,13 +98,6 @@ class Outputs:
                 self.flags.cpu().numpy())
 
 
-def packed(pics):
-    import torch
-    d = torch.cat([torch.from_numpy(np.ascontiguousarray(p).reshape(-1)) for p in pics]).cuda()
-    wh = np.array([(p.shape[1], p.shape[0]) for p in pics], np.int32).reshape(-1, 2)
-    return d, wh
-
-
 def as_png(jpeg_bytes):
     ok, buf = cv2.imencode(".png", cv2.imdecode(np.frombuffer(jpeg_bytes, np.uint8), cv2.IMREAD_COLOR))
     assert ok
@@ -140,10 +129,6 @@ def reference(cb, mode_val, batches, flags):
     ccm = ref.get_ccm()
     ref.close()
     return out, ccm
-
-
-def same_ccm(a, b):
-    return (a is None) == (b is None) and (a is None or np.array_equal(a, b))
 
 
 @pytest.mark.parametrize("mode_val", [4, 68])

@@ -16,11 +16,8 @@ pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
-from test_gpu_receivers import cb, entries, frames  # noqa: E402,F401  (fixtures)
-from test_gpu_receivers_pictures_plan import bounds_of, direct, fresh, pool  # noqa: E402
-from test_gpu_receivers_plan import graph_kernel_nodes  # noqa: E402
-from test_gpu_detect import RECV, contexts, exact_pictures, rendered  # noqa: E402
-from test_gpu_detect_receivers import Out  # noqa: E402
+from gpu_support import cb, entries, frames  # noqa: E402,F401  (fixtures)
+from gpu_support import Out, RECV, bounds_of, contexts, direct, exact_pictures, fresh, graph_kernel_nodes, pool, rendered  # noqa: E402
 
 MODES = [68, 67, 66, 4]
 

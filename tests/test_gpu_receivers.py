@@ -16,43 +16,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
 import chain_batches as CB  # noqa: E402
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
-
-
-def same_ccm(a, b):
-    return (a is None) == (b is None) and (a is None or np.array_equal(a, b))
-
-
-@pytest.fixture(scope="module")
-def frames():
-    """the crafted frames under the frame cast (0, 1, 3, 4 fit their own matrix; 2 has no header), then the same five with the
-    encoder's anchors pasted in and dimmed to 80 % (5 .. 9): the crafted frames have no anchor white, these have one, so CC_SIMPLE
-    gives the two halves different matrices"""
-    fr = np.stack(CB.crafted(CB.CAST_FRAMES))
-    lit = np.stack([CB.with_anchors(f) for f in fr])
-    return np.concatenate([fr, np.rint(lit * np.float32(0.8)).astype(np.uint8)])
-
-
-@pytest.fixture(scope="module")
-def entries(cb, frames):
-    """entry states: inactive, fitted from another frame (crafted frames 0 and 4), the identity"""
-    import torch
-    ctx = cb.Context(68, max_frames=1)
-    out = torch.zeros((1, ctx.info.data_bytes), dtype=torch.uint8, device="cuda")
-    mask = torch.zeros(1, dtype=torch.int32, device="cuda")
-    fits = []
-    for i in (0, 4):
-        ctx.set_ccm(None)
-        d = torch.from_numpy(frames[i:i + 1]).cuda()
-        ctx.decode_chunks_dev(d.data_ptr(), 1, out.data_ptr(), mask.data_ptr(), flags=cb.FLAG_CC_FIT)
-        fits.append(ctx.get_ccm())
-    assert fits[0] is not None and fits[1] is not None and not np.array_equal(fits[0], fits[1])
-    return [None, fits[0], np.eye(3, dtype=np.float32), fits[1]]
+from gpu_support import cb, entries, frames  # noqa: F401  (fixtures)
+from gpu_support import camera_call, layouts, same_ccm
 
 
 # ------------------------------------------------------------------------------------------------------------------- frames
@@ -186,49 +151,6 @@ def test_scale_more_frames_than_four_waves(cb, frames, entries):
 
 
 # ------------------------------------------------------------------------------------------------------------------- camera
-def layouts(pics):
-    """the pictures as CUDA tensors in mixed layouts and pitches: RGB, BGR, planar, padded RGB, RGBA, in turn"""
-    import torch
-    ts, orders = [], []
-    for i, p in enumerate(pics):
-        t = torch.from_numpy(np.ascontiguousarray(p)).cuda()
-        k = i % 5
-        if k == 1:
-            t, o = t.flip(2).contiguous(), "bgr"
-        elif k == 2:
-            t, o = t.permute(2, 0, 1).contiguous(), "rgb"
-        elif k == 3:
-            h, w, _ = t.shape
-            big = torch.zeros((h, w + 13, 3), dtype=torch.uint8, device="cuda")
-            big[:, :w] = t
-            t, o = big[:, :w], "rgb"
-        elif k == 4:
-            t, o = torch.cat([t, torch.full_like(t[:, :, :1], 77)], 2).contiguous(), "rgba"
-        else:
-            o = "rgb"
-        ts.append(t)
-        orders.append(o)
-    return ts, orders
-
-
-def camera_call(cb, ctx, ts, orders, flags, receiver_of=None, states=None):
-    import torch
-    n = len(ts)
-    chunks = torch.full((n, ctx.info.data_bytes), 0xA5, dtype=torch.uint8, device="cuda")
-    mask = torch.full((n,), -1, dtype=torch.int32, device="cuda")
-    status = torch.full((n,), 7, dtype=torch.int32, device="cuda")
-    ff = torch.full((n,), 0xEE, dtype=torch.uint8, device="cuda")
-    torch.cuda.synchronize()
-    if receiver_of is None:
-        ctx.scan_extract_decode_chunks_pictures_dev(ts, chunks.data_ptr(), mask.data_ptr(), status.data_ptr(), ff.data_ptr(), flags=flags,
-                                                    order=orders)
-    else:
-        ctx.scan_extract_decode_chunks_receivers_dev(ts, receiver_of, states, chunks.data_ptr(), mask.data_ptr(), status.data_ptr(),
-                                                     ff.data_ptr(), flags=flags, order=orders)
-    ctx.sync()
-    return chunks.cpu().numpy(), mask.cpu().numpy(), status.cpu().numpy(), ff.cpu().numpy(), ctx.camera_transforms(n)
-
-
 def check_camera(cb, mode, pics, of, entries, flags):
     of = np.asarray(of, np.int32)
     ts, orders = layouts(pics)

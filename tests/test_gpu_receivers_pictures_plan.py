@@ -17,57 +17,15 @@ pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
-import chain_batches as CB  # noqa: E402
-from test_gpu_receivers import cb, entries, frames, same_ccm  # noqa: E402,F401  (fixtures and helpers)
-from test_gpu_receivers_plan import graph_kernel_nodes  # noqa: E402
+from gpu_support import cb, entries, frames  # noqa: E402,F401  (fixtures)
+from gpu_support import KINDS, as_tensor, bounds_of, direct, fresh, graph_kernel_nodes, pool, resized  # noqa: E402
 
 FLAGS = {"0": 0, "cc_simple": 4, "cc_fit": 8, "sharpen_if_needed|cc_fit": 0x20 | 8}
-KINDS = ["rgb", "bgr", "planar", "pitched", "rgba", "bgra"]
-
-
-def resized(p, short):
-    import cv2
-    f = short / min(p.shape[:2])
-    return cv2.resize(p, (round(p.shape[1] * f), round(p.shape[0] * f)), interpolation=cv2.INTER_LINEAR if f > 1 else cv2.INTER_AREA)
-
-
-def pool(mode):
-    """the golden photographs and pictures of the mode at native size (landscape and portrait), upscales to 5 and 9 taps, downscales"""
-    base = CB.camera_pictures() if mode == 68 else CB.legacy_pictures()
-    photo = base[0]
-    s = min(photo.shape[:2])
-    up5 = resized(photo, 1.7 * s if 1500 <= 1.7 * s < 2500 else 1800)
-    return base + [np.ascontiguousarray(np.transpose(photo, (1, 0, 2))), up5, resized(photo, 2600), resized(base[-1], 0.6 * min(base[-1].shape[:2]))]
 
 
 def radius(w, h):
     s = min(w, h)
     return 1 if s < 1500 else (2 if s < 2500 else 4)
-
-
-def as_tensor(p, kind):
-    """picture p as a fresh CUDA tensor (its own allocation) in one of the layouts, and its order"""
-    import torch
-    t = torch.from_numpy(np.ascontiguousarray(p)).cuda()
-    if kind == "bgr":
-        return t.flip(2).contiguous(), "bgr"
-    if kind == "planar":
-        return t.permute(2, 0, 1).contiguous(), "rgb"
-    if kind == "pitched":
-        h, w, _ = t.shape
-        big = torch.zeros((h, w + 13, 3), dtype=torch.uint8, device="cuda")
-        big[:, :w] = t
-        return big[:, :w], "rgb"
-    if kind == "rgba":
-        return torch.cat([t, torch.full_like(t[:, :, :1], 77)], 2).contiguous(), "rgba"
-    if kind == "bgra":
-        return torch.cat([t.flip(2), torch.full_like(t[:, :, :1], 99)], 2).contiguous(), "bgra"
-    return t, "rgb"
-
-
-def bounds_of(pics):
-    s = [min(p.shape[:2]) for p in pics]
-    return (min(s), max(s), max(max(p.shape[:2]) for p in pics))
 
 
 class Plan:
@@ -107,22 +65,6 @@ class Plan:
         return [t.cpu().numpy() for t in (self.chunks, self.mask, self.status, self.flags)]
 
 
-def direct(cb, ref, ts, orders, of, states, flags):
-    import torch
-    n = len(ts)
-    if n == 0:
-        return None
-    chunks = torch.full((n, ref.info.data_bytes), 0xA5, dtype=torch.uint8, device="cuda")
-    mask = torch.full((n,), -1, dtype=torch.int32, device="cuda")
-    status = torch.full((n,), 7, dtype=torch.int32, device="cuda")
-    ff = torch.full((n,), 0xEE, dtype=torch.uint8, device="cuda")
-    torch.cuda.synchronize()
-    ref.scan_extract_decode_chunks_receivers_dev(ts, np.asarray(of, np.int32), states, chunks.data_ptr(), mask.data_ptr(), status.data_ptr(),
-                                                 ff.data_ptr(), flags=flags, order=orders)
-    ref.sync()
-    return [t.cpu().numpy() for t in (chunks, mask, status, ff)], ref.camera_transforms(n), ref.frame_ccms(n)
-
-
 def launch_and_check(cb, slots, ts, orders, of, n_receivers, refused, states, ref, ref_states, flags, launch=None):
     """one launch (of the descriptors and map already written) against the direct call on its accepted non-empty slots.  launch:
     a replay of an outer graph instead, which leaves the context's host state -- the transforms' picture count -- alone"""
@@ -147,12 +89,6 @@ def launch_and_check(cb, slots, ts, orders, of, n_receivers, refused, states, re
     assert (got[1][refused] == 0).all() and (got[2][refused] == cb.EXTRACT_REFUSED).all()
     assert torch.equal(states, ref_states)
     return got
-
-
-def fresh(pics, rng):
-    """every picture in a random layout, each in a new allocation"""
-    out = [as_tensor(p, KINDS[int(rng.integers(len(KINDS)))]) for p in pics]
-    return [t for t, _ in out], [o for _, o in out]
 
 
 @pytest.mark.parametrize("flag", list(FLAGS))

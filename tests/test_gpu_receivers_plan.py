@@ -3,7 +3,6 @@ device memory and grouped on the device at every launch.  The expected result of
 (cb200_scan_extract_decode_chunks_receivers_dev) on a second context with its own state table, on the launch's non-empty slots
 alone, in batch order: records, masks, frame flags, statuses, transforms, frame CCMs and states, bit for bit.  Empty slots (a
 receiver outside [0, n_receivers)) give mask 0 and status EXTRACT_EMPTY and touch no state."""
-import ctypes as C
 import os
 import sys
 import time
@@ -17,7 +16,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
 import chain_batches as CB  # noqa: E402
-from test_gpu_receivers import cb, entries, frames, layouts, same_ccm  # noqa: E402,F401  (fixtures and helpers)
+from gpu_support import cb, entries, frames  # noqa: E402,F401  (fixtures)
+from gpu_support import direct, graph_kernel_nodes, layouts, same_ccm  # noqa: E402
 
 INT_MIN, INT_MAX = -2 ** 31, 2 ** 31 - 1
 EXTRA_KERNELS = 1                      # k_receivers_order: every other kernel of the graph is the direct receivers call's
@@ -54,23 +54,6 @@ class Slots:
 
     def records(self):
         return [t.cpu().numpy() for t in (self.chunks, self.mask, self.status, self.flags)]
-
-
-def direct(cb, ref, ts, orders, of, states, flags):
-    """the direct receivers call on ref: records, transforms, frame CCMs (nothing for an empty batch)"""
-    import torch
-    n = len(ts)
-    if n == 0:
-        return None
-    chunks = torch.full((n, ref.info.data_bytes), 0xA5, dtype=torch.uint8, device="cuda")
-    mask = torch.full((n,), -1, dtype=torch.int32, device="cuda")
-    status = torch.full((n,), 7, dtype=torch.int32, device="cuda")
-    ff = torch.full((n,), 0xEE, dtype=torch.uint8, device="cuda")
-    torch.cuda.synchronize()
-    ref.scan_extract_decode_chunks_receivers_dev(ts, np.asarray(of, np.int32), states, chunks.data_ptr(), mask.data_ptr(), status.data_ptr(),
-                                                 ff.data_ptr(), flags=flags, order=orders)
-    ref.sync()
-    return [t.cpu().numpy() for t in (chunks, mask, status, ff)], ref.camera_transforms(n), ref.frame_ccms(n)
 
 
 def launch_and_check(cb, ctx, plan, slots, of, n_receivers, states, ref, ref_states, flags):
@@ -200,20 +183,6 @@ def test_more_than_1024_slots(cb, entries):
     plan.close()
     ctx.close()
     ref.close()
-
-
-def graph_kernel_nodes(graph):
-    cuda = C.CDLL("libcuda.so.1")
-    count = C.c_size_t(0)
-    assert cuda.cuGraphGetNodes(C.c_void_p(graph), None, C.byref(count)) == 0
-    nodes = (C.c_void_p * count.value)()
-    assert cuda.cuGraphGetNodes(C.c_void_p(graph), nodes, C.byref(count)) == 0
-    kinds = []
-    for nd in nodes:
-        t = C.c_int(-1)
-        assert cuda.cuGraphNodeGetType(C.c_void_p(nd), C.byref(t)) == 0
-        kinds.append(t.value)
-    return kinds.count(0)                                                  # CU_GRAPH_NODE_TYPE_KERNEL
 
 
 @pytest.mark.parametrize("flag", list(FLAGS))

@@ -7,17 +7,12 @@ import pytest
 
 import oracle_lib as ol
 from scan_oracle_lib import ScanOracle, join
-from test_scan_core_host import pictures
+from gpu_support import cb  # noqa: F401  (fixtures)
+from cpu_support import pictures
 
 pytestmark = pytest.mark.gpu
 
 SO = ScanOracle()
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def _check(ctx, pics):

@@ -9,17 +9,12 @@ import pytest
 
 from ragged_samples import BIG, GLOB, sample
 from scan_oracle_lib import ScanOracle, join
-from test_gpu_sharpen_select import ORA, _cli_loop, check_dense
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import ORA, check_dense, pad, sharpen_cli_loop
 
 pytestmark = pytest.mark.gpu
 
 SO = ScanOracle()
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 def radius(w, h):
@@ -39,10 +34,6 @@ def word_path(pics):
         out.append((w % 4 == 0, off % 4 == 0))
         off += w * h
     return out
-
-
-def pad(rgb, top, bottom, left, right):
-    return cv2.copyMakeBorder(rgb, top, bottom, left, right, cv2.BORDER_CONSTANT, value=(0, 0, 0))
 
 
 # ------------------------------------------------------------------------------------------------ scan
@@ -141,7 +132,7 @@ def cli_loop(m, pics, cc, monkeypatch):
                 seen["ccm"] = ORA.get_ccm()
         set_ccm(m9)
     monkeypatch.setattr(ORA, "set_ccm", spy)
-    out = _cli_loop(m, pics, cc)
+    out = sharpen_cli_loop(m, pics, cc)
     monkeypatch.setattr(ORA, "set_ccm", set_ccm)
     assert seen["calls"] == 2
     return out, seen["ccm"]

@@ -7,48 +7,12 @@ import numpy as np
 import pytest
 
 from oracle_lib import load_sample
-from scan_oracle_lib import ScanOracle
-from test_gpu_parity import ORA, synth_frames
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import ORA, POOL, check_dense, dense, frame_pool, oracle, sharpen_cli_loop
 
 pytestmark = pytest.mark.gpu
 
 MODES = [68, 4, 8, 67, 66]
-POOL = 12                  # per mode: 4 clean frames, 4 with 1 % noise tiles (exact walk), 4 blurred (sigma 1.6) + noise
-_pools, _oracle = {}, {}
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
-
-
-def pool(mode_val):
-    if mode_val not in _pools:
-        m, _, clean = synth_frames(mode_val, 4, seed=700 + mode_val)
-        noisy = synth_frames(mode_val, 4, seed=710 + mode_val, error_rate=0.01, noise_tiles=True)[2]
-        base = synth_frames(mode_val, 4, seed=720 + mode_val)[2]
-        rng = np.random.default_rng(730 + mode_val)
-        blurred = []
-        for b in base:
-            b = cv2.GaussianBlur(b, (0, 0), 1.6).astype(np.int16) + np.rint(rng.normal(0, 6, b.shape)).astype(np.int16)
-            blurred.append(np.clip(b, 0, 255).astype(np.uint8))
-        _pools[mode_val] = (m, np.concatenate([clean, noisy, np.stack(blurred)]))
-    return _pools[mode_val]
-
-
-def oracle(mode_val, p, sharpen, cc):
-    """Decoder::decode_fountain of pool frame p by a fresh reference decoder: (good bytes, dense chunks, chunk mask)"""
-    key = (mode_val, p, bool(sharpen), cc)
-    if key not in _oracle:
-        m, frames = pool(mode_val)
-        ORA.set_ccm(None)
-        try:
-            good, chunks, mask = ORA.decode_fountain(m, frames[p], sharpen=bool(sharpen), color_correction=cc)
-        finally:
-            ORA.set_ccm(None)
-        _oracle[key] = (good, chunks.copy(), mask)
-    return _oracle[key]
 
 
 def selection(mode_val, n, seed):
@@ -64,19 +28,6 @@ def differs(mode_val, p, cc=0):
     return a[2] != b[2] or not np.array_equal(a[1], b[1])
 
 
-def check_dense(m, chunks, count, mask, want, what):
-    good, wchunks, wmask = want
-    assert mask == wmask and count * m.chunk_size == good, what
-    assert np.array_equal(chunks[:count], wchunks[:count]), what
-
-
-def dense(m, slots, mask):
-    """the fixed-slot records of cb200_decode_chunks_dev as escrow_buffer_writer's dense order"""
-    rows = slots.reshape(m.chunks_per_frame, m.chunk_size)
-    keep = [q for q in range(m.chunks_per_frame) if mask >> q & 1]
-    return len(keep), rows[keep]
-
-
 def premise(mode_val, idx, sel):
     # some frames of each kind decode differently under the other choice
     assert any(differs(mode_val, int(p)) for p, s in zip(idx, sel) if s)
@@ -88,7 +39,7 @@ def premise(mode_val, idx, sel):
 def test_mixed_selection_matches_oracle_every_mode(cb, mode_val):
     """a 40-frame batch (both kinds in K1's band schedule) with an irregular selection, colour correction 0 and 1 and, where the
     reference fits a CCM, 2 against the oracle decoding the batch in order with one decoder state"""
-    m, frames = pool(mode_val)
+    m, frames = frame_pool(mode_val)
     n = 40
     idx, sel = selection(mode_val, n, 11)
     batch = frames[idx]
@@ -123,7 +74,7 @@ def test_mixed_selection_matches_oracle_every_mode(cb, mode_val):
 
 def _device_batch(mode_val, idx):
     import torch
-    m, frames = pool(mode_val)
+    m, frames = frame_pool(mode_val)
     dev = torch.device("cuda")
     return m, torch.from_numpy(frames).to(dev)[torch.from_numpy(idx).to(dev)].contiguous()
 
@@ -197,38 +148,13 @@ def _camera_batch():
     return np.stack([pics[0], pics[1], noise, pics[3], pics[2]])
 
 
-def _cli_loop(m, pics, cc):
-    """the reference CLI's decode loop with --preprocess -1: scan, Corners, warp, decode with sharpen iff NEEDS_SHARPEN, one
-    decoder state in picture order; FAILURE pictures are skipped"""
-    so = ScanOracle()
-    an, W, H = 30, m.image_size_x, m.image_size_y
-    dst = np.array([[an, an], [W - an, an], [an, H - an], [W - an, H - an]], np.float32)
-    out = []
-    ORA.set_ccm(None)
-    try:
-        for rgb in pics:
-            anchors, _ = so.scan(rgb)
-            if anchors is None or len(anchors) < 4:
-                out.append((0, None, None))
-                continue
-            xy = so.corners(anchors)
-            status = 1 if so.is_granular_scale(xy, W, H) else 2
-            frame = cv2.warpPerspective(rgb, cv2.getPerspectiveTransform(np.array(xy, np.float32).reshape(4, 2), dst), (W, H),
-                                        flags=cv2.INTER_LINEAR)
-            good, chunks, mask = ORA.decode_fountain(m, frame, sharpen=status == 2, color_correction=cc)
-            out.append((status, xy, (good, chunks.copy(), mask)))
-    finally:
-        ORA.set_ccm(None)
-    return out
-
-
 def test_camera_batch_matches_the_cli_loop(cb):
     import torch
     pics = _camera_batch()
     n = len(pics)
     m = ORA.mode(4)
     for cc, ccf in ((0, 0), (2, cb.FLAG_CC_FIT)):
-        want = _cli_loop(m, pics, cc)
+        want = sharpen_cli_loop(m, pics, cc)
         assert sorted({w[0] for w in want}) == [0, 1, 2]
         assert any(w[0] == 2 and w[2][0] > 0 for w in want)
         ctx = cb.Context(4, max_frames=n)
@@ -270,7 +196,7 @@ def test_cpp_decoder_per_frame_overload(cb, tmp_path):
     libdir = os.path.join(root, "libcimbar_b200", "lib")
     subprocess.check_call(["g++", "-std=c++17", "-O1", "-o", exe, os.path.join(root, "tests", "cpp", "decoder_sharpen_test.cpp"),
                            "-L" + libdir, "-lcb200", "-Wl,-rpath," + libdir])
-    m, frames = pool(68)
+    m, frames = frame_pool(68)
     batch = np.stack([load_sample("b/tr_0.png"), load_sample("b/ex2434.jpg"), frames[8], load_sample("b/ex380.jpg"),
                       load_sample("b/tr_1.png"), frames[4], frames[9]])
     pattern = "0110101"

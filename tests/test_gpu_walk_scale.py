@@ -13,7 +13,8 @@ import numpy as np
 import pytest
 
 from oracle_lib import load_sample
-from test_gpu_parity import ORA, synth_frames
+from gpu_support import cb  # noqa: F401  (fixtures)
+from gpu_support import ORA, synth_frames
 
 pytestmark = pytest.mark.gpu
 
@@ -21,12 +22,6 @@ HEAP_SMEM = 1023                # heap entries a walk keeps in shared memory whe
 HEAP_SMEM_FEW = 8191            # ... and when it is not
 POOL_FLAGGED = 26               # the pool: 2 photographs + 12 frames with 1 % and 12 with 8 % noise tiles ...
 POOL_CLEAN = 3                  # ... + 3 clean frames = 29, a prime, so that neighbours in a batch never repeat with a short period
-
-
-@pytest.fixture(scope="module")
-def cb():
-    import libcimbar_b200 as cb
-    return cb
 
 
 @pytest.fixture(scope="module")

@@ -4,21 +4,19 @@ numpy restatement of include/cb200.h in tests/group_fixtures.py; then the rule o
 of synthetic captures of distinct frames, which must group by frame."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from group_fixtures import assign
+from host_harness import build_harness
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("group_core") / "group_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(ROOT, "tests", "cpp", "group_core_host.cpp")])
-    L = C.CDLL(so)
+    L = build_harness(tmp_path_factory, "group_core_host")
     L.gc_agree.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     L.gc_agree_packed.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     L.gc_match.argtypes = [C.c_int, C.c_int]

@@ -1,10 +1,6 @@
 """The device JPEG decoder's functions (libcimbar_b200/csrc/jpeg_core.cuh: parse, segment decoder, ISLOW IDCT, fancy upsampling,
 YCbCr -> RGB, EXIF orientation -- what jpeg.cu's kernels run) compiled for the host and pinned against cv2: every golden JPEG and
 every file of the generated matrix decodes to exactly cv2.imread + cvtColor(BGR2RGB), and cb200_jpeg_info gives cv2's size."""
-import ctypes as C
-import os
-import subprocess
-
 import cv2
 import numpy as np
 import pytest
@@ -12,28 +8,9 @@ import pytest
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
 from jpeg_matrix import cv2_rgb, golden_files, matrix
+from cpu_support import core, decode  # noqa: F401
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FILES = golden_files() + matrix()
-
-
-@pytest.fixture(scope="module")
-def core(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("jpeg_core") / "jpeg_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(ROOT, "tests", "cpp", "jpeg_core_host.cpp")])
-    lib = C.CDLL(so)
-    lib.jc_decode.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_int]
-    lib.jc_info.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_int]
-    return lib
-
-
-def decode(core, data, like=None):
-    want = cv2_rgb(data if like is None else like)
-    out = np.zeros(want.size + 16, np.uint8)
-    wh = np.zeros(2, np.int32)
-    why = C.create_string_buffer(256)
-    rc = core.jc_decode(data, len(data), out.ctypes.data, out.size, wh.ctypes.data, why, 256)
-    return rc, why.value.decode(), wh, out, want
 
 
 def test_premise_the_matrix_covers_the_layouts():

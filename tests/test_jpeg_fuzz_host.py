@@ -5,7 +5,6 @@ chooses; and damaged files, decoded under AddressSanitizer and UndefinedBehavior
 exactly what cv2 gives for the same bytes -- except for pictures with blocks whose IDCT leaves the range where libjpeg-turbo's C and
 SIMD IDCTs agree (jpeg_core.cuh idct_islow), where cv2's bytes depend on how it was built."""
 import collections
-import ctypes as C
 import os
 import struct
 import subprocess
@@ -18,7 +17,7 @@ import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
 from jpeg_fuzz import RESTARTS, corpus, mutations, orphaned_ff, restart_class, walk
 from jpeg_matrix import SAMPLING, cv2_rgb
-from test_jpeg_core_host import core, decode  # noqa: F401  (the host build as a fixture)
+from cpu_support import core, decode, decode_wide  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FILES = corpus()
@@ -123,18 +122,6 @@ def test_damaged_files_are_reported_or_decode_like_cv2(tmp_path):
     # premise: every kind of damage is there, and both verdicts, with pictures that differ from the undamaged file's
     assert {k for k, _ in seen} == {"flip", "truncate", "unstuff", "swap"} and {rc for _, rc in seen} == {0, -2}, seen
     assert changed >= 10, changed
-
-
-def decode_wide(core, data):  # noqa: F811  (the fixture's library)
-    """(rc, wide, rgb or None) of the host build's jc_decode_wide"""
-    core.jc_decode_wide.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_int, C.c_void_p]
-    wh = np.zeros(2, np.int32)
-    why = C.create_string_buffer(256)
-    assert core.jc_info(data, len(data), wh.ctypes.data, why, 256) == 0, why.value
-    out = np.zeros(3 * int(wh[0]) * int(wh[1]), np.uint8)
-    wide = np.zeros(1, np.int32)
-    rc = core.jc_decode_wide(data, len(data), out.ctypes.data, out.size, wh.ctypes.data, why, 256, wide.ctypes.data)
-    return rc, int(wide[0]), out.reshape(wh[1], wh[0], 3) if rc == 0 else None
 
 
 def test_every_byte_after_an_orphaned_ff_is_corrupt_data(core):  # noqa: F811

@@ -10,30 +10,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
-
-U = np.uint32
-NT = 128
-
-
-def prmt(a, b, sel):
-    """__byte_perm(a, b, sel) on arrays of uint32."""
-    a = a.astype(np.uint64); b = b.astype(np.uint64)
-    src = a | (b << np.uint64(32))
-    out = np.zeros_like(a)
-    for i in range(4):
-        n = (sel >> (4 * i)) & 0x7
-        out |= ((src >> np.uint64(8 * n)) & np.uint64(0xFF)) << np.uint64(8 * i)
-    return out.astype(U)
-
-
-def vmaxu2(a, b):
-    lo = np.maximum(a & U(0xFFFF), b & U(0xFFFF)); hi = np.maximum(a >> U(16), b >> U(16))
-    return (lo | (hi << U(16))).astype(U)
-
-
-def vminu2(a, b):
-    lo = np.minimum(a & U(0xFFFF), b & U(0xFFFF)); hi = np.minimum(a >> U(16), b >> U(16))
-    return (lo | (hi << U(16))).astype(U)
+from cpu_support import NT, U, prmt, vmaxu2, vminu2
 
 
 def umulhi(a, b):

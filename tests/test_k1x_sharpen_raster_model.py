@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
-from test_k1_sharpen_model import prmt, vmaxu2, vminu2, U, NT
+from cpu_support import NT, U, prmt, vmaxu2, vminu2
 
 BAND = 64
 

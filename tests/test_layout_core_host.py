@@ -3,24 +3,20 @@ numpy and cv2: the gray k_scan_blur4 takes (byte fetch and word path) is cvtColo
 pairs k_deskew reads are that copy's pixels, in every layout, at odd widths, unaligned bases and padded pitches.  The GPU test
 (tests/test_gpu_camera_layouts.py) compares the whole camera call."""
 import ctypes as C
-import os
-import subprocess
 
 import cv2
 import numpy as np
 import pytest
 
 import libcimbar_b200 as cb
+from host_harness import build_harness
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LAYOUTS = {"rgb": cb.LAYOUT_RGB, "bgr": cb.LAYOUT_BGR, "rgba": cb.LAYOUT_RGBA, "bgra": cb.LAYOUT_BGRA, "planar": cb.LAYOUT_RGB_PLANAR}
 
 
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("layout_core") / "layout_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(ROOT, "tests", "cpp", "layout_core_host.cpp")])
-    lib = C.CDLL(so)
+    lib = build_harness(tmp_path_factory, "layout_core_host")
     lib.lc_gray.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p]
     lib.lc_taps.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
     lib.lc_picture_abi.argtypes = [C.c_void_p]

@@ -2,8 +2,6 @@
 what png.cu's kernels run) compiled for the host and pinned against cv2: every golden PNG and every file of the generated matrix
 decodes to exactly cv2.imread + cvtColor(BGR2RGB), and cb200_png_info gives cv2's size for each file the camera path takes."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -11,16 +9,14 @@ import pytest
 import libcimbar_b200 as cb
 from libcimbar_b200 import build as cbbuild
 from png_matrix import cv2_rgb, golden_files, matrix, premise
+from host_harness import build_harness
 
-ROOT = os.path.dirname(os.path.abspath(os.path.dirname(__file__)))
 FILES = golden_files() + matrix()
 
 
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("png_core") / "png_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(ROOT, "tests", "cpp", "png_core_host.cpp")])
-    lib = C.CDLL(so)
+    lib = build_harness(tmp_path_factory, "png_core_host")
     lib.pc_decode.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_int]
     lib.pc_info.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_int]
     return lib

@@ -4,23 +4,19 @@ both bits of one pair; a valid word sharpens a picture as the call with those fl
 extract status 2); and it keeps its receiver's CCM unchanged without a CC bit, or with CC_FIT in a mode that never fits.  All 64
 values of the six flag bits, and 100 000 random 32-bit words."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import libcimbar_b200 as cb
+from host_harness import build_harness
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PER_RECEIVER = cb.FLAG_SHARPEN | cb.FLAG_SHARPEN_IF_NEEDED | cb.FLAG_CC_SIMPLE | cb.FLAG_CC_FIT
 
 
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("receiver_flags") / "receiver_flags_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(ROOT, "tests", "cpp", "receiver_flags_host.cpp")])
-    lib = C.CDLL(so)
+    lib = build_harness(tmp_path_factory, "receiver_flags_host")
     lib.rf_rules.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     return lib
 

@@ -4,20 +4,16 @@ scan), against a sequential carry per receiver: a picture takes the fit of its r
 else its receiver's entry state, and each receiver's last picture writes the exit state.  The GPU test (tests/test_gpu_receivers.py)
 compares whole calls."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from host_harness import build_harness
 
 
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("receivers_core") / "receivers_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(ROOT, "tests", "cpp", "receivers_core_host.cpp")])
-    lib = C.CDLL(so)
+    lib = build_harness(tmp_path_factory, "receivers_core_host")
     lib.rc_carry.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.rc_order.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     return lib

@@ -9,6 +9,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from host_harness import build_harness
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INT_MIN, INT_MAX = -2 ** 31, 2 ** 31 - 1
 
@@ -24,9 +26,7 @@ def exe(tmp_path_factory):
 def make_order(tmp_path_factory):
     """make_order through the existing host harness of the carry (tests/cpp/receivers_core_host.cpp)"""
     import ctypes as C
-    so = str(tmp_path_factory.mktemp("receivers_core") / "receivers_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(ROOT, "tests", "cpp", "receivers_core_host.cpp")])
-    lib = C.CDLL(so)
+    lib = build_harness(tmp_path_factory, "receivers_core_host")
     lib.rc_order.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
 
     def run(of, receivers):

@@ -2,51 +2,24 @@
 host and run as a one-thread CTA against the oracle -- the logic check that is possible without a GPU.  The GPU parity test
 (tests/test_gpu_scan.py) runs the same comparisons through the C ABI."""
 import ctypes as C
-import os
-import subprocess
 
-import cv2
 import numpy as np
 import pytest
 
 import oracle_lib as ol
 from scan_oracle_lib import ScanOracle, join
+from host_harness import build_harness
+from cpu_support import pictures
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = ScanOracle()
 
 
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("scan_core") / "scan_core_host.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so,
-                           os.path.join(ROOT, "tests", "cpp", "scan_core_host.cpp")])
-    lib = C.CDLL(so)
+    lib = build_harness(tmp_path_factory, "scan_core_host", "-ffp-contract=off")
     lib.sc_scan.argtypes = [C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint), C.POINTER(C.c_int)]
     lib.sc_sort_check.argtypes = [C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     return lib
-
-
-def pictures():
-    """camera pictures, clean frames, rotations, shrunken and enlarged copies, and pictures without a code"""
-    out = []
-    for s in ("6bit/4_30_f0_627.jpg", "6bit/4_30_f2_734.jpg", "6bit/4_30_f2_246.jpg", "6bit/4_30_f1_360.jpg",
-              "6bit/4color_ecc30_fountain_0.png", "b/ex2434.jpg", "b/tr_0.png"):
-        out.append((s, ol.load_sample(s)))
-    cam = out[0][1]
-    out.append(("627 rot90", np.ascontiguousarray(np.rot90(cam))))
-    out.append(("627 rot180", np.ascontiguousarray(np.rot90(cam, 2))))
-    out.append(("627 x0.6", cv2.resize(cam, None, fx=0.6, fy=0.6, interpolation=cv2.INTER_AREA)))
-    out.append(("627 x1.7 (blur 5)", cv2.resize(cam, None, fx=1.7, fy=1.7)))
-    out.append(("627 cropped (anchor cut off)", np.ascontiguousarray(cam[:, 260:])))
-    out.append(("627 odd width (1277 x 957: no 4-byte aligned rows)", np.ascontiguousarray(cam[2:959, 1:1278])))
-    rng = np.random.default_rng(3)
-    out.append(("noise", rng.integers(0, 256, (480, 640, 3), dtype=np.uint8)))
-    out.append(("black", np.zeros((300, 400, 3), np.uint8)))
-    pad = np.full((1400, 1500, 3), 40, np.uint8)
-    pad[150:1174, 300:1324] = ol.load_sample("b/tr_1.png")
-    out.append(("clean frame on a dark table", pad))
-    return out
 
 
 @pytest.mark.parametrize("name,rgb", pictures(), ids=[p[0] for p in pictures()])
