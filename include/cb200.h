@@ -297,6 +297,18 @@ typedef struct cb200_picture {
    and the flags and outputs cb200_scan_extract_decode_chunks_ragged_dev refuses. */
 int cb200_scan_extract_decode_chunks_pictures_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags, uint8_t* d_chunks,
                                                   uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status);
+/* cb200_deskew_dev for n pictures described by pics[0 .. n) (HOST memory, read before the call returns), each in its own layout, size
+   and allocation: frame f = cv::warpPerspective(packed RGB copy of picture f, m9 + 9 f, Size(image_size_x, image_size_y),
+   INTER_LINEAR) (border constant 0) into d_dst + f x image_size_x x image_size_y x 3.  m9: n x 9 doubles on the HOST (the forward
+   transforms, e.g. cb200_camera_transforms of a camera call on the same pictures).  Enqueue-only on the context's stream: the call
+   returns without waiting for the device, the kernel does not wait for work on other streams that writes the pictures or d_dst, and
+   the pictures and d_dst belong to the stream until it passes the call.  CB200_ERR_ARG, before any CUDA call, for what
+   cb200_scan_extract_decode_chunks_pictures_dev refuses of the pictures (with its messages: short side 60 .. 4499 -- smaller
+   pictures go through cb200_deskew_dev), a null context, m9 or d_dst.  While the context has camera plans, a call of more pictures
+   than they reserved is refused as cb200_deskew_dev's is, naming the buffer: like that call it reserves the context's deskew frames
+   and exact walk workspace for n frames, which the plans froze, though it writes neither.  CB200_ERR_ARG with nothing enqueued for a
+   singular transform ("singular perspective transform"). */
+int cb200_deskew_pictures_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, const double* m9, uint8_t* d_dst);
 /* ---- several pictures of one frame ----------------------------------------------------------------------------------------------
 
    cb200_scan_extract_decode_chunks_pictures_dev plus one decode per group of pictures of the same frame, so that a frame no single

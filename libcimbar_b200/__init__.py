@@ -48,7 +48,7 @@ EXPORTS = [
     "cb200_camera_plan_create_receivers_pictures_dev", "cb200_camera_plan_create_detect_receivers_pictures_dev",
     "cb200_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_receivers_pictures_flags_dev",
     "cb200_detect_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_detect_receivers_pictures_flags_dev",
-    "cb200_scan_extract_decode_chunks_combined_dev", "cb200_scan_extract_decode_chunks_grouped_dev",
+    "cb200_scan_extract_decode_chunks_combined_dev", "cb200_scan_extract_decode_chunks_grouped_dev", "cb200_deskew_pictures_dev",
 ]
 
 
@@ -134,6 +134,7 @@ def load_library():
     lib.cb200_perspective_transform.argtypes = [vp, vp, vp]
     lib.cb200_deskew_dev.argtypes = [vp, u8p, C.c_int, C.c_int, C.c_int, vp, u8p]
     lib.cb200_deskew.argtypes = [vp, u8p, C.c_int, C.c_int, C.c_int, vp, u8p]
+    lib.cb200_deskew_pictures_dev.argtypes = [vp, vp, C.c_int, vp, u8p]
     lib.cb200_extract_decode_fountain.argtypes = [vp, u8p, C.c_int, C.c_int, C.c_int, vp, C.c_uint32, u8p, u32p, u32p, u8p]
     lib.cb200_extract_decode_fountain_dev.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_uint32, u8p, u32p, u32p, u8p]
     lib.cb200_scan.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
@@ -590,6 +591,16 @@ class Context:
         out = np.zeros((n, self.info.image_size_y, self.info.image_size_x, 3), dtype=np.uint8)
         _check(self.lib.cb200_deskew(self._h, src.ctypes.data, w, h, n, m.ctypes.data, out.ctypes.data))
         return out
+
+    def deskew_pictures_dev(self, tensors, m9, d_dst, order="rgb"):
+        """cv::warpPerspective of a list of uint8 CUDA tensors, each in its own layout and allocation (see picture(); order: one
+        string, or one per tensor), with the forward transforms m9 (n x 3 x 3 float64, host) into n frames of the mode's size at the
+        device address d_dst (cb200_deskew_pictures_dev).  Enqueue-only; keep the tensors alive until the stream has passed the call"""
+        descs = picture_descriptors(tensors, order)
+        m = np.ascontiguousarray(m9, dtype=np.float64).reshape(-1, 9)
+        if m.shape[0] != len(tensors):
+            raise Cb200Error(f"{m.shape[0]} transforms for {len(tensors)} pictures")
+        _check(self.lib.cb200_deskew_pictures_dev(self._h, descs.ctypes.data, len(tensors), m.ctypes.data, d_dst))
 
     def extract_decode_fountain(self, src, corners, flags=0):
         """camera images + their four anchor centres (tl, tr, bl, br) -> fountain chunks; the deskewed frames stay on the device"""

@@ -180,7 +180,8 @@ static int deskew_run(cb200_ctx* c, const CameraBatch& b, const double* m9, uint
     for (int f = 0; f < n; ++f) {
         if (!extract::invert3(m9 + (size_t)f * 9, inv + (size_t)f * 9)) return fail(CB200_ERR_ARG, "singular perspective transform");
         const cb200_picture& p = b.pics[(size_t)f];
-        desc[f] = PicDesc{reinterpret_cast<uint64_t>(p.data), 0, p.w, p.h, 0, 0, (uint64_t)p.row_pitch, 0, p.layout};
+        const uint64_t plane = p.layout == CB200_LAYOUT_RGB_PLANAR ? (uint64_t)p.plane_pitch : 0;     // ignored in the other layouts
+        desc[f] = PicDesc{reinterpret_cast<uint64_t>(p.data), 0, p.w, p.h, 0, 0, (uint64_t)p.row_pitch, plane, p.layout};
     }
     rc = c->upload.send(c->stream, slot, d->d_table, table_bytes); if (rc) return rc;
     const double* d_inv = reinterpret_cast<const double*>(d->d_table.get());
@@ -268,6 +269,18 @@ int cb200_deskew_dev(cb200_ctx* c, const uint8_t* d_src, int src_w, int src_h, i
 {
     CameraBatch b;
     int rc = deskew_batch(d_src, src_w, src_h, n, false, b);
+    if (rc || (rc = check_spans(b))) return rc;
+    if (!c || !m9 || !d_dst) return fail(CB200_ERR_ARG, !c ? "null context" : "null argument");
+    rc = check_frozen_deskew(c, n); if (rc) return rc;
+    if (n == 0) return CB200_OK;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    return deskew_run(c, b, m9, d_dst);
+}
+
+int cb200_deskew_pictures_dev(cb200_ctx* c, const cb200_picture* pics, int n, const double* m9, uint8_t* d_dst)
+{
+    CameraBatch b;
+    int rc = picture_batch(pics, n, b);
     if (rc || (rc = check_spans(b))) return rc;
     if (!c || !m9 || !d_dst) return fail(CB200_ERR_ARG, !c ? "null context" : "null argument");
     rc = check_frozen_deskew(c, n); if (rc) return rc;
