@@ -189,7 +189,7 @@ __device__ bool moore_penrose_lsm(const float* actual, const float* desired, int
     for (int i = 0; i < N * 3; ++i) z[i] = 0;
     double threshold = 0;
     for (int i = 0; i < 3; ++i) threshold = dadd(threshold, (double)W[i]);
-    threshold = dmul(threshold, (double)2.384185791015625e-07f);
+    threshold = dmul(threshold, (double)4.440892098500626e-16f);     // SVBkSb's (float)(DBL_EPSILON * 2) = 2^-51 (DESIGN §3)
     for (int i = 0; i < 3; ++i) {
         double wi = W[i];
         if (fabs(wi) <= threshold) continue;

@@ -47,8 +47,17 @@ __device__ __forceinline__ uint32_t best_color_ccm(const float* ccm, const Mode&
     const float r = dot3_rn(ccm[0], ccm[1], ccm[2], r0, g0, b0);
     const float g = dot3_rn(ccm[3], ccm[4], ccm[5], r0, g0, b0);
     const float b = dot3_rn(ccm[6], ccm[7], ccm[8], r0, g0, b0);
-    const float mx = fmaxf(fmaxf(r, g), fmaxf(b, 1.0f));
-    float mn = fminf(fminf(r, g), fminf(b, 48.0f));
+    // std::max({r, g, b, 1.0f}) / std::min({r, g, b, 48.0f}) are max_element / min_element: first element wins, a later one
+    // replaces it only when `<` holds.  So a NaN in r is both the max and the min (every channel then casts to 0), a NaN in g or
+    // b is skipped.  fmaxf / fminf would skip a NaN in r as well.  Only a matrix from cb200_set_ccm gets there (NaN in row 0 but
+    // not in every row); a zero von Kries denominator makes all three channels NaN, where both rules give the same colour
+    float mx = r, mn = r;
+    if (mx < g) mx = g;
+    if (mx < b) mx = b;
+    if (mx < 1.0f) mx = 1.0f;
+    if (g < mn) mn = g;
+    if (b < mn) mn = b;
+    if (48.0f < mn) mn = 48.0f;
     if (mn >= mx) mn = 0.0f;
     // float adjust = 255.0 / (max - min): a double division rounded to float in the reference.  For a float divisor d that
     // is the correctly rounded SINGLE quotient: the double quotient could only mis-round if it sat exactly on a float

@@ -573,6 +573,12 @@ unsigned cbo_best_color(float r, float g, float b, unsigned num_colors, unsigned
     return best_fit;
 }
 
+void cbo_best_colors(const uint8_t* means, int n, unsigned num_colors, unsigned color_mode, const float* ccm, uint8_t* out)
+{
+    for (int i = 0; i < n; ++i)
+        out[i] = (uint8_t)cbo_best_color((float)means[3 * i], (float)means[3 * i + 1], (float)means[3 * i + 2], num_colors, color_mode, ccm);
+}
+
 /* CimbDecoder's thread_local color_correction (CimbDecoder.cpp:69-85): set by update_color_correction, used by every
    get_best_color until replaced.  NULL deactivates it (TestableCimbDecoder::internal_ccm() = color_correction()). */
 static __thread float g_ccm[9];
@@ -709,8 +715,10 @@ static void jacobi_svd_f32(float* At, int astep, float* Wout, float* Vt, int m, 
     }
     for (int i = 0; i < n; ++i) Wout[i] = (float)W[i];
     for (int i = 0; i < n; ++i) {
-        /* (singular values <= FLT_MIN would get a random unit vector from cv::RNG(0x12345678): cannot happen for 3 colour
-           columns that span the colour space; treated as zero here) */
+        /* OpenCV gives a singular value <= FLT_MIN a random unit vector from cv::RNG(0x12345678) as its column of vt.  Grey
+           or equal rows do reach it (W = 0 exactly), but the result cannot depend on that vector: backSubst drops every
+           w <= threshold = sum(W) * 2^-51, and sum(W) >= |white| >= sqrt(3) (calculateWhite's floor of 1 per channel), so the
+           threshold is far above FLT_MIN and the column is never used.  A zero column stands in for it here. */
         double sd = W[i];
         float s = (float)(sd > (double)FLT_MIN ? 1 / sd : 0.);
         for (int k = 0; k < m; ++k) At[i * astep + k] *= s;
@@ -726,9 +734,11 @@ int cbo_moore_penrose_lsm(const float* actual, const float* desired, int rows, f
     /* SVD of y: u = Vt^T (3 x 3), vt = At (3 x N).  backSubst with no rhs: z (N x 3) = sum_i vt_i^T * (u column i / w_i) */
     float z[16 * 3];
     for (int i = 0; i < N * 3; ++i) z[i] = 0;
+    /* SVBkSb's threshold for the float SVD is sum(W) * (float)(DBL_EPSILON * 2) = sum(W) * 2^-51, not FLT_EPSILON's: on grey or
+       rank-2 colour rows the Jacobi sweeps leave a residual singular value of ~1e-8 sum(W) that OpenCV inverts (fits of 1e6..1e9) */
     double threshold = 0;
     for (int i = 0; i < 3; ++i) threshold += W[i];
-    threshold *= (float)(FLT_EPSILON * 2);
+    threshold *= (float)(DBL_EPSILON * 2);
     for (int i = 0; i < 3; ++i) {
         double wi = W[i];
         if (fabs(wi) <= threshold) continue;
@@ -795,6 +805,14 @@ int cbo_header_after_symbols(const uint8_t* blocks, const uint8_t* ok, unsigned 
 /* CimbReader::init_ccm, CimbReader.cpp:169-267 (color_correction == 2): colours the header predicts at the head of every
    colour-stream chunk -> per-colour average of the observed cell means -> + anchor white -> least-squares 3x3 fit.
    hdr/radioactive as left by the symbol pass.  Returns 1 and fills out when a matrix results, 0 when the reference bails. */
+static __thread float g_fit_actual[16 * 3], g_fit_desired[16 * 3];
+static __thread int g_fit_rows = 0;
+int cbo_last_fit_rows(float* actual, float* desired)
+{
+    memcpy(actual, g_fit_actual, sizeof(float) * 3 * (size_t)g_fit_rows);
+    memcpy(desired, g_fit_desired, sizeof(float) * 3 * (size_t)g_fit_rows);
+    return g_fit_rows;
+}
 int cbo_init_ccm(const cbo_mode* m, const uint8_t* rgb, int w, int h, const uint8_t hdr_in[6], unsigned radioactive, float out[9])
 {
     if ((hdr_in[0] | hdr_in[1] | hdr_in[2] | hdr_in[3]) == 0) return 0;
@@ -851,6 +869,9 @@ int cbo_init_ccm(const cbo_mode* m, const uint8_t* rgb, int w, int h, const uint
         desired[rows * 3] = desired[rows * 3 + 1] = desired[rows * 3 + 2] = 255.0f;
         ++rows;
     }
+    g_fit_rows = rows;
+    memcpy(g_fit_actual, actual, sizeof(float) * 3 * (size_t)rows);
+    memcpy(g_fit_desired, desired, sizeof(float) * 3 * (size_t)rows);
     return cbo_moore_penrose_lsm(actual, desired, rows, out);
 }
 

@@ -105,6 +105,8 @@ const uint64_t* cbo_tile_hashes(void);
 void cbo_avg_color(const uint8_t* rgb, int w, int x, int y, int cell_size, uint8_t out[3]);
 /* P9: CimbDecoder::get_best_color (CimbDecoder.cpp:168-200); ccm = 9 floats row-major or NULL */
 unsigned cbo_best_color(float r, float g, float b, unsigned num_colors, unsigned color_mode, const float* ccm);
+/* cbo_best_color of n integer means (r, g, b bytes), one call for a batch */
+void cbo_best_colors(const uint8_t* means, int n, unsigned num_colors, unsigned color_mode, const float* ccm, uint8_t* out);
 void cbo_palette(unsigned index, unsigned num_colors, unsigned color_mode, uint8_t rgb[3]);
 
 /* P3+P4+P5+P6+P8+P9+P7+P10: Decoder::do_decode / do_decode_coupled with use_ecc=false
@@ -126,6 +128,8 @@ int cbo_header_after_symbols(const uint8_t* blocks, const uint8_t* ok, unsigned 
                              uint8_t hdr[6], unsigned* radioactive_out);
 /* CimbReader::init_ccm (CimbReader.cpp:169-267); returns 1 when a matrix was fitted */
 int cbo_init_ccm(const cbo_mode* m, const uint8_t* rgb, int w, int h, const uint8_t hdr[6], unsigned radioactive, float out[9]);
+/* the N x 3 actual / desired rows the calling thread's last cbo_init_ccm fitted (white last); returns N (0 before any fit) */
+int cbo_last_fit_rows(float* actual, float* desired);
 /* Decoder::decode_fountain(img, stream, should_preprocess, color_correction) incl. color_correction == 2 */
 int cbo_decode_fountain_cc(const cbo_mode* m, const uint8_t* rgb, int w, int h, int needs_sharpen, int color_correction,
                            uint8_t* chunks_out, uint32_t* mask);

@@ -99,6 +99,8 @@ class Oracle:
         L.cbo_simple_ccm.argtypes = [C.POINTER(Mode), u8p, C.c_int, C.c_int, C.POINTER(C.c_float)]
         L.cbo_moore_penrose_lsm.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_float)]
         L.cbo_init_ccm.argtypes = [C.POINTER(Mode), u8p, C.c_int, C.c_int, u8p, C.c_uint, C.POINTER(C.c_float)]
+        L.cbo_best_colors.argtypes = [u8p, C.c_int, C.c_uint, C.c_uint, C.POINTER(C.c_float), u8p]
+        L.cbo_last_fit_rows.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float)]
         L.cbo_decode_fountain_cc.argtypes = [C.POINTER(Mode), u8p, C.c_int, C.c_int, C.c_int, C.c_int, u8p, C.POINTER(C.c_uint32)]
 
     def mode(self, mode_val=68):
@@ -163,6 +165,20 @@ class Oracle:
         a = np.ascontiguousarray(actual, np.float32); d = np.ascontiguousarray(desired, np.float32); o = np.zeros(9, np.float32)
         self.lib.cbo_moore_penrose_lsm(_ptr(a, C.c_float), _ptr(d, C.c_float), a.shape[0], _ptr(o, C.c_float))
         return o.reshape(3, 3)
+
+    def best_colors(self, means, num_colors, color_mode, ccm):
+        """cbo_best_color of every row of means ((n, 3) bytes) under ccm (9 floats, or None)"""
+        means = np.ascontiguousarray(means, dtype=np.uint8).reshape(-1, 3)
+        out = np.zeros(len(means), np.uint8)
+        cm = None if ccm is None else _ptr(np.ascontiguousarray(ccm, np.float32).reshape(9), C.c_float)
+        self.lib.cbo_best_colors(_ptr(means), len(means), num_colors, color_mode, cm, _ptr(out))
+        return out
+
+    def last_fit_rows(self):
+        """the actual / desired rows (N x 3 float32 each, white last) of the calling thread's last init_ccm"""
+        a, d = np.zeros(48, np.float32), np.zeros(48, np.float32)
+        n = self.lib.cbo_last_fit_rows(_ptr(a, C.c_float), _ptr(d, C.c_float))
+        return a[:3 * n].reshape(n, 3), d[:3 * n].reshape(n, 3)
 
     def init_ccm(self, m, rgb, hdr6, radioactive):
         rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
