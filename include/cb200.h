@@ -494,6 +494,43 @@ int cb200_camera_plan_create_receivers_pictures_flags_dev(cb200_ctx* ctx, const 
                                                           cb200_receiver_state* d_states, const uint32_t* d_receiver_flags, uint8_t* d_chunks,
                                                           uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status,
                                                           cb200_camera_plan** out);
+/* ---- grouped receivers: the pictures of one frame found within each receiver of a receivers batch ------------------------------
+
+   cb200_scan_extract_decode_chunks_grouped_dev for a decode service: the receivers call (or its flags form) plus one decode per group
+   of pictures of one frame, where a group never mixes receivers.  Two sessions that receive the same file show the same frames; their
+   pictures form separate groups, each decoded from its own session's pictures with its own session's colour correction.
+   Per picture: records, masks, frame flags, extract statuses, cb200_camera_transforms, cb200_get_frame_ccms and every d_states[r]
+   afterwards are bit for bit those of cb200_scan_extract_decode_chunks_receivers_dev on the same arguments (the _flags_ form:
+   cb200_scan_extract_decode_chunks_receivers_flags_dev).  The context's own CCM is neither read nor written.
+   The rule is the grouped call's, with match(i, j) also requiring receiver_of[i] == receiver_of[j]: within a receiver, in batch
+   order, a picture with extract status 1 or 2 joins the group of the earliest earlier leader of its own receiver that it matches and
+   whose group has fewer than 16 pictures, else it becomes a leader.  Groups are numbered in their leaders' batch order, across all
+   receivers.  A refused receiver's pictures (an invalid flags word: status CB200_EXTRACT_REFUSED) take part in no group.
+   d_group_of, d_group_count, d_group_chunks, d_group_mask and d_group_used are as for the grouped call (n / 2 slots);
+   d_group_receiver (device, n / 2 int32) gets the receiver of each group, whose fountain sink takes the group's record, and -1 past
+   the count, where the slots also get a zeroed record, mask 0 and 0 pictures.  n = 0 or 1 gives count 0.
+   So for every receiver r: on a context whose CCM is set to d_states[r] on entry (the _flags_ form: with flags | d_receiver_flags[r]),
+   cb200_scan_extract_decode_chunks_grouped_dev on r's pictures alone, in batch order, gives r's groups in slot order: the same records,
+   masks, used counts, and members (mapped back to batch indices).
+   Enqueue-only, with the receivers call's waits: the picture table, the map and the lists the pairing reads travel in its one
+   upload, and it launches six kernels more than the receivers call on the same batch.  The pairing's work grows with the sum over
+   receivers of their pictures squared, and no part of the call depends on n_receivers beyond what the receivers call does.
+   CB200_ERR_ARG, before any CUDA call: the flags form's table first, as in cb200_scan_extract_decode_chunks_receivers_flags_dev; then
+   the receiver arguments and a context linked to a CCM chain, as in the receivers call; then what the grouped call refuses, in its
+   order (the flags, the pictures, CB200_FLAG_NO_FALLBACK, a null group output -- d_group_receiver included --, the context, a null
+   output, n > max_frames), whatever n is. */
+int cb200_scan_extract_decode_chunks_grouped_receivers_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags,
+                                                           const int32_t* receiver_of, int n_receivers, cb200_receiver_state* d_states,
+                                                           uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                                                           int32_t* d_extract_status, int32_t* d_group_of, int32_t* d_group_count,
+                                                           uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used,
+                                                           int32_t* d_group_receiver);
+int cb200_scan_extract_decode_chunks_grouped_receivers_flags_dev(cb200_ctx* ctx, const cb200_picture* pics, int n, uint32_t flags,
+                                                                 const int32_t* receiver_of, int n_receivers, cb200_receiver_state* d_states,
+                                                                 const uint32_t* d_receiver_flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                                                 uint8_t* d_frame_flags, int32_t* d_extract_status, int32_t* d_group_of,
+                                                                 int32_t* d_group_count, uint8_t* d_group_chunks, uint32_t* d_group_mask,
+                                                                 int32_t* d_group_used, int32_t* d_group_receiver);
 /* cb200_camera_plan_create_detect_receivers (below) with its descriptors in DEVICE memory too, read at each launch within bounds, as
    above.  A slot is EMPTY exactly as in that plan (receiver out of range, or no candidate bit below n_modes): its descriptor is not
    read.  A non-empty slot whose descriptor is refused as above gets status CB200_EXTRACT_REFUSED and otherwise what an empty slot

@@ -49,6 +49,7 @@ EXPORTS = [
     "cb200_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_receivers_pictures_flags_dev",
     "cb200_detect_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_detect_receivers_pictures_flags_dev",
     "cb200_scan_extract_decode_chunks_combined_dev", "cb200_scan_extract_decode_chunks_grouped_dev", "cb200_deskew_pictures_dev",
+    "cb200_scan_extract_decode_chunks_grouped_receivers_dev", "cb200_scan_extract_decode_chunks_grouped_receivers_flags_dev",
 ]
 
 
@@ -186,6 +187,8 @@ def load_library():
     lib.cb200_scan_extract_decode_chunks_pictures_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_combined_dev.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_grouped_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.cb200_scan_extract_decode_chunks_grouped_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp] + [vp] * 10
+    lib.cb200_scan_extract_decode_chunks_grouped_receivers_flags_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp] + [vp] * 10
     lib.cb200_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp]
     lib.cb200_camera_plan_create_receivers.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, vp, vp]
@@ -849,6 +852,30 @@ class Context:
         _check(self.lib.cb200_scan_extract_decode_chunks_receivers_flags_dev(self._h, C.cast(descs, C.c_void_p), len(pictures), flags,
                                                                              of.ctypes.data, count, ptr, _flags_table(receiver_flags, count),
                                                                              d_chunks, d_mask, d_flags, d_status))
+
+    def scan_extract_decode_chunks_grouped_receivers_dev(self, pictures, receiver_of, states, d_chunks, d_mask, d_status, d_group_of,
+                                                         d_group_count, d_group_chunks, d_group_mask, d_group_used, d_group_receiver,
+                                                         d_flags=None, flags=0, order="rgb", receiver_flags=None):
+        """scan_extract_decode_chunks_receivers_dev plus the grouped call's groups found within each receiver
+        (cb200_scan_extract_decode_chunks_grouped_receivers_dev, or its _flags_ form with receiver_flags): a group never mixes
+        receivers, and d_group_receiver (int32, len(pictures) // 2 slots in device memory, -1 past the count) names the receiver of
+        each group, whose session takes its record.  The other outputs are as for scan_extract_decode_chunks_grouped_dev.
+        Enqueue-only"""
+        orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+        if len(orders) != len(pictures):
+            raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+        of = _receiver_map(receiver_of, len(pictures))
+        ptr, count = _states_ptr(states)
+        descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+        groups = (d_group_of, d_group_count, d_group_chunks, d_group_mask, d_group_used, d_group_receiver)
+        if receiver_flags is None:
+            _check(self.lib.cb200_scan_extract_decode_chunks_grouped_receivers_dev(
+                self._h, C.cast(descs, C.c_void_p), len(pictures), flags, of.ctypes.data, count, ptr, d_chunks, d_mask, d_flags, d_status,
+                *groups))
+            return
+        _check(self.lib.cb200_scan_extract_decode_chunks_grouped_receivers_flags_dev(
+            self._h, C.cast(descs, C.c_void_p), len(pictures), flags, of.ctypes.data, count, ptr, _flags_table(receiver_flags, count),
+            d_chunks, d_mask, d_flags, d_status, *groups))
 
     def camera_plan(self, wh, flags, pictures, chunks, mask, frame_flags, status):
         """scan_extract_decode_chunks_dev for pictures of sizes wh (n x (w, h), host) with these flags, captured once in a CUDA graph

@@ -21,6 +21,7 @@ namespace combine {
 
 constexpr int kMaxGroup = 16;       // pictures with one group index: the vote loop's bound, larger groups are refused
 constexpr uint8_t kValueBits = 0x7F;
+constexpr int kPairTile = 64;       // pictures per side of a k_pair_match tile (group.cu)
 
 // the winning value of k participating pictures' value bits v[0 .. k) and walk distances d[0 .. k), both in batch order (k >= 1)
 CB_HD uint8_t vote(const uint8_t* v, const uint8_t* d, int k)
@@ -124,18 +125,94 @@ CB_HD int differing_symbols(uint32_t a, uint32_t b)
 
 // match rows: row i holds bit j (word j / 32, bit j % 32) set iff match(i, j), for j < i; bits from i on are not read.  open: one bit
 // per picture, set while it is a leader whose group has fewer than kMaxGroup pictures.  open_matches: word w of row i's candidates
-CB_HD uint32_t open_matches(const uint32_t* row, const uint32_t* open, int i, int w)
+// j in [from, i) (from: the first picture of i's segment, below)
+CB_HD uint32_t open_matches(const uint32_t* row, const uint32_t* open, int i, int w, int from = 0)
 {
-    if (w > i >> 5) return 0;
+    if (w > i >> 5 || w < from >> 5) return 0;
     const uint32_t below = w < i >> 5 ? ~0u : (1u << (i & 31)) - 1u;
-    return row[w] & open[w] & below;
+    const uint32_t above = w > from >> 5 ? ~0u : ~((1u << (from & 31)) - 1u);
+    return row[w] & open[w] & below & above;
 }
 
-// picture i joins leader j (j == i: i leads a new group); size[] counts each leader's pictures
-CB_HD void join(int i, int j, int32_t* size, uint32_t* open)
+// picture i joins leader j (j == i: i leads a new group); size[] counts each leader's pictures.  shared: on the device, the open bits
+// change atomically, because k_assign_groups' warps work on segments that may share a word of `open` (several segments)
+CB_HD void join(int i, int j, int32_t* size, uint32_t* open, bool shared = false)
 {
+#if defined(__CUDA_ARCH__)
+    if (shared) {
+        if (j == i) { size[i] = 1; atomicOr(&open[i >> 5], 1u << (i & 31)); return; }
+        if (++size[j] == kMaxGroup) atomicAnd(&open[j >> 5], ~(1u << (j & 31)));
+        return;
+    }
+#endif
     if (j == i) { size[i] = 1; open[i >> 5] |= 1u << (i & 31); return; }
     if (++size[j] == kMaxGroup) open[j >> 5] &= ~(1u << (j & 31));
+}
+
+// ---- receivers (cb200_scan_extract_decode_chunks_grouped_receivers_dev): match(i, j) also requires receiver_of[i] == receiver_of[j].
+// The pictures are taken in the receiver-major order (receivers_core.cuh make_order: a stable counting sort of the receiver map), in
+// which each receiver's pictures form one segment [s, e) of positions, in batch order.  The match rows are indexed by position, so a
+// picture's candidates are the positions [s, p) of its own segment and the rule inside a segment is the one above.  The grouped call is
+// the one-receiver case: one segment, the identity order.
+//   pair_tiles: the kPairTile-position tile pairs (I, J <= I) of k_pair_match that hold at least one same-receiver pair p > q, each
+//               once, in increasing (I, J) order.  Their number is at most sum over segments of (tiles the segment spans)^2: it grows
+//               with the sum of n_r^2, and neither it nor the work depends on the number of receivers.
+//   segment_starts: the first position of every segment, then n.
+//   assign_segment: the assignment over one segment's positions: lead[p] = the position of p's leader (-1: does not take part).
+//   number_groups: groups numbered in their leaders' batch order, across the segments (lead and size indexed by batch index here).
+inline void pair_tiles(const int32_t* of, const int32_t* order, int n, int tile, std::vector<int32_t>& ij)
+{
+    std::vector<uint64_t> keys;
+    for (int s = 0, e; s < n; s = e) {
+        for (e = s + 1; e < n && of[order[e]] == of[order[s]]; ++e) {}
+        if (e - s < 2) continue;
+        const int t0 = s / tile, t1 = (e - 1) / tile;
+        for (int I = t0; I <= t1; ++I)
+            for (int J = t0; J <= I; ++J) {
+                // a diagonal tile needs two of the segment's positions in it
+                if (I == J && std::min(e, (I + 1) * tile) - std::max(s, I * tile) < 2) continue;
+                keys.push_back((uint64_t)I << 32 | (uint32_t)J);
+            }
+    }
+    std::sort(keys.begin(), keys.end());
+    keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+    ij.resize(2 * keys.size());
+    for (size_t k = 0; k < keys.size(); ++k) { ij[2 * k] = (int32_t)(keys[k] >> 32); ij[2 * k + 1] = (int32_t)(uint32_t)keys[k]; }
+}
+
+inline void segment_starts(const int32_t* of, const int32_t* order, int n, std::vector<int32_t>& starts)
+{
+    starts.clear();
+    for (int p = 0; p < n; ++p)
+        if (p == 0 || of[order[p]] != of[order[p - 1]]) starts.push_back(p);
+    starts.push_back(n);
+}
+
+// order: NULL for the identity.  k_assign_groups runs the same loop in one warp per segment, searching a row's words 32 at a time
+inline void assign_segment(const uint32_t* rows, size_t words, const int32_t* status, const int32_t* order, int s, int e, int32_t* lead,
+                           int32_t* size, uint32_t* open)
+{
+    for (int p = s; p < e; ++p) {
+        lead[p] = -1;
+        if (!takes_part(status[order ? order[p] : p])) continue;
+        int j = p;
+        for (int w = s >> 5; w <= p >> 5 && j == p; ++w) {
+            const uint32_t x = open_matches(rows + (size_t)p * words, open, p, w, s);
+            if (x) j = 32 * w + __builtin_ctz(x);
+        }
+        join(p, j, size, open);
+        lead[p] = j;
+    }
+}
+
+inline int number_groups(const int32_t* lead, const int32_t* size, int n, int32_t* group_of)
+{
+    std::vector<int32_t> number((size_t)n, -1);
+    int groups = 0;
+    for (int i = 0; i < n; ++i)
+        if (lead[i] == i && size[i] >= 2) number[(size_t)i] = groups++;
+    for (int i = 0; i < n; ++i) group_of[i] = lead[i] < 0 ? -1 : number[(size_t)lead[i]];
+    return groups;
 }
 
 // the assignment of the rule over n pictures' match rows (`words` words each) and extract statuses: group_of[0 .. n), returns the
@@ -144,22 +221,26 @@ inline int assign_groups(const uint32_t* rows, size_t words, const int32_t* stat
 {
     std::vector<uint32_t> open(words ? words : 1, 0u);
     std::vector<int32_t> size((size_t)n, 0), lead((size_t)n, -1);
-    for (int i = 0; i < n; ++i) {
-        if (!takes_part(status[i])) continue;
-        int j = i;
-        for (int w = 0; w <= i >> 5 && j == i; ++w) {
-            const uint32_t x = open_matches(rows + (size_t)i * words, open.data(), i, w);
-            if (x) j = 32 * w + __builtin_ctz(x);
-        }
-        join(i, j, size.data(), open.data());
-        lead[(size_t)i] = j;
+    assign_segment(rows, words, status, nullptr, 0, n, lead.data(), size.data(), open.data());
+    return number_groups(lead.data(), size.data(), n, group_of);
+}
+
+// the receivers form: rows indexed by position of the receiver-major order (map: the n receivers, then the order), statuses and
+// group_of by batch index.  Each segment is assigned on its own, then the leaders are numbered in batch order.  Returns the count
+inline int assign_receivers(const uint32_t* rows, size_t words, const int32_t* status, const int32_t* map, int n, int32_t* group_of)
+{
+    const int32_t* order = map + n;
+    std::vector<int32_t> starts;
+    segment_starts(map, order, n, starts);
+    std::vector<uint32_t> open(words ? words : 1, 0u);
+    std::vector<int32_t> psize((size_t)n, 0), plead((size_t)n, -1), size((size_t)n, 0), lead((size_t)n, -1);
+    for (size_t k = 0; k + 1 < starts.size(); ++k)
+        assign_segment(rows, words, status, order, starts[k], starts[k + 1], plead.data(), psize.data(), open.data());
+    for (int p = 0; p < n; ++p) {
+        lead[(size_t)order[p]] = plead[(size_t)p] < 0 ? -1 : order[plead[(size_t)p]];
+        size[(size_t)order[p]] = psize[(size_t)p];
     }
-    std::vector<int32_t> number((size_t)n, -1);
-    int groups = 0;
-    for (int i = 0; i < n; ++i)
-        if (lead[(size_t)i] == i && size[(size_t)i] >= 2) number[(size_t)i] = groups++;
-    for (int i = 0; i < n; ++i) group_of[i] = lead[(size_t)i] < 0 ? -1 : number[(size_t)lead[(size_t)i]];
-    return groups;
+    return number_groups(lead.data(), size.data(), n, group_of);
 }
 
 }  // namespace combine

@@ -329,7 +329,8 @@ struct cb200_ctx {
     cb200::DevBuf<uint8_t> d_combined;
     cb200::DevBuf<cb200::CellTrace> d_traces;
     // a grouped camera call (cb200_scan_extract_decode_chunks_grouped_dev): the pictures' match rows (n x ceil(n / 32) words) and the
-    // group table (n / 2 + 1 offsets, n members) followed by the assignment's scratch (2 n), both grown through grow()
+    // group table (n / 2 + 1 offsets, n members) followed by the assignment's scratch (2 n; 4 n for a grouped receivers call), both
+    // grown through grow()
     cb200::DevBuf<uint32_t> d_pairs;
     cb200::DevBuf<int32_t> d_groups;
     int ccm_frames = 0;              // frames of the last call that took the fitted-CCM route (cb200_get_frame_ccms)
@@ -363,8 +364,12 @@ inline void begin_timed_call(cb200_ctx* c) { if (c->timing) { c->cur = (int)(c->
 inline void mark(cb200_ctx* c) { if (c->timing && c->ev_count[c->cur] < 8) cudaEventRecord(c->ev[c->cur][c->ev_count[c->cur]++], c->stream); }
 
 // the groups of a grouped camera call's n >= 2 pictures, enqueued: the match rows into c->d_pairs, then d_group_of, d_group_count and
-// the group table of n / 2 slots in c->d_groups (offsets, members), from the final cell bytes and the extract statuses (group.cu)
-int find_groups(cb200_ctx* c, int n, const int32_t* d_status, int32_t* d_group_of, int32_t* d_group_count);
+// the group table of n / 2 slots in c->d_groups (offsets, members), from the final cell bytes and the extract statuses (group.cu).
+// lists: NULL for one receiver; else a grouped receivers call's device lists, all from its one upload: the receivers map
+// (Receivers::d_map: receivers, then the receiver-major order), the tile pairs k_pair_match takes (combine::pair_tiles), the segment
+// starts (combine::segment_starts, segs + 1 entries), and the output of each group's receiver.  Its c->d_groups holds 2 n ints more
+struct GroupLists { const int32_t* d_map; const int2* d_tiles; int ntiles; const int32_t* d_starts; int segs; int32_t* d_group_receiver; };
+int find_groups(cb200_ctx* c, int n, const int32_t* d_status, int32_t* d_group_of, int32_t* d_group_count, const GroupLists* lists = nullptr);
 
 // the groups of a combined camera call (cb200_scan_extract_decode_chunks_combined_dev): the host group_of (n entries), the number of
 // groups m and whether its three group outputs are all non-null.  check_groups: CB200_ERR_ARG for CB200_FLAG_NO_FALLBACK with m > 0,

@@ -966,17 +966,17 @@ int check_groups(uint32_t flags, const CameraGroups& g, int n)
     return CB200_OK;
 }
 
-// the combined and grouped calls' own buffers: the groups' cells and the pictures' traces, and with `pairs` (the grouped call) the
-// match rows and the group table with the assignment's scratch.  With live plans grow() makes no CUDA call and refuses what would
-// grow, so the calls run this before any CUDA call then
-static int combine_reserve(cb200_ctx* c, int n, int m, bool pairs)
+// the combined and grouped calls' own buffers: the groups' cells and the pictures' traces, and with `pairs` (the grouped calls) the
+// match rows and the group table with the assignment's scratch (`receivers`: the grouped receivers call's, 2 n ints more).  With
+// live plans grow() makes no CUDA call and refuses what would grow, so the calls run this before any CUDA call then
+static int combine_reserve(cb200_ctx* c, int n, int m, bool pairs, bool receivers = false)
 {
     const size_t cells = (size_t)c->mode.num_cells;
     int rc;
     if ((rc = grow(c, c->d_combined, (size_t)m * cells, "combined cells")) || (rc = grow(c, c->d_traces, (size_t)n * cells, "cell traces")))
         return rc;
     if (pairs && ((rc = grow(c, c->d_pairs, (size_t)n * (((size_t)n + 31) / 32), "match rows")) ||
-                  (rc = grow(c, c->d_groups, (size_t)m + 1 + 3 * (size_t)n, "group table"))))
+                  (rc = grow(c, c->d_groups, (size_t)m + 1 + (receivers ? 5 : 3) * (size_t)n, "group table"))))
         return rc;
     return CB200_OK;
 }
@@ -1014,18 +1014,20 @@ static int combine_empty(cb200_ctx* c, int m, uint8_t* d_group_chunks, uint32_t*
     return CB200_OK;
 }
 
-// camera_enqueue with the walk's traces kept and `tail` (or nothing) behind the picture table, at *d_tail on the device
+// camera_enqueue with the walk's traces kept and `tail` (or nothing) behind the picture table, at *d_tail on the device.  recv: a
+// grouped receivers call's receivers, whose map goes up between the table and the tail
 static int combine_pictures(cb200_ctx* c, const CameraBatch& b, int m, bool pairs, const std::vector<uint8_t>* tail, const uint8_t** d_tail,
-                            uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status)
+                            uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status,
+                            Receivers* recv = nullptr)
 {
     const int n = b.n();
     int rc;
-    if ((rc = combine_reserve(c, n, m, pairs)) || (rc = camera_reserve(c, b))) return rc;
+    if ((rc = combine_reserve(c, n, m, pairs, recv != nullptr)) || (rc = camera_reserve(c, b))) return rc;
     uint8_t* frames;
     if ((rc = deskew_frames(c, n, &frames))) return rc;
     const PicDesc* d_desc;
-    if ((rc = camera_scan(c, b, nullptr, &d_desc, nullptr, tail, d_tail))) return rc;
-    return camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, nullptr,
+    if ((rc = camera_scan(c, b, nullptr, &d_desc, recv, tail, d_tail))) return rc;
+    return camera_after_scan(c, c, b, d_desc, flags, frames, true, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, recv, nullptr,
                              c->d_traces);
 }
 
@@ -1080,6 +1082,33 @@ static int grouped_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, u
     int rc = combine_pictures(c, b, slots, true, nullptr, nullptr, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status);
     if (rc) return rc;
     if ((rc = find_groups(c, n, d_extract_status, d_group_of, d_group_count))) return rc;
+    return combine_groups(c, slots, c->d_groups, flags, d_extract_status, d_group_chunks, d_group_mask, d_group_used);
+}
+
+// ---- the grouped receivers call (cb200_scan_extract_decode_chunks_grouped_receivers_dev): the grouped call's rule within each
+// receiver.  After the argument checks, n >= 2: the receivers call with traces, whose one upload carries the picture table, the map
+// and the host lists of find_groups (combine::pair_tiles' tile pairs, then combine::segment_starts); find_groups with those lists;
+// combine_groups over the n / 2 slots.  Six launches more than the receivers call, and no wait of its own
+static int grouped_receivers_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, Receivers& r, uint8_t* d_chunks,
+                                     uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, int32_t* d_group_of,
+                                     int32_t* d_group_count, uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used,
+                                     int32_t* d_group_receiver)
+{
+    const int n = b.n(), slots = n / 2;
+    const int32_t* order = r.map.data() + n;
+    std::vector<int32_t> tiles, starts;
+    combine::pair_tiles(r.map.data(), order, n, combine::kPairTile, tiles);
+    combine::segment_starts(r.map.data(), order, n, starts);
+    std::vector<uint8_t> tail(sizeof(int32_t) * (tiles.size() + starts.size()));
+    memcpy(tail.data(), tiles.data(), sizeof(int32_t) * tiles.size());
+    memcpy(tail.data() + sizeof(int32_t) * tiles.size(), starts.data(), sizeof(int32_t) * starts.size());
+    const uint8_t* d_tail;
+    int rc = combine_pictures(c, b, slots, true, &tail, &d_tail, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &r);
+    if (rc) return rc;
+    const int ntiles = (int)(tiles.size() / 2);
+    const GroupLists lists = {r.d_map, reinterpret_cast<const int2*>(d_tail), ntiles, reinterpret_cast<const int32_t*>(d_tail) + 2 * (size_t)ntiles,
+                              (int)starts.size() - 1, d_group_receiver};
+    if ((rc = find_groups(c, n, d_extract_status, d_group_of, d_group_count, &lists))) return rc;
     return combine_groups(c, slots, c->d_groups, flags, d_extract_status, d_group_chunks, d_group_mask, d_group_used);
 }
 
@@ -1268,6 +1297,68 @@ int cb200_scan_extract_decode_chunks_receivers_flags_dev(cb200_ctx* c, const cb2
     auto build = [&](CameraBatch& b) { return picture_batch(pics, n, b); };
     const ReceiverArgs ra = {receiver_of, n, n_receivers, d_states, d_receiver_flags};
     return scan_extract_decode_dev(c, build, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, &ra);
+}
+
+// both grouped receivers entry points (ra->d_words: the flags form's table, checked by the caller).  The receivers call's checks,
+// then the grouped call's (check_camera_call with the groups: NO_FALLBACK and the six group outputs before the context)
+static int grouped_receivers(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, const ReceiverArgs& ra, uint8_t* d_chunks,
+                             uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, int32_t* d_group_of,
+                             int32_t* d_group_count, uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used,
+                             int32_t* d_group_receiver)
+{
+    CameraBatch b;
+    int rc = check_receivers(c, ra.of, ra.n, ra.count, ra.d_states); if (rc) return rc;
+    auto build = [&](CameraBatch& bb) { return picture_batch(pics, n, bb); };
+    const CameraGroups groups = {nullptr, 0, d_group_of && d_group_count && d_group_chunks && d_group_mask && d_group_used && d_group_receiver,
+                                 true};
+    rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output", &groups);
+    if (rc) return rc;
+    const int nb = b.n();
+    if (nb == 0) {
+        rc = empty_stripe(c, flags, true);
+    } else {
+        if ((rc = check_frozen_camera(c, b.wh.data(), nb)) ||
+            (nb >= 2 && !c->plans.empty() && (rc = combine_reserve(c, nb, nb / 2, true, true))))
+            return rc;
+        CK(cudaSetDevice(c->device), "cudaSetDevice");
+        Receivers r(ra.of, nb, ra.count, ra.d_states);
+        if ((r.d_words = ra.d_words)) { r.refused_bytes(nb); r.receivers = ra.count; }
+        if (nb >= 2)
+            return grouped_receivers_enqueue(c, b, flags, r, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, d_group_of,
+                                             d_group_count, d_group_chunks, d_group_mask, d_group_used, d_group_receiver);
+        rc = camera_enqueue(c, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, nullptr, &r);
+    }
+    if (rc) return rc;
+    // fewer than two pictures form no group, and there are no slots
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    CK(cudaMemsetAsync(d_group_of, 0xFF, sizeof(int32_t) * (size_t)nb, c->stream), "memset group_of");
+    CK(cudaMemsetAsync(d_group_count, 0, sizeof(int32_t), c->stream), "memset group count");
+    return CB200_OK;
+}
+
+int cb200_scan_extract_decode_chunks_grouped_receivers_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags,
+                                                           const int32_t* receiver_of, int n_receivers, cb200_receiver_state* d_states,
+                                                           uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                                                           int32_t* d_extract_status, int32_t* d_group_of, int32_t* d_group_count,
+                                                           uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used,
+                                                           int32_t* d_group_receiver)
+{
+    const ReceiverArgs ra = {receiver_of, n, n_receivers, d_states, nullptr};
+    return grouped_receivers(c, pics, n, flags, ra, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, d_group_of, d_group_count,
+                             d_group_chunks, d_group_mask, d_group_used, d_group_receiver);
+}
+
+int cb200_scan_extract_decode_chunks_grouped_receivers_flags_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags,
+                                                                 const int32_t* receiver_of, int n_receivers, cb200_receiver_state* d_states,
+                                                                 const uint32_t* d_receiver_flags, uint8_t* d_chunks, uint32_t* d_chunk_mask,
+                                                                 uint8_t* d_frame_flags, int32_t* d_extract_status, int32_t* d_group_of,
+                                                                 int32_t* d_group_count, uint8_t* d_group_chunks, uint32_t* d_group_mask,
+                                                                 int32_t* d_group_used, int32_t* d_group_receiver)
+{
+    int rc = check_receiver_flags(d_receiver_flags, flags); if (rc) return rc;
+    const ReceiverArgs ra = {receiver_of, n, n_receivers, d_states, d_receiver_flags};
+    return grouped_receivers(c, pics, n, flags, ra, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, d_group_of, d_group_count,
+                             d_group_chunks, d_group_mask, d_group_used, d_group_receiver);
 }
 
 int cb200_camera_transforms(cb200_ctx* c, double* m9_out, int n)
