@@ -346,6 +346,53 @@ int cb200_scan_extract_decode_chunks_grouped_dev(cb200_ctx* ctx, const cb200_pic
                                                  uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status,
                                                  int32_t* d_group_of, int32_t* d_group_count, uint8_t* d_group_chunks,
                                                  uint32_t* d_group_mask, int32_t* d_group_used);
+/* ---- grouped pictures across calls: a group history ---------------------------------------------------------------------------
+
+   A camera loop hands over one picture, or a few, per call, and a frame's pictures often fall into two calls, where the grouped call
+   cannot meet them.  A history keeps, on the device, the pictures of earlier calls that have not yet given a whole frame, and
+   cb200_scan_extract_decode_chunks_grouped_history_dev groups each batch against them as if they came first in the batch.
+   A history belongs to one context and holds at most `capacity` (H, 1 .. 256) pictures, oldest first.  For each it keeps the final
+   cell bytes (after colour correction) and walk distances its own call decoded, and a tag: call_number << 32 | batch index, where
+   call_number counts the history's accepted calls since create or reset, from 0.
+   A call on n pictures, with h pictures in the history:
+     per picture: records, masks, frame flags, extract statuses, cb200_camera_transforms, the sharpen selection, the CCM carry and
+             cb200_get_frame_ccms are bit for bit those of cb200_scan_extract_decode_chunks_pictures_dev on the same arguments.
+     positions: the history's pictures at [0, h), oldest first, then the batch at [h, h + n).  A history picture is always eligible,
+             a batch picture iff its extract status is 1 or 2.  The grouped call's match and assignment run over the positions
+             unchanged (half the cells' symbol bits agree; each picture joins the earliest open leader; at most 16 per group).
+     groups: a leader with at least one other member and at least one batch member (a group of history pictures only is not
+             decoded again), numbered in the leaders' position order.  d_group_of (n entries) gets each batch picture's group or -1,
+             d_group_count the count.  d_group_chunks / d_group_mask / d_group_used are n slots (each group may be one batch picture
+             with a history leader): slots [0, count) the vote of the members in position order (so "earliest" is the oldest
+             picture), decoded as by the combined call; the other slots a zeroed record, mask 0 and 0 pictures.
+     new history: a record is complete when its mask has all chunks_per_frame bits set (as it does when every block decodes); a
+             group is done when its record or one of its batch members' own records is complete.  In position order the history
+             keeps every history picture not in a done group and every eligible batch picture whose own record is not complete and
+             that is not in a done group; of those the last H stay.  A decoded frame's pictures leave at once, the rest first in,
+             first out.
+     n = 0: the history and every output stay untouched; the call still counts.
+   With an empty history (a new one, or after reset) the call gives exactly the grouped call's d_group_of, count and slots
+   [0, count); only the slot count differs (n, not n / 2).
+   Enqueue-only, with the pictures call's waits and none of its own: h stays on the device, so the launches are sized for H + n
+   positions; the call launches nine kernels more than the pictures call and makes three device-to-device copies.  The history's
+   buffers are the call's: one history serves one sequence of calls on its context's stream.
+   CB200_ERR_ARG, before any CUDA call: everything the grouped call refuses, in its order (CB200_FLAG_NO_FALLBACK and a null group
+   output included); then a null history or one created on another context.  While the context has camera plans, a call whose
+   context buffers would grow is refused as the grouped call's is.
+     create: CB200_ERR_ARG for a null out, a null context, a capacity outside [1, 256].
+     reset: enqueued on the context's stream: h = 0, call number 0.
+     read: synchronises the context's stream; *count = h and tags[0 .. min(h, max)) the tags, oldest first.  CB200_ERR_ARG for a
+             null history, a null count, max < 0, null tags with max > 0.
+     destroy: frees the history; call it before cb200_destroy of its context. */
+typedef struct cb200_group_history cb200_group_history;
+int cb200_group_history_create(cb200_ctx* ctx, int capacity, cb200_group_history** out);
+int cb200_group_history_reset(cb200_group_history* h);
+int cb200_group_history_read(cb200_group_history* h, int64_t* tags, int max, int32_t* count);
+int cb200_group_history_destroy(cb200_group_history* h);
+int cb200_scan_extract_decode_chunks_grouped_history_dev(cb200_ctx* ctx, cb200_group_history* h, const cb200_picture* pics, int n,
+                                                         uint32_t flags, uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                                                         int32_t* d_extract_status, int32_t* d_group_of, int32_t* d_group_count,
+                                                         uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used);
 /* ---- receivers: pictures of many decoders in one batch ------------------------------------------------------------------------
 
    A batch of the calls above is one decoder: under CC_FIT a picture without a usable header takes the matrix of the picture before

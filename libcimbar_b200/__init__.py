@@ -50,6 +50,8 @@ EXPORTS = [
     "cb200_detect_scan_extract_decode_chunks_receivers_flags_dev", "cb200_camera_plan_create_detect_receivers_pictures_flags_dev",
     "cb200_scan_extract_decode_chunks_combined_dev", "cb200_scan_extract_decode_chunks_grouped_dev", "cb200_deskew_pictures_dev",
     "cb200_scan_extract_decode_chunks_grouped_receivers_dev", "cb200_scan_extract_decode_chunks_grouped_receivers_flags_dev",
+    "cb200_group_history_create", "cb200_group_history_reset", "cb200_group_history_read", "cb200_group_history_destroy",
+    "cb200_scan_extract_decode_chunks_grouped_history_dev",
 ]
 
 
@@ -187,6 +189,11 @@ def load_library():
     lib.cb200_scan_extract_decode_chunks_pictures_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_combined_dev.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp, vp, vp]
     lib.cb200_scan_extract_decode_chunks_grouped_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.cb200_group_history_create.argtypes = [vp, C.c_int, C.POINTER(C.c_void_p)]
+    lib.cb200_group_history_reset.argtypes = [vp]
+    lib.cb200_group_history_read.argtypes = [vp, vp, C.c_int, vp]
+    lib.cb200_group_history_destroy.argtypes = [vp]
+    lib.cb200_scan_extract_decode_chunks_grouped_history_dev.argtypes = [vp, vp, vp, C.c_int, C.c_uint32] + [vp] * 9
     lib.cb200_scan_extract_decode_chunks_grouped_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp] + [vp] * 10
     lib.cb200_scan_extract_decode_chunks_grouped_receivers_flags_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp] + [vp] * 10
     lib.cb200_decode_chunks_receivers_dev.argtypes = [vp, vp, C.c_int, C.c_uint32, vp, C.c_int, vp, vp, vp, vp]
@@ -825,6 +832,27 @@ class Context:
             self._h, C.cast(descs, C.c_void_p), len(pictures), flags, d_chunks, d_mask, d_flags, d_status, d_group_of, d_group_count,
             d_group_chunks, d_group_mask, d_group_used))
 
+    def group_history(self, capacity):
+        """a group history of this context holding at most `capacity` (1 .. 256) pictures (cb200_group_history_create), for
+        scan_extract_decode_chunks_grouped_history_dev.  Close it before the context"""
+        h = C.c_void_p()
+        _check(self.lib.cb200_group_history_create(self._h, capacity, C.byref(h)))
+        return GroupHistory(self, h, capacity)
+
+    def scan_extract_decode_chunks_grouped_history_dev(self, pictures, history, d_chunks, d_mask, d_status, d_group_of, d_group_count,
+                                                       d_group_chunks, d_group_mask, d_group_used, d_flags=None, flags=0, order="rgb"):
+        """scan_extract_decode_chunks_grouped_dev over the pictures of earlier calls that have not yet given a whole frame, then the
+        batch (cb200_scan_extract_decode_chunks_grouped_history_dev): `history` (group_history) comes first in the positions, a group
+        needs a picture of this batch, and the history keeps what is left undecoded.  d_group_of / d_group_count as for the grouped
+        call; d_group_chunks / d_group_mask / d_group_used are len(pictures) slots in device memory.  Enqueue-only"""
+        orders = [order] * len(pictures) if isinstance(order, str) else list(order)
+        if len(orders) != len(pictures):
+            raise Cb200Error(f"{len(orders)} orders for {len(pictures)} pictures")
+        descs = (Picture * max(1, len(pictures)))(*[picture(t, o) for t, o in zip(pictures, orders)])
+        _check(self.lib.cb200_scan_extract_decode_chunks_grouped_history_dev(
+            self._h, None if history is None else history._h, C.cast(descs, C.c_void_p), len(pictures), flags, d_chunks, d_mask, d_flags,
+            d_status, d_group_of, d_group_count, d_group_chunks, d_group_mask, d_group_used))
+
     def decode_chunks_receivers_dev(self, d_rgb, n, receiver_of, states, d_chunks, d_mask, d_flags=None, flags=0):
         """decode_chunks_dev for frames of several receivers: frame i belongs to receiver receiver_of[i] (host), each receiver decodes
         with its own state in `states` (receiver_states) and leaves its new one there.  Enqueue-only"""
@@ -1059,6 +1087,34 @@ class Context:
 
     def render_frames_dev(self, d_cellvals, n, d_rgb_out):
         _check(self.lib.cb200_render_frames_dev(self._h, d_cellvals, n, d_rgb_out))
+
+
+class GroupHistory:
+    """a group history (cb200_group_history_*) of one context: reset() empties it in stream order, tags() synchronises and returns its
+    pictures' tags (call_number << 32 | batch index, oldest first) as an int64 numpy array.  Close it before its context"""
+
+    def __init__(self, ctx, handle, capacity):
+        self.ctx, self._h, self.capacity = ctx, handle, capacity
+
+    def reset(self):
+        _check(self.ctx.lib.cb200_group_history_reset(self._h))
+
+    def tags(self):
+        tags = np.zeros(self.capacity, np.int64)
+        count = C.c_int32()
+        _check(self.ctx.lib.cb200_group_history_read(self._h, tags.ctypes.data, self.capacity, C.byref(count)))
+        return tags[:count.value].copy()
+
+    def close(self):
+        if self._h and self.ctx._h:
+            self.ctx.lib.cb200_group_history_destroy(self._h)
+        self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class CameraPlan:

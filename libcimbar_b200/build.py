@@ -16,7 +16,7 @@ OBJ = os.path.join(HERE, "lib", "obj")
 LIB = os.path.join(HERE, "lib", "libcb200.so")
 SOURCES = ["api.cu", "k1_decode.cu", "k1x_flood.cu", "k2_rs.cu", "render.cu", "encode.cu", "host_sink.cu", "ccm.cu",
            "gather.cu", "chain.cu", "deskew.cu", "scan.cu", "files.cu", "jpeg.cu", "png.cu", "plan.cu",
-           "detect.cu", "group.cu"]
+           "detect.cu", "group.cu", "history.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 

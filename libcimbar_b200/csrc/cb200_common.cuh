@@ -28,6 +28,7 @@ public:
         if (e == cudaSuccess) cap_ = count; else p_ = nullptr;
         return e;
     }
+    void swap(Buffer& o) { T* p = p_; p_ = o.p_; o.p_ = p; const size_t c = cap_; cap_ = o.cap_; o.cap_ = c; }
     T* get() const { return p_; }
     operator T*() const { return p_; }
     size_t capacity() const { return cap_; }   // elements

@@ -243,5 +243,69 @@ inline int assign_receivers(const uint32_t* rows, size_t words, const int32_t* s
     return number_groups(lead.data(), size.data(), n, group_of);
 }
 
+// ---- a history (cb200_scan_extract_decode_chunks_grouped_history_dev): the grouped call's rule over a batch that follows the
+// undecoded pictures of earlier calls.  The device lays out N = H + n positions: history slot s < H holds the s-th oldest history
+// picture when s < h (position status 1: always eligible) and is empty otherwise (status 0: never eligible); batch picture i sits
+// at position first = H plus i with its extract status.  The empty slots take part in nothing, so the assignment over the positions
+// is the rule's over [0, h) followed by the batch.  Then:
+//   groups:   a group of the assignment that has a batch member (its last member, in position order, lies at or after `first`);
+//             the others (history pictures only) are not decoded again.  Numbered in their leaders' position order.
+//   complete: a record whose chunk mask has all chunks_per_frame bits set (k_chunk_mask sets them all when every block decodes).
+//   done:     a group whose record is complete or one of whose batch members' own records is complete.
+//   keep:     a position that is eligible, is in no done group and, in the batch, whose own record is not complete; of those the
+//             last H stay, oldest first (keep_destination), so the pictures of a decoded frame leave at once and the rest first in,
+//             first out.
+// history_number and history_keep are the host restatements of k_history_groups and k_history_keep (history.cu), which apply the
+// same helpers per position
+CB_HD int32_t history_slot_status(int s, int h) { return s < h ? 1 : 0; }
+
+CB_HD uint32_t complete_mask(int chunks_per_frame) { return chunks_per_frame >= 32 ? ~0u : (1u << chunks_per_frame) - 1u; }
+
+CB_HD bool complete(uint32_t mask, int chunks_per_frame) { return mask == complete_mask(chunks_per_frame); }
+
+CB_HD bool has_batch_member(int last_member, int first) { return last_member >= first; }
+
+CB_HD bool keeps(int p, int first, int32_t status, bool own_complete, bool group_done)
+{
+    return takes_part(status) && !group_done && (p < first || !own_complete);
+}
+
+// the slot of the rank-th of `kept` kept positions among the last `capacity` of them, or < 0 when it leaves
+CB_HD int keep_destination(int rank, int kept, int capacity) { return rank - (kept > capacity ? kept - capacity : 0); }
+
+// the groups of the call from the assignment over the positions (of[0 .. N), m groups): pos_group[p] = p's group of the call or -1.
+// Returns the number of groups
+inline int history_number(const int32_t* of, int N, int first, int m, int32_t* pos_group)
+{
+    std::vector<int32_t> last((size_t)(m > 0 ? m : 0), -1), number((size_t)(m > 0 ? m : 0), -1);
+    for (int p = 0; p < N; ++p) if (of[p] >= 0) last[(size_t)of[p]] = p;
+    int groups = 0;
+    for (int g = 0; g < m; ++g) if (has_batch_member(last[(size_t)g], first)) number[(size_t)g] = groups++;
+    for (int p = 0; p < N; ++p) pos_group[p] = of[p] < 0 ? -1 : number[(size_t)of[p]];
+    return groups;
+}
+
+// the new history: own[i] the batch pictures' chunk masks, gmask[g] the groups' (count groups), status the positions'.  src[s] = the
+// position of the new slot s (s < the returned h); the history keeps `capacity` pictures at most
+inline int history_keep(const int32_t* status, int N, int first, const uint32_t* own, const int32_t* pos_group, int count,
+                        const uint32_t* gmask, int chunks_per_frame, int capacity, int32_t* src)
+{
+    std::vector<uint8_t> done((size_t)(count > 0 ? count : 0), 0);
+    for (int g = 0; g < count; ++g) done[(size_t)g] = complete(gmask[g], chunks_per_frame);
+    for (int p = first; p < N; ++p)
+        if (pos_group[p] >= 0 && complete(own[p - first], chunks_per_frame)) done[(size_t)pos_group[p]] = 1;
+    std::vector<int32_t> kept;
+    for (int p = 0; p < N; ++p) {
+        const bool own_complete = p >= first && complete(own[p - first], chunks_per_frame);
+        if (keeps(p, first, status[p], own_complete, pos_group[p] >= 0 && done[(size_t)pos_group[p]])) kept.push_back(p);
+    }
+    int h = 0;
+    for (int r = 0; r < (int)kept.size(); ++r) {
+        const int s = keep_destination(r, (int)kept.size(), capacity);
+        if (s >= 0) { src[s] = kept[(size_t)r]; h = s + 1; }
+    }
+    return h;
+}
+
 }  // namespace combine
 }  // namespace cb200

@@ -368,8 +368,29 @@ inline void mark(cb200_ctx* c) { if (c->timing && c->ev_count[c->cur] < 8) cudaE
 // lists: NULL for one receiver; else a grouped receivers call's device lists, all from its one upload: the receivers map
 // (Receivers::d_map: receivers, then the receiver-major order), the tile pairs k_pair_match takes (combine::pair_tiles), the segment
 // starts (combine::segment_starts, segs + 1 entries), and the output of each group's receiver.  Its c->d_groups holds 2 n ints more
+// d_cellvals: the pictures' final cells when they are not c->d_cellvals (a history's staging region, whose positions are the pictures)
 struct GroupLists { const int32_t* d_map; const int2* d_tiles; int ntiles; const int32_t* d_starts; int segs; int32_t* d_group_receiver; };
-int find_groups(cb200_ctx* c, int n, const int32_t* d_status, int32_t* d_group_of, int32_t* d_group_count, const GroupLists* lists = nullptr);
+int find_groups(cb200_ctx* c, int n, const int32_t* d_status, int32_t* d_group_of, int32_t* d_group_count, const GroupLists* lists = nullptr,
+                const uint8_t* d_cellvals = nullptr);
+
+// a group history (cb200_group_history, history.cu): two staging regions of H history slots followed by a batch (cell bytes, traces,
+// position statuses), used alternately, and the history's scratch.  history_check: CB200_ERR_ARG for a null history or one of
+// another context (no CUDA call).  history_positions: H.  history_reserve: the history's own buffers for a batch of n (after the
+// argument checks; a CUDA call when they grow).  history_groups: the batch's final cells, traces and statuses (c->d_cellvals,
+// c->d_traces, d_status) copied behind the history, the grouped call's pairing and assignment over the H + n positions, then the
+// groups with a batch member (k_history_groups) into d_group_of, d_group_count and the table of n slots *st describes.
+// history_settle: the new history from the batch's and the groups' chunk masks (k_history_keep, k_history_copy) into the other
+// region.  history_skip: a call without pictures, counted
+struct HistoryStage { const uint8_t* cells; const CellTrace* traces; const int32_t* status; const int32_t* table; };
+int history_check(const cb200_ctx* c, const cb200_group_history* h);
+int history_positions(const cb200_group_history* h);
+int history_reserve(cb200_ctx* c, cb200_group_history* h, int n);
+int history_groups(cb200_ctx* c, cb200_group_history* h, int n, const int32_t* d_status, int32_t* d_group_of, int32_t* d_group_count,
+                   HistoryStage* st);
+int history_settle(cb200_ctx* c, cb200_group_history* h, int n, const uint32_t* d_chunk_mask, const int32_t* d_group_count,
+                   const uint32_t* d_group_mask);
+constexpr int kMaxHistory = 256;
+void history_skip(cb200_group_history* h);
 
 // the groups of a combined camera call (cb200_scan_extract_decode_chunks_combined_dev): the host group_of (n entries), the number of
 // groups m and whether its three group outputs are all non-null.  check_groups: CB200_ERR_ARG for CB200_FLAG_NO_FALLBACK with m > 0,

@@ -207,13 +207,15 @@ __global__ void __launch_bounds__(32 * kAssignWarps) k_assign_groups(int n, int 
     }
 }
 
-int find_groups(cb200_ctx* c, int n, const int32_t* d_status, int32_t* d_group_of, int32_t* d_group_count, const GroupLists* lists)
+int find_groups(cb200_ctx* c, int n, const int32_t* d_status, int32_t* d_group_of, int32_t* d_group_count, const GroupLists* lists,
+                const uint8_t* d_cellvals)
 {
     const Mode& md = c->mode;
     const int slots = n / 2;
     const long long tiles = (n + kPairTile - 1) / kPairTile;
     const unsigned grid = lists ? (unsigned)std::max(lists->ntiles, 1) : (unsigned)(tiles * (tiles + 1) / 2);
-    k_pair_match<<<grid, kPairThreads, 0, c->stream>>>(n, md.num_cells, md.symbol_bits, c->d_cellvals, d_status, c->d_pairs,
+    k_pair_match<<<grid, kPairThreads, 0, c->stream>>>(n, md.num_cells, md.symbol_bits, d_cellvals ? d_cellvals : c->d_cellvals.get(),
+                                                        d_status, c->d_pairs,
                                                         lists ? lists->d_map : nullptr, lists ? lists->d_tiles : nullptr,
                                                         lists ? lists->ntiles : 0);
     count_launch();

@@ -1033,14 +1033,17 @@ static int combine_pictures(cb200_ctx* c, const CameraBatch& b, int m, bool pair
 
 // the vote and the decode of the m groups of the table at d_table (offsets[0 .. m], then the members): the route of a call without
 // colour correction (k2_rs_fused_launch: the frame-pair kernel where it applies), the chunk masks, and mask 0 for a group without
-// pictures (k_mask_failed on the counts).  Four launches
+// pictures (k_mask_failed on the counts).  The members' cells and traces: the context's (d_cellvals, d_traces), or a history's
+// staging region (members are then its positions).  Four launches
 static int combine_groups(cb200_ctx* c, int m, const int32_t* d_table, uint32_t flags, const int32_t* d_extract_status, uint8_t* d_group_chunks,
-                          uint32_t* d_group_mask, int32_t* d_group_used)
+                          uint32_t* d_group_mask, int32_t* d_group_used, const uint8_t* d_cellvals = nullptr,
+                          const CellTrace* d_traces = nullptr)
 {
     const Mode& md = c->mode;
     const long long threads = (long long)m * md.num_cells;
     k_combine<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(m, md.num_cells, d_table, d_table + m + 1, d_extract_status,
-                                                                       c->d_cellvals, c->d_traces, c->d_combined, d_group_used);
+                                                                       d_cellvals ? d_cellvals : c->d_cellvals.get(),
+                                                                       d_traces ? d_traces : c->d_traces.get(), c->d_combined, d_group_used);
     count_launch();
     CK(cudaGetLastError(), "combine launch");
     const uint16_t* idx = (flags & CB200_FLAG_NO_INTERLEAVE) ? c->d_idx_ident.get() : c->d_idx.get();
@@ -1083,6 +1086,35 @@ static int grouped_enqueue(cb200_ctx* c, const CameraBatch& b, uint32_t flags, u
     if (rc) return rc;
     if ((rc = find_groups(c, n, d_extract_status, d_group_of, d_group_count))) return rc;
     return combine_groups(c, slots, c->d_groups, flags, d_extract_status, d_group_chunks, d_group_mask, d_group_used);
+}
+
+// ---- the grouped history call (cb200_scan_extract_decode_chunks_grouped_history_dev): the grouped call over a batch that follows a
+// history's pictures.  Its own buffers on the context: n voted frames and traces, and the pairing and assignment over N = H + n
+// positions.  With live plans grow() refuses before any CUDA call
+static int history_reserve_ctx(cb200_ctx* c, int N, int n)
+{
+    int rc;
+    if ((rc = combine_reserve(c, n, n, false)) || (rc = grow(c, c->d_pairs, (size_t)N * (((size_t)N + 31) / 32), "match rows")) ||
+        (rc = grow(c, c->d_groups, (size_t)(N / 2) + 1 + 3 * (size_t)N, "group table")))
+        return rc;
+    return CB200_OK;
+}
+
+// after the argument checks, n >= 1: the pictures call with traces; history_groups (the batch staged behind the history, the
+// pairing, the assignment and the groups with a batch member); the vote and decode of n slots from the staging region; history_settle
+// (the new history).  Nine launches more than the pictures call (three more than the grouped call), three device copies, no wait
+static int grouped_history_enqueue(cb200_ctx* c, cb200_group_history* h, const CameraBatch& b, uint32_t flags, uint8_t* d_chunks,
+                                   uint32_t* d_chunk_mask, uint8_t* d_frame_flags, int32_t* d_extract_status, int32_t* d_group_of,
+                                   int32_t* d_group_count, uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    const int n = b.n();
+    int rc;
+    if ((rc = history_reserve_ctx(c, history_positions(h) + n, n)) || (rc = history_reserve(c, h, n))) return rc;
+    if ((rc = combine_pictures(c, b, n, false, nullptr, nullptr, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status))) return rc;
+    HistoryStage st;
+    if ((rc = history_groups(c, h, n, d_extract_status, d_group_of, d_group_count, &st))) return rc;
+    if ((rc = combine_groups(c, n, st.table, flags, st.status, d_group_chunks, d_group_mask, d_group_used, st.cells, st.traces))) return rc;
+    return history_settle(c, h, n, d_chunk_mask, d_group_count, d_group_mask);
 }
 
 // ---- the grouped receivers call (cb200_scan_extract_decode_chunks_grouped_receivers_dev): the grouped call's rule within each
@@ -1277,6 +1309,31 @@ int cb200_scan_extract_decode_chunks_grouped_dev(cb200_ctx* c, const cb200_pictu
     CK(cudaMemsetAsync(d_group_of, 0xFF, sizeof(int32_t) * (size_t)nb, c->stream), "memset group_of");
     CK(cudaMemsetAsync(d_group_count, 0, sizeof(int32_t), c->stream), "memset group count");
     return CB200_OK;
+}
+
+int cb200_scan_extract_decode_chunks_grouped_history_dev(cb200_ctx* c, cb200_group_history* h, const cb200_picture* pics, int n, uint32_t flags,
+                                                         uint8_t* d_chunks, uint32_t* d_chunk_mask, uint8_t* d_frame_flags,
+                                                         int32_t* d_extract_status, int32_t* d_group_of, int32_t* d_group_count,
+                                                         uint8_t* d_group_chunks, uint32_t* d_group_mask, int32_t* d_group_used)
+{
+    CameraBatch b;
+    auto build = [&](CameraBatch& bb) { return picture_batch(pics, n, bb); };
+    const CameraGroups groups = {nullptr, 0, d_group_of && d_group_count && d_group_chunks && d_group_mask && d_group_used, true};
+    int rc = check_camera_call(c, flags, build, b, d_chunks && d_chunk_mask && d_extract_status ? nullptr : "null output", &groups);
+    if (rc || (rc = history_check(c, h))) return rc;
+    const int nb = b.n();
+    if (nb == 0) {
+        // the history and the group outputs stay as they are; the call is counted
+        if ((rc = empty_stripe(c, flags, true))) return rc;
+        history_skip(h);
+        return CB200_OK;
+    }
+    if ((rc = check_frozen_camera(c, b.wh.data(), nb)) ||
+        (!c->plans.empty() && (rc = history_reserve_ctx(c, history_positions(h) + nb, nb))))
+        return rc;
+    CK(cudaSetDevice(c->device), "cudaSetDevice");
+    return grouped_history_enqueue(c, h, b, flags, d_chunks, d_chunk_mask, d_frame_flags, d_extract_status, d_group_of, d_group_count,
+                                   d_group_chunks, d_group_mask, d_group_used);
 }
 
 int cb200_scan_extract_decode_chunks_receivers_dev(cb200_ctx* c, const cb200_picture* pics, int n, uint32_t flags, const int32_t* receiver_of,
